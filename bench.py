@@ -1,7 +1,7 @@
 """Headline benchmark: FL rounds/sec (device-timed, max over ranks) -- CIFAR-10 ResNet-18, FedAvg, bf16,
 num_agents = number of GPUs, local_ep=2, bs=256, 50,000 synthetic CIFAR-shaped training images (BASELINE.json).
 
-    python bench.py [--gpus N --steps K --warmup W] [--impl ours|reference]
+    python bench.py [--gpus N --steps K --warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -9,6 +9,10 @@ A "step" is one federated round = every agent trains local_ep epochs on its shar
 parallel) + fused aggregation / server step / parameter hand-off.  Total work per round is fixed (the 50k-image
 dataset is split over the agents), so scaling is STRONG.  Evaluation is outside the timed region for both arms
 (BASELINE.md section 2).  Rank 0 prints ONE JSON line.
+
+--dump-outputs DIR (ours): after the timed rounds, rank 0 writes what the last timed round produced -- the global parameter
+vector after aggregation, the round's summed training loss and its flipped-coordinate count -- as DIR/<name>.npy (float32 /
+float64, at most 64 MB), so two builds run with the same arguments (same seeded inputs) can be compared output for output.
 """
 from __future__ import annotations
 
@@ -51,11 +55,35 @@ def parse():
     p.add_argument("--agent_frac", type=float, default=1.0, help="fraction of the agents sampled per round (reference --agent_frac)")
     p.add_argument("--pattern_type", type=str, default="plus")
     p.add_argument("--no_fused_handoff", action="store_true", help="ours: keep round_init + the aggregation kernel's barrier-out (A/B of the hand-off fusion)")
+    p.add_argument("--dump-outputs", dest="dump_outputs", type=str, default=None, metavar="DIR",
+                   help="ours: write the outputs of the last timed round as DIR/<name>.npy")
     return p.parse_args()
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(eng, out_dir, write=True):
+    """Outputs of the round that just ran, as a caller of FLEngine.run_round receives them: the global parameters (float32; a fixed,
+    seeded sample of them if the whole vector would exceed the size limit), the summed training loss and the flipped count (float64)."""
+    import numpy as np
+    loss, flipped = eng.round_result()          # collective on multi-GPU runs: every rank takes part, rank 0 writes
+    w = eng.global_params().float().cpu().numpy()
+    if not write:
+        return
+    os.makedirs(out_dir, exist_ok=True)
+    budget = (DUMP_LIMIT_BYTES - (1 << 20)) // 4
+    if w.size > budget:
+        idx = np.sort(np.random.default_rng(0).choice(w.size, size=budget, replace=False))
+        np.save(os.path.join(out_dir, "global_params_sample_index.npy"), idx.astype(np.float64))
+        w = w[idx]
+    np.save(os.path.join(out_dir, "global_params.npy"), w)
+    np.save(os.path.join(out_dir, "train_loss_sum.npy"), np.array([loss], dtype=np.float64))
+    np.save(os.path.join(out_dir, "flipped.npy"), np.array([flipped], dtype=np.float64))
+
+
 class ClockSampler:
-    """nvidia-smi clock / throttle-reason sampler running DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clock / throttle-reason sampler running DURING the timed region (clocks and throttle reasons are part of every timing)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -106,7 +134,7 @@ def config_dict(a, n, impl):
             "num_corrupt": a.num_corrupt, "poison_frac": a.poison_frac, "agent_frac": a.agent_frac, "seq_len": None,
             "parallelism": f"agent-parallel: {k} agent(s) on {n} GPU(s)" if impl == "ours" else f"{k} agent(s) sequential on 1 GPU (reference design)",
             "l2_policy": "inputs larger than L2: each step streams a fresh batch from the 150 MB device-resident dataset plus "
-                         "4x45 MB flat parameter/grad/momentum buffers and >100 MB of activations (L2 = 126 MB)",
+                         "4x45 MB flat parameter/grad/momentum buffers and >100 MB of activations (H100 L2 = 50 MB)",
             "timed_region": "local training of all agents + aggregation + parameter hand-off; evaluation excluded"}
 
 
@@ -212,15 +240,6 @@ def run_ours(a):
     cuda = dev.type == "cuda"
     notes = []
     eng = make_engine(a.trainer)
-    if a.trainer == "auto" and eng.trainer.name == "native" and n == 1:
-        # safety net for the headline number (single process only: a rank-local fallback would desynchronise ranks): if the
-        # sm_100a executor cannot run on this box, fall back to the torch trainer and SAY SO in the JSON
-        try:
-            eng.run_round(0)
-            torch.cuda.synchronize(dev)
-        except Exception as e:  # noqa: BLE001
-            notes.append(f"native trainer failed ({type(e).__name__}: {str(e)[:120]}); fell back to trainer=torch")
-            eng = make_engine("torch")
 
     def sync():
         ctx.barrier()
@@ -255,6 +274,9 @@ def run_ours(a):
     clocks = ClockSampler(dev.index or 0) if (ctx.is_main and cuda) else None
     ms, _, _, _, info = timed(a.steps, a.warmup + 1, False)
     ck = clocks.stop() if clocks else {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["cpu run"]}
+    if a.dump_outputs:
+        dump_outputs(eng, a.dump_outputs, write=ctx.is_main)
+        ctx.barrier()
     phases = eng.timer.elapsed()
     e2e = None
     if not a.no_e2e:

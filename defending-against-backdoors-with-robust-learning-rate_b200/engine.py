@@ -100,13 +100,12 @@ class FLEngine:
         n_flight = int(getattr(args, "agents_in_flight", 0))
         if n_flight <= 0:
             # auto: two agents in flight whenever this rank hosts more than one (native trainer on CUDA).  The small reference CNNs are
-            # launch / latency bound at batch 256 (FMNIST CNN, 10 agents, one B200: 160 -> 120 ms per round); the large models run
-            # one-wave kernels in lock step whose ragged tails a second agent's kernels fill (ResNet-18, 8 agents, one B200:
-            # 1008.6 -> 887.6 ms per round, profiles/r2_step_ab.md c27).  One agent per rank (the multi-GPU headline): nothing to overlap.
+            # launch / latency bound at batch 256; the large models run one-wave kernels in lock step whose ragged tails a second
+            # agent's kernels fill.  One agent per rank (the multi-GPU headline): nothing to overlap.
             # Native trainer only: the autograd trainer drives cuDNN from PyTorch's backward threads (see below).
             n_flight = 2 if (dev.type == "cuda" and self.trainer.name == "native") else 1
         if n_flight > 1 and dev.type == "cuda" and self.trainer.name != "native":
-            # measured (scripts/stress_inflight.py torch 2): two autograd trainers replaying cuDNN / cuBLAS graphs on two streams dead-lock
+            # two autograd trainers replaying cuDNN / cuBLAS graphs on two streams dead-lock
             # the device within a few rounds (library kernels whose CTAs wait for each other while the other graph holds the SMs)
             if ctx.is_main:
                 print(f"[engine] --agents_in_flight {n_flight} needs the native trainer; the {self.trainer.name} trainer trains one agent at a time")

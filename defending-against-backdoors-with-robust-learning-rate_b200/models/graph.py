@@ -4,7 +4,7 @@ A model is a short list of ``Node``s over named activation slots.  The same IR d
 
 * ``GraphNet`` (this file): a ``torch.nn.Module`` that interprets the IR with torch ops -- the CPU / oracle /
   "torch trainer" path -- whose parameters are *views into one flat fp32 buffer*, and
-* ``models.native.NativeNet``: the sm_100a executor (hand-written forward/backward kernels, no autograd).
+* ``models.native.NativeNet``: the sm_90a executor (hand-written forward/backward kernels, no autograd).
 
 Flat layout (one buffer per role: params ``w``, grads ``g``, momentum ``m``):
 

@@ -9,7 +9,7 @@ per-tensor optimizer state, no zero_grad (every gradient is overwritten).  The p
     BN(batch stats) + residual add + ReLU in one pass; BN backward in two (reduce, apply) passes
     avg-pool + flatten + linear head + softmax cross-entropy
 
-Each primitive has two back-ends selected per op in ``self.impl``: ``"sm100"`` -- the hand-written tcgen05/TMA
+Each primitive has two back-ends selected per op in ``self.impl``: ``"sm100"`` -- the hand-written wgmma/TMA
 kernels of ops/csrc (gemm.cu / conv.cu / norm.cu) -- and ``"aten"`` -- the same math through library calls on the
 same buffers, used as the in-place numerical oracle for the kernels (tests/test_gpu_native.py) and for shapes a
 kernel does not cover yet.  ``NativeTrainer`` captures the whole step (gather -> forward -> loss -> backward -> fused
@@ -31,11 +31,9 @@ from .graph import FlatLayout
 ACT = torch.bfloat16   # default activation / GEMM-operand dtype on GPU (tests may run the plan in fp32 on CPU)
 # Weight gradients are off the critical path of the backward pass (nothing but the optimizer reads them): every conv weight-gradient
 # kernel is queued on a side stream (forked / joined with events, so it becomes a parallel branch of the captured step graph) while the
-# data-gradient / BatchNorm chain continues on the main stream.  Measured on B200: ResNet-18 round 1065.7 -> 1030.0 ms (same box,
-# profiles/r2_step_ab.md).  RLR_WGRAD_OVERLAP=0 serialises them again.
+# data-gradient / BatchNorm chain continues on the main stream.  RLR_WGRAD_OVERLAP=0 serialises them again.
 # partial-sum slots of the per-channel reductions: with N > 1 the CTAs of channel_reduce_kernel spread their atomics over N buffers
-# (consumers sum them) and the reductions run four / three CTAs per SM instead of two.  Measured on B200 (profiles/r2_step_ab.md):
-# 4 slots = +3.3 % round time, i.e. the two-CTA grid of round 1 stays the default; the knob is kept for re-measurement.
+# (consumers sum them) and the reductions run four / three CTAs per SM instead of two; default 1 (the two-CTA grid).
 # Dropout after a max-pool or a Linear+ReLU is fused into that producer (SURVEY.md K5): the pooling kernel / the GEMM epilogue applies the
 # Philox keep-mask, the backward recomputes it (pool) or reads it off the output together with the ReLU mask (linear).  RLR_FUSE_DROPOUT=0
 # restores the stand-alone dropout kernels.
@@ -375,7 +373,7 @@ class NativeNet:
         gout = self.G(self.out_tid, B)
         if dlogits.data_ptr() != gout.data_ptr():
             gout.copy_(dlogits.reshape(gout.shape))
-        ops.zero_(self.g)        # tcgen05 weight gradients are split-K reductions (red.add) into the flat buffer
+        ops.zero_(self.g)        # wgmma weight gradients are added into the flat buffer
         ops.zero_(self.dsum_arena)
         self._side = None
         if WGRAD_OVERLAP and self.device.type == "cuda":
@@ -419,7 +417,7 @@ class NativeNet:
         x, y = self.T(op.x, B), self.T(op.y, B)
         bias = self.pw.get(op.name + ".bias")
         # BatchNorm statistics: fused into the conv epilogue (FUSE_BN_STATS) or taken by one streaming pass over the conv output
-        # while it is still L2-resident (default: measured cheaper than the in-epilogue reduction, profiles/r1c notes)
+        # while it is still L2-resident (default: cheaper than the in-epilogue reduction)
         stats = op.saved.get("stats") if (train and op.saved.get("want_stats") and (self.fuse_bn_stats or self._epilogue_stats_free(op))) else None
         op.saved["stats_done"] = stats is not None
         if self.impl["conv_fwd"] == "sm100" and ops.conv_supported(op.in_shape, a, "fwd"):
@@ -565,7 +563,7 @@ class NativeTrainer:
     def __init__(self, layout, args, device, max_shard: int, impl="auto"):
         self.layout, self.args = layout, args
         self.device = torch.device(device)
-        assert self.device.type == "cuda", "the native trainer runs on sm_100a devices only"
+        assert self.device.type == "cuda", "the native trainer runs on sm_90a devices only"
         n = layout.n_total
         self.w = torch.zeros(n, dtype=torch.float32, device=device)
         self.wb = torch.zeros(n, dtype=torch.bfloat16, device=device)

@@ -2,7 +2,7 @@
 
 Every op has two implementations behind one Python signature:
 
-* **native** -- a hand-written sm_100a kernel from ``ops/_C.so`` (sources in ``ops/csrc``), used whenever the tensors
+* **native** -- a hand-written sm_90a kernel from ``ops/_C.so`` (sources in ``ops/csrc``), used whenever the tensors
   live on a CUDA device.  If the extension is missing on a GPU box the op raises -- there is no silent eager fallback.
 * **oracle** -- a plain fp32/fp64 PyTorch re-statement of the same semantics, used on CPU (the plumbing config and the
   CPU test-suite) and as the numerical reference the GPU tests compare the kernels against.
@@ -162,7 +162,7 @@ def gather_normalize(data, idxs, mean, std, dtype=torch.float32, nhwc=False, c_p
 def gather_im2col(data, idxs, mean, std, k, pad, out, cursor=None, targets=None, out_labels=None, batch=None):
     """Batch assembly fused with the first layer's im2col (SURVEY.md K1+K2, tiny-K stems: C*k*k <= 64): row (b, ho, wo) of ``out``
     [B*Ho*Wo, 64] (bf16) is the k x k x C patch of the normalised image around that output pixel in (tap, channel) order, zero
-    padded -- the A operand of the stem convolution as a single-k-block tcgen05 GEMM.  Same cursor / label contract as
+    padded -- the A operand of the stem convolution as a single-k-block wgmma GEMM.  Same cursor / label contract as
     ``gather_normalize``."""
     N, H, W, C = data.shape
     B = int(batch if batch is not None else idxs.shape[0])

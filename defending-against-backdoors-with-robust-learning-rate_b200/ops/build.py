@@ -1,10 +1,10 @@
-"""In-tree build of the native extension ``ops/_C.so`` for sm_100a.
+"""In-tree build of the native extension ``ops/_C.so`` for sm_90a (H100).
 
 ``python -m rlr_b200.ops.build`` (or ``__graft_entry__.build()``): every ``csrc/*.cu`` is compiled by nvcc with
-``-gencode arch=compute_100a,code=sm_100a -lineinfo`` (cross-compiles without a GPU), every ``csrc/*.cpp`` by g++
-against the torch headers, and the objects are linked into ``ops/_C.so``.  The .so is git-ignored but travels to
-the GPU box with the gpurun snapshot, so nothing is JIT-compiled there.  Objects are rebuilt only when the source
-or a header changed (content hash), so iterating on one kernel costs seconds.
+``-gencode arch=compute_90a,code=sm_90a -lineinfo`` (cross-compiles without a GPU), every ``csrc/*.cpp`` by g++
+against the torch headers, and the objects are linked into ``ops/_C.so``.  The .so is git-ignored; nothing is
+JIT-compiled at run time.  Objects are rebuilt only when the source or a header changed (content hash), so iterating
+on one kernel costs seconds.
 """
 from __future__ import annotations
 
@@ -19,7 +19,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_build")
 TARGET = os.path.join(HERE, "_C.so")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 
@@ -33,18 +33,8 @@ def _torch_paths():
     return inc, lib, abi
 
 
-def _cutlass_include():
-    """Vendored CUTLASS/CuTe header tree (flashinfer ships one); optional, used for cross-checking only."""
-    try:
-        import flashinfer  # noqa: F401
-        p = os.path.join(os.path.dirname(flashinfer.__file__), "data", "cutlass", "include")
-        return [p] if os.path.isdir(p) else []
-    except Exception:  # noqa: BLE001
-        return []
-
-
 def _hash(paths, extra=""):
-    """Content hash that is independent of where the repo lives (the gpurun box unpacks it under a scratch path)."""
+    """Content hash that is independent of where the repository lives (include / library paths are left out)."""
     h = hashlib.sha256(" ".join(a for a in extra.split() if not a.startswith(("-I", "-L"))).encode())
     for p in sorted(paths, key=os.path.basename):
         with open(p, "rb") as f:
@@ -104,11 +94,11 @@ def build(verbose: bool = False, force: bool = False) -> str:
             for name in ex.map(do, jobs):
                 if verbose:
                     print(f"[build] compiled {name}")
-    for name, out in logs.items():  # keep ptxas -v output for profiles/ (registers, spills, smem)
+    for name, out in logs.items():  # keep ptxas -v output (registers, spills, smem) next to the objects
         with open(os.path.join(OBJ, name + ".log"), "w") as fh:
             fh.write(out)
     if jobs or force or not os.path.exists(TARGET):
-        tmp = TARGET + ".tmp"       # link to a temporary name and rename: a gpurun snapshot taken meanwhile never sees half a file
+        tmp = TARGET + ".tmp"       # link to a temporary name and rename: a concurrent reader never sees half a file
         link = ["g++", "-shared", "-o", tmp, *objs, f"-L{torch_lib}", "-L/usr/local/cuda/lib64",
                 "-lc10", "-ltorch_cpu", "-ltorch", "-ltorch_python", "-lc10_cuda", "-ltorch_cuda", "-lcudart",
                 f"-Wl,-rpath,{torch_lib}", "-Wl,-rpath,/usr/local/cuda/lib64"]

@@ -1,4 +1,4 @@
-// Fused federated server step for sm_100a: one pass over the flat parameter vector that
+// Fused federated server step for sm_90a: one pass over the flat parameter vector that
 //   * reads every participating agent's local parameters w_k (local HBM, or a PEER GPU's HBM through
 //     NVLink/NVSwitch-mapped pointers) and forms the update d_k = w_k - w_g in registers (never materialised),
 //   * takes the per-coordinate sign vote  s = |sum_k sign(d_k)|  ->  lr = +server_lr if s >= theta else -server_lr

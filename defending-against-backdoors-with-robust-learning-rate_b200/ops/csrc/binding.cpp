@@ -1,4 +1,4 @@
-// Python bindings (pybind11 through torch/extension.h) for the sm_100a kernels and the small native runtime
+// Python bindings (pybind11 through torch/extension.h) for the sm_90a kernels and the small native runtime
 // pieces (CUDA-IPC symmetric buffers).  All launches go to the CURRENT torch CUDA stream so they compose with
 // stream capture (CUDA graphs) and with torch ops on the same stream.
 #include <torch/extension.h>
@@ -266,7 +266,7 @@ at::Tensor tensor_from_ptr(int64_t ptr, std::vector<int64_t> sizes, at::ScalarTy
 void register_gemm_bindings(py::module_& m);  // gemm_binding.cpp
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-    m.doc() = "b200-robust-fl sm_100a kernels";
+    m.doc() = "robust-fl sm_90a kernels";
     m.def("fused_aggregate", &fused_aggregate, py::arg("w_agent_ptrs"), py::arg("weights"), py::arg("scales"), py::arg("total_weight"),
           py::arg("w_global_ptr"), py::arg("out_ptrs"), py::arg("out_bf16_ptrs"), py::arg("use_multimem"), py::arg("begin"), py::arg("end"),
           py::arg("n_vote"), py::arg("mode"), py::arg("theta"), py::arg("server_lr"), py::arg("noise_std"), py::arg("seed"),

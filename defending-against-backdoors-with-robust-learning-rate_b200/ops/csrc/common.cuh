@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a kernels of b200-robust-fl.
+// Shared device helpers for the sm_90a kernels of robust-fl.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -18,7 +18,7 @@ constexpr int kWarp = 32;
 
 // ---- programmatic dependent launch (PDL) ------------------------------------------------------------------------------------
 // Kernels launched through launch_kernel() with PDL enabled (RLR_PDL=1 / set_pdl) may start while their predecessor in the stream
-// is still draining: they run their prologue (barrier init, TMEM allocation, tensor-map prefetch, index arithmetic) and then block
+// is still draining: they run their prologue (barrier init, tensor-map prefetch, index arithmetic) and then block
 // in pdl_wait() until the predecessor grid has completed and its memory is visible.  Rules every such kernel follows: NO global
 // memory access before pdl_wait(); pdl_wait() is executed by every thread; pdl_trigger() (lets the successor start launching)
 // comes after it.  Without the launch attribute both instructions are no-ops, so the same kernels serve plain launches.
@@ -41,6 +41,33 @@ inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+
+// ---- deterministic cross-CTA reductions ---------------------------------------------------------------------------------------
+// A reduction over CTAs never adds into its output with float atomics (their order, and so the rounding, changes from run to run):
+// every CTA writes its partial result to a slot of a scratch buffer and ordered_sum_kernel adds the slots in a fixed order.
+// Scratch memory comes from the framework's stream-ordered caching allocator (gemm_binding.cpp), so it is safe to release right
+// after the launches that use it and it is captured with the rest of a CUDA graph.
+void* scratch_alloc(size_t bytes, cudaStream_t st);
+void scratch_free(void* p);
+struct Scratch {
+    void* p;
+    Scratch(size_t bytes, cudaStream_t st) : p(scratch_alloc(bytes, st)) {}
+    ~Scratch() { scratch_free(p); }
+    Scratch(const Scratch&) = delete;
+    Scratch& operator=(const Scratch&) = delete;
+    template <typename T> T* as() const { return static_cast<T*>(p); }
+};
+// out[i] += part[0][i] + part[1][i] + ... + part[nparts-1][i]   (part = [nparts][n])
+template <typename T>
+__global__ void __launch_bounds__(256) ordered_sum_kernel(T* __restrict__ out, const T* __restrict__ part, int nparts, long long n) {
+    pdl_wait();
+    pdl_trigger();
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        T s = part[i];
+        for (int j = 1; j < nparts; ++j) s += part[(size_t)j * n + i];
+        out[i] += s;
+    }
 }
 
 __device__ __forceinline__ unsigned long long gtimer() {     // nanosecond timer common to all SMs
@@ -195,6 +222,14 @@ __device__ __forceinline__ uint32_t dropout_keep8(const DropSpec& d, long long q
 #pragma unroll
     for (int i = 0; i < 8; ++i) keep |= (uint32_t)(((r[i >> 1] >> (16 * (i & 1))) & 0xffffu) >= d.thr) << i;
     return keep;
+}
+
+template <typename T>
+inline cudaError_t launch_ordered_sum(T* out, const T* part, int nparts, long long n, cudaStream_t st) {
+    long long blocks = (n + 255) / 256;
+    if (blocks > 1024) blocks = 1024;
+    if (blocks < 1) blocks = 1;
+    return launch_kernel(ordered_sum_kernel<T>, dim3((unsigned)blocks), dim3(256), (size_t)0, st, out, part, nparts, n);
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {

@@ -1,42 +1,40 @@
-// Persistent tcgen05 3x3 / stride-1 convolution for 64-channel inputs with SHARED-MEMORY HALO REUSE (sm_100a).
+// Persistent wgmma 3x3 / stride-1 convolution for 64-channel inputs with SHARED-MEMORY HALO REUSE (sm_90a).
 //
 // The generic implicit-GEMM kernel (gemm.cu) fetches one 128x64 input tile per filter tap, i.e. it re-reads every input
-// pixel 9 times from L2 (TMA bypasses L1), which makes the 64-channel 32x32 layers L2-bandwidth bound (profiles/r1a_ncu).
+// pixel 9 times from L2 (TMA bypasses L1), which makes the 64-channel 32x32 layers L2-bandwidth bound.
 // Here an output tile is 16 rows x 8 columns of one image and its whole receptive field -- 18 x 10 pixels x 64 channels,
 // stored with a 16-pixel row pitch = 36 KB -- is loaded ONCE by a single 4-D TMA box (zero fill at the borders = padding).
 // The A operand of tap (dy,dx) is then just a *view* into that halo: 16 groups (image rows) of 8 pixel-rows, group stride
 // SBO = 16 px * 128 B = 2048 B, start address offset by (dy*16 + dx) * 128 B.  That start is not aligned to the 1024-byte
-// swizzle atom; measured on B200 (tests/test_gpu_native.py::test_conv3x3_halo_kernel): the tensor core applies the 128-byte
-// swizzle as a function of the ABSOLUTE shared-memory address bits, exactly like the TMA unit that wrote the tile, so the
-// shifted view is read correctly with the descriptor's base-offset field left at 0 (setting it to (addr>>7)&7 is wrong).
-// All 9 x 64 x 64 filter taps
-// (72 KB) stay resident in shared memory for the lifetime of the persistent CTA, so per output tile the kernel moves 36 KB
-// instead of 216 KB and becomes tensor/epilogue bound.  Accumulators are double-buffered in TMEM (2 x 64 columns) so the
-// epilogue of tile i (bias / ReLU / residual-accumulate / bf16 / coalesced stores / BatchNorm statistics) overlaps the
-// MMAs of tile i+1.  Used for the stem and layer1 forward convolutions and layer1 data gradients of ResNet-18 and the
-// 64-channel VGG layers.
+// swizzle atom; the descriptor's base-offset field is 0 by default (bo_mode 0, the swizzle follows the absolute shared-memory
+// address bits like the TMA unit that wrote the tile) or (addr >> 7) & 7 (bo_mode 1); tests/test_gpu_native.py checks both.
+// All 9 x 64 x 64 filter taps (72 KB) stay resident in shared memory for the lifetime of the persistent CTA, so per output tile
+// the kernel moves 36 KB instead of 216 KB.  The two consumer warpgroups take alternate tiles, each computing the whole 128 x 64
+// tile (two m64n64 wgmma per k-step) into registers and running its own epilogue (bias / ReLU / residual-accumulate / bf16 /
+// coalesced stores / BatchNorm statistics) from its own staging tile, so one warpgroup's epilogue overlaps the other's MMAs.
+// Used for the stem and layer1 forward convolutions and layer1 data gradients of ResNet-18 and the 64-channel VGG layers.
 #include <cuda.h>
 
 #include "common.cuh"
 #include "gemm.h"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace rlr {
 
-using namespace umma;
+using namespace wg;
 
 cudaError_t make_tmap_bf16(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                            const uint32_t* box, const uint32_t* elem_strides = nullptr);  // gemm.cu
 
-constexpr int HL_THREADS = 192;
+constexpr int HL_THREADS = 256 + 32;                  // two consumer warpgroups + the TMA producer warp
 constexpr int HL_TH = 16, HL_TW = 8;                  // output tile: 16 rows x 8 cols = 128 pixels
 constexpr int HL_PITCH = 16;                          // halo row pitch in pixels (8 + 2 halo + 6 pad) -> SBO = 2048 B
 constexpr int HL_HALO_BYTES = (HL_TH + 2) * HL_PITCH * 128;   // 36864
 constexpr int HL_W_BYTES = 9 * 64 * 128;              // 73728: [tap][cout 64][cin 64] bf16, K-major, one n-tile
 constexpr int HL_STAGES = 3;
 constexpr int HL_PITCH_OUT = 64 * 2 + 16;             // staging row pitch (bytes)
-constexpr int HL_STAGING = 128 * HL_PITCH_OUT + 2 * 64 * 4;
-constexpr int HL_SMEM = HL_W_BYTES + HL_STAGES * HL_HALO_BYTES + HL_STAGING + 1024 + 1024;
+constexpr int HL_STAGING = 128 * HL_PITCH_OUT;        // per warpgroup
+constexpr int HL_SMEM = HL_W_BYTES + HL_STAGES * HL_HALO_BYTES + 2 * HL_STAGING + 1024 + 1024;
 
 struct HaloParams {
     int NB, H, W;                 // OUTPUT spatial size; input = output + 2 - 2*pad
@@ -48,23 +46,16 @@ struct HaloParams {
     float* stats;
     int relu, accumulate;
     long long* dbg;               // optional per-tile clock64 timeline of CTA 0 (tuning aid): [tile][8]
-    int bo_mode;                  // 0 (correct on B200): base-offset field 0;  1: (addr >> 7) & 7 -- kept for the experiment
+    int bo_mode;                  // 0: descriptor base-offset field 0;  1: (addr >> 7) & 7
 };
 
 struct __align__(8) HaloShared {
     uint64_t w_full;
     uint64_t halo_full[HL_STAGES];
     uint64_t halo_empty[HL_STAGES];
-    uint64_t acc_full[2];
-    uint64_t acc_empty[2];
-    uint32_t tmem_base;
-    uint32_t pad;
+    float red[128];               // per-CTA column sums (sum, sum of squares)
+    float bias[64];
 };
-
-__device__ __forceinline__ uint64_t desc_sw128_bo(uint32_t saddr, uint32_t sbo_bytes, uint32_t base_offset) {
-    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) |
-           (1ull << 46) | ((uint64_t)(base_offset & 7u) << 49) | (2ull << 61);
-}
 
 template <bool kStats, bool kAcc>
 __global__ void __launch_bounds__(HL_THREADS, 1)
@@ -73,28 +64,26 @@ umma_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_c
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* s_w = smem;                                   // 72 KB resident filter
     uint8_t* s_halo = smem + HL_W_BYTES;                   // 3 x 36 KB ring
-    uint8_t* s_stage = s_halo + HL_STAGES * HL_HALO_BYTES; // epilogue staging + stats scratch
-    HaloShared* sh = reinterpret_cast<HaloShared*>(s_stage + HL_STAGING);
+    uint8_t* s_stage = s_halo + HL_STAGES * HL_HALO_BYTES; // 2 epilogue staging tiles
+    HaloShared* sh = reinterpret_cast<HaloShared*>(s_stage + 2 * HL_STAGING);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile_n = blockIdx.y;
+    const int col0 = tile_n * 64;
 
-    if (warp == 0 && lane == 0) { prefetch_tmap(&tmX); prefetch_tmap(&tmW); }
-    if (warp == 1 && lane == 0) {
+    if (warp == 8 && lane == 0) {
+        prefetch_tmap(&tmX); prefetch_tmap(&tmW);
         mbar_init(&sh->w_full, 1);
-        for (int s = 0; s < HL_STAGES; ++s) { mbar_init(&sh->halo_full[s], 1); mbar_init(&sh->halo_empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&sh->acc_full[a], 1); mbar_init(&sh->acc_empty[a], 128); }
+        for (int s = 0; s < HL_STAGES; ++s) { mbar_init(&sh->halo_full[s], 1); mbar_init(&sh->halo_empty[s], 4); }
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc(&sh->tmem_base, 128);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_acc = sh->tmem_base;
+    if (threadIdx.x < 128) sh->red[threadIdx.x] = 0.f;
     const int tiles_per_img = p.tiles_h * p.tiles_w;
-    pdl_wait();        // nothing above read or wrote global memory
+    pdl_wait();
     pdl_trigger();
+    if (threadIdx.x < 64) sh->bias[threadIdx.x] = (p.bias && col0 + (int)threadIdx.x < p.N) ? p.bias[col0 + threadIdx.x] : 0.f;
+    __syncthreads();
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ===================== producer: filter once, then one halo box per tile =====================================
         if (lane == 0) {
             mbar_expect_tx(&sh->w_full, HL_W_BYTES);
@@ -110,149 +99,137 @@ umma_conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_c
                 if (++stage == HL_STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer ==========================================================================
-        if (lane == 0) {
-            constexpr uint32_t idesc = idesc_bf16(128, 64, 0, 0);
-            mbar_wait(&sh->w_full, 0);
-            int stage = 0, acc = 0;
-            uint32_t phase = 0, acc_phase = 0;
-            const uint32_t w_base = smem_u32(s_w);
-            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-                const bool trace = p.dbg && blockIdx.x == 0 && blockIdx.y == 0;
-                const int tix = (tile - blockIdx.x) / gridDim.x;
-                if (trace) p.dbg[tix * 8 + 0] = clock64();
-                mbar_wait(&sh->acc_empty[acc], acc_phase ^ 1);       // epilogue has drained this accumulator
-                if (trace) p.dbg[tix * 8 + 1] = clock64();
-                mbar_wait(&sh->halo_full[stage], phase);
-                if (trace) p.dbg[tix * 8 + 2] = clock64();
-                tc_fence_after();
-                const uint32_t halo = smem_u32(s_halo + stage * HL_HALO_BYTES);
-                const uint32_t d_tmem = tmem_acc + acc * 64;
-#pragma unroll
-                for (int t = 0; t < 9; ++t) {
-                    const int dy = t / 3, dx = t - dy * 3;
-                    const uint32_t a0 = halo + (dy * HL_PITCH + dx) * 128;
-                    const uint32_t bo = p.bo_mode ? ((a0 >> 7) & 7u) : 0u;
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint64_t da = desc_sw128_bo(a0 + k * 32, HL_PITCH * 128, bo);
-                        const uint64_t db = smem_desc_sw128(w_base + t * 8192 + k * 32, 16, 1024);
-                        umma_bf16(d_tmem, da, db, idesc, (t > 0 || k > 0) ? 1u : 0u);
-                    }
-                }
-                umma_commit(&sh->halo_empty[stage]);
-                umma_commit(&sh->acc_full[acc]);
-                if (trace) p.dbg[tix * 8 + 3] = clock64();
-                if (++stage == HL_STAGES) { stage = 0; phase ^= 1; }
-                acc ^= 1;
-                if (acc == 0) acc_phase ^= 1;
-            }
-        }
     } else {
-        // ===================== epilogue (128 threads) ================================================================
-        const int et = threadIdx.x - 64;
-        const int lane_base = (warp & 3) * 32;
-        const int row = lane_base + lane;
-        const int col0 = tile_n * 64;
-        float* red = reinterpret_cast<float*>(s_stage + 128 * HL_PITCH_OUT);
+        // ===================== consumers: warpgroup wgi takes the tiles of ordinal q = wgi, wgi + 2, ... ====================
+        const int wgi = threadIdx.x >> 7, t = threadIdx.x & 127;
+        uint8_t* stage_buf = s_stage + wgi * HL_STAGING;
+        const int r0 = frag_row(t, 0);                         // rows r0 (+8) of each 64-row half
         __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out);
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        if (kStats) red[et] = 0.f;                                 // per-CTA statistics, flushed once at the end
-        // without statistics the same 512 bytes hold this n-tile's bias values: read once per CTA, not once per element and tile
-        const bool bias_smem = !kStats && p.bias != nullptr;
-        if (bias_smem) {
-            if (et < 64) red[et] = (col0 + et < p.N) ? p.bias[col0 + et] : 0.f;
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-        }
-        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        float st1[16], st2[16];                                // statistics of this thread's 16 columns over all its tiles
+#pragma unroll
+        for (int i = 0; i < 16; ++i) { st1[i] = 0.f; st2[i] = 0.f; }
+        const uint32_t w_base = smem_u32(s_w);
+        mbar_wait(&sh->w_full, 0);
+        for (int q = wgi;; q += 2) {
+            const int tile = blockIdx.x + q * gridDim.x;
+            if (tile >= p.num_tiles) break;
+            const int stage = q % HL_STAGES;
+            const uint32_t phase = (uint32_t)(q / HL_STAGES) & 1u;
             const int n = tile / tiles_per_img, r = tile - n * tiles_per_img;
             const int h0 = (r / p.tiles_w) * HL_TH, w0 = (r % p.tiles_w) * HL_TW;
-            // residual-accumulate operand: issue all loads BEFORE waiting for the accumulator so their latency overlaps the MMAs
+            // residual-accumulate operand: issue all loads BEFORE the MMAs so their latency overlaps them
             uint4 oldv[8];
             if (kAcc) {
 #pragma unroll
                 for (int it = 0; it < 8; ++it) {
-                    const int idx = et + it * 128, rr = idx >> 3, ch = idx & 7;
+                    const int idx = t + it * 128, rr = idx >> 3, ch = idx & 7;
                     const int h = h0 + (rr >> 3), w = w0 + (rr & 7);
                     oldv[it] = make_uint4(0, 0, 0, 0);
                     if (col0 + ch * 8 < p.N && h < p.H && w < p.W)
                         oldv[it] = *reinterpret_cast<const uint4*>(out + (((size_t)n * p.H + h) * p.W + w) * p.ldc + col0 + ch * 8);
                 }
             }
-            const bool trace = p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && et == 0;
-            const int tix = (tile - blockIdx.x) / gridDim.x;
-            if (trace) p.dbg[tix * 8 + 4] = clock64();
-            mbar_wait(&sh->acc_full[acc], acc_phase);
-            if (trace) p.dbg[tix * 8 + 5] = clock64();
-            tc_fence_after();
+            const bool trace = p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && t == 0;
+            if (trace) p.dbg[q * 8 + 0] = clock64();
+            mbar_wait(&sh->halo_full[stage], phase);
+            if (trace) p.dbg[q * 8 + 2] = clock64();
+            const uint32_t halo = smem_u32(s_halo + stage * HL_HALO_BYTES);
+            float acc[2][32];
 #pragma unroll
-            for (int c0 = 0; c0 < 64; c0 += 32) {
-                uint32_t v[32];
-                tmem_ld_32x32(tmem_acc + ((uint32_t)lane_base << 16) + acc * 64 + c0, v);
-                uint32_t packed[16];
-                float f1[32], f2[32];
+            for (int m = 0; m < 2; ++m)
 #pragma unroll
-                for (int j = 0; j < 32; j += 2) {
-                    float a = __uint_as_float(v[j]), b = __uint_as_float(v[j + 1]);
-                    if (bias_smem) { a += red[c0 + j]; b += red[c0 + j + 1]; }
-                    else if (p.bias && col0 + c0 + j < p.N) { a += p.bias[col0 + c0 + j]; b += p.bias[col0 + c0 + j + 1]; }
-                    if (p.relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
-                    packed[j >> 1] = pack_bf16x2(a, b);
-                    if (kStats) {   // statistics of the bf16-rounded values that BatchNorm will read back
-                        const float2 rq = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&packed[j >> 1]));
-                        f1[j] = rq.x; f1[j + 1] = rq.y; f2[j] = rq.x * rq.x; f2[j + 1] = rq.y * rq.y;
+                for (int i = 0; i < 32; ++i) acc[m][i] = 0.f;
+            wgmma_fence();
+#pragma unroll
+            for (int tp = 0; tp < 9; ++tp) {
+                const int dy = tp / 3, dx = tp - dy * 3;
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const uint64_t db = smem_desc_sw128(w_base + tp * 8192 + k * 32, 16, 1024);
+#pragma unroll
+                    for (int m = 0; m < 2; ++m) {                  // rows 64 m .. 64 m + 63 = image rows 8 m .. 8 m + 7 of the tile
+                        const uint32_t a0 = halo + (dy * HL_PITCH + dx) * 128 + m * 8 * HL_PITCH * 128 + k * 32;
+                        const uint32_t bo = p.bo_mode ? ((a0 >> 7) & 7u) : 0u;
+                        wgmma_bf16<64, 0, 0>(acc[m], smem_desc_sw128(a0, 16, HL_PITCH * 128, bo), db, (tp > 0 || k > 0) ? 1u : 0u);
                     }
                 }
-                uint4* dst = reinterpret_cast<uint4*>(s_stage + row * HL_PITCH_OUT + c0 * 2);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) dst[q] = make_uint4(packed[4 * q], packed[4 * q + 1], packed[4 * q + 2], packed[4 * q + 3]);
-                if (kStats) {   // every tile row is a valid pixel (the launcher refuses statistics on partial tiles): warp-level column sums
-                    const float c1 = warp_transpose_sum32(f1, lane), c2 = warp_transpose_sum32(f2, lane);
-                    atomicAdd(&red[c0 + lane], c1);
-                    atomicAdd(&red[64 + c0 + lane], c2);
-                }
             }
-            tc_fence_before();
-            mbar_arrive(&sh->acc_empty[acc]);                        // 128 arrivals release the accumulator to the MMA warp
-            if (trace) p.dbg[tix * 8 + 6] = clock64();
-            asm volatile("bar.sync 1, 128;" ::: "memory");
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_acc(acc[0]);
+            fence_acc(acc[1]);
+            if (lane == 0) mbar_arrive(&sh->halo_empty[stage]);   // 4 arrivals (this warpgroup's warps) release the halo stage
+            if (trace) p.dbg[q * 8 + 3] = clock64();
+#pragma unroll
+            for (int m = 0; m < 2; ++m)
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const int c = frag_col(t, 4 * j);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        float a = acc[m][4 * j + 2 * h], b = acc[m][4 * j + 2 * h + 1];
+                        a += sh->bias[c]; b += sh->bias[c + 1];
+                        if (p.relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
+                        const uint32_t packed = pack_bf16x2(a, b);
+                        if (kStats) {   // statistics of the bf16-rounded values that BatchNorm will read back (whole tiles only)
+                            const float2 rq = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&packed));
+                            st1[2 * j] += rq.x; st1[2 * j + 1] += rq.y;
+                            st2[2 * j] += rq.x * rq.x; st2[2 * j + 1] += rq.y * rq.y;
+                        }
+                        *reinterpret_cast<uint32_t*>(stage_buf + (m * 64 + r0 + 8 * h) * HL_PITCH_OUT + c * 2) = packed;
+                    }
+                }
+            named_bar(1 + wgi, 128);
+            if (trace) p.dbg[q * 8 + 6] = clock64();
             // coalesced stores: tile row rr = g*8 + px  ->  image pixel (h0+g, w0+px)
 #pragma unroll
             for (int it = 0; it < 8; ++it) {
-                const int idx = et + it * 128;
+                const int idx = t + it * 128;
                 const int rr = idx >> 3, ch = idx & 7;
                 if (col0 + ch * 8 >= p.N) continue;
                 const int h = h0 + (rr >> 3), w = w0 + (rr & 7);
                 if (h >= p.H || w >= p.W) continue;
                 const size_t gi = ((size_t)n * p.H + h) * p.W + w;
-                uint4 val = *reinterpret_cast<const uint4*>(s_stage + rr * HL_PITCH_OUT + ch * 16);
+                uint4 val = *reinterpret_cast<const uint4*>(stage_buf + rr * HL_PITCH_OUT + ch * 16);
                 uint4* gp = reinterpret_cast<uint4*>(out + gi * p.ldc + col0 + ch * 8);
                 if (kAcc) {
                     const __nv_bfloat162* o2 = reinterpret_cast<const __nv_bfloat162*>(&oldv[it]);
                     __nv_bfloat162* v2 = reinterpret_cast<__nv_bfloat162*>(&val);
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        const float2 a = __bfloat1622float2(v2[q]), b = __bfloat1622float2(o2[q]);
-                        v2[q] = __floats2bfloat162_rn(a.x + b.x, a.y + b.y);
+                    for (int qq = 0; qq < 4; ++qq) {
+                        const float2 a = __bfloat1622float2(v2[qq]), b = __bfloat1622float2(o2[qq]);
+                        v2[qq] = __floats2bfloat162_rn(a.x + b.x, a.y + b.y);
                     }
                 }
                 *gp = val;
             }
-            asm volatile("bar.sync 1, 128;" ::: "memory");           // staging may be overwritten by the next tile
-            if (trace) p.dbg[tix * 8 + 7] = clock64();
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1;
+            named_bar(1 + wgi, 128);                                // staging may be overwritten by this warpgroup's next tile
+            if (trace) p.dbg[q * 8 + 7] = clock64();
         }
-        // one global reduction per CTA and channel (instead of per tile), spread over kStatSlots slots to cut same-address
-        // contention in L2; bn_finalize sums the slots
-        if (kStats && col0 + (et & 63) < p.N)
-            atomicAdd(p.stats + (size_t)(blockIdx.x % kStatSlots) * 2 * p.N + (et < 64 ? 0 : p.N) + col0 + (et & 63), red[et]);
+        if (kStats) {
+            // column sums over the 8 lanes sharing this thread's columns, then one shared atomic per column and warp
+#pragma unroll
+            for (int i = 0; i < 16; ++i)
+#pragma unroll
+                for (int o = 4; o < 32; o <<= 1) {
+                    st1[i] += __shfl_xor_sync(0xffffffffu, st1[i], o);
+                    st2[i] += __shfl_xor_sync(0xffffffffu, st2[i], o);
+                }
+            if (lane < 4)
+#pragma unroll
+                for (int i = 0; i < 16; ++i) {
+                    const int c = frag_col(t, 2 * (i & ~1)) + (i & 1);
+                    atomicAdd(&sh->red[c], st1[i]);
+                    atomicAdd(&sh->red[64 + c], st2[i]);
+                }
+            named_bar(3, 256);
+            // one global reduction per CTA and channel (instead of per tile), spread over kStatSlots slots to cut same-address
+            // contention in L2; bn_finalize sums the slots
+            if (threadIdx.x < 128 && col0 + (threadIdx.x & 63) < p.N)
+                atomicAdd(p.stats + (size_t)(blockIdx.x % kStatSlots) * 2 * p.N + (threadIdx.x < 64 ? 0 : p.N) + col0 + (threadIdx.x & 63),
+                          sh->red[threadIdx.x]);
+        }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_acc, 128);
 }
 
 // y[NB][H][W][Cout] = conv3x3(x[NB][Hin][Win][64], w[Cout][9*64]), stride 1, padding pad = (H - Hin + 2) / 2 in {0, 1, 2} (valid / same /

@@ -1,33 +1,31 @@
-// Three-taps-per-MMA variant of the persistent 3x3 / stride-1 halo convolution for 64 input channels (opt-in: RLR_HALO3=1, not yet
-// measured on hardware).
+// Three-taps-per-MMA variant of the persistent 3x3 / stride-1 halo convolution for 64 input channels (opt-in: RLR_HALO3=1).
 //
-// conv_halo.cu issues nine N = 64 MMAs per 16-deep k-step (one per filter tap); those are bounded by shared-memory operand
-// bandwidth (6 KB per MMA, ~70 clk instead of 16; docs/NOTES_ROUND1.md).  Here the three taps of a filter ROW share one A view:
+// conv_halo.cu issues nine N = 64 MMAs per 16-deep k-step (one per filter tap).  Here the three taps of a filter ROW share one A view:
 //   D_j[h][w] = sum_ci x[h + dy - 1][w] * W[dy][j][ci][:]      for j = 0, 1, 2 at once  ->  one N = 192 MMA per (dy, k-step)
-// (B = the three consecutive 64 x 64 tap tiles of the resident filter, 192 rows, K-major), i.e. 3 MMAs of 10 KB instead of 9 of
-// 6 KB, and the column shift of the taps moves into the epilogue:
+// (B = the three consecutive 64 x 64 tap tiles of the resident filter, 192 rows, K-major), and the column shift of the taps moves
+// into the epilogue:
 //   out[h][c] = D_0[h][c - 1] + D_1[h][c] + D_2[h][c + 1]
-// Tile rows are (h, w) = 16 x 8 accumulator lanes with w the fast index, so "c -+ 1" is the neighbouring lane of the same 8-lane
-// group: two warp shuffles per value.  Only the six interior columns of a tile have both neighbours, so tiles advance by 6 columns
-// (8-column A views overlapping by 2): 75 % of the MMA rows are useful, against 3x fewer and 1.8x cheaper-per-tap MMAs.
+// Tile rows are (h, w) = 16 x 8 with w the fast index; in the wgmma accumulator fragment w = lane / 4, so "c -+ 1" is the value held
+// four lanes away: two warp shuffles per value.  Only the six interior columns of a tile have both neighbours, so tiles advance by 6
+// columns (8-column A views overlapping by 2): 75 % of the MMA rows are useful.
 // The halo box shrinks to 8 x 18 pixels (18 KB, row-group pitch 1024 B = the swizzle atom, so the three A views start atom-aligned).
-// Accumulators: 2 x 192 TMEM columns (double-buffered), filter resident (72 KB), 4-stage halo ring.
+// Two consumer warpgroups (image rows 0-7 / 8-15 of the tile, 96 accumulator registers each), filter resident (72 KB), 4-stage halo ring.
 #include <cuda.h>
 
 #include "common.cuh"
 #include "gemm.h"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace rlr {
 
-using namespace umma;
+using namespace wg;
 
 cudaError_t make_tmap_bf16(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                            const uint32_t* box, const uint32_t* elem_strides = nullptr);  // gemm.cu
 
 namespace {
 
-constexpr int H3_THREADS = 192;
+constexpr int H3_THREADS = 256 + 32;
 constexpr int H3_TH = 16, H3_TWD = 8, H3_VALID = 6;      // 16 x 8 accumulator rows per tile, 6 output columns of them valid
 constexpr int H3_HALO_BYTES = (H3_TH + 2) * H3_TWD * 128; // 18432
 constexpr int H3_W_BYTES = 9 * 64 * 128;                  // 73728
@@ -35,7 +33,6 @@ constexpr int H3_STAGES = 4;
 constexpr int H3_PITCH_OUT = 64 * 2 + 16;
 constexpr int H3_STAGING = 128 * H3_PITCH_OUT;
 constexpr int H3_SMEM = H3_W_BYTES + H3_STAGES * H3_HALO_BYTES + H3_STAGING + 1024 + 1024;
-constexpr int H3_ACC_COLS = 192;
 
 struct Halo3Params {
     int NB, H, W;
@@ -50,10 +47,6 @@ struct __align__(8) Halo3Shared {
     uint64_t w_full;
     uint64_t halo_full[H3_STAGES];
     uint64_t halo_empty[H3_STAGES];
-    uint64_t acc_full[2];
-    uint64_t acc_empty[2];
-    uint32_t tmem_base;
-    uint32_t pad;
 };
 
 template <bool kAcc>
@@ -68,23 +61,18 @@ umma_conv3x3_halo3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tile_n = blockIdx.y;
 
-    if (warp == 0 && lane == 0) { prefetch_tmap(&tmX); prefetch_tmap(&tmW); }
-    if (warp == 1 && lane == 0) {
+    if (warp == 8 && lane == 0) {
+        prefetch_tmap(&tmX); prefetch_tmap(&tmW);
         mbar_init(&sh->w_full, 1);
-        for (int s = 0; s < H3_STAGES; ++s) { mbar_init(&sh->halo_full[s], 1); mbar_init(&sh->halo_empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&sh->acc_full[a], 1); mbar_init(&sh->acc_empty[a], 128); }
+        for (int s = 0; s < H3_STAGES; ++s) { mbar_init(&sh->halo_full[s], 1); mbar_init(&sh->halo_empty[s], 8); }
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc(&sh->tmem_base, 512);          // 2 x 192 columns -> next power of two
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_acc = sh->tmem_base;
     const int tiles_per_img = p.tiles_h * p.tiles_w;
     pdl_wait();
     pdl_trigger();
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ===================== producer: filter once, then one 8 x 18 pixel box per tile ==================================
         if (lane == 0) {
             mbar_expect_tx(&sh->w_full, H3_W_BYTES);
@@ -100,92 +88,74 @@ umma_conv3x3_halo3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
                 if (++stage == H3_STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer: 3 filter rows x 4 k-steps of N = 192 ===========================================
-        if (lane == 0) {
-            constexpr uint32_t idesc = idesc_bf16(128, 192, 0, 0);
-            mbar_wait(&sh->w_full, 0);
-            int stage = 0, acc = 0;
-            uint32_t phase = 0, acc_phase = 0;
-            const uint32_t w_base = smem_u32(s_w);
-            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-                mbar_wait(&sh->acc_empty[acc], acc_phase ^ 1);
-                mbar_wait(&sh->halo_full[stage], phase);
-                tc_fence_after();
-                const uint32_t halo = smem_u32(s_halo + stage * H3_HALO_BYTES);
-                const uint32_t d_tmem = tmem_acc + acc * H3_ACC_COLS;
-#pragma unroll
-                for (int dy = 0; dy < 3; ++dy) {
-                    const uint32_t a0 = halo + dy * H3_TWD * 128;            // box row dy: 1024-byte (atom) aligned
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint64_t da = smem_desc_sw128(a0 + k * 32, 16, 1024);
-                        const uint64_t db = smem_desc_sw128(w_base + dy * 3 * 8192 + k * 32, 16, 1024);   // taps (dy,0..2): 192 rows
-                        umma_bf16(d_tmem, da, db, idesc, (dy > 0 || k > 0) ? 1u : 0u);
-                    }
-                }
-                umma_commit(&sh->halo_empty[stage]);
-                umma_commit(&sh->acc_full[acc]);
-                if (++stage == H3_STAGES) { stage = 0; phase ^= 1; }
-                acc ^= 1;
-                if (acc == 0) acc_phase ^= 1;
-            }
-        }
     } else {
-        // ===================== epilogue: shift-add of the three tap blocks, bias / ReLU / accumulate, stores ==============
-        const int et = threadIdx.x - 64;
-        const int lane_base = (warp & 3) * 32;
-        const int row = lane_base + lane;                       // accumulator row = h * 8 + w
+        // ===================== consumers: 3 filter rows x 4 k-steps of N = 192, shift-add, bias / ReLU / accumulate, stores =====
+        const int et = threadIdx.x;
+        const int wgi = et >> 7, t = et & 127;
+        const int r0 = wgi * 64 + frag_row(t, 0);               // accumulator rows r0, r0 + 8 (row = h * 8 + w, w = lane / 4)
         const int col0 = tile_n * 64;
+        const uint32_t w_base = smem_u32(s_w);
         __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out);
-        int acc = 0;
-        uint32_t acc_phase = 0;
+        int stage = 0;
+        uint32_t phase = 0;
+        mbar_wait(&sh->w_full, 0);
         for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
             const int n = tile / tiles_per_img, r = tile - n * tiles_per_img;
             const int h0 = (r / p.tiles_w) * H3_TH, oc0 = (r % p.tiles_w) * H3_VALID;    // first OUTPUT column of the tile
-            uint4 oldv[8];
+            uint4 oldv[4];
             if (kAcc) {
 #pragma unroll
-                for (int it = 0; it < 8; ++it) {
-                    const int idx = et + it * 128, rr = idx >> 3, ch = idx & 7;
+                for (int it = 0; it < 4; ++it) {
+                    const int idx = et + it * 256, rr = idx >> 3, ch = idx & 7;
                     const int wl = rr & 7, h = h0 + (rr >> 3), c = oc0 + wl - 1;
                     oldv[it] = make_uint4(0, 0, 0, 0);
                     if (wl >= 1 && wl <= H3_VALID && col0 + ch * 8 < p.N && h < p.H && c < p.W)
                         oldv[it] = *reinterpret_cast<const uint4*>(out + (((size_t)n * p.H + h) * p.W + c) * p.ldc + col0 + ch * 8);
                 }
             }
-            mbar_wait(&sh->acc_full[acc], acc_phase);
-            tc_fence_after();
-            const uint32_t t0 = tmem_acc + ((uint32_t)lane_base << 16) + acc * H3_ACC_COLS;
+            mbar_wait(&sh->halo_full[stage], phase);
+            const uint32_t halo = smem_u32(s_halo + stage * H3_HALO_BYTES) + wgi * 8 * 1024;   // image rows 8 wgi .. 8 wgi + 7
+            float acc[96];
 #pragma unroll
-            for (int c0 = 0; c0 < 64; c0 += 32) {
-                uint32_t d0[32], d1[32], d2[32];
-                tmem_ld_32x32(t0 + c0, d0);                    // tap column j = 0: contributes to the output one lane to the right
-                tmem_ld_32x32(t0 + 64 + c0, d1);
-                tmem_ld_32x32(t0 + 128 + c0, d2);              // j = 2: contributes to the output one lane to the left
-                uint32_t packed[16];
+            for (int i = 0; i < 96; ++i) acc[i] = 0.f;
+            wgmma_fence();
 #pragma unroll
-                for (int j = 0; j < 32; j += 2) {
-                    float a = __uint_as_float(d1[j]) + __shfl_up_sync(0xffffffffu, __uint_as_float(d0[j]), 1) +
-                              __shfl_down_sync(0xffffffffu, __uint_as_float(d2[j]), 1);
-                    float b = __uint_as_float(d1[j + 1]) + __shfl_up_sync(0xffffffffu, __uint_as_float(d0[j + 1]), 1) +
-                              __shfl_down_sync(0xffffffffu, __uint_as_float(d2[j + 1]), 1);
-                    if (p.bias && col0 + c0 + j < p.N) { a += p.bias[col0 + c0 + j]; b += p.bias[col0 + c0 + j + 1]; }
-                    if (p.relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
-                    packed[j >> 1] = pack_bf16x2(a, b);
-                }
-                uint4* dst = reinterpret_cast<uint4*>(s_stage + row * H3_PITCH_OUT + c0 * 2);
+            for (int dy = 0; dy < 3; ++dy) {
+                const uint32_t a0 = halo + dy * H3_TWD * 128;            // box row dy: 1024-byte (atom) aligned
 #pragma unroll
-                for (int q = 0; q < 4; ++q) dst[q] = make_uint4(packed[4 * q], packed[4 * q + 1], packed[4 * q + 2], packed[4 * q + 3]);
+                for (int k = 0; k < 4; ++k)
+                    wgmma_bf16<192, 0, 0>(acc, smem_desc_sw128(a0 + k * 32, 16, 1024),
+                                          smem_desc_sw128(w_base + dy * 3 * 8192 + k * 32, 16, 1024),   // taps (dy,0..2): 192 rows
+                                          (dy > 0 || k > 0) ? 1u : 0u);
             }
-            tc_fence_before();
-            mbar_arrive(&sh->acc_empty[acc]);
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            // stores: accumulator row rr = (h, wl); wl = 1..6 are the valid output columns oc0 + wl - 1 (lanes 0 and 7 of a group mixed
-            // in values of the neighbouring image row and are dropped)
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_acc(acc);
+            if (lane == 0) mbar_arrive(&sh->halo_empty[stage]);
+            if (++stage == H3_STAGES) { stage = 0; phase ^= 1; }
 #pragma unroll
-            for (int it = 0; it < 8; ++it) {
-                const int idx = et + it * 128, rr = idx >> 3, ch = idx & 7;
+            for (int j = 0; j < 8; ++j) {
+                const int c = frag_col(t, 4 * j);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    float v[2];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int i = 4 * j + 2 * h + e;
+                        // tap column j = 0 contributes to the output one pixel (4 lanes) to the right, j = 2 one pixel to the left
+                        v[e] = acc[32 + i] + __shfl_up_sync(0xffffffffu, acc[i], 4) + __shfl_down_sync(0xffffffffu, acc[64 + i], 4);
+                        if (p.bias && col0 + c + e < p.N) v[e] += p.bias[col0 + c + e];
+                        if (p.relu) v[e] = fmaxf(v[e], 0.f);
+                    }
+                    *reinterpret_cast<uint32_t*>(s_stage + (r0 + 8 * h) * H3_PITCH_OUT + c * 2) = pack_bf16x2(v[0], v[1]);
+                }
+            }
+            named_bar(1, 256);
+            // stores: accumulator row rr = (h, wl); wl = 1..6 are the valid output columns oc0 + wl - 1 (w = 0 and 7 lack a neighbour
+            // and are dropped)
+#pragma unroll
+            for (int it = 0; it < 4; ++it) {
+                const int idx = et + it * 256, rr = idx >> 3, ch = idx & 7;
                 const int wl = rr & 7, h = h0 + (rr >> 3), c = oc0 + wl - 1;
                 if (wl < 1 || wl > H3_VALID || col0 + ch * 8 >= p.N || h >= p.H || c >= p.W) continue;
                 uint4 val = *reinterpret_cast<const uint4*>(s_stage + rr * H3_PITCH_OUT + ch * 16);
@@ -201,14 +171,9 @@ umma_conv3x3_halo3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_
                 }
                 *gp = val;
             }
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1;
+            named_bar(1, 256);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_acc, 512);
 }
 
 }  // namespace

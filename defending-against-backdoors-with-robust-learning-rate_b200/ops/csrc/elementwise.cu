@@ -157,7 +157,7 @@ cudaError_t launch_gather_normalize(const void* data, int in_is_float, const int
     const float4 m4 = make_float4(mu[0], mu[1], mu[2], mu[3]), s4 = make_float4(is[0], is[1], is[2], is[3]);
     const int HW = H * W, total = B * HW, threads = 256, blocks = (total + threads - 1) / threads;
     const float sc = in_is_float ? 1.0f : (1.0f / 255.0f);
-    if (!nchw && out_kind == 1 && c_pad > C && c_pad % 8 == 0) {      // channel-padded bf16 NHWC (stem input of the tcgen05 conv)
+    if (!nchw && out_kind == 1 && c_pad > C && c_pad % 8 == 0) {      // channel-padded bf16 NHWC (stem input of the wgmma conv)
         const long long tot = (long long)total * (c_pad / 8);
         const int nb = (int)((tot + 255) / 256);
         if (in_is_float) gather_normalize_padded_kernel<float><<<nb, 256, 0, st>>>((const float*)data, idx, cursor, targets, (__nv_bfloat16*)out, out_labels, B, HW, C, c_pad, m4, s4, sc);
@@ -278,14 +278,14 @@ static inline int grid_for(long long n4, int threads, int num_sms, int per_sm) {
 cudaError_t launch_round_init(const float* w_global, float* w_local, __nv_bfloat16* w_bf16, float* mom, long long n,
                               cudaStream_t st) {
     if (n & 3) return cudaErrorInvalidValue;
-    round_init_kernel<<<grid_for(n / 4, 256, 148, 8), 256, 0, st>>>(w_global, w_local, w_bf16, mom, n / 4);
+    round_init_kernel<<<grid_for(n / 4, 256, 132, 8), 256, 0, st>>>(w_global, w_local, w_bf16, mom, n / 4);
     return cudaGetLastError();
 }
 
 // ------------------------------------------------------------------------------------------------------------
 // fused clip_grad_norm_(.,max) + SGD(momentum) [+ ||w-w0||^2 for PGD] over flat buffers   (src/agent.py:50-60)
 // ------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) sqnorm_kernel(const float* __restrict__ x, long long n4, double* out) {
+__global__ void __launch_bounds__(256) sqnorm_kernel(const float* __restrict__ x, long long n4, double* part /*[gridDim.x]*/) {
     __shared__ double scratch[32];
     double acc = 0.0;
     for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n4; q += (long long)gridDim.x * blockDim.x) {
@@ -293,11 +293,15 @@ __global__ void __launch_bounds__(256) sqnorm_kernel(const float* __restrict__ x
         acc += (double)(v.x * v.x + v.y * v.y) + (double)(v.z * v.z + v.w * v.w);
     }
     const double tot = block_sum<double>(acc, scratch);
-    if (threadIdx.x == 0) atomicAdd(out, tot);
+    if (threadIdx.x == 0) part[blockIdx.x] = tot;
 }
 cudaError_t launch_sqnorm(const float* x, long long n, double* out, int num_sms, cudaStream_t st) {
     if (n & 3) return cudaErrorInvalidValue;
-    sqnorm_kernel<<<grid_for(n / 4, 256, num_sms, 4), 256, 0, st>>>(x, n / 4, out);
+    const int grid = grid_for(n / 4, 256, num_sms, 4);
+    Scratch part((size_t)grid * sizeof(double), st);
+    sqnorm_kernel<<<grid, 256, 0, st>>>(x, n / 4, part.as<double>());
+    RLR_CUDA_CHECK(cudaGetLastError());
+    RLR_CUDA_CHECK(launch_ordered_sum(out, part.as<double>(), grid, 1LL, st));
     return cudaGetLastError();
 }
 
@@ -385,7 +389,7 @@ cudaError_t launch_pgd_project(float* w, const float* w0, __nv_bfloat16* w_bf16,
 // ------------------------------------------------------------------------------------------------------------
 template <typename T>
 __global__ void softmax_xent_kernel(const T* __restrict__ logits, const int64_t* __restrict__ labels, T* __restrict__ dlogits,
-                                    float* loss_sum, int* correct, int B, int C, float grad_scale) {
+                                    float* loss_part /*[gridDim.x]*/, int* correct, int B, int C, float grad_scale) {
     __shared__ float scratch[32];
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     float loss = 0.f;
@@ -408,7 +412,7 @@ __global__ void softmax_xent_kernel(const T* __restrict__ logits, const int64_t*
             for (int c = 0; c < C; ++c) dlogits[(int64_t)b * C + c] = (T)((v[c] * inv - (c == y ? 1.f : 0.f)) * grad_scale);
     }
     const float tot = block_sum<float>(loss, scratch);
-    if (threadIdx.x == 0 && loss_sum) atomicAdd(loss_sum, tot);
+    if (threadIdx.x == 0 && loss_part) loss_part[blockIdx.x] = tot;
     if (correct) {
         const int nok = __syncthreads_count(ok);
         if (threadIdx.x == 0 && nok) atomicAdd(correct, nok);
@@ -418,8 +422,12 @@ cudaError_t launch_softmax_xent(const void* logits, int kind, const int64_t* lab
                                 int* correct, int B, int C, float grad_scale, cudaStream_t st) {
     if (C > 32 || B <= 0) return cudaErrorInvalidValue;
     const int threads = 128, blocks = (B + threads - 1) / threads;
-    if (kind == 0) softmax_xent_kernel<float><<<blocks, threads, 0, st>>>((const float*)logits, labels, (float*)dlogits, loss_sum, correct, B, C, grad_scale);
-    else softmax_xent_kernel<__nv_bfloat16><<<blocks, threads, 0, st>>>((const __nv_bfloat16*)logits, labels, (__nv_bfloat16*)dlogits, loss_sum, correct, B, C, grad_scale);
+    Scratch part((size_t)blocks * sizeof(float), st);                 // per-block loss sums, added into loss_sum in block order
+    float* lp = loss_sum ? part.as<float>() : nullptr;
+    if (kind == 0) softmax_xent_kernel<float><<<blocks, threads, 0, st>>>((const float*)logits, labels, (float*)dlogits, lp, correct, B, C, grad_scale);
+    else softmax_xent_kernel<__nv_bfloat16><<<blocks, threads, 0, st>>>((const __nv_bfloat16*)logits, labels, (__nv_bfloat16*)dlogits, lp, correct, B, C, grad_scale);
+    RLR_CUDA_CHECK(cudaGetLastError());
+    if (loss_sum) RLR_CUDA_CHECK(launch_ordered_sum(loss_sum, part.as<float>(), blocks, 1LL, st));
     return cudaGetLastError();
 }
 

@@ -1,7 +1,7 @@
-// tcgen05 / TMEM / TMA GEMM and implicit-GEMM convolution for sm_100a (forward and data-gradient of every conv /
-// linear layer of the model zoo; replaces the cuDNN / cuBLAS calls behind src/models.py:22-31,47-58 and autograd).
+// wgmma / TMA GEMM and implicit-GEMM convolution for sm_90a (forward and data-gradient of every conv / linear layer of the
+// model zoo; replaces the cuDNN / cuBLAS calls behind src/models.py:22-31,47-58 and autograd).
 //
-//   C[M, N] = A[M, K] * B[N, K]^T      bf16 operands (K-major, 128-byte swizzled tiles), fp32 accumulation in TMEM
+//   C[M, N] = A[M, K] * B[N, K]^T      bf16 operands (K-major, 128-byte swizzled tiles), fp32 accumulation in registers
 //
 // * plain mode: A is a row-major [M][K] matrix (linear layers).
 // * conv mode : A is never materialised.  The activation tensor is NHWC; for filter tap (dy,dx) the 128 x 64 A tile of
@@ -10,28 +10,30 @@
 //   read a parity-split copy of the input ([4][N][H/2][W/2][C], see space_to_depth in norm.cu) through per-tap plane
 //   offsets, so they use the same kernel.  The data-gradient of a 3x3/s1 conv is the same kernel on dY with the
 //   tap-flipped, transposed filter.
-// * warp-specialised CTA (192 threads): warp 0 = TMA producer, warp 1 = single-thread tcgen05.mma issuer,
-//   warps 2-5 = epilogue (tcgen05.ld TMEM->registers, bias / ReLU / residual-accumulate, bf16 pack, staging through
-//   shared memory for fully coalesced 16-byte global stores, and per-channel sum / sum-of-squares reductions that feed
-//   BatchNorm -- fused here so the conv output is not re-read for statistics).
-// * 4-stage (BN=64) / 3-stage (BN=128) smem ring with full/empty mbarriers; tcgen05.commit releases stages; two CTAs
-//   are resident per SM (<= 113 KB smem, <= 128 TMEM columns each) so one CTA's epilogue overlaps the other's mainloop.
+// * warp-specialised CTA (320 threads): warps 0-7 = two consumer warpgroups, each issuing the m64 wgmma of its half of the
+//   128-row tile and then running the epilogue on its accumulator registers (bias / ReLU / dropout, bf16 pack, staging through
+//   shared memory for TMA tensor stores or fully coalesced 16-byte global stores, and per-channel sum / sum-of-squares
+//   reductions that feed BatchNorm -- fused here so the conv output is not re-read for statistics); warp 8 = TMA producer,
+//   warp 9 = second TMA producer for the B tiles.
+// * 4-stage (BN=64) / 3-stage (BN=128) smem ring with full/empty mbarriers; a stage is released once the wgmma group that read
+//   it has retired; two CTAs are resident per SM (<= 113 KB smem each) so one CTA's epilogue overlaps the other's mainloop.
 #include <cuda.h>
 #include <stdlib.h>
 
 #include "common.cuh"
 #include "gemm.h"
 #include "stem_gather.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace rlr {
 
-using namespace umma;
+using namespace wg;
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int kThreads = 192;
-constexpr int kEpiThreads = 128;
+constexpr int kConsumers = 256;                 // two warpgroups
+constexpr int kThreads = kConsumers + 64;       // + producer warps 8, 9
+constexpr int kEpiThreads = kConsumers;
 
 template <int BN, int kOcc = 2>
 struct TileCfg {
@@ -51,9 +53,9 @@ struct TileCfg {
 struct __align__(8) SharedTail {
     uint64_t full[4];
     uint64_t empty[4];
-    uint64_t tmem_full;
-    uint32_t tmem_base;
-    uint32_t pad;
+    uint64_t pad0;
+    uint32_t pad1;
+    uint32_t pad2;
     int row_index[BM];   // global output row of each tile row, -1 = masked
 };
 static_assert(sizeof(SharedTail) <= 640, "the bias slice starts 640 bytes into the tail");
@@ -61,7 +63,7 @@ static_assert(sizeof(SharedTail) <= 640, "the bias slice starts 640 bytes into t
 template <int BN, bool kStats, bool kBMN, int kOcc = 2>
 __global__ void __launch_bounds__(kThreads, kOcc)
 umma_conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC,
-                      const ConvGemmParams p) {
+                       const ConvGemmParams p) {
     using Cfg = TileCfg<BN, kOcc>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -81,19 +83,15 @@ umma_conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         w0 = tw_i * p.TW; h0 = th_i * p.TH; n0 = tn_i * p.TN;
     }
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         prefetch_tmap(&tmA);
         prefetch_tmap(&tmB);
         if (p.tma_store) prefetch_tmap(&tmC);
-    }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&tail->full[s], (p.split_prod || p.b_src) ? 2 : 1); mbar_init(&tail->empty[s], 1); }
-        mbar_init(&tail->tmem_full, 1);
+        for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&tail->full[s], (p.split_prod || p.b_src) ? 2 : 1); mbar_init(&tail->empty[s], 8); }
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc(&tail->tmem_base, BN);
-    if (warp >= 2) {   // each epilogue thread owns one tile row: resolve its global output row once
-        const int r = threadIdx.x - 64;
+    if (threadIdx.x < BM) {   // resolve the global output row of every tile row once
+        const int r = threadIdx.x;
         int gi;
         if (p.mode == 1) {
             const int tw = r % p.TW, th = (r / p.TW) % p.TH, tn = r / (p.TW * p.TH);
@@ -105,15 +103,12 @@ umma_conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         }
         tail->row_index[r] = gi;
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_acc = tail->tmem_base;
-    pdl_wait();        // everything above touched only parameters, shared memory and TMEM
+    pdl_wait();        // everything above touched only parameters and shared memory
     pdl_trigger();
     if (dbg && threadIdx.x == 0) dbg[1] = (long long)gtimer();
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ================================ TMA producer =====================================================================
         if (p.b_src) {
             // stem GEMM (ONE k-block, mode 0): the A tile is requested first, then -- while it is in flight -- the whole warp builds the
@@ -124,15 +119,15 @@ umma_conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
             }
             stem_gather_b(p, smem + Cfg::kABytes, BN, tile_n, lane);               // stage 0's B slot
             if (lane == 0) mbar_arrive(&tail->full[0]);
-        } else
-        if (lane == 0) {
+        } else if (lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
             for (int kb = 0; kb < p.num_kb; ++kb) {
                 mbar_wait(&tail->empty[stage], phase ^ 1);
                 uint8_t* sa = smem + stage * Cfg::kStageBytes;
                 uint8_t* sb = sa + Cfg::kABytes;
-                mbar_expect_tx(&tail->full[stage], (p.b_src || p.split_prod) ? Cfg::kABytes : Cfg::kStageBytes);
+                mbar_expect_tx(&tail->full[stage], p.split_prod ? Cfg::kABytes : Cfg::kStageBytes);
+                if (dbg && kb == 0) dbg[2] = (long long)gtimer();
                 if (p.mode == 1) {
                     const int tap = kb / p.cblocks, cb = kb - tap * p.cblocks;
                     tma_load_4d(&tmA, &tail->full[stage], sa, cb * BK, w0 * p.in_stride + p.dw[tap], h0 * p.in_stride + p.dh[tap],
@@ -140,8 +135,8 @@ umma_conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                 } else {
                     tma_load_2d(&tmA, &tail->full[stage], sa, kb * BK, tile_m * BM);
                 }
-                if (p.b_src || p.split_prod) {
-                    // B tile already written by the warp above / loaded by the second producer (warp 2)
+                if (p.split_prod) {
+                    // B tile loaded by the second producer (warp 9)
                 } else if (kBMN) {
                     // data gradient: B[k = co][n = ci] is a 64 x 64 box of the ORIGINAL filter W[co][tap][ci] (ci contiguous ->
                     // MN-major operand); one box per 64-wide ci group.  No transposed filter copy is ever materialised.
@@ -154,38 +149,9 @@ umma_conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                 if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        // ================================ MMA issuer (one thread) ==============================================================
-        if (lane == 0) {
-            constexpr uint32_t idesc = idesc_bf16(BM, BN, 0, kBMN ? 1 : 0);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int kb = 0; kb < p.num_kb; ++kb) {
-                mbar_wait(&tail->full[stage], phase);
-                tc_fence_after();
-                if (dbg && kb == 0) dbg[3] = (long long)gtimer();
-                const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-                const uint32_t sb = sa + Cfg::kABytes;
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k) {
-                    const uint64_t da = smem_desc_sw128(sa + k * 32, 16, 1024);
-                    // K-major B: 32-byte k-slices inside the 128-byte rows; MN-major B: 16 k-rows (2 KB) per slice, N groups 8 KB apart
-                    const uint64_t db = kBMN ? smem_desc_sw128(sb + k * 2048, 8192, 1024) : smem_desc_sw128(sb + k * 32, 16, 1024);
-                    umma_bf16(tmem_acc, da, db, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                }
-                umma_commit(&tail->empty[stage]);   // frees this smem stage once the MMAs above have read it
-                if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-            }
-            umma_commit(&tail->tmem_full);          // accumulator complete
-            if (dbg) dbg[4] = (long long)gtimer();
-        }
-    } else {
-        // ================================ epilogue (4 warps, 128 threads) =======================================================
-        const int et = threadIdx.x - 64;                 // 0..127
-        const int lane_base = (warp & 3) * 32;           // TMEM lanes this warp may access
-        const int row = lane_base + lane;                // tile row held by this thread
-        if (p.split_prod && warp == 2 && lane == 0) {
-            // second TMA producer: the B (filter) tiles of every k-block -- an independent request stream next to warp 0's A stream
+    } else if (warp == 9) {
+        if (p.split_prod && lane == 0) {
+            // second TMA producer: the B (filter) tiles of every k-block -- an independent request stream next to warp 8's A stream
             int stage = 0;
             uint32_t phase = 0;
             for (int kb = 0; kb < p.num_kb; ++kb) {
@@ -202,86 +168,87 @@ umma_conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                 if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
             }
         }
-        // the tile's bias values go to shared memory while the main loop runs (128 dependent global loads per thread in the epilogue
-        // cost 2.4 us per launch, scripts/bench_small_gemm.py)
+    } else {
+        // ================================ consumers: 2 warpgroups x 64 rows ==================================================
+        const int et = threadIdx.x;                      // 0..255
+        const int wgi = et >> 7, t = et & 127;
         const int col0 = tile_n * BN;
         const bool has_bias = !kBMN && p.bias != nullptr;   // data gradients (MN-major B) never carry a bias
-        if (has_bias) {
-            float* bw = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(tail) + 640);
-            for (int i = et; i < BN; i += kEpiThreads) bw[i] = (col0 + i < p.N) ? p.bias[col0 + i] : 0.f;
-            asm volatile("bar.sync 1, 128;" ::: "memory");
+        // the tile's bias values go to shared memory while the main loop runs
+        float* bias_w = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(tail) + 640);
+        if (has_bias)
+            for (int i = et; i < BN; i += kEpiThreads) bias_w[i] = (col0 + i < p.N) ? p.bias[col0 + i] : 0.f;
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        {
+            int stage = 0;
+            uint32_t phase = 0;
+            consumer_mainloop<BN, Cfg::kStages, Cfg::kStageBytes, Cfg::kABytes, kBMN>(
+                acc, smem, tail->full, tail->empty, p.num_kb, (uint32_t)wgi * 64 * 128, p.b_src ? smem_u32(smem + Cfg::kABytes) : 0u,
+                stage, phase, lane);
         }
-        __syncwarp();
-        mbar_wait(&tail->tmem_full, 0);
-        tc_fence_after();
-        const float* bias_s = reinterpret_cast<const float*>(reinterpret_cast<const uint8_t*>(tail) + 640);
+        if (dbg && et == 0) dbg[4] = (long long)gtimer();
+        named_bar(1, kEpiThreads);                       // both warpgroups are done with the ring (and the bias slice is written)
         if (dbg && et == 0) dbg[5] = (long long)gtimer();
+        const float* bias_s = bias_w;
         uint8_t* staging = smem;                         // operand ring is idle now: reuse it
         float* red = reinterpret_cast<float*>(staging + Cfg::kStagingBytes);   // [2][BN] per-tile column sums
-        const int gi_row = tail->row_index[row];
-        const bool row_ok = gi_row >= 0;
+        const int r0 = wgi * 64 + frag_row(t, 0);        // this thread's two tile rows: r0, r0 + 8
+        int gi_r[2];
+        gi_r[0] = tail->row_index[r0];
+        gi_r[1] = tail->row_index[r0 + 8];
         if (kStats) {
             for (int i = et; i < 2 * BN; i += kEpiThreads) red[i] = 0.f;
-            asm volatile("bar.sync 1, 128;" ::: "memory");
+            named_bar(1, kEpiThreads);
         }
         const bool tma_out = !kStats && p.tma_store;
-        // TMEM -> registers two 32-column loads at a time (one wait for both), bias / ReLU / bf16 pack, -> staging tile.
+        // registers -> bias / ReLU / dropout / bf16 pack -> staging tile.
         // Staging layout: TMA-store path = 128-byte-swizzled [64-channel group][128 rows][128 B] tiles (what cp.async.bulk.tensor reads);
         //                 accumulate / statistics path = padded row pitch for the coalesced read-modify-write stores below.
 #pragma unroll
-        for (int c0 = 0; c0 < BN; c0 += 64) {
-            uint32_t vv[2][32];
-            tmem_ld_32x32_nowait(tmem_acc + ((uint32_t)lane_base << 16) + c0, vv[0]);
-            tmem_ld_32x32_nowait(tmem_acc + ((uint32_t)lane_base << 16) + c0 + 32, vv[1]);
-            tmem_ld_wait();
+        for (int j = 0; j < BN / 8; ++j) {
+            const int c = frag_col(t, 4 * j);            // even column of this thread inside the 8-column group j
+            float s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const int cc = c0 + h * 32;
-                uint32_t (&v)[32] = vv[h];
-                uint32_t packed[16];
-                uint32_t keep8 = 0xffu;
-                float f1[32], f2[32];
-#pragma unroll
-                for (int j = 0; j < 32; j += 2) {
-                    float a = __uint_as_float(v[j]), b = __uint_as_float(v[j + 1]);
-                    if (has_bias) { a += bias_s[cc + j]; b += bias_s[cc + j + 1]; }
-                    if (p.relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
-                    if (p.drop.thr) {   // fused dropout (linear layers): one Philox call per 8 output columns of this row
-                        if ((j & 7) == 0) keep8 = dropout_keep8(p.drop, ((long long)(gi_row < 0 ? 0 : gi_row) * p.ldc + col0 + cc + j) >> 3);
-                        a = (keep8 >> (j & 7) & 1) ? a * p.drop.scale : 0.f;
-                        b = (keep8 >> ((j & 7) + 1) & 1) ? b * p.drop.scale : 0.f;
-                    }
-                    packed[j >> 1] = pack_bf16x2(a, b);
-                    if (kStats) {   // statistics of the bf16-rounded values BatchNorm will read back; masked rows count as zero
-                        const float2 rq = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&packed[j >> 1]));
-                        f1[j] = row_ok ? rq.x : 0.f; f1[j + 1] = row_ok ? rq.y : 0.f;
-                        f2[j] = f1[j] * f1[j]; f2[j + 1] = f1[j + 1] * f1[j + 1];
-                    }
+                const int row = r0 + 8 * h, gi_row = gi_r[h];
+                float a = acc[4 * j + 2 * h], b = acc[4 * j + 2 * h + 1];
+                if (has_bias) { a += bias_s[c]; b += bias_s[c + 1]; }
+                if (p.relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
+                if (p.drop.thr) {   // fused dropout (linear layers): keep-mask of the 8-column group of this row
+                    const uint32_t keep8 = dropout_keep8(p.drop, ((long long)(gi_row < 0 ? 0 : gi_row) * p.ldc + col0 + 8 * j) >> 3);
+                    a = (keep8 >> (c & 7) & 1) ? a * p.drop.scale : 0.f;
+                    b = (keep8 >> ((c & 7) + 1) & 1) ? b * p.drop.scale : 0.f;
                 }
-                if (tma_out) {
-                    uint8_t* gbase = staging + (cc >> 6) * (BM * 128) + row * 128;     // 64-channel group tile, this thread's 128-byte row
-                    const int ch0 = (cc & 63) >> 3;                                    // first 16-byte chunk of this 32-column piece
-#pragma unroll
-                    for (int q = 0; q < 4; ++q)
-                        *reinterpret_cast<uint4*>(gbase + (((ch0 + q) ^ (row & 7)) << 4)) =
-                            make_uint4(packed[4 * q], packed[4 * q + 1], packed[4 * q + 2], packed[4 * q + 3]);
-                } else {
-                    uint4* dst = reinterpret_cast<uint4*>(staging + row * Cfg::kPitch + cc * 2);
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) dst[q] = make_uint4(packed[4 * q], packed[4 * q + 1], packed[4 * q + 2], packed[4 * q + 3]);
+                const uint32_t packed = pack_bf16x2(a, b);
+                if (kStats && gi_row >= 0) {   // statistics of the bf16-rounded values BatchNorm will read back; masked rows count as zero
+                    const float2 rq = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&packed));
+                    s1[0] += rq.x; s1[1] += rq.y; s2[0] += rq.x * rq.x; s2[1] += rq.y * rq.y;
                 }
-                if (kStats) {   // warp-level column sums (31 shuffles each), 4 warps meet in shared memory
-                    const float c1 = warp_transpose_sum32(f1, lane), c2 = warp_transpose_sum32(f2, lane);
-                    atomicAdd(&red[cc + lane], c1);
-                    atomicAdd(&red[BN + cc + lane], c2);
+                if (tma_out)
+                    *reinterpret_cast<uint32_t*>(staging + (c >> 6) * (BM * 128) + row * 128 + ((((c & 63) >> 3) ^ (row & 7)) << 4) + (c & 7) * 2) = packed;
+                else
+                    *reinterpret_cast<uint32_t*>(staging + row * Cfg::kPitch + c * 2) = packed;
+            }
+            if (kStats) {   // column sums over the 8 lanes that share this thread's columns, then the warps meet in shared memory
+#pragma unroll
+                for (int o = 4; o < 32; o <<= 1)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        s1[e] += __shfl_xor_sync(0xffffffffu, s1[e], o);
+                        s2[e] += __shfl_xor_sync(0xffffffffu, s2[e], o);
+                    }
+                if (lane < 4) {
+                    atomicAdd(&red[c], s1[0]); atomicAdd(&red[c + 1], s1[1]);
+                    atomicAdd(&red[BN + c], s2[0]); atomicAdd(&red[BN + c + 1], s2[1]);
                 }
             }
         }
         if (tma_out) {
             fence_proxy_async_smem();                        // generic-proxy staging writes -> TMA (async proxy) reads
-            tc_fence_before();
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            if (dbg && et == 0) dbg[2] = (long long)gtimer();
+            named_bar(1, kEpiThreads);
+            if (dbg && et == 0) dbg[6] = (long long)gtimer();
             if (et == 0) {
                 // one TMA tensor store per 64-channel group: the box is the tile's pixel box of the NHWC output (rows / columns outside
                 // the tensor are clipped by the TMA unit) -- no per-thread address arithmetic, fully coalesced, asynchronous
@@ -294,11 +261,12 @@ umma_conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                 tma_store_commit();
             }
             if (p.stats) {
-                // BatchNorm statistics of this tile while the TMA unit drains it: thread = one output column (BN = 64: two threads per
-                // column, 64 rows each), walking the staged bf16 tile -- exactly the values BatchNorm will read back -- down its rows
-                // (masked rows skipped); ONE pair of global reductions per column and CTA, spread over kStatSlots partial buffers
-                const int c = BN == 128 ? et : (et & 63);
-                const int r_lo = BN == 128 ? 0 : (et >> 6) * (BM / 2), r_hi = BN == 128 ? BM : r_lo + BM / 2;
+                // BatchNorm statistics of this tile while the TMA unit drains it: kEpiThreads / BN threads per output column, each walking
+                // the staged bf16 tile -- exactly the values BatchNorm will read back -- down its share of the rows (masked rows skipped);
+                // ONE pair of global reductions per thread, spread over the stat_slots partial buffers
+                constexpr int kPerCol = kEpiThreads / BN, kRows = BM / kPerCol;
+                const int c = et % BN;
+                const int r_lo = (et / BN) * kRows, r_hi = r_lo + kRows;
                 const uint8_t* colp = staging + (c >> 6) * (BM * 128) + (c & 7) * 2;
                 const int chunk = (c & 63) >> 3;
                 float s1 = 0.f, s2 = 0.f;
@@ -314,24 +282,21 @@ umma_conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                     atomicAdd(dst + p.N, s2);
                 }
             }
-            if (et == 0) {
-                tma_store_wait_read();
-                if (dbg) dbg[6] = (long long)gtimer();
-            }
+            if (et == 0) tma_store_wait_read();
         } else {
-        tc_fence_before();
-        asm volatile("bar.sync 1, 128;" ::: "memory");   // epilogue-only named barrier: staging tile complete
-        if (dbg && et == 0) dbg[2] = (long long)gtimer();   // TMEM -> registers -> shared staging done
+        named_bar(1, kEpiThreads);                       // staging tile complete
+        if (dbg && et == 0) dbg[6] = (long long)gtimer();
         // ---- coalesced 16-byte stores (optionally accumulating into the existing output) ----
         constexpr int kChunks = BN * 2 / 16;             // 16 B chunks per row
         __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out);
-        constexpr int kIters = BM * kChunks / kEpiThreads;   // 8 (BN=64) / 16 (BN=128) chunks per thread
+        constexpr int kIters = BM * kChunks / kEpiThreads;   // 4 (BN=64) / 8 (BN=128) chunks per thread
+        constexpr int kBatch = kIters < 8 ? kIters : 8;
 #pragma unroll
-        for (int it0 = 0; it0 < kIters; it0 += 8) {
-            uint4 oldv[8];
-            if (p.accumulate) {                             // batch the read-modify-write loads: one latency per 8 chunks
+        for (int it0 = 0; it0 < kIters; it0 += kBatch) {
+            uint4 oldv[kBatch];
+            if (p.accumulate) {                             // batch the read-modify-write loads: one latency per batch
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
+                for (int j = 0; j < kBatch; ++j) {
                     const int idx = et + (it0 + j) * kEpiThreads, r = idx / kChunks, ch = idx - r * kChunks;
                     const int gi = tail->row_index[r];
                     oldv[j] = make_uint4(0, 0, 0, 0);
@@ -339,7 +304,7 @@ umma_conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                 }
             }
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
+            for (int j = 0; j < kBatch; ++j) {
                 const int idx = et + (it0 + j) * kEpiThreads, r = idx / kChunks, ch = idx - r * kChunks;
                 const int gi = tail->row_index[r];
                 if (gi < 0 || col0 + ch * 8 >= p.N) continue;     // masked row / column chunk beyond Cout
@@ -356,20 +321,15 @@ umma_conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                 *reinterpret_cast<uint4*>(out + (size_t)gi * p.ldc + col0 + ch * 8) = val;
             }
         }
-        if (dbg && et == 0) dbg[6] = (long long)gtimer();      // end of this thread's share of the epilogue stores
         // ---- per-channel statistics: one global reduction per column and tile, spread over kStatSlots partial buffers ----
         if (kStats) {
-            asm volatile("bar.sync 1, 128;" ::: "memory");   // (also orders the smem atomics above; the bar before the stores did too)
+            named_bar(1, kEpiThreads);                   // (also orders the smem atomics above; the bar before the stores did too)
             for (int i = et; i < 2 * BN; i += kEpiThreads)
                 if (col0 + (i % BN) < p.N)
                     atomicAdd(p.stats + (size_t)(blockIdx.x % kStatSlots) * 2 * p.N + (i < BN ? 0 : p.N) + col0 + (i % BN), red[i]);
         }
         }   // !tma_out
     }
-    // ---- teardown ----------------------------------------------------------------------------------------------------------
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_acc, BN);
 }
 
 // =====================================================================================================================
@@ -413,15 +373,15 @@ cudaError_t make_tmap_bf16(CUtensorMap* map, const void* base, int rank, const u
     return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 
-// gemm_persistent.cu (opt-in, RLR_PERSISTENT_CONV=1): one CTA per SM looping over tiles, double-buffered TMEM accumulators
+// gemm_persistent.cu (opt-in, RLR_PERSISTENT_CONV=1): one CTA per SM looping over tiles, operand ring running ahead of the epilogue
 template <int BN>
 cudaError_t launch_persistent_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvGemmParams& p, int m_tiles, int num_sms,
                                  cudaStream_t st, int occ = 1);
 
-// 0: two CTAs per SM for every tile | 1 (default, measured -1.4 % / round): three for the 64-wide tile | 2 (measured: 1072 vs 1065 ms, no gain): also
-// for the 128-wide tile (2-stage ring).  -1: take RLR_CONV_OCC3 from the environment on first use.
+// 0: two CTAs per SM for every tile | 1 (default): three for the 64-wide tile.  Levels above 1 select 1: three 320-thread CTAs of the
+// 128-wide tile would need 64 accumulator registers of a 64-register budget per thread.  -1: take RLR_CONV_OCC3 from the environment on first use.
 static int g_occ3 = -1;
-void set_conv_occ3(int level) { g_occ3 = level < 0 ? 0 : (level > 2 ? 2 : level); }
+void set_conv_occ3(int level) { g_occ3 = level < 0 ? 0 : (level > 1 ? 1 : level); }
 static int conv_occ3() {
     if (g_occ3 < 0) { const char* e = getenv("RLR_CONV_OCC3"); set_conv_occ3(e ? atoi(e) : 1); }
     return g_occ3;
@@ -443,41 +403,13 @@ static cudaError_t launch_bn_occ3(const CUtensorMap& tmA, const CUtensorMap& tmB
     return launch_kernel(umma_conv_gemm_kernel<BN, false, false, 3>, grid, dim3(kThreads), Cfg::kSmemBytes, st, tmA, tmB, tmC, p);
 }
 
-// gemm_2cta.cu (opt-in, RLR_CONV_2CTA=1): CTA pairs, tcgen05.mma.cta_group::2 with M = 256, half of the B tile per CTA
-template <int BN>
-cudaError_t launch_2cta_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvGemmParams& p, int m_tiles, cudaStream_t st, int deep);
-// 0 off | 1 pairs with two CTAs per SM (96 KB rings) | 2 deep variant: one CTA per SM with a 192 KB ring whenever the grid fits in one wave
-static int g_2cta = -1;
-static int g_pair_min_ctas = -1;
-void set_conv_2cta(int on) { g_2cta = on < 0 ? 0 : (on > 2 ? 2 : on); }
 static int sm_count() {
     static const int sms = [] {
         int dev = 0, n = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 148;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 132;
         return n;
     }();
     return sms;
-}
-// tile width of the CTA-pair kernel for an M-tiles x N problem, 0 = use the single-CTA kernels (flag off, shape not eligible, or
-// too few pairs to cover the SMs)
-static int pair_bn(int m_tiles, int N, bool eligible) {
-    if (g_2cta < 0) { const char* e = getenv("RLR_CONV_2CTA"); set_conv_2cta(e ? atoi(e) : 0); }
-    if (g_pair_min_ctas < 0) { const char* e = getenv("RLR_PAIR_MIN_CTAS"); g_pair_min_ctas = e ? atoi(e) : 96; }
-    if (!g_2cta || !eligible || N % 128) return 0;
-    const int ctas_m = (m_tiles + 1) / 2 * 2;
-    // N = 256 tiles halve the bytes per FLOP again (A tile shared by 256 output channels): worth it even when the pairs leave some SMs idle
-    int bn = (N % 256 == 0) ? 256 : 128;
-    if (bn == 256 && ctas_m * (N / 256) < g_pair_min_ctas) bn = 128;
-    if (ctas_m * (N / bn) < g_pair_min_ctas) return 0;
-    return bn;
-}
-static int pair_deep(int m_tiles, int N, int bn) {
-    const int ctas = (m_tiles + 1) / 2 * 2 * (N / bn);
-    return (g_2cta == 2 && ctas <= sm_count()) ? 1 : 0;
-}
-static cudaError_t launch_pair(int bn2, const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvGemmParams& p, int m_tiles, cudaStream_t st) {
-    const int deep = pair_deep(m_tiles, p.N, bn2);
-    return bn2 == 256 ? launch_2cta_bn<256>(tmA, tmB, p, m_tiles, st, deep) : launch_2cta_bn<128>(tmA, tmB, p, m_tiles, st, deep);
 }
 
 static int g_persistent = -1;   // -1: take RLR_PERSISTENT_CONV from the environment on first use
@@ -535,12 +467,12 @@ static cudaError_t launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, con
     p.tma_store = 0;
     if (tma_store_enabled() && !p.accumulate && ((reinterpret_cast<uintptr_t>(p.out) & 15) == 0) && make_out_tmap(&tmC, p) == cudaSuccess)
         p.tma_store = 1;
-    if (g_split_prod < 0) { const char* e = getenv("RLR_SPLIT_PRODUCER"); g_split_prod = (e && atoi(e) == 0) ? 0 : 1; }   // default on: -2.2 % per round (profiles/r2_step_ab.md)
+    if (g_split_prod < 0) { const char* e = getenv("RLR_SPLIT_PRODUCER"); g_split_prod = (e && atoi(e) == 0) ? 0 : 1; }   // default on
     p.split_prod = (g_split_prod && !p.b_src) ? 1 : 0;
     if (p.b_src && !p.stats && p.N <= BN) {
         // stem GEMM: ONE k-block per output tile, so a one-tile CTA is all fixed cost (set-up, the filter gather, a lone TMA round trip).
         // The persistent kernel builds the B tile once per SM, streams the A tiles through its ring and overlaps every tile's epilogue
-        // with the next tile's MMAs (double-buffered TMEM).  RLR_STEM_PERSISTENT=0 restores the one-tile-per-CTA launch.
+        // with the next tile's operand loads.  RLR_STEM_PERSISTENT=0 restores the one-tile-per-CTA launch.
         // (RLR_STEM_PERSISTENT=1: one CTA per SM with the deep ring; default 2: two CTAs per SM, 3-stage rings -- the tiles are epilogue bound)
         static const int stem_persistent = [] { const char* e = getenv("RLR_STEM_PERSISTENT"); return e ? atoi(e) : 2; }();
         if (stem_persistent && m_tiles >= 2 * sm_count())
@@ -549,7 +481,8 @@ static cudaError_t launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, con
     if (!p.stats && !p.b_src && persistent_sms() > 0 && m_tiles * ((p.N + BN - 1) / BN) > persistent_sms())
         return launch_persistent_bn<BN>(tmA, tmB, p, m_tiles, persistent_sms(), st);
     // statistics ride on the TMA-store epilogue of the plain instantiation (runtime p.stats); without TMA stores: the kStats variant below
-    if ((!p.stats || p.tma_store) && conv_occ3() >= (BN == 64 ? 1 : 2)) return launch_bn_occ3<BN>(tmA, tmB, tmC, p, m_tiles, st);
+    if constexpr (BN == 64)
+        if ((!p.stats || p.tma_store) && conv_occ3() >= 1) return launch_bn_occ3<BN>(tmA, tmB, tmC, p, m_tiles, st);
     static bool configured = false;
     if (!configured) {
         RLR_CUDA_CHECK(cudaFuncSetAttribute(umma_conv_gemm_kernel<BN, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
@@ -571,11 +504,10 @@ cudaError_t launch_gemm_bf16(const void* A, const void* B, void* out, int M, int
     if (K % BK || N % 8 || M <= 0) return cudaErrorInvalidValue;
     if (drop && drop->thr && (accumulate || stats || ldc % 8)) return cudaErrorInvalidValue;
     const int m_tiles = (M + BM - 1) / BM;
-    const int bn2 = pair_bn(m_tiles, N, stats == nullptr);
-    int bn = bn2 ? bn2 : pick_bn(N);
-    {   // opt-in (RLR_GEMM_SMALL_BN64=1; measured 256x128x1024: 15.2 -> 11.5 us, 256x256x128: 11.2 -> 9.3 us, profiles/raw/r2_experiments_summary.txt): small-batch linear layers (M = 256: two M tiles) get twice the CTAs
+    int bn = pick_bn(N);
+    {   // opt-in (RLR_GEMM_SMALL_BN64=1): small-batch linear layers (M = 256: two M tiles) get twice the CTAs
         static const int small64 = [] { const char* e = getenv("RLR_GEMM_SMALL_BN64"); return e ? atoi(e) : 0; }();
-        if (small64 && !bn2 && bn == 128 && m_tiles * (N / 128) < sm_count()) bn = 64;
+        if (small64 && bn == 128 && m_tiles * (N / 128) < sm_count()) bn = 64;
     }
     CUtensorMap tmA, tmB;
     {
@@ -585,17 +517,13 @@ cudaError_t launch_gemm_bf16(const void* A, const void* B, void* out, int M, int
     }
     {
         const uint64_t d[2] = {(uint64_t)K, (uint64_t)N}, s[1] = {(uint64_t)ldb * 2};
-        const uint32_t b[2] = {BK, (uint32_t)(bn2 ? bn2 / 2 : bn)};       // CTA pair: each CTA stages half of the B tile
+        const uint32_t b[2] = {BK, (uint32_t)bn};
         RLR_CUDA_CHECK(make_tmap_bf16(&tmB, B, 2, d, s, b));
     }
     ConvGemmParams p{};
     p.M = M; p.N = N; p.num_kb = K / BK; p.mode = 0; p.in_stride = 1; p.out_stride = 1;
     p.out = out; p.ldc = ldc; p.bias = bias; p.stats = stats; p.relu = relu; p.accumulate = accumulate;
-    if (drop && drop->thr) {      // fused dropout lives in the single-CTA kernel's epilogue
-        p.drop = *drop;
-        return bn == 128 ? launch_bn<128>(tmA, tmB, p, m_tiles, st) : launch_bn<64>(tmA, tmB, p, m_tiles, st);
-    }
-    if (bn2) return launch_pair(bn2, tmA, tmB, p, m_tiles, st);
+    if (drop && drop->thr) p.drop = *drop;      // fused dropout lives in the epilogue
     return bn == 128 ? launch_bn<128>(tmA, tmB, p, m_tiles, st) : launch_bn<64>(tmA, tmB, p, m_tiles, st);
 }
 
@@ -637,9 +565,9 @@ cudaError_t launch_conv_bf16(const void* x, const void* w, void* out, int NB, in
     int bn = pick_bn(Cout);
     ConvGemmParams p{};
     {   // few M tiles (deep layers at small batch / 4x4 maps): prefer the 64-wide tile so the grid covers all SMs
-        static const int small_bn64 = [] { const char* e = getenv("RLR_SMALL_BN64"); return e ? atoi(e) : 1; }();   // measured +2.4 %
+        static const int small_bn64 = [] { const char* e = getenv("RLR_SMALL_BN64"); return e ? atoi(e) : 1; }();
         const long long px = (long long)NB * Ho * Wo;
-        if (small_bn64 && bn == 128 && ((px + BM - 1) / BM) * (Cout / 128) < 148) bn = 64;
+        if (small_bn64 && bn == 128 && ((px + BM - 1) / BM) * (Cout / 128) < sm_count()) bn = 64;
     }
     // output tile: TW x TH x TN = 128 output pixels, TW/TH powers of two covering the image
     int TW = pow2_ceil(Wo); if (TW > BM) TW = BM;
@@ -673,15 +601,11 @@ cudaError_t launch_conv_bf16(const void* x, const void* w, void* out, int NB, in
         const uint64_t d[2] = {cols, (uint64_t)Cin}, s[1] = {cols * 2};
         const uint32_t b[2] = {64, BK};
         RLR_CUDA_CHECK(make_tmap_bf16(&tmB, w, 2, d, s, b));
-        const int bn2 = pair_bn(m_tiles, Cout, true);      // CTA pair: each CTA loads the 64-wide groups of its half of the tile
-        if (bn2) return launch_pair(bn2, tmA, tmB, p, m_tiles, st);
     } else {
         const uint64_t K = (uint64_t)ntaps * Cin;
         const uint64_t d[2] = {K, (uint64_t)Cout}, s[1] = {K * 2};
-        const int bn2 = pair_bn(m_tiles, Cout, stats == nullptr);
-        const uint32_t b[2] = {BK, (uint32_t)(bn2 ? bn2 / 2 : bn)};       // CTA pair: each CTA stages half of the filter tile
+        const uint32_t b[2] = {BK, (uint32_t)bn};
         RLR_CUDA_CHECK(make_tmap_bf16(&tmB, w, 2, d, s, b));
-        if (bn2) return launch_pair(bn2, tmA, tmB, p, m_tiles, st);
     }
     return bn == 128 ? launch_bn<128>(tmA, tmB, p, m_tiles, st) : launch_bn<64>(tmA, tmB, p, m_tiles, st);
 }

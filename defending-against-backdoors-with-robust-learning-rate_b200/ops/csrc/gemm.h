@@ -1,4 +1,5 @@
-// tcgen05 / TMA GEMM + implicit-GEMM convolution launchers (gemm.cu, wgrad.cu) and the memory-bound layer kernels
+// wgmma / TMA GEMM + implicit-GEMM convolution launchers (gemm.cu, wgrad.cu) and the memory-bound layer kernels
+// (the tensor-core kernels keep their historical umma_* names; all of them issue Hopper wgmma, see wgmma.cuh)
 // (norm.cu).  Raw pointers + stream; bindings in gemm_binding.cpp.
 #pragma once
 #include <cuda_runtime.h>
@@ -60,15 +61,13 @@ cudaError_t launch_stem_gemm_bf16(const void* A, const void* W, void* out, int M
                                   cudaStream_t st);
 // programmatic dependent launch for the hot kernels (common.cuh: launch_kernel / pdl_wait); default: RLR_PDL env, off
 void set_pdl(int on);
-// gemm_splitk.cu (opt-in): small-M / deep-K GEMM, grid.z CTAs share a tile's k range and add fp32 partials into `ws` ([M][N], zero on
-// entry and left zero), then one finishing pass applies bias / ReLU and packs bf16
+// gemm_splitk.cu: small-M / deep-K GEMM, grid.z CTAs share a tile's k range and store fp32 partials into per-split slots of stream
+// scratch memory, then one finishing pass adds them in split order, applies bias / ReLU and packs bf16 (`ws` is not used)
 cudaError_t launch_gemm_splitk_bf16(const void* A, const void* B, void* out, float* ws, int M, int N, int K, const float* bias, int relu,
                                     int num_sms, cudaStream_t st, const DropSpec* drop = nullptr);
-// opt-in CTA-pair kernel (gemm_2cta.cu: tcgen05.mma.cta_group::2, M = 256, half a B tile per CTA); default: RLR_CONV_2CTA env, off
-void set_conv_2cta(int on);
 // opt-in persistent tile scheduler for the generic conv / GEMM kernel (gemm_persistent.cu); default: RLR_PERSISTENT_CONV env
 void set_persistent_conv(int on);
-// three CTAs per SM: level 0 never, 1 (default) for the 64-wide tile, 2 also for the 128-wide tile (RLR_CONV_OCC3 env)
+// three CTAs per SM: level 0 never, 1 (default) for the 64-wide tile (RLR_CONV_OCC3 env; higher levels select 1)
 void set_conv_occ3(int level);
 // per-CTA timeline buffer for the NEXT launches of the generic conv / GEMM kernel (nullptr = off); see ConvGemmParams::dbg
 void set_conv_tma_store(int on);           // epilogue via TMA tensor stores (default on; RLR_TMA_STORE=0)
@@ -88,7 +87,7 @@ cudaError_t launch_conv3x3_halo_bf16(const void* x, const void* w, void* out, in
 cudaError_t launch_conv3x3_halo3_bf16(const void* x, const void* w, void* out, int NB, int H, int W, int Cout, const float* bias, int relu,
                                       int accumulate, int num_sms, cudaStream_t st);
 
-// ---- wgrad.cu: MN-major tcgen05 weight gradients (fp32, accumulated with red.add) -----------------------------------
+// ---- wgrad.cu: MN-major wgmma weight gradients (fp32, added into dW; split-K partials summed in split order) ---------
 cudaError_t launch_conv_wgrad_bf16(const void* dy, const void* x, float* dW, int NB, int planes, int Hin, int Win, int Cin, int Cin_valid,
                                    int Ho, int Wo, int Cout, int ntaps, const int* dh, const int* dw, const int* dplane, int num_sms,
                                    cudaStream_t st, int in_stride = 1);

@@ -1,12 +1,21 @@
-// Python bindings for the tcgen05 GEMM / implicit-GEMM conv kernels (gemm.cu) and the NHWC layer kernels (norm.cu).
+// Python bindings for the wgmma GEMM / implicit-GEMM conv kernels (gemm.cu) and the NHWC layer kernels (norm.cu).
 #include <torch/extension.h>
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <c10/cuda/CUDAStream.h>
+#include <c10/cuda/CUDACachingAllocator.h>
 
 #include <vector>
 
 #include "gemm.h"
+
+namespace rlr {
+// scratch memory of the deterministic reductions (common.cuh): PyTorch's caching allocator, ordered on the launch stream
+void* scratch_alloc(size_t bytes, cudaStream_t st) {
+    return c10::cuda::CUDACachingAllocator::raw_alloc_with_stream(bytes < 256 ? 256 : bytes, st);
+}
+void scratch_free(void* p) { c10::cuda::CUDACachingAllocator::raw_delete(p); }
+}  // namespace rlr
 
 namespace {
 inline cudaStream_t cur_stream() { return c10::cuda::getCurrentCUDAStream().stream(); }
@@ -336,7 +345,6 @@ void linear_small_bwd2(at::Tensor x, at::Tensor dy, at::Tensor w, c10::optional<
 void register_gemm_bindings(py::module_& m) {
     m.attr("STAT_SLOTS") = rlr::kStatSlots;
     m.def("set_persistent_conv", [](bool on) { rlr::set_persistent_conv(on ? 1 : 0); });
-    m.def("set_conv_2cta", [](int64_t mode) { rlr::set_conv_2cta((int)mode); });   // 0 off | 1 CTA pairs | 2 + deep single-wave variant
     m.def("set_pdl", [](bool on) { rlr::set_pdl(on ? 1 : 0); });
     m.def("set_conv_occ3", [](int64_t level) { rlr::set_conv_occ3((int)level); });
     m.def("set_conv_tma_store", [](bool on) { rlr::set_conv_tma_store(on ? 1 : 0); });

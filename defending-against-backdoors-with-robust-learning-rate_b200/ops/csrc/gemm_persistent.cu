@@ -1,26 +1,25 @@
-// Persistent variant of the implicit-GEMM conv / GEMM kernel of gemm.cu (opt-in: RLR_PERSISTENT_CONV=1).
+// Persistent variant of the implicit-GEMM conv / GEMM kernel of gemm.cu (opt-in: RLR_PERSISTENT_CONV=1; default for the stem GEMM).
 //
-// Same operands, tap tables and epilogue semantics as umma_conv_gemm_kernel, but ONE CTA per SM loops over output tiles
-// (tile = blockIdx.x, += gridDim.x; consecutive tiles share the filter n-tile), with a deeper operand ring (7 x 24 KB for
-// BN = 64, 5 x 32 KB for BN = 128), a dedicated staging tile and DOUBLE-BUFFERED TMEM accumulators (2 x BN columns): the
-// producer and the MMA thread run straight through tile boundaries while the four epilogue warps drain tile i during the
-// main loop of tile i+1 -- the structure validated in conv_halo.cu.  No statistics path (BatchNorm statistics are taken by
-// the streaming pass, see models/native.py).
+// Same operands, tap tables and epilogue semantics as umma_conv_gemm_kernel, but the CTA loops over output tiles (tile = blockIdx.x,
+// += gridDim.x; consecutive tiles share the filter n-tile) with a deeper operand ring (7 x 24 KB for BN = 64, 5 x 32 KB for BN = 128)
+// and a dedicated staging tile: the producer warp runs straight through tile boundaries, so the operands of tile i+1 are in flight
+// while the two consumer warpgroups (64 rows each) run the epilogue of tile i.  No statistics path (BatchNorm statistics are taken
+// by the streaming pass, see models/native.py).
 #include <cuda.h>
 
 #include "common.cuh"
 #include "gemm.h"
 #include "stem_gather.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace rlr {
 
-using namespace umma;
+using namespace wg;
 
-constexpr int PBM = 128, PBK = 64, PThreads = 192;
+constexpr int PBM = 128, PBK = 64, PConsumers = 256, PThreads = PConsumers + 32;
 
 // kOcc = 1: one CTA per SM with a deep ring (7 x 24 KB / 5 x 32 KB).  kOcc = 2: two CTAs per SM with a 3-stage ring -- for the stem GEMM,
-// whose one-k-block tiles are EPILOGUE bound: two CTAs give the SM two epilogue warp-groups (and two TMA streams) to drain them.
+// whose one-k-block tiles are EPILOGUE bound: two CTAs give the SM two sets of epilogue warpgroups (and two TMA streams) to drain them.
 template <int BN, int kOcc = 1>
 struct PCfg {
     static constexpr int kStages = kOcc == 2 ? 3 : (BN == 64 ? 7 : 5);
@@ -37,10 +36,6 @@ struct PCfg {
 struct __align__(8) PShared {
     uint64_t full[8];
     uint64_t empty[8];
-    uint64_t acc_full[2];
-    uint64_t acc_empty[2];
-    uint32_t tmem_base;
-    uint32_t pad;
     int row_index[PBM];
 };
 static_assert(sizeof(PShared) <= 704, "the bias slice starts 704 bytes into the tail");
@@ -48,7 +43,7 @@ static_assert(sizeof(PShared) <= 704, "the bias slice starts 704 bytes into the 
 template <int BN, bool kBMN, int kOcc = 1>
 __global__ void __launch_bounds__(PThreads, kOcc)
 umma_conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvGemmParams p,
-                                 const int m_tiles, const int total_tiles) {
+                                  const int m_tiles, const int total_tiles) {
     using Cfg = PCfg<BN, kOcc>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -56,17 +51,12 @@ umma_conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const 
     PShared* sh = reinterpret_cast<PShared*>(staging + Cfg::kStagingBytes);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-    if (warp == 0 && lane == 0) { prefetch_tmap(&tmA); prefetch_tmap(&tmB); }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&sh->full[s], 1); mbar_init(&sh->empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&sh->acc_full[a], 1); mbar_init(&sh->acc_empty[a], 128); }
+    if (warp == 8 && lane == 0) {
+        prefetch_tmap(&tmA); prefetch_tmap(&tmB);
+        for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&sh->full[s], 1); mbar_init(&sh->empty[s], 8); }
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc(&sh->tmem_base, 2 * BN);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_acc = sh->tmem_base;
 
     // tile -> (tile_m, tile_n) and image-space origin
     auto origin = [&](int tile, int& tile_m, int& tile_n, int& n0, int& h0, int& w0) {
@@ -78,9 +68,10 @@ umma_conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const 
         }
     };
 
-    if (warp == 0) {
+    if (warp == 8) {
         // stem GEMM (b_src: one k-block, one n-tile): the B tile is built ONCE per CTA by this warp in the B slot of stage 0 (no stage ever
-        // loads a B tile in this mode, so the slot is never overwritten) and every tile's MMAs read it there; per tile only A is fetched
+        // loads a B tile in this mode, so the slot is never overwritten) and every tile's MMAs read it there; per tile only A is fetched.
+        // The first full[0] arrival orders the gather before every consumer read of the slot.
         if (p.b_src) stem_gather_b(p, smem + Cfg::kABytes, BN, 0, lane);
         if (lane == 0) {
             int stage = 0;
@@ -109,56 +100,29 @@ umma_conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const 
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = idesc_bf16(PBM, BN, 0, kBMN ? 1 : 0);
-            int stage = 0, acc = 0;
-            uint32_t phase = 0, acc_phase = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                mbar_wait(&sh->acc_empty[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_acc + acc * BN;
-                for (int kb = 0; kb < p.num_kb; ++kb) {
-                    mbar_wait(&sh->full[stage], phase);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-                    const uint32_t sb = p.b_src ? smem_u32(smem + Cfg::kABytes) : sa + Cfg::kABytes;
-#pragma unroll
-                    for (int k = 0; k < PBK / 16; ++k) {
-                        const uint64_t da = smem_desc_sw128(sa + k * 32, 16, 1024);
-                        const uint64_t db = kBMN ? smem_desc_sw128(sb + k * 2048, 8192, 1024) : smem_desc_sw128(sb + k * 32, 16, 1024);
-                        umma_bf16(d_tmem, da, db, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                    }
-                    umma_commit(&sh->empty[stage]);
-                    if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(&sh->acc_full[acc]);
-                acc ^= 1;
-                if (acc == 0) acc_phase ^= 1;
-            }
-        }
     } else {
-        const int et = threadIdx.x - 64;
-        const int lane_base = (warp & 3) * 32;
-        const int row = lane_base + lane;
+        const int et = threadIdx.x;                 // 0..255
+        const int wgi = et >> 7, t = et & 127;
+        const int r0 = wgi * 64 + frag_row(t, 0);   // this thread's two tile rows: r0, r0 + 8
         __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out);
         constexpr int kChunks = BN * 2 / 16;
-        constexpr int kIters = PBM * kChunks / 128;
-        int acc = 0;
-        uint32_t acc_phase = 0;
+        constexpr int kIters = PBM * kChunks / PConsumers;
+        constexpr int kBatch = kIters < 8 ? kIters : 8;
         float* bias_s = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(sh) + 704);
         int bias_tile_n = -1;
+        int stage = 0;
+        uint32_t phase = 0;
+        const uint32_t b_fixed = p.b_src ? smem_u32(smem + Cfg::kABytes) : 0u;
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
             int tile_m, tile_n, n0, h0, w0;
             origin(tile, tile_m, tile_n, n0, h0, w0);
             const int col0 = tile_n * BN;
             if (p.bias && tile_n != bias_tile_n) {   // (re)load this n-tile's bias values; consecutive tiles share the n-tile
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                for (int i = et; i < BN; i += 128) bias_s[i] = (col0 + i < p.N) ? p.bias[col0 + i] : 0.f;
-                asm volatile("bar.sync 1, 128;" ::: "memory");
+                for (int i = et; i < BN; i += PConsumers) bias_s[i] = (col0 + i < p.N) ? p.bias[col0 + i] : 0.f;
                 bias_tile_n = tile_n;
             }
-            {   // global output row of my tile row (-1 = masked); staging / row_index of the previous tile are free (end-of-tile barrier)
+            if (et < PBM) {   // global output row of every tile row (-1 = masked); the previous tile's readers are past the end-of-tile barrier
+                const int row = et;
                 int gi;
                 if (p.mode == 1) {
                     const int tw = row % p.TW, th = (row / p.TW) % p.TH, tn = row / (p.TW * p.TH);
@@ -171,42 +135,39 @@ umma_conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const 
                 }
                 sh->row_index[row] = gi;
             }
-            mbar_wait(&sh->acc_full[acc], acc_phase);
-            tc_fence_after();
+            float acc[BN / 2];
 #pragma unroll
-            for (int c0 = 0; c0 < BN; c0 += 32) {
-                uint32_t v[32];
-                tmem_ld_32x32(tmem_acc + ((uint32_t)lane_base << 16) + acc * BN + c0, v);
-                uint32_t packed[16];
+            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+            consumer_mainloop<BN, Cfg::kStages, Cfg::kStageBytes, Cfg::kABytes, kBMN>(acc, smem, sh->full, sh->empty, p.num_kb,
+                                                                                       (uint32_t)wgi * 64 * 128, b_fixed, stage, phase, lane);
+            named_bar(1, PConsumers);                // bias slice and row_index of this tile are written
 #pragma unroll
-                for (int j = 0; j < 32; j += 2) {
-                    float a = __uint_as_float(v[j]), b = __uint_as_float(v[j + 1]);
-                    if (p.bias) { a += bias_s[c0 + j]; b += bias_s[c0 + j + 1]; }
+            for (int j = 0; j < BN / 8; ++j) {
+                const int c = frag_col(t, 4 * j);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    float a = acc[4 * j + 2 * h], b = acc[4 * j + 2 * h + 1];
+                    if (p.bias) { a += bias_s[c]; b += bias_s[c + 1]; }
                     if (p.relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
-                    packed[j >> 1] = pack_bf16x2(a, b);
+                    *reinterpret_cast<uint32_t*>(staging + (r0 + 8 * h) * Cfg::kPitch + c * 2) = pack_bf16x2(a, b);
                 }
-                uint4* dst = reinterpret_cast<uint4*>(staging + row * Cfg::kPitch + c0 * 2);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) dst[q] = make_uint4(packed[4 * q], packed[4 * q + 1], packed[4 * q + 2], packed[4 * q + 3]);
             }
-            tc_fence_before();
-            mbar_arrive(&sh->acc_empty[acc]);                  // accumulator drained: the MMA thread may start tile i+2 in it
-            asm volatile("bar.sync 1, 128;" ::: "memory");    // staging tile + row_index complete
+            named_bar(1, PConsumers);                // staging tile complete
 #pragma unroll
-            for (int it0 = 0; it0 < kIters; it0 += 8) {
-                uint4 oldv[8];
+            for (int it0 = 0; it0 < kIters; it0 += kBatch) {
+                uint4 oldv[kBatch];
                 if (p.accumulate) {
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const int idx = et + (it0 + j) * 128, r = idx / kChunks, ch = idx - r * kChunks;
+                    for (int j = 0; j < kBatch; ++j) {
+                        const int idx = et + (it0 + j) * PConsumers, r = idx / kChunks, ch = idx - r * kChunks;
                         const int gi = sh->row_index[r];
                         oldv[j] = make_uint4(0, 0, 0, 0);
                         if (gi >= 0 && col0 + ch * 8 < p.N) oldv[j] = *reinterpret_cast<const uint4*>(out + (size_t)gi * p.ldc + col0 + ch * 8);
                     }
                 }
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const int idx = et + (it0 + j) * 128, r = idx / kChunks, ch = idx - r * kChunks;
+                for (int j = 0; j < kBatch; ++j) {
+                    const int idx = et + (it0 + j) * PConsumers, r = idx / kChunks, ch = idx - r * kChunks;
                     const int gi = sh->row_index[r];
                     if (gi < 0 || col0 + ch * 8 >= p.N) continue;
                     uint4 val = *reinterpret_cast<const uint4*>(staging + r * Cfg::kPitch + ch * 16);
@@ -222,14 +183,9 @@ umma_conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const 
                     *reinterpret_cast<uint4*>(out + (size_t)gi * p.ldc + col0 + ch * 8) = val;
                 }
             }
-            asm volatile("bar.sync 1, 128;" ::: "memory");    // staging / row_index may be overwritten by the next tile
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1;
+            named_bar(1, PConsumers);                // staging / row_index / bias slice may be overwritten by the next tile
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_acc, 2 * BN);
 }
 
 template <int BN>

@@ -1,4 +1,4 @@
-// Host-callable launchers of the sm_100a kernels (raw pointers + stream; no torch headers so the .cu
+// Host-callable launchers of the sm_90a kernels (raw pointers + stream; no torch headers so the .cu
 // translation units compile in seconds).  Python bindings live in binding.cpp.
 #pragma once
 #include <cuda_runtime.h>

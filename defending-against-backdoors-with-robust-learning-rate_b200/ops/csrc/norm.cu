@@ -2,7 +2,7 @@
 // BatchNorm (training statistics, fused normalise + residual add + ReLU, two-pass backward), ReLU backward, 2x2
 // max-pool, global average pool, dropout (Philox), space-to-depth for strided convs, filter transpose for dgrad, and
 // the tiny classifier heads.  They replace the ATen elementwise / cuDNN-BN calls behind autograd in the reference's
-// local step (src/agent.py:46-48) and are what the tcgen05 conv kernels hand their outputs to.
+// local step (src/agent.py:46-48) and are what the wgmma conv kernels hand their outputs to.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -39,10 +39,9 @@ static inline bool chan_ok(int C) { return C >= 8 && C <= 2048 && (C % 8) == 0 &
 template <int MODE, bool kRecompute = false>
 __global__ void __launch_bounds__(256, MODE == 0 ? 4 : 3) channel_reduce_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy,
                                                                const __nv_bfloat16* __restrict__ y, const float* __restrict__ mean_rstd,
-                                                               float* out, long long M, int C, int relu,
+                                                               float* __restrict__ part /*[gridDim.x][ncols] partial sums*/, long long M, int C, int relu,
                                                                const float* __restrict__ gamma = nullptr, const float* __restrict__ beta = nullptr,
-                                                               int out_cols = 0 /*0: both rows (2C values) | C: only the first row (bias gradients)*/,
-                                                               int nslots = 1 /*partial buffers out[nslots][2][C]: CTA b adds into slot b % nslots*/) {
+                                                               int out_cols = 0 /*0: both rows (2C values) | C: only the first row (bias gradients)*/) {
     // relu: 0 none | 1 mask = (y > 0) from the stored output | 2 mask recomputed as (x * scale + shift > 0) with exactly the
     // expression of bn_apply_kernel -- BatchNorm + ReLU without a residual: the output tensor is not read at all
     extern __shared__ float sh[];   // [rpi][2][C] per-row-slot partials (16 KB for every C)
@@ -61,8 +60,8 @@ __global__ void __launch_bounds__(256, MODE == 0 ? 4 : 3) channel_reduce_kernel(
             for (int i = 0; i < 8; ++i) { msc[i] = gamma[cg * 8 + i] * rs[i]; msh[i] = beta[cg * 8 + i] - mu[i] * msc[i]; }
         }
     }
-    // U rows per iteration with every load issued before the first use: one 16-byte load per thread in flight reaches only
-    // ~20 % (forward statistics) / ~48 % (backward) of the HBM roofline (profiles/r1c_ncu_bn_kernels.md)
+    // U rows per iteration with every load issued before the first use: one 16-byte load per thread in flight leaves the kernel
+    // far below the HBM roofline
     constexpr int U = MODE == 0 ? 4 : 2;
     const long long stride = (long long)gridDim.x * rpi;
     for (long long r0 = (long long)blockIdx.x * rpi + ry; r0 < M; r0 += stride * U) {
@@ -104,26 +103,30 @@ __global__ void __launch_bounds__(256, MODE == 0 ? 4 : 3) channel_reduce_kernel(
         }
     }
     // block reduction without atomics: every thread parks its 16 partial sums in its row slot, then each thread sums a few
-    // columns over the rpi slots (conflict-free) and issues ONE global atomic per column and block
+    // columns over the rpi slots (conflict-free) and stores ONE partial per column and block
     float* mine = sh + (size_t)ry * 2 * C + cg * 8;
 #pragma unroll
     for (int i = 0; i < 8; ++i) { mine[i] = a[i]; mine[C + i] = b[i]; }
     __syncthreads();
     const int ncols = out_cols > 0 ? out_cols : 2 * C;
-    float* dst = out + (size_t)(blockIdx.x % nslots) * 2 * C;       // same-address atomics spread over the slots
+    float* dst = part + (size_t)blockIdx.x * ncols;                  // this CTA's slot; launch_ordered_sum adds the slots into out
     for (int i = threadIdx.x; i < ncols; i += 256) {
         float t = 0.f;
         for (int r = 0; r < rpi; ++r) t += sh[(size_t)r * 2 * C + i];
-        atomicAdd(dst + i, t);
+        dst[i] = t;
     }
 }
 
+// The per-CTA partial sums are added into slot 0 of the [nslots][2][C] output in CTA order (deterministic); nslots >= 4 selects
+// four CTAs per SM instead of two.
 cudaError_t launch_channel_stats(const __nv_bfloat16* x, long long M, int C, float* stats, int num_sms, cudaStream_t st, int only_sum, int nslots) {
     if (!chan_ok(C) || nslots < 1) return cudaErrorInvalidValue;
     const int rpi = 256 / (C / 8);
-    // four CTAs per SM (twice the bytes in flight of the two-CTA grid) once the atomics have slots to spread over
-    return launch_kernel(channel_reduce_kernel<0, false>, dim3(rows_grid(M, rpi * 8, num_sms, nslots >= 4 ? 4 : 2)), dim3(256),
-                         (size_t)rpi * 2 * C * sizeof(float), st, x, nullptr, nullptr, nullptr, stats, M, C, 0, nullptr, nullptr, only_sum ? C : 0, nslots);
+    const int grid = rows_grid(M, rpi * 8, num_sms, nslots >= 4 ? 4 : 2), ncols = only_sum ? C : 2 * C;
+    Scratch part((size_t)grid * ncols * sizeof(float), st);
+    RLR_CUDA_CHECK(launch_kernel(channel_reduce_kernel<0, false>, dim3(grid), dim3(256), (size_t)rpi * 2 * C * sizeof(float), st, x, nullptr,
+                                 nullptr, nullptr, part.as<float>(), M, C, 0, nullptr, nullptr, only_sum ? C : 0));
+    return launch_ordered_sum(stats, part.as<float>(), grid, (long long)ncols, st);
 }
 cudaError_t launch_bn_bwd_reduce(const __nv_bfloat16* dy, const __nv_bfloat16* y, const __nv_bfloat16* x, const float* mean_rstd,
                                  float* dsum, long long M, int C, int relu, int num_sms, cudaStream_t st, const float* gamma,
@@ -132,8 +135,14 @@ cudaError_t launch_bn_bwd_reduce(const __nv_bfloat16* dy, const __nv_bfloat16* y
     const int rpi = 256 / (C / 8);
     const int grid = rows_grid(M, rpi * 8, num_sms, nslots >= 3 ? 3 : 2);
     const size_t smem = (size_t)rpi * 2 * C * sizeof(float);
-    if (relu == 2) return launch_kernel(channel_reduce_kernel<1, true>, dim3(grid), dim3(256), smem, st, x, dy, y, mean_rstd, dsum, M, C, relu, gamma, beta, 0, nslots);
-    return launch_kernel(channel_reduce_kernel<1, false>, dim3(grid), dim3(256), smem, st, x, dy, y, mean_rstd, dsum, M, C, relu, nullptr, nullptr, 0, nslots);
+    Scratch part((size_t)grid * 2 * C * sizeof(float), st);
+    if (relu == 2)
+        RLR_CUDA_CHECK(launch_kernel(channel_reduce_kernel<1, true>, dim3(grid), dim3(256), smem, st, x, dy, y, mean_rstd, part.as<float>(), M, C,
+                                     relu, gamma, beta, 0));
+    else
+        RLR_CUDA_CHECK(launch_kernel(channel_reduce_kernel<1, false>, dim3(grid), dim3(256), smem, st, x, dy, y, mean_rstd, part.as<float>(), M, C,
+                                     relu, nullptr, nullptr, 0));
+    return launch_ordered_sum(dsum, part.as<float>(), grid, 2LL * C, st);
 }
 
 __global__ void bn_finalize_kernel(const float* __restrict__ stats, int slots, float* __restrict__ mean_rstd, float* running_mean,
@@ -205,7 +214,7 @@ __global__ void __launch_bounds__(256, kMinBlocks) bn_apply_kernel(const __nv_bf
         sh[i] = beta[c] - mean * sc[i];
     }
     // U rows per thread in flight (all loads issued before the first use): one 16-byte load per thread and iteration leaves the kernel
-    // latency-bound at ~3.9 TB/s (32 KB in flight per SM); measured same-box A/B in profiles/r2_step_ab.md
+    // latency-bound (32 KB in flight per SM)
     const long long stride = (long long)gridDim.x * rpi;
     for (long long r0 = (long long)blockIdx.x * rpi + ry; r0 < M; r0 += stride * U) {
         uint4 xr[U], rr[U];
@@ -240,8 +249,7 @@ cudaError_t launch_bn_apply(const __nv_bfloat16* x, const __nv_bfloat16* res, __
     if (!chan_ok(C)) return cudaErrorInvalidValue;
     const int rpi = 256 / (C / 8);
     BnFinalize fin{fin_mode, stats, slots, count, eps, momentum, running_mean, running_var};
-    // rows per thread in flight: 1 (default) | 4 (RLR_BN_UNROLL=4).  Four rows look better in isolation but cost +0.7 % per round on
-    // B200 inside the step (profiles/r2_step_ab.md) -- the same verdict as in round 1, now from a same-box A/B
+    // rows per thread in flight: 1 (default) | 4 (RLR_BN_UNROLL=4)
     static const int unroll = [] { const char* e = getenv("RLR_BN_UNROLL"); return e ? atoi(e) : 1; }();
     // RLR_BN_OCC=1: register caps that let one more CTA per SM be resident (more loads in flight through occupancy instead of unrolling)
     static const int occ = [] { const char* e = getenv("RLR_BN_OCC"); return e ? atoi(e) : 0; }();
@@ -462,14 +470,14 @@ cudaError_t launch_maxpool2_fwd(const __nv_bfloat16* x, __nv_bfloat16* y, uint8_
                                 uint64_t seed, const long long* step, uint64_t stream) {
     if (C % 8) return cudaErrorInvalidValue;
     const long long total = (long long)B * (H / 2) * (W / 2) * (C / 8);
-    maxpool2_fwd_kernel<<<rows_grid(total, 256, 148, 8), 256, 0, st>>>(x, y, idx, B, H, W, C, make_drop(drop_p, seed, step, stream));
+    maxpool2_fwd_kernel<<<rows_grid(total, 256, 132, 8), 256, 0, st>>>(x, y, idx, B, H, W, C, make_drop(drop_p, seed, step, stream));
     return cudaGetLastError();
 }
 cudaError_t launch_maxpool2_bwd(const __nv_bfloat16* dy, const uint8_t* idx, __nv_bfloat16* dx, int B, int H, int W, int C, cudaStream_t st, float drop_p,
                                 uint64_t seed, const long long* step, uint64_t stream, const __nv_bfloat16* zmask) {
     if (C % 8 || H < 2 || W < 2) return cudaErrorInvalidValue;
     const long long total = (long long)B * (H / 2) * (W / 2) * (C / 8);
-    maxpool2_bwd_kernel<<<rows_grid(total, 256, 148, 8), 256, 0, st>>>(dy, idx, dx, zmask, B, H, W, C, make_drop(drop_p, seed, step, stream));
+    maxpool2_bwd_kernel<<<rows_grid(total, 256, 132, 8), 256, 0, st>>>(dy, idx, dx, zmask, B, H, W, C, make_drop(drop_p, seed, step, stream));
     return cudaGetLastError();
 }
 
@@ -554,12 +562,12 @@ __global__ void __launch_bounds__(256) dropout_bwd_kernel(const __nv_bfloat16* _
 cudaError_t launch_dropout_fwd(const __nv_bfloat16* x, __nv_bfloat16* y, uint8_t* mask, long long n, float p, uint64_t seed,
                                const long long* step, uint64_t stream, cudaStream_t st) {
     if (n % 8) return cudaErrorInvalidValue;
-    dropout_fwd_kernel<<<rows_grid(n / 8, 256, 148, 8), 256, 0, st>>>(x, y, mask, n / 8, p, seed, step, stream);
+    dropout_fwd_kernel<<<rows_grid(n / 8, 256, 132, 8), 256, 0, st>>>(x, y, mask, n / 8, p, seed, step, stream);
     return cudaGetLastError();
 }
 cudaError_t launch_dropout_bwd(const __nv_bfloat16* dy, const uint8_t* mask, __nv_bfloat16* dx, long long n, float p, cudaStream_t st) {
     if (n % 8) return cudaErrorInvalidValue;
-    dropout_bwd_kernel<<<rows_grid(n / 8, 256, 148, 8), 256, 0, st>>>(dy, mask, dx, n / 8, 1.0f / (1.0f - p));
+    dropout_bwd_kernel<<<rows_grid(n / 8, 256, 132, 8), 256, 0, st>>>(dy, mask, dx, n / 8, 1.0f / (1.0f - p));
     return cudaGetLastError();
 }
 
@@ -680,7 +688,7 @@ cudaError_t launch_filter_gather_transpose(const __nv_bfloat16* w, __nv_bfloat16
     for (int i = 0; i < nsub; ++i) tl.t[i] = taps[i];
     const long long total = (long long)Cout * nsub * Cin;
     const long long blocks = (total + 255) / 256;
-    filter_gather_transpose_kernel<<<(int)(blocks > 148 * 16 ? 148 * 16 : blocks), 256, 0, st>>>(w, wt, Cout, T, Cin, tl);
+    filter_gather_transpose_kernel<<<(int)(blocks > 132 * 16 ? 132 * 16 : blocks), 256, 0, st>>>(w, wt, Cout, T, Cin, tl);
     return cudaGetLastError();
 }
 
@@ -697,7 +705,7 @@ __global__ void filter_transpose_kernel(const __nv_bfloat16* __restrict__ w, __n
 }
 cudaError_t launch_filter_transpose(const __nv_bfloat16* w, __nv_bfloat16* wt, int Cout, int ntaps, int Cin, cudaStream_t st) {
     const long long total = (long long)Cout * ntaps * Cin;
-    filter_transpose_kernel<<<(int)((total + 255) / 256 > 148 * 16 ? 148 * 16 : (total + 255) / 256), 256, 0, st>>>(w, wt, Cout, ntaps, Cin);
+    filter_transpose_kernel<<<(int)((total + 255) / 256 > 132 * 16 ? 132 * 16 : (total + 255) / 256), 256, 0, st>>>(w, wt, Cout, ntaps, Cin);
     return cudaGetLastError();
 }
 
@@ -786,16 +794,17 @@ __global__ void __launch_bounds__(256) linear_small_bwd_kernel(const __nv_bfloat
         }
     }
 }
-// v2 (opt-in, RLR_HEAD_V2): the weight/bias gradient of the classifier head is spread over (K/64) x (B/16) blocks that stage their
-// 16 dy rows in shared memory and add their partial sums with float atomics -- dW/db must be ZERO on entry (the native plan zeroes
-// the flat gradient once per step).  v1 used K/64 blocks that each walked the whole batch (30 us for a 256 x 512 x 10 layer).
+// v2 (RLR_HEAD_V2): the weight/bias gradient of the classifier head is spread over (K/64) x (B/16) blocks that stage their
+// 16 dy rows in shared memory; block (kc, bs) stores its partial sums in slot bs of `pw` ([B/16][N][K]) / `pb` ([B/16][N]) and
+// launch_linear_small_bwd2 adds the slots into dW / db in a fixed order.  v1 used K/64 blocks that each walked the whole batch (30 us for a 256 x 512 x 10 layer).
 __global__ void __launch_bounds__(256) linear_small_bwd2_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy,
                                                                   const __nv_bfloat16* __restrict__ w, __nv_bfloat16* __restrict__ dx,
-                                                                  float* __restrict__ dw, float* __restrict__ db, int B, int K, int N,
+                                                                  float* __restrict__ pw, float* __restrict__ pb, int B, int K, int N,
                                                                   int accumulate_dx, int kchunks, int bsplit) {
     pdl_wait();
     pdl_trigger();
     __shared__ float sdy[16][32];
+    __shared__ float sred[4][64];
     const int wblocks = kchunks * bsplit;
     if ((int)blockIdx.x < wblocks) {
         const int kc = blockIdx.x % kchunks, bs = blockIdx.x / kchunks;
@@ -813,19 +822,20 @@ __global__ void __launch_bounds__(256) linear_small_bwd2_kernel(const __nv_bfloa
             const int b = b0 + rg * 4 + r;
             xv[r] = (k < K && b < B) ? __bfloat162float(x[(size_t)b * K + k]) : 0.f;
         }
-        if (k < K) {
-            for (int n = 0; n < N; ++n) {
-                float a = 0.f;
+        for (int n = 0; n < N; ++n) {
+            float a = 0.f;
 #pragma unroll
-                for (int r = 0; r < 4; ++r) a += xv[r] * sdy[rg * 4 + r][n];
-                atomicAdd(dw + (size_t)n * K + k, a);
-            }
+            for (int r = 0; r < 4; ++r) a += xv[r] * sdy[rg * 4 + r][n];
+            sred[rg][kk] = a;
+            __syncthreads();
+            if (rg == 0 && k < K) pw[((size_t)bs * N + n) * K + k] = ((sred[0][kk] + sred[1][kk]) + sred[2][kk]) + sred[3][kk];
+            __syncthreads();
         }
-        if (kc == 0 && db && threadIdx.x < N) {
+        if (kc == 0 && pb && threadIdx.x < N) {
             float a = 0.f;
 #pragma unroll
             for (int r = 0; r < 16; ++r) a += sdy[r][threadIdx.x];
-            atomicAdd(db + threadIdx.x, a);
+            pb[(size_t)bs * N + threadIdx.x] = a;
         }
     } else if (dx) {                                       // dx[b][k] = sum_n dy[b][n] w[n][k], two columns per thread
         const long long total2 = (long long)B * (K / 2);
@@ -850,8 +860,13 @@ cudaError_t launch_linear_small_bwd2(const __nv_bfloat16* x, const __nv_bfloat16
     const int kchunks = (K + 63) / 64, bsplit = (B + 15) / 16;
     long long dxb = dx ? ((long long)B * (K / 2) + 255) / 256 : 0;
     if (dxb > 592) dxb = 592;
-    return launch_kernel(linear_small_bwd2_kernel, dim3(kchunks * bsplit + (int)dxb), dim3(256), (size_t)0, st, x, dy, w, dx, dw, db, B, K, N,
-                         accumulate_dx, kchunks, bsplit);
+    Scratch part(((size_t)bsplit * N * K + (size_t)bsplit * N) * sizeof(float), st);
+    float* pw = part.as<float>();
+    float* pb = db ? pw + (size_t)bsplit * N * K : nullptr;
+    RLR_CUDA_CHECK(launch_kernel(linear_small_bwd2_kernel, dim3(kchunks * bsplit + (int)dxb), dim3(256), (size_t)0, st, x, dy, w, dx, pw, pb, B,
+                                 K, N, accumulate_dx, kchunks, bsplit));
+    RLR_CUDA_CHECK(launch_ordered_sum(dw, pw, bsplit, (long long)N * K, st));
+    return db ? launch_ordered_sum(db, pb, bsplit, (long long)N, st) : cudaSuccess;
 }
 
 // v2 forward: 8 samples per 256-thread block, one warp per sample, the whole weight matrix staged in shared memory once per block

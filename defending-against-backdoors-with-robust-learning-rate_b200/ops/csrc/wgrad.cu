@@ -1,11 +1,12 @@
-// tcgen05 weight-gradient kernel for sm_100a:   dW[co][tap][ci] = sum_pix dY[pix][co] * X[pix (+) tap][ci]
+// wgmma weight-gradient kernels for sm_90a:   dW[co][tap][ci] = sum_pix dY[pix][co] * X[pix (+) tap][ci]
 //
 // The reduction runs over PIXELS, which is the slow dimension of both NHWC operands, so both MMA operands are
-// MN-major: a k-block is 64 pixels, the A tile is dY[64 pix][128 co] (two 64-channel TMA boxes) and the B tile of
-// tap t is X[64 shifted pix][64 ci] (one 4-D TMA box, zero-filled at the borders = padding).  One CTA keeps the
-// accumulators of up to THREE taps (one filter row) in TMEM (3 x 64 fp32 columns) so each dY tile is loaded once per
-// filter row, runs a contiguous slice of the pixel range (split-K over CTAs) and reduces its 128 x 64 x taps partial
-// result into the fp32 flat gradient buffer with red.global.add.f32 (the buffer is zeroed once per step).
+// MN-major: a k-block is 64 pixels, the A tile is dY[64 pix][128 co] (two 64-channel TMA boxes, one per consumer warpgroup) and
+// the B tile of tap t is X[64 shifted pix][64 ci] (one 4-D TMA box, zero-filled at the borders = padding).  One CTA keeps the
+// accumulators of up to THREE taps (one filter row: one m64n192 wgmma per warpgroup and k-step) in registers so each dY tile is
+// loaded once per filter row, runs a contiguous slice of the pixel range (split-K over CTAs) and reduces its 128 x 64 x taps
+// partial result into a slot of a scratch buffer; the slots are then added into the fp32 flat gradient in split order, so the
+// result does not depend on CTA scheduling (one split: the CTA adds its tile straight into the gradient).
 // Plain mode (mode 0) is the same kernel on 2-D operands: dW[n][k] = sum_b dY[b][n] X[b][k] for linear layers.
 // Replaces cuDNN wgrad / cuBLAS GEMM^T behind loss.backward() (reference src/agent.py:48).
 #include <cuda.h>
@@ -13,11 +14,11 @@
 
 #include "common.cuh"
 #include "gemm.h"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace rlr {
 
-using namespace umma;
+using namespace wg;
 
 cudaError_t make_tmap_bf16(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                            const uint32_t* box, const uint32_t* elem_strides = nullptr);  // gemm.cu
@@ -25,14 +26,13 @@ cudaError_t make_tmap_bf16(CUtensorMap* map, const void* base, int rank, const u
 constexpr int WG_BM = 128, WG_BK = 64;                        // co tile, pixels per k-block
 constexpr int WG_STAGES = 3;
 constexpr int WG_A_BYTES = 2 * 64 * WG_BK * 2;                // two 64-channel groups x 64 pixel rows x 128 B
-constexpr int WG_THREADS = 192;
+constexpr int WG_THREADS = 256 + 32;                          // two consumer warpgroups + the TMA producer warp
 template <int BNW>                                            // ci tile width: 64 or 128 channels
 struct WgCfg {
     static constexpr int kGroups = BNW / 64;
     static constexpr int kBBytes = kGroups * 64 * WG_BK * 2;  // per tap
     static constexpr int kStageBytes = WG_A_BYTES + 3 * kBBytes;   // 40 KB / 64 KB
     static constexpr int kSmem = WG_STAGES * kStageBytes + 2048;
-    static constexpr int kTmemCols = BNW == 64 ? 256 : 512;   // 3 taps x BNW fp32 columns, power of two
 };
 
 struct WgradParams {
@@ -49,56 +49,72 @@ struct WgradParams {
     int ci_tiles;
     int Cout, Cin_valid;      // rows / columns of dW that exist (Cin_valid < 64 for the channel-padded stem)
     float* dW;                // [Cout][T][Cin_valid] fp32 (accumulated)
+    float* part;              // split-K > 1: [splits][Cout][T][Cin_valid] partial gradients (one slot per blockIdx.z)
 };
 
 struct __align__(8) WgShared {
     uint64_t full[WG_STAGES];
     uint64_t empty[WG_STAGES];
-    uint64_t tmem_full;
-    uint32_t tmem_base;
 };
 
-template <int BNW>
+// acc column c of warpgroup row `co` (fragment layout) -> dW[co][tap0 + c / BNW][ci0 + c % BNW], pairs of adjacent columns per thread;
+// with `part` the values are stored into this split's slot of the partial buffer instead of being added into dW
+template <int NACC, int BNW>
+__device__ __forceinline__ void wgrad_flush(const float (&acc)[NACC / 2], float* dW, float* part, int co, int Cout, int T, int tap0, int ci0,
+                                            int Cin_valid, int t) {
+    if (part) dW = part + (size_t)blockIdx.z * Cout * T * Cin_valid;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int row = co + 8 * h;
+        if (row >= Cout) continue;
+#pragma unroll
+        for (int j = 0; j < NACC / 8; ++j) {
+            const int c = frag_col(t, 4 * j), tap = c / BNW, ci = ci0 + c % BNW;
+            float* dst = dW + ((size_t)row * T + tap0 + tap) * Cin_valid + ci;
+            const float a = acc[4 * j + 2 * h], b = acc[4 * j + 2 * h + 1];
+            if (part) {
+                if (ci < Cin_valid) dst[0] = a;
+                if (ci + 1 < Cin_valid) dst[1] = b;
+            } else if ((Cin_valid & 1) == 0) {
+                if (ci < Cin_valid) asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(a), "f"(b) : "memory");
+            } else {
+                if (ci < Cin_valid) atomicAdd(dst, a);
+                if (ci + 1 < Cin_valid) atomicAdd(dst + 1, b);
+            }
+        }
+    }
+}
+
+template <int BNW, int kTaps>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const WgradParams p) {
     using Cfg = WgCfg<BNW>;
     constexpr int WG_BN = BNW, WG_B_BYTES = Cfg::kBBytes, WG_STAGE_BYTES = Cfg::kStageBytes;
+    constexpr int NACC = kTaps * BNW;                         // 64, 128 or 192 accumulator columns
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     WgShared* sh = reinterpret_cast<WgShared*>(smem + WG_STAGES * WG_STAGE_BYTES);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int co_tile = blockIdx.x / p.ci_tiles, ci_tile = blockIdx.x - co_tile * p.ci_tiles;
-    const int tap0 = blockIdx.y * p.ntaps_cta;
+    const int tap0 = blockIdx.y * kTaps;
     const int kb_begin = blockIdx.z * p.kb_per_cta;
     const int kb_end = min(p.num_kb, kb_begin + p.kb_per_cta);
     const int nkb = kb_end - kb_begin;
 
-    if (warp == 0 && lane == 0) { prefetch_tmap(&tmA); prefetch_tmap(&tmB); }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&sh->full[s], 1); mbar_init(&sh->empty[s], 1); }
-        mbar_init(&sh->tmem_full, 1);
+    if (warp == 8 && lane == 0) {
+        prefetch_tmap(&tmA); prefetch_tmap(&tmB);
+        for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&sh->full[s], 1); mbar_init(&sh->empty[s], 8); }
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc(&sh->tmem_base, Cfg::kTmemCols);
-    if (p.a_groups == 1) {   // upper 64 rows of the M=128 tile do not exist: keep that operand half at zero
-        for (int s = 0; s < WG_STAGES; ++s) {
-            uint4* z = reinterpret_cast<uint4*>(smem + s * WG_STAGE_BYTES + 8192);
-            for (int i = threadIdx.x; i < 8192 / 16; i += WG_THREADS) z[i] = make_uint4(0, 0, 0, 0);
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_acc = sh->tmem_base;
-    pdl_wait();        // prologue above: parameters, shared memory, TMEM only
+    pdl_wait();        // prologue above: parameters and shared memory only
     pdl_trigger();
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
-            const uint32_t bytes = p.a_groups * 8192 + p.ntaps_cta * WG_B_BYTES;
+            const uint32_t bytes = p.a_groups * 8192 + kTaps * WG_B_BYTES;
             for (int i = 0; i < nkb; ++i) {
                 const int kb = kb_begin + i;
                 mbar_wait(&sh->empty[stage], phase ^ 1);
@@ -110,7 +126,7 @@ umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     const int w0 = tw_i * p.TW, h0 = th_i * p.TH, n0 = tn_i * p.TN;
                     for (int g = 0; g < p.a_groups; ++g)
                         tma_load_4d(&tmA, &sh->full[stage], sa + g * 8192, co_tile * WG_BM + g * 64, w0, h0, n0);
-                    for (int t = 0; t < p.ntaps_cta; ++t)
+                    for (int t = 0; t < kTaps; ++t)
                         for (int g = 0; g < Cfg::kGroups; ++g)
                             tma_load_4d(&tmB, &sh->full[stage], sb + t * WG_B_BYTES + g * 8192, ci_tile * WG_BN + g * 64,
                                         w0 * p.in_stride + p.dw[tap0 + t], h0 * p.in_stride + p.dh[tap0 + t], n0 + p.dn[tap0 + t]);
@@ -123,81 +139,49 @@ umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = idesc_bf16(WG_BM, WG_BN, 1, 1);   // both operands MN-major
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int i = 0; i < nkb; ++i) {
-                mbar_wait(&sh->full[stage], phase);
-                tc_fence_after();
-                const uint32_t sa = smem_u32(smem + stage * WG_STAGE_BYTES);
-                const uint32_t sb = sa + WG_A_BYTES;
-                if (BNW == 64 && p.ntaps_cta == 3) {
-                    // the three tap tiles are 64-channel groups 8 KB apart: one N = 192 MMA (LBO = 8192) covers all of them,
-                    // which lifts the instruction out of the smem-bandwidth-bound N = 64 regime
-                    constexpr uint32_t idesc3 = idesc_bf16(WG_BM, 192, 1, 1);
-#pragma unroll
-                    for (int k = 0; k < WG_BK / 16; ++k) {
-                        const uint64_t da = smem_desc_sw128(sa + k * 2048, 8192, 1024);
-                        const uint64_t db = smem_desc_sw128(sb + k * 2048, 8192, 1024);
-                        umma_bf16(tmem_acc, da, db, idesc3, (i > 0 || k > 0) ? 1u : 0u);
-                    }
-                } else {
-                    for (int t = 0; t < p.ntaps_cta; ++t) {
-#pragma unroll
-                        for (int k = 0; k < WG_BK / 16; ++k) {   // 16 pixel rows (2 swizzle atoms) per MMA
-                            const uint64_t da = smem_desc_sw128(sa + k * 2048, 8192, 1024);
-                            const uint64_t db = smem_desc_sw128(sb + t * WG_B_BYTES + k * 2048, 8192, 1024);
-                            umma_bf16(tmem_acc + t * WG_BN, da, db, idesc, (i > 0 || k > 0) ? 1u : 0u);
-                        }
-                    }
-                }
-                umma_commit(&sh->empty[stage]);
-                if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-            }
-            umma_commit(&sh->tmem_full);
-        }
     } else if (nkb > 0) {
-        const int lane_base = (warp & 3) * 32;
-        const int co = co_tile * WG_BM + lane_base + lane;
-        mbar_wait(&sh->tmem_full, 0);
-        tc_fence_after();
-        for (int t = 0; t < p.ntaps_cta; ++t) {
+        // warpgroup wgi: output channels co_tile * 128 + 64 wgi + [0, 64) = A group wgi; it idles (but still releases stages) when that
+        // group does not exist (a_groups == 1)
+        const int wgi = threadIdx.x >> 7, t = threadIdx.x & 127;
+        const bool active = wgi < p.a_groups;
+        float acc[NACC / 2];
 #pragma unroll
-            for (int c0 = 0; c0 < WG_BN; c0 += 32) {
-                uint32_t v[32];
-                tmem_ld_32x32(tmem_acc + ((uint32_t)lane_base << 16) + t * WG_BN + c0, v);
-                if (co < p.Cout) {
-                    float* dst = p.dW + ((size_t)co * p.T + tap0 + t) * p.Cin_valid + ci_tile * WG_BN + c0;
-                    if ((p.Cin_valid & 3) == 0) {
-                        // 16-byte vector reductions (REDG.E.ADD.F32x4): 4x fewer L2 atomic operations
+        for (int i = 0; i < NACC / 2; ++i) acc[i] = 0.f;
+        int stage = 0, prev = -1;
+        uint32_t phase = 0;
+        for (int i = 0; i < nkb; ++i) {
+            mbar_wait(&sh->full[stage], phase);
+            if (active) {
+                const uint32_t sa = smem_u32(smem + stage * WG_STAGE_BYTES) + wgi * 8192;
+                const uint32_t sb = smem_u32(smem + stage * WG_STAGE_BYTES) + WG_A_BYTES;
+                wgmma_fence();
 #pragma unroll
-                        for (int j = 0; j < 32; j += 4)
-                            if (ci_tile * WG_BN + c0 + j < p.Cin_valid)
-                                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + j), "f"(__uint_as_float(v[j])),
-                                             "f"(__uint_as_float(v[j + 1])), "f"(__uint_as_float(v[j + 2])), "f"(__uint_as_float(v[j + 3]))
-                                             : "memory");
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (ci_tile * WG_BN + c0 + j < p.Cin_valid) atomicAdd(dst + j, __uint_as_float(v[j]));
-                    }
+                for (int k = 0; k < WG_BK / 16; ++k) {   // 16 pixel rows (2 swizzle atoms) per MMA
+                    // B: the tap tiles (and 64-wide ci groups inside them) are N groups 8 KB apart -> one MMA covers all kTaps taps
+                    wgmma_bf16<NACC, 1, 1>(acc, smem_desc_sw128(sa + k * 2048, 8192, 1024), smem_desc_sw128(sb + k * 2048, 8192, 1024),
+                                           (i > 0 || k > 0) ? 1u : 0u);
                 }
+                wgmma_commit();
+                wgmma_wait<1>();
             }
+            if (prev >= 0 && lane == 0) mbar_arrive(&sh->empty[prev]);
+            prev = stage;
+            if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
+        }
+        if (active) {
+            wgmma_wait<0>();
+            fence_acc(acc);
+            wgrad_flush<NACC, BNW>(acc, p.dW, p.part, co_tile * WG_BM + wgi * 64 + frag_row(t, 0), p.Cout, p.T, tap0, ci_tile * WG_BN, p.Cin_valid, t);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_acc, Cfg::kTmemCols);
 }
 
-template <int BNW>
+template <int BNW, int kTaps>
 static cudaError_t launch_wg(const CUtensorMap& tmA, const CUtensorMap& tmB, WgradParams& p, int co_tiles, int tap_groups,
                              int num_sms, cudaStream_t st) {
     static bool configured = false;
     if (!configured) {
-        RLR_CUDA_CHECK(cudaFuncSetAttribute(umma_wgrad_kernel<BNW>, cudaFuncAttributeMaxDynamicSharedMemorySize, WgCfg<BNW>::kSmem));
+        RLR_CUDA_CHECK(cudaFuncSetAttribute(umma_wgrad_kernel<BNW, kTaps>, cudaFuncAttributeMaxDynamicSharedMemorySize, WgCfg<BNW>::kSmem));
         configured = true;
     }
     // split-K so that the grid is (at most) a whole number of waves of one CTA per SM: no ragged tail wave
@@ -210,7 +194,12 @@ static cudaError_t launch_wg(const CUtensorMap& tmA, const CUtensorMap& tmB, Wgr
     p.kb_per_cta = (p.num_kb + splits - 1) / splits;
     splits = (p.num_kb + p.kb_per_cta - 1) / p.kb_per_cta;
     dim3 grid(co_tiles * p.ci_tiles, tap_groups, splits);
-    return launch_kernel(umma_wgrad_kernel<BNW>, grid, dim3(WG_THREADS), (size_t)WgCfg<BNW>::kSmem, st, tmA, tmB, p);
+    if (splits == 1) return launch_kernel(umma_wgrad_kernel<BNW, kTaps>, grid, dim3(WG_THREADS), (size_t)WgCfg<BNW>::kSmem, st, tmA, tmB, p);
+    const long long plane = (long long)p.Cout * p.T * p.Cin_valid;
+    Scratch part((size_t)splits * plane * sizeof(float), st);
+    p.part = part.as<float>();
+    RLR_CUDA_CHECK(launch_kernel(umma_wgrad_kernel<BNW, kTaps>, grid, dim3(WG_THREADS), (size_t)WgCfg<BNW>::kSmem, st, tmA, tmB, p));
+    return launch_ordered_sum(p.dW, p.part, splits, plane, st);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -222,7 +211,7 @@ static cudaError_t launch_wg(const CUtensorMap& tmA, const CUtensorMap& tmB, Wgr
 // (see conv_halo.cu).  The three dx taps of a filter row are the SAME view shifted by one pixel (128 B), i.e. three
 // 64-channel "N groups" with a leading-dimension byte offset of 128: one N = 192 MMA per k-step computes all three, which
 // moves the instruction out of the smem-bandwidth-bound N = 64 regime.  grid.y = 3 filter rows (3 x 192 columns do not fit
-// TMEM).  L2 traffic per 128 pixels: 3 x (36 + 16..32) KB instead of 3 x 2 x (24 + 8..16) KB.
+// registers).  L2 traffic per 128 pixels: 3 x (36 + 16..32) KB instead of 3 x 2 x (24 + 8..16) KB.
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int WH_STAGES = 3;
 constexpr int WH_A_BYTES = 2 * 128 * 128;                      // up to two 64-channel groups x 128 pixel rows x 128 B
@@ -236,6 +225,7 @@ struct WgHaloParams {
     int a_groups;
     int Cout, Cin_valid;
     float* dW;                // [Cout][9][Cin_valid]
+    float* part;              // split-K > 1: [splits][Cout][9][Cin_valid] partial gradients
 };
 
 __global__ void __launch_bounds__(WG_THREADS, 1)
@@ -245,34 +235,22 @@ umma_wgrad_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     WgShared* sh = reinterpret_cast<WgShared*>(smem + WH_STAGES * WH_STAGE_BYTES);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int co_tile = blockIdx.x;
-    const int dy = blockIdx.y, tap0 = dy * 3, ntaps = 3;
+    const int dy = blockIdx.y, tap0 = dy * 3;
     const int kb_begin = blockIdx.z * p.kb_per_cta;
     const int kb_end = min(p.num_kb, kb_begin + p.kb_per_cta);
     const int nkb = kb_end - kb_begin;
     const int tiles_per_img = p.tiles_h * p.tiles_w;
 
-    if (warp == 0 && lane == 0) { prefetch_tmap(&tmA); prefetch_tmap(&tmB); }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < WH_STAGES; ++s) { mbar_init(&sh->full[s], 1); mbar_init(&sh->empty[s], 1); }
-        mbar_init(&sh->tmem_full, 1);
+    if (warp == 8 && lane == 0) {
+        prefetch_tmap(&tmA); prefetch_tmap(&tmB);
+        for (int s = 0; s < WH_STAGES; ++s) { mbar_init(&sh->full[s], 1); mbar_init(&sh->empty[s], 8); }
         fence_barrier_init();
     }
-    if (warp == 2) tmem_alloc(&sh->tmem_base, 256);
-    if (p.a_groups == 1) {
-        for (int s = 0; s < WH_STAGES; ++s) {
-            uint4* z = reinterpret_cast<uint4*>(smem + s * WH_STAGE_BYTES + 16384);
-            for (int i = threadIdx.x; i < 16384 / 16; i += WG_THREADS) z[i] = make_uint4(0, 0, 0, 0);
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_acc = sh->tmem_base;
-    pdl_wait();        // prologue above: parameters, shared memory, TMEM only
+    pdl_wait();        // prologue above: parameters and shared memory only
     pdl_trigger();
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
@@ -290,59 +268,39 @@ umma_wgrad_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
                 if (++stage == WH_STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = idesc_bf16(WG_BM, 192, 1, 1);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int i = 0; i < nkb; ++i) {
-                mbar_wait(&sh->full[stage], phase);
-                tc_fence_after();
-                const uint32_t sa = smem_u32(smem + stage * WH_STAGE_BYTES);
-                const uint32_t halo = sa + WH_A_BYTES;
+    } else if (nkb > 0) {
+        const int wgi = threadIdx.x >> 7, t = threadIdx.x & 127;
+        const bool active = wgi < p.a_groups;
+        float acc[96];
+#pragma unroll
+        for (int i = 0; i < 96; ++i) acc[i] = 0.f;
+        int stage = 0, prev = -1;
+        uint32_t phase = 0;
+        for (int i = 0; i < nkb; ++i) {
+            mbar_wait(&sh->full[stage], phase);
+            if (active) {
+                const uint32_t sa = smem_u32(smem + stage * WH_STAGE_BYTES) + wgi * 16384;
+                const uint32_t halo = smem_u32(smem + stage * WH_STAGE_BYTES) + WH_A_BYTES;
+                wgmma_fence();
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {                     // 16 pixels = output rows 2j, 2j+1 of the tile
-                    const uint64_t da = smem_desc_sw128(sa + j * 2048, 16384, 1024);
                     // N groups 0,1,2 = taps dx = 0,1,2: same halo view shifted by one pixel -> LBO = 128 B; SBO = one image row
-                    const uint64_t db = smem_desc_sw128(halo + ((2 * j + dy) * 16) * 128, 128, 2048);
-                    umma_bf16(tmem_acc, da, db, idesc, (i > 0 || j > 0) ? 1u : 0u);
+                    wgmma_bf16<192, 1, 1>(acc, smem_desc_sw128(sa + j * 2048, 16384, 1024),
+                                          smem_desc_sw128(halo + ((2 * j + dy) * 16) * 128, 128, 2048), (i > 0 || j > 0) ? 1u : 0u);
                 }
-                umma_commit(&sh->empty[stage]);
-                if (++stage == WH_STAGES) { stage = 0; phase ^= 1; }
+                wgmma_commit();
+                wgmma_wait<1>();
             }
-            umma_commit(&sh->tmem_full);
+            if (prev >= 0 && lane == 0) mbar_arrive(&sh->empty[prev]);
+            prev = stage;
+            if (++stage == WH_STAGES) { stage = 0; phase ^= 1; }
         }
-    } else if (nkb > 0) {
-        const int lane_base = (warp & 3) * 32;
-        const int co = co_tile * WG_BM + lane_base + lane;
-        mbar_wait(&sh->tmem_full, 0);
-        tc_fence_after();
-        for (int t = 0; t < ntaps; ++t) {
-#pragma unroll
-            for (int c0 = 0; c0 < 64; c0 += 32) {
-                uint32_t v[32];
-                tmem_ld_32x32(tmem_acc + ((uint32_t)lane_base << 16) + t * 64 + c0, v);
-                if (co < p.Cout) {
-                    float* dst = p.dW + ((size_t)co * 9 + tap0 + t) * p.Cin_valid + c0;
-                    if ((p.Cin_valid & 3) == 0) {
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4)
-                            if (c0 + j < p.Cin_valid)
-                                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + j), "f"(__uint_as_float(v[j])),
-                                             "f"(__uint_as_float(v[j + 1])), "f"(__uint_as_float(v[j + 2])), "f"(__uint_as_float(v[j + 3]))
-                                             : "memory");
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (c0 + j < p.Cin_valid) atomicAdd(dst + j, __uint_as_float(v[j]));
-                    }
-                }
-            }
+        if (active) {
+            wgmma_wait<0>();
+            fence_acc(acc);
+            wgrad_flush<192, 64>(acc, p.dW, p.part, co_tile * WG_BM + wgi * 64 + frag_row(t, 0), p.Cout, 9, tap0, 0, p.Cin_valid, t);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_acc, 256);
 }
 
 // dW[Cout][9][Cin_valid] += wgrad3x3(dy[NB][H][W][Cout], x[NB][H][W][64]); stride 1, pad 1, H % 16 == 0, W % 8 == 0
@@ -378,7 +336,12 @@ cudaError_t launch_conv_wgrad_halo_bf16(const void* dy, const void* x, float* dW
         const uint32_t b[4] = {64, 16, 18, 1};
         RLR_CUDA_CHECK(make_tmap_bf16(&tmB, x, 4, d, s, b));
     }
-    return launch_kernel(umma_wgrad_halo_kernel, dim3(co_tiles, 3, splits), dim3(WG_THREADS), (size_t)WH_SMEM, st, tmA, tmB, p);
+    if (splits == 1) return launch_kernel(umma_wgrad_halo_kernel, dim3(co_tiles, 3, splits), dim3(WG_THREADS), (size_t)WH_SMEM, st, tmA, tmB, p);
+    const long long plane = (long long)Cout * 9 * Cin_valid;
+    Scratch part((size_t)splits * plane * sizeof(float), st);
+    p.part = part.as<float>();
+    RLR_CUDA_CHECK(launch_kernel(umma_wgrad_halo_kernel, dim3(co_tiles, 3, splits), dim3(WG_THREADS), (size_t)WH_SMEM, st, tmA, tmB, p));
+    return launch_ordered_sum(dW, p.part, splits, plane, st);
 }
 
 static int pow2_ceil_(int x) { int q = 1; while (q < x) q <<= 1; return q; }
@@ -399,9 +362,10 @@ cudaError_t launch_conv_wgrad_bf16(const void* dy, const void* x, float* dW, int
     p.num_kb = p.tiles_w * p.tiles_h * ((NB + TN - 1) / TN);
     p.T = ntaps; p.ntaps_cta = ntaps == 9 ? 3 : 1;
     for (int t = 0; t < ntaps; ++t) { p.dh[t] = (int8_t)dh[t]; p.dw[t] = (int8_t)dw[t]; p.dn[t] = dplane[t] * NB; }
-    const bool wide = (Cin % 128 == 0) && (Cin_valid == Cin);
+    // 128-wide ci tiles only for one-tap filters: three taps of 128 channels would need 192 accumulator registers per thread
+    const bool wide = (Cin % 128 == 0) && (Cin_valid == Cin) && ntaps == 1;
     p.ci_tiles = wide ? Cin / 128 : Cin / 64; p.Cout = Cout; p.Cin_valid = Cin_valid; p.dW = dW;
-    p.a_groups = (Cout % 128 == 0) ? 2 : 1;
+    p.a_groups = Cout > 64 ? 2 : 1;        // the second 64-channel box is zero-filled beyond Cout
     const int co_tiles = (Cout + WG_BM - 1) / WG_BM;
     CUtensorMap tmA, tmB;
     {
@@ -417,8 +381,8 @@ cudaError_t launch_conv_wgrad_bf16(const void* dy, const void* x, float* dW, int
         const uint32_t es[4] = {1, (uint32_t)in_stride, (uint32_t)in_stride, 1};
         RLR_CUDA_CHECK(make_tmap_bf16(&tmB, x, 4, d, s, b, in_stride > 1 ? es : nullptr));
     }
-    return wide ? launch_wg<128>(tmA, tmB, p, co_tiles, ntaps / p.ntaps_cta, num_sms, st)
-                : launch_wg<64>(tmA, tmB, p, co_tiles, ntaps / p.ntaps_cta, num_sms, st);
+    if (wide) return launch_wg<128, 1>(tmA, tmB, p, co_tiles, ntaps, num_sms, st);
+    return ntaps == 9 ? launch_wg<64, 3>(tmA, tmB, p, co_tiles, 3, num_sms, st) : launch_wg<64, 1>(tmA, tmB, p, co_tiles, 1, num_sms, st);
 }
 
 // dW[N][K] += dy[B][N]^T x[B][K]     (N, K multiples of 64)
@@ -428,7 +392,7 @@ cudaError_t launch_linear_wgrad_bf16(const void* dy, const void* x, float* dW, i
     p.mode = 0; p.num_kb = (B + WG_BK - 1) / WG_BK; p.T = 1; p.ntaps_cta = 1; p.in_stride = 1;
     const bool wide = K % 128 == 0;
     p.ci_tiles = wide ? K / 128 : K / 64; p.Cout = N; p.Cin_valid = K; p.dW = dW;
-    p.a_groups = (N % 128 == 0) ? 2 : 1;
+    p.a_groups = N > 64 ? 2 : 1;
     const int co_tiles = (N + WG_BM - 1) / WG_BM;
     CUtensorMap tmA, tmB;
     {
@@ -441,7 +405,7 @@ cudaError_t launch_linear_wgrad_bf16(const void* dy, const void* x, float* dW, i
         const uint32_t b[2] = {64, WG_BK};
         RLR_CUDA_CHECK(make_tmap_bf16(&tmB, x, 2, d, s, b));
     }
-    return wide ? launch_wg<128>(tmA, tmB, p, co_tiles, 1, num_sms, st) : launch_wg<64>(tmA, tmB, p, co_tiles, 1, num_sms, st);
+    return wide ? launch_wg<128, 1>(tmA, tmB, p, co_tiles, 1, num_sms, st) : launch_wg<64, 1>(tmA, tmB, p, co_tiles, 1, num_sms, st);
 }
 
 }  // namespace rlr

@@ -1,5 +1,5 @@
 """Layer primitives of the native executor (models/native.py), each with an ``sm100`` back-end (hand-written kernels
-of ops/csrc: gemm.cu = tcgen05/TMEM/TMA implicit-GEMM convolution + GEMM, norm.cu = NHWC bf16 layer kernels) and an
+of ops/csrc: gemm.cu = wgmma/TMA implicit-GEMM convolution + GEMM, norm.cu = NHWC bf16 layer kernels) and an
 ``aten`` back-end (the same math through PyTorch library calls on the same buffers: CPU path + in-place oracle).
 
 Reference call sites these primitives replace (SURVEY.md 2.4 rows K2-K8): the ``nn.Conv2d`` / ``nn.Linear`` / ``max_pool2d`` /
@@ -18,29 +18,27 @@ STAT_SLOTS = 16         # conv epilogues spread their BatchNorm statistics over 
 USE_WGRAD_HALO = True   # 3x3/s1/p1, 64 input channels: halo-reuse weight-gradient kernel (wgrad.cu)
 # Stride-2 convolutions without parity-split copies: the forward conv and the weight gradient read the original input through a
 # TMA box with element strides 2, and the four parity planes of the data gradient are stored straight into dX (strided epilogue
-# rows) -- no space_to_depth / depth_to_space passes.  Measured on B200 (profiles/r2_conv_layers.md): stride-2 forward 37 -> 21 us
-# (layer2), data gradient 68 -> 49 us, 1x1 shortcut 30 -> 15 us; whole ResNet-18 round -4.6 %.  RLR_STRIDED_TMA=0 restores the copies.
+# rows) -- no space_to_depth / depth_to_space passes.  RLR_STRIDED_TMA=0 restores the copies.
 USE_STRIDED_TMA = bool(int(os.environ.get("RLR_STRIDED_TMA", "1")))
 # Stem convolutions (Cin * k * k <= 64, stride 1): gather the k x k x Cin patch of every output pixel into ONE 64-wide K block
-# (im2col_small, or -- in the training step -- directly by the batch-assembly kernel gather_im2col) and run the plain tcgen05 GEMM on
+# (im2col_small, or -- in the training step -- directly by the batch-assembly kernel gather_im2col) and run the plain wgmma GEMM on
 # it, instead of k*k k-blocks of a 64-channel zero-padded input; the weight gradient is a [Cout x 64] GEMM over the same matrix.
-# Verified on B200 (tests/test_gpu_variants.py::test_im2col_stem_conv_and_wgrad, tests/test_gpu_native.py::test_stem_gemm_*);
+# Tested by tests/test_gpu_variants.py::test_im2col_stem_conv_and_wgrad and tests/test_gpu_native.py::test_stem_gemm_*;
 # RLR_IM2COL_STEM=0 restores the padded conv.
 USE_IM2COL_STEM = bool(int(os.environ.get("RLR_IM2COL_STEM", "1")))
 # BatchNorm(+ReLU, no residual) backward without reading the layer output: the mask is recomputed from x with the forward's own
-# scale/shift expression.  Measured on B200: within noise on the round, one activation read less per backward pass; default on
-# (RLR_BN_RECOMPUTE=0 reads the stored output instead).
+# scale/shift expression: one activation read less per backward pass; default on (RLR_BN_RECOMPUTE=0 reads the stored output instead).
 USE_BN_RECOMPUTE = bool(int(os.environ.get("RLR_BN_RECOMPUTE", "1")))
 # 3x3/s1/p1 convs with 64 input channels: three filter taps per N = 192 MMA with a lane shift-add epilogue (conv_halo3.cu) instead of
-# nine N = 64 MMAs per k-step.  Measured on B200: correct, +7 % per round (epilogue shuffles, 33 % more tiles): opt-in (RLR_HALO3=1).
+# nine N = 64 MMAs per k-step (33 % more tiles, shuffles in the epilogue): opt-in (RLR_HALO3=1).
 USE_HALO3 = bool(int(os.environ.get("RLR_HALO3", "0")))
 # halo-reuse kernel also for valid / full 3x3 convs and sizes that are not whole 16x8 tiles (reference CNNs: conv2 and its data gradient)
 USE_HALO_ANY = bool(int(os.environ.get("RLR_HALO_ANY", "1")))
 # Dense layers with few output tiles and a deep reduction (FMNIST CNN fc1: 256 x 128 x 9216): split-K GEMM with an fp32 workspace
 # (gemm_splitk.cu).  Verified and default on (RLR_SPLITK=0 runs the single-pass GEMM).
 USE_SPLITK = bool(int(os.environ.get("RLR_SPLITK", "1")))
-# Classifier-head kernels v2 (weights staged in shared memory, weight gradient spread over K/64 x B/16 blocks with float atomics).
-# Measured on B200: 49 -> 13 us per step; default on (RLR_HEAD_V2=0 restores the first kernels).
+# Classifier-head kernels v2 (weights staged in shared memory, weight gradient spread over K/64 x B/16 blocks, partials summed in a fixed order).
+# Default on (RLR_HEAD_V2=0 restores the first kernels).
 USE_HEAD_V2 = bool(int(os.environ.get("RLR_HEAD_V2", "1")))
 
 
@@ -86,7 +84,7 @@ def scratch(tag, shape, dtype, device):
 # convolution
 # =====================================================================================================================
 def conv_supported(in_shape, a, kind):
-    """Can the tcgen05 implicit-GEMM kernel run this conv?  ``in_shape`` = (H, W, Cin)."""
+    """Can the wgmma implicit-GEMM kernel run this conv?  ``in_shape`` = (H, W, Cin)."""
     h, w, cin = in_shape
     k, s, p, cout = a["k"], a.get("stride", 1), a.get("pad", 0), a["cout"]
     if k not in (1, 3) or s not in (1, 2) or cout % 8:
@@ -228,7 +226,7 @@ def _conv2d_dgrad_s2(e, dy, w, dx, pad, accumulate):
     """Stride-2 data gradient by input parity: input pixel (2a+pi, 2b+pj) only receives the taps with
     (pi + pad - dy) and (pj + pad - dx) even, from output pixel (a + (pi+pad-dy)/2, b + (pj+pad-dx)/2).  Each parity
     plane is therefore a small stride-1 convolution of dY with a sub-filter (1/2/2/4 taps for 3x3, pad 1); the four
-    planes are computed by the tcgen05 conv kernel into a parity-split buffer and interleaved by depth_to_space, or (strided
+    planes are computed by the wgmma conv kernel into a parity-split buffer and interleaved by depth_to_space, or (strided
     mode) stored directly at their pixels of dX."""
     Cout, k, _, Cin = w.shape
     B, Ho, Wo, _ = dy.shape
@@ -487,12 +485,12 @@ def dropout_bwd(dy, mask, dx, p, impl):
 # linear
 # =====================================================================================================================
 def linear_fused_dropout_ok(N, K):
-    """Can dropout be fused into this linear layer's GEMM epilogue (tcgen05 GEMM / split-K finishing pass)?"""
+    """Can dropout be fused into this linear layer's GEMM epilogue (wgmma GEMM / split-K finishing pass)?"""
     return N > 32 and K % 64 == 0 and N % 64 == 0
 
 
 def linear_fwd(x, w, bias, y, relu, impl, drop=None):
-    """y[B,N] = x[B,K] w[N,K]^T + b (ReLU).  N <= 32: CUDA-core head kernel; otherwise the tcgen05 GEMM.  ``drop`` = (p, seed, step
+    """y[B,N] = x[B,K] w[N,K]^T + b (ReLU).  N <= 32: CUDA-core head kernel; otherwise the wgmma GEMM.  ``drop`` = (p, seed, step
     counter tensor, node id): dropout fused into the GEMM epilogue after bias / ReLU (SURVEY.md K5); the backward pass reads the
     combined ReLU-and-dropout mask off the output (``relu_bwd_(..., scale=1/(1-p))``)."""
     N, K = w.shape

@@ -23,7 +23,7 @@ def _default_device():
 
 def build_parser() -> argparse.ArgumentParser:
     p = argparse.ArgumentParser(
-        description="Federated learning with the Robust Learning Rate backdoor defense (B200-native engine)")
+        description="Federated learning with the Robust Learning Rate backdoor defense (H100-native engine)")
     # ---- reference flags (names/defaults: src/options.py:7-70) ----
     p.add_argument("--data", type=str, default="fmnist", help="dataset: fmnist | fedemnist | cifar10")
     p.add_argument("--num_agents", type=int, default=10, help="number of agents: K")
@@ -53,7 +53,7 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--dtype", type=str, default="bf16", choices=("fp32", "bf16"),
                    help="activation/GEMM-operand dtype on GPU (master params, updates, aggregation stay fp32)")
     p.add_argument("--backend", type=str, default="auto", choices=("auto", "fused", "nccl", "gloo", "local"),
-                   help="aggregation transport: fused = P2P/multicast sm_100a kernel; nccl/gloo = all_gather + kernel")
+                   help="aggregation transport: fused = P2P/multicast sm_90a kernel; nccl/gloo = all_gather + kernel")
     p.add_argument("--agents_in_flight", type=int, default=0,
                    help="agents a GPU trains CONCURRENTLY when it hosts several per round (one trainer + CUDA stream each); helps the "
                         "small launch-bound CNNs, costs one set of activation buffers per extra agent.  0 = auto (2 for models under 4 M "
@@ -66,7 +66,7 @@ def build_parser() -> argparse.ArgumentParser:
                         "all_reduce per-coordinate vote / weighted-sum partials (avg, sign, RLR: O(N) traffic per rank); "
                         "auto = reduce when the ranks span several hosts")
     p.add_argument("--trainer", type=str, default="auto", choices=("auto", "native", "torch"),
-                   help="local-training executor: native = sm_100a kernels, torch = autograd oracle (CPU / baseline)")
+                   help="local-training executor: native = sm_90a kernels, torch = autograd oracle (CPU / baseline)")
     p.add_argument("--class_per_agent", type=int, default=10,
                    help="classes per agent in the partitioner (10 = IID like the reference's calls; fewer = label-skewed non-IID; "
                         "reference distribute_data parameter, src/utils.py:58)")

@@ -20,7 +20,7 @@ fp64 passes of ``Aggregation.aggregate_updates`` (src/aggregation.py:19-75) and 
 
 Hand-off fused with the next round's first GEMM (``enable_handoff``; SURVEY.md A9 / 5.8): the kernel then has NO barrier-out.  Rank r
 publishes its slice in every peer's ready word and exits; the consumer of the broadcast is the first local step of the next round
-(``models.native.NativeTrainer``): the producer warp of the stem convolution's tcgen05 GEMM acquires the ready word(s) of the slice(s)
+(``models.native.NativeTrainer``): the producer warp of the stem convolution's wgmma GEMM acquires the ready word(s) of the slice(s)
 that hold its filter -- it reads that filter straight out of the multicast bf16 shadow -- and a one-warp ``acquire_slices`` kernel
 queued right behind it waits for the remaining slices, so the first-layer GEMM overlaps the rest of the broadcast.  The separate
 ``round_init`` pass (w <- w_global, bf16 shadow, momentum <- 0) does not exist on that path: the first optimizer step reads

@@ -3,7 +3,7 @@
 ``TorchTrainer`` runs the IR with PyTorch autograd (cuDNN/cuBLAS on GPU): it is the CPU path, the numerical oracle
 for the native kernels, and the "ours-in-torch" baseline of BASELINE.md.  Everything around the forward/backward is
 already the engine's own: device-resident data + gather kernel, flat buffers, fused clip+SGD(+PGD) kernel, CUDA-graph
-capture of the whole step.  ``models.native.NativeTrainer`` replaces forward/backward with sm_100a kernels behind the
+capture of the whole step.  ``models.native.NativeTrainer`` replaces forward/backward with sm_90a kernels behind the
 same interface.
 
 One local step (reference src/agent.py:41-60): zero grads -> forward -> CE loss -> backward -> clip_grad_norm_(10) ->

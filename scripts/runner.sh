@@ -1,5 +1,5 @@
 #!/bin/bash
-# Canned experiment suites of the B200 engine.  The three dataset suites reproduce the experiment grid of the reference launcher
+# Canned experiment suites of the engine.  The three dataset suites reproduce the experiment grid of the reference launcher
 # (src/runner.sh:12-38: {no attack, backdoor attack, attack + Robust LR} x {FMNIST, CIFAR-10, Fed-EMNIST}); the last suite adds the
 # ResNet-18 / VGG-11 configs of BASELINE.json.
 #

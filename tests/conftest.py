@@ -6,11 +6,11 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
-REF_SRC = "/root/reference/src"
+GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_outputs.pt")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -30,17 +30,7 @@ def pytest_collection_modifyitems(config, items):
 
 
 @pytest.fixture(scope="session")
-def reference_modules():
-    """The reference's own modules (utils / aggregation / agent) for differential tests; skipped if not mounted.
-    They are imported under their bare names with cwd=src semantics, like the reference requires."""
-    src = REF_SRC if os.path.isdir(REF_SRC) else os.path.join(ROOT, "baseline", "_ref", "src")
-    if not os.path.isdir(src):
-        pytest.skip("reference sources not available")
-    sys.path.insert(0, src)
-    try:
-        import importlib
-        mods = {name: importlib.import_module(name) for name in ("utils", "aggregation", "models")}
-    finally:
-        sys.path.remove(src)
-    mods["src"] = src
-    return mods
+def reference_outputs():
+    """Outputs of the reference implementation for the differential tests' seeded inputs (scripts/make_reference_golden.py)."""
+    import torch
+    return torch.load(GOLDEN, weights_only=False)

@@ -1,6 +1,4 @@
 """Server step semantics (src/aggregation.py:19-75; SURVEY.md 3.4) incl. differential tests against the reference class."""
-from types import SimpleNamespace
-
 import pytest
 import torch
 from hypothesis import given, settings, strategies as st
@@ -35,40 +33,36 @@ def test_rlr_flips_sign_not_zero_and_zero_abstains():
 
 @pytest.mark.parametrize("aggr", ["avg", "comed", "sign"])
 @pytest.mark.parametrize("theta", [0, 1, 3, 5])
-def test_matches_reference_class(reference_modules, aggr, theta):
+def test_matches_reference_class(reference_outputs, aggr, theta):
     K, n = 5, 2000
     w0, ws = _mk(K, n, seed=theta)
     sizes = {i: 100 + 7 * i for i in range(K)}
-    args = SimpleNamespace(aggr=aggr, robustLR_threshold=theta, server_lr=0.7 if aggr == "sign" else 1.0, noise=0, clip=0, device="cpu")
-    model = torch.nn.Linear(n, 1, bias=False)
-    model.weight.data.copy_(w0.view(1, n))
-    ref = reference_modules["aggregation"].Aggregation(sizes, n, None, args, None)
-    ref.aggregate_updates(model, {i: (ws[i].double() - w0) for i in range(K)}, 1)
-    ours, _ = ops.aggregate_oracle(w0, ws, [sizes[i] for i in range(K)], aggr, theta, args.server_lr)
-    torch.testing.assert_close(ours, model.weight.data.view(-1), atol=1e-7, rtol=1e-6)
+    server_lr = 0.7 if aggr == "sign" else 1.0
+    ref = reference_outputs[f"aggregate/{aggr}/{theta}"]       # the reference class's aggregate_updates on a Linear model holding w0
+    ours, _ = ops.aggregate_oracle(w0, ws, [sizes[i] for i in range(K)], aggr, theta, server_lr)
+    torch.testing.assert_close(ours, ref, atol=1e-7, rtol=1e-6)
     # and the public class (CPU path of the fused op)
     a = make_args(aggr=aggr, robustLR_threshold=theta, server_lr=0.7)
     wg = w0.clone()
     Aggregation(sizes, n, None, a).aggregate_updates(wg, {i: ws[i] for i in range(K)}, 1, n_vote=n)
-    torch.testing.assert_close(wg, model.weight.data.view(-1), atol=1e-7, rtol=1e-6)
+    torch.testing.assert_close(wg, ref, atol=1e-7, rtol=1e-6)
 
 
-def test_reference_named_helpers_match_reference(reference_modules):
+def test_reference_named_helpers_match_reference(reference_outputs):
     K, n = 4, 500
     w0, ws = _mk(K, n, seed=3)
     ups = {i: (ws[i].double() - w0) for i in range(K)}
     sizes = {i: 10 * (i + 1) for i in range(K)}
-    args = SimpleNamespace(aggr="avg", robustLR_threshold=3, server_lr=1.0, noise=0, clip=0.5, device="cpu")
-    ref = reference_modules["aggregation"].Aggregation(sizes, n, None, args, None)
+    ref = lambda name: reference_outputs[f"helpers/{name}"]  # noqa: E731  (reference Aggregation, robustLR_threshold=3, clip=0.5)
     ours = Aggregation(sizes, n, None, make_args(robustLR_threshold=3, clip=0.5))
-    torch.testing.assert_close(ours.compute_robustLR(ups), ref.compute_robustLR({k: v.clone() for k, v in ups.items()}))
-    torch.testing.assert_close(ours.agg_avg(ups), ref.agg_avg(ups))
-    torch.testing.assert_close(ours.agg_comed(ups), ref.agg_comed(ups))
-    torch.testing.assert_close(ours.agg_sign(ups), ref.agg_sign(ups))
-    a, b = {k: v.clone() for k, v in ups.items()}, {k: v.clone() for k, v in ups.items()}
-    ours.clip_updates(a); ref.clip_updates(b)
+    torch.testing.assert_close(ours.compute_robustLR(ups), ref("robustLR"))
+    torch.testing.assert_close(ours.agg_avg(ups), ref("avg"))
+    torch.testing.assert_close(ours.agg_comed(ups), ref("comed"))
+    torch.testing.assert_close(ours.agg_sign(ups), ref("sign"))
+    a = {k: v.clone() for k, v in ups.items()}
+    ours.clip_updates(a)
     for k in a:
-        torch.testing.assert_close(a[k], b[k])
+        torch.testing.assert_close(a[k], ref("clipped")[k])
 
 
 def test_tail_coordinates_get_plain_mean_and_no_vote():

@@ -1,4 +1,4 @@
-"""GPU numerics: every sm_100a kernel of ops/csrc vs. its plain-PyTorch fp32/fp64 oracle (run with -m gpu)."""
+"""GPU numerics: every sm_90a kernel of ops/csrc vs. its plain-PyTorch fp32/fp64 oracle (run with -m gpu)."""
 import pytest
 import torch
 

@@ -1,6 +1,6 @@
 """Multi-GPU: the fused P2P aggregate+broadcast kernel (peer reads over NVLink, multicast / per-peer stores, in-kernel
 flag barriers) against the fp64 oracle and against the NCCL all_gather baseline.  Needs >= 2 GPUs
-(``gpurun --gpus 2 -- python -m pytest tests/test_gpu_multi.py -m gpu``)."""
+(``python -m pytest tests/test_gpu_multi.py -m gpu`` on a multi-GPU machine); skips on one GPU."""
 import os
 import socket
 import sys

@@ -1,4 +1,4 @@
-"""GPU numerics of the tcgen05 GEMM / implicit-GEMM convolution kernels (gemm.cu), the NHWC layer kernels (norm.cu)
+"""GPU numerics of the wgmma GEMM / implicit-GEMM convolution kernels (gemm.cu), the NHWC layer kernels (norm.cu)
 and the native executor against plain PyTorch fp32 references of the same ops."""
 import pytest
 import torch
@@ -304,7 +304,7 @@ def test_native_net_sm100_vs_fp32_autograd(model, B):
 
 @pytest.mark.parametrize("model", ["resnet18", "cnn_cifar"])
 def test_native_trainer_learns_like_torch_trainer(model):
-    """A few federated rounds on separable synthetic data: the sm_100a trainer must learn (and roughly track the torch
+    """A few federated rounds on separable synthetic data: the sm_90a trainer must learn (and roughly track the torch
     trainer); also exercises CUDA-graph capture of the native step, the ragged last batch and evaluation."""
     from rlr_b200.engine import FLEngine
     from rlr_b200.options import make_args
@@ -346,7 +346,7 @@ def test_conv3x3_halo_kernel(B, H, W, Cout, acc):
         errs[bo] = _rel(y, ref)
         if bo == 0:
             s_ok = acc or torch.allclose(stats.sum(0)[0], y.float().sum((0, 1, 2)), rtol=2e-3, atol=0.5)
-    # bo=0 (base-offset field zero) is the mode that is correct on B200: the swizzle follows absolute smem address bits
+    # bo=0 (base-offset field zero) is the default mode: the swizzle follows absolute smem address bits
     print("halo conv rel err by base-offset mode:", errs)
     assert errs[0] < 1e-2, errs
     assert s_ok
@@ -451,7 +451,7 @@ def test_persistent_conv_matches_default(B, H, W, Cin, Cout, k, s, p):
 @pytest.mark.parametrize("N,kvalid,M,relu", [(64, 27, 1000, True), (32, 9, 300, False), (128, 27, 4096, True), (64, 64, 129, False),
                                              (64, 27, 65536 + 77, True), (32, 9, 173056, True), (128, 27, 40000, False)])   # persistent path (>= 2 tiles per SM)
 def test_stem_gemm_gathers_unpadded_filter(N, kvalid, M, relu):
-    """Stem convolution as one 64-deep tcgen05 GEMM whose B tile is gathered + zero-padded + swizzled by the producer warp from the
+    """Stem convolution as one 64-deep wgmma GEMM whose B tile is gathered + zero-padded + swizzled by the producer warp from the
     UN-padded filter (stem_gather.cuh; the same path reads the multicast broadcast buffer behind ready flags).  Small M: one tile per
     CTA (gemm.cu); from two tiles per SM upwards: the persistent kernel (gemm_persistent.cu) that builds the B tile once per SM."""
     torch.manual_seed(N + kvalid + M)
@@ -505,7 +505,7 @@ def test_fused_handoff_equals_round_init_path(model):
 
 
 def test_fused_dropout_kernels():
-    """Dropout fused into its producers (SURVEY.md K5): max-pool kernel, tcgen05 GEMM epilogue, split-K finishing pass.  Keep fraction and
+    """Dropout fused into its producers (SURVEY.md K5): max-pool kernel, wgmma GEMM epilogue, split-K finishing pass.  Keep fraction and
     1/(1-p) scaling, determinism in (seed, step, node), fresh masks per step, and forward/backward mask consistency (the pooling backward
     recomputes the Philox mask; the linear backward reads ReLU-and-dropout off the output)."""
     torch.manual_seed(5)
@@ -530,7 +530,7 @@ def test_fused_dropout_kernels():
     step += 1
     y3 = torch.empty_like(y0); ops.maxpool2_fwd(x, y3, idx1, "sm100", (p, 7, step, 3))
     assert not torch.equal(y1, y3)                                                # next step -> fresh mask
-    # ---- Linear + ReLU + dropout: tcgen05 GEMM epilogue (K = 128) and split-K finishing pass (K = 2048) ----
+    # ---- Linear + ReLU + dropout: wgmma GEMM epilogue (K = 128) and split-K finishing pass (K = 2048) ----
     for K in (128, 2048):
         xx = torch.randn(256, K, device=DEV).to(BF)
         ww = (torch.randn(128, K, device=DEV) / K ** 0.5).to(BF)

@@ -1,5 +1,5 @@
 """The native executor's plan (fusion, hand-derived backward, residual gradient accumulation) against PyTorch autograd, run on
-CPU in fp32 through the `aten` back-end.  The sm_100a kernels behind the same plan are checked in tests/test_gpu_native.py."""
+CPU in fp32 through the `aten` back-end.  The sm_90a kernels behind the same plan are checked in tests/test_gpu_native.py."""
 import pytest
 import torch
 

@@ -319,7 +319,7 @@ def test_native_plan_with_kernel_conv_paths_matches_library_convs(fake, monkeypa
     monkeypatch.setattr(nn, "USE_STRIDED_TMA", mode == "strided")
     monkeypatch.setattr(nn, "USE_IM2COL_STEM", mode == "stem")
     import rlr_b200.models.native as native_mod
-    monkeypatch.setattr(native_mod, "EPILOGUE_BN_STATS", True)     # opt-in path (measured slower on B200): keep its plumbing covered
+    monkeypatch.setattr(native_mod, "EPILOGUE_BN_STATS", True)     # opt-in path: keep its plumbing covered
     torch.manual_seed(0)
     lay = get_layout(model)
     for nd in lay.nodes:

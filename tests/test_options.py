@@ -1,6 +1,4 @@
 """CLI parity with the reference flag table (src/options.py:4-74, SURVEY.md 5.6)."""
-import sys
-
 import pytest
 
 from rlr_b200.options import args_parser, finalize_args, make_args, print_exp_details
@@ -16,14 +14,8 @@ def test_defaults_match_reference_table():
         assert getattr(a, k) == v, k
 
 
-def test_defaults_match_reference_parser(reference_modules, monkeypatch):
-    sys.path.insert(0, reference_modules["src"])
-    try:
-        import options as ref_options
-    finally:
-        sys.path.remove(reference_modules["src"])
-    monkeypatch.setattr(sys, "argv", ["federated.py"])
-    ref = vars(ref_options.args_parser())
+def test_defaults_match_reference_parser(reference_outputs):
+    ref = reference_outputs["options/defaults"]          # vars(args_parser()) of the reference's options.py, without "device"
     ours = vars(args_parser([]))
     for k, v in ref.items():
         if k == "device":

@@ -59,21 +59,25 @@ def test_fedemnist_patterns():
     assert abs(float(cp[rows[0], cols[0]]) - (0.8 - vals[0])) < 1e-6
 
 
-@pytest.mark.parametrize("ds,pat,agent", [("cifar10", "plus", -1), ("cifar10", "plus", 0), ("cifar10", "plus", 1), ("cifar10", "plus", 2),
-                                          ("cifar10", "plus", 3), ("cifar10", "square", -1), ("fmnist", "plus", -1),
-                                          ("fmnist", "square", -1), ("fmnist", "copyright", -1), ("fmnist", "apple", -1),
-                                          ("fedemnist", "plus", -1), ("fedemnist", "square", -1), ("fedemnist", "copyright", -1),
-                                          ("fedemnist", "apple", -1)])
-def test_add_pattern_matches_reference(reference_modules, ds, pat, agent, monkeypatch):
-    monkeypatch.chdir(reference_modules["src"])  # '../watermark.png' is cwd-relative (src/utils.py:233)
+PATTERN_CASES = [("cifar10", "plus", -1), ("cifar10", "plus", 0), ("cifar10", "plus", 1), ("cifar10", "plus", 2), ("cifar10", "plus", 3),
+                 ("cifar10", "square", -1), ("fmnist", "plus", -1), ("fmnist", "square", -1), ("fmnist", "copyright", -1),
+                 ("fmnist", "apple", -1), ("fedemnist", "plus", -1), ("fedemnist", "square", -1), ("fedemnist", "copyright", -1),
+                 ("fedemnist", "apple", -1)]
+
+
+def pattern_input(ds):
     g = torch.Generator().manual_seed(0)
     if ds == "cifar10":
-        x = torch.randint(0, 256, (32, 32, 3), generator=g, dtype=torch.uint8)
-    elif ds == "fmnist":
-        x = torch.randint(0, 256, (28, 28), generator=g, dtype=torch.uint8)
-    else:
-        x = torch.rand(1, 28, 28, generator=g)
-    ref = reference_modules["utils"].add_pattern_bd(x.clone() if ds != "cifar10" else x.numpy().copy(), ds, pattern_type=pat, agent_idx=agent)
+        return torch.randint(0, 256, (32, 32, 3), generator=g, dtype=torch.uint8)
+    if ds == "fmnist":
+        return torch.randint(0, 256, (28, 28), generator=g, dtype=torch.uint8)
+    return torch.rand(1, 28, 28, generator=g)
+
+
+@pytest.mark.parametrize("ds,pat,agent", PATTERN_CASES)
+def test_add_pattern_matches_reference(reference_outputs, ds, pat, agent):
+    x = pattern_input(ds)
+    ref = reference_outputs[f"pattern/{ds}/{pat}/{agent}"].numpy()     # the reference's add_pattern_bd on the same image
     ours = add_pattern_bd(x.squeeze(0) if ds == "fedemnist" else x, ds, pat, agent)
     if ds == "fedemnist":
         np.testing.assert_allclose(ours.numpy(), np.asarray(ref, dtype=np.float32), atol=1e-6)

@@ -45,7 +45,7 @@ inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block
 
 // ---- deterministic cross-CTA reductions ---------------------------------------------------------------------------------------
 // A reduction over CTAs never adds into its output with float atomics (their order, and so the rounding, changes from run to run):
-// every CTA writes its partial result to a slot of a scratch buffer and ordered_sum_kernel adds the slots in a fixed order.
+// every CTA writes its partial result to a slot of a scratch buffer and launch_ordered_sum adds the slots in a fixed order.
 // Scratch memory comes from the framework's stream-ordered caching allocator (gemm_binding.cpp), so it is safe to release right
 // after the launches that use it and it is captured with the rest of a CUDA graph.
 void* scratch_alloc(size_t bytes, cudaStream_t st);
@@ -68,6 +68,40 @@ __global__ void __launch_bounds__(256) ordered_sum_kernel(T* __restrict__ out, c
         for (int j = 1; j < nparts; ++j) s += part[(size_t)j * n + i];
         out[i] += s;
     }
+}
+
+// Same sums as ordered_sum_kernel for many partials (the per-CTA slots of a grid-wide reduction: hundreds of parts of a few hundred
+// columns).  One thread per element walking hundreds of dependent-order loads leaves a handful of CTAs latency-bound, so here a CTA
+// takes 32 columns: all eight warps stage 64 parts at a time into shared memory with independent coalesced loads, and warp 0 adds
+// the staged rows in part order -- the additions, and so the rounding, are exactly those of ordered_sum_kernel.
+template <typename T>
+__global__ void __launch_bounds__(256) ordered_sum_cols_kernel(T* __restrict__ out, const T* __restrict__ part, int nparts, long long n) {
+    constexpr int kRows = 64, kPerWarp = kRows / 8;
+    __shared__ T tile[kRows][33];
+    pdl_wait();
+    pdl_trigger();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long col = (long long)blockIdx.x * 32 + lane;
+    T s = T(0);
+    for (int j0 = 0; j0 < nparts; j0 += kRows) {
+        T v[kPerWarp];
+#pragma unroll
+        for (int q = 0; q < kPerWarp; ++q) {
+            const int j = j0 + warp + 8 * q;
+            v[q] = (j < nparts && col < n) ? part[(size_t)j * n + col] : T(0);
+        }
+#pragma unroll
+        for (int q = 0; q < kPerWarp; ++q) tile[warp + 8 * q][lane] = v[q];
+        __syncthreads();
+        if (warp == 0) {
+            const int rows = nparts - j0 < kRows ? nparts - j0 : kRows;
+            int r = 0;
+            if (j0 == 0) { s = tile[0][lane]; r = 1; }
+            for (; r < rows; ++r) s += tile[r][lane];
+        }
+        __syncthreads();
+    }
+    if (warp == 0 && col < n) out[col] += s;
 }
 
 __device__ __forceinline__ unsigned long long gtimer() {     // nanosecond timer common to all SMs
@@ -226,6 +260,8 @@ __device__ __forceinline__ uint32_t dropout_keep8(const DropSpec& d, long long q
 
 template <typename T>
 inline cudaError_t launch_ordered_sum(T* out, const T* part, int nparts, long long n, cudaStream_t st) {
+    if (nparts >= 16)
+        return launch_kernel(ordered_sum_cols_kernel<T>, dim3((unsigned)((n + 31) / 32)), dim3(256), (size_t)0, st, out, part, nparts, n);
     long long blocks = (n + 255) / 256;
     if (blocks > 1024) blocks = 1024;
     if (blocks < 1) blocks = 1;

@@ -96,6 +96,9 @@ cudaError_t launch_conv_wgrad_halo_bf16(const void* dy, const void* x, float* dW
 cudaError_t launch_linear_wgrad_bf16(const void* dy, const void* x, float* dW, int B, int N, int K, int num_sms, cudaStream_t st);
 
 // ---- norm.cu: NHWC bf16 layer kernels -----------------------------------------------------------------------------
+// out[i] += part[0][i] + part[1][i] + ... in part order (common.cuh launch_ordered_sum, the reduction behind every cross-CTA sum)
+cudaError_t launch_ordered_sum_f32(float* out, const float* part, int nparts, long long n, cudaStream_t st);
+cudaError_t launch_ordered_sum_f64(double* out, const double* part, int nparts, long long n, cudaStream_t st);
 // per-channel sum / sum of squares of x[M][C]
 // only_sum: accumulate just sum x into stats[0..C) (bias gradients written straight into the flat gradient)
 cudaError_t launch_channel_stats(const __nv_bfloat16* x, long long M, int C, float* stats /*[nslots][2][C], accumulates*/, int num_sms, cudaStream_t st,

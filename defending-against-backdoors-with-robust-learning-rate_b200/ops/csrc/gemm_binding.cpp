@@ -187,6 +187,19 @@ void linear_wgrad_bf16(at::Tensor dy, at::Tensor x, at::Tensor dW) {
     check(rlr::launch_linear_wgrad_bf16(bf(dy), bf(x), f32(dW), B, N, K, num_sms(), cur_stream()), "linear_wgrad_bf16");
 }
 
+// out[i] += part[0][i] + part[1][i] + ... in part order (the fixed-order reduction behind every cross-CTA sum); float32 / float64
+void ordered_sum(at::Tensor out, at::Tensor part) {
+    c10::cuda::CUDAGuard g(out.device());
+    TORCH_CHECK(out.is_contiguous() && part.is_contiguous() && part.dim() == 2 && part.size(1) == out.numel() &&
+                part.scalar_type() == out.scalar_type(), "ordered_sum: out [n], part [nparts][n]");
+    const int nparts = (int)part.size(0);
+    const long long n = out.numel();
+    if (out.scalar_type() == at::kDouble)
+        check(rlr::launch_ordered_sum_f64(out.data_ptr<double>(), part.data_ptr<double>(), nparts, n, cur_stream()), "ordered_sum");
+    else
+        check(rlr::launch_ordered_sum_f32(out.data_ptr<float>(), part.data_ptr<float>(), nparts, n, cur_stream()), "ordered_sum");
+}
+
 void channel_stats(at::Tensor x, at::Tensor stats) {
     c10::cuda::CUDAGuard g(x.device());
     const int C = x.size(-1);
@@ -367,6 +380,7 @@ void register_gemm_bindings(py::module_& m) {
     m.def("linear_wgrad_bf16", &linear_wgrad_bf16);
     m.def("conv_wgrad_halo_bf16", &conv_wgrad_halo_bf16);
     m.def("channel_stats", &channel_stats);
+    m.def("ordered_sum", &ordered_sum);
     m.def("bias_grad", &bias_grad);
     m.def("bn_finalize", &bn_finalize);
     m.def("bn_apply", &bn_apply);

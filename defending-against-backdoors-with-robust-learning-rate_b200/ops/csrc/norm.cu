@@ -117,6 +117,13 @@ __global__ void __launch_bounds__(256, MODE == 0 ? 4 : 3) channel_reduce_kernel(
     }
 }
 
+cudaError_t launch_ordered_sum_f32(float* out, const float* part, int nparts, long long n, cudaStream_t st) {
+    return launch_ordered_sum(out, part, nparts, n, st);
+}
+cudaError_t launch_ordered_sum_f64(double* out, const double* part, int nparts, long long n, cudaStream_t st) {
+    return launch_ordered_sum(out, part, nparts, n, st);
+}
+
 // The per-CTA partial sums are added into slot 0 of the [nslots][2][C] output in CTA order (deterministic); nslots >= 4 selects
 // four CTAs per SM instead of two.
 cudaError_t launch_channel_stats(const __nv_bfloat16* x, long long M, int C, float* stats, int num_sms, cudaStream_t st, int only_sum, int nslots) {

@@ -1,0 +1,263 @@
+"""Per-kernel profile of one training step of the bench.py workload (ResNet-18, CIFAR shape, batch 256, one GPU).
+
+    python scripts/profile_step.py [--out DIR] [--replays N] [--bs 256]
+
+Builds the engine exactly as ``bench.py`` does, runs one warm-up round (which captures the training-step CUDA graph), then
+replays the captured full-batch step ``--replays`` times under ``torch.profiler`` with CUDA activities.  The kernels inside the
+graph are listed one by one; the script writes DIR/profile_step.md (and .json) with one row per kernel name: calls and
+microseconds per step, share of the step and, for the implicit-GEMM conv / GEMM kernel, its FLOP, L2 operand bytes and achieved
+TFLOP/s per launch shape.  FLOP and bytes come from the launch shapes (``launch_record`` below), recorded by wrapping the
+extension's conv / GEMM entry points during the warm-up round.  The card's name, power limit and maximum SM clock are read in
+the same run (read-only nvidia-smi query).
+"""
+from __future__ import annotations
+
+import argparse
+import collections
+import json
+import os
+import subprocess
+import sys
+import tempfile
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+BM, BK = 128, 64        # gemm.cu tile rows / k-block depth
+KERNEL = "umma_conv_gemm_kernel"
+
+
+def _pow2_ceil(x):
+    p = 1
+    while p < x:
+        p <<= 1
+    return p
+
+
+def conv_tiles(NB, Ho, Wo):
+    """m-tiles of launch_conv_bf16: TW x TH x TN = 128-pixel boxes."""
+    TW = min(_pow2_ceil(Wo), BM)
+    TH = _pow2_ceil(Ho)
+    if TW * TH > BM:
+        TH = BM // TW
+    TN = BM // (TW * TH)
+    return -(-Wo // TW) * -(-Ho // TH) * -(-NB // TN)
+
+
+def pick_bn(N, m_tiles, sms, conv):
+    """Tile width launch_conv_bf16 / launch_gemm_bf16 choose (RLR_SMALL_BN64 default on for convs)."""
+    bn = 128 if N % 128 == 0 else 64
+    if conv and bn == 128 and m_tiles * (N // 128) < sms and int(os.environ.get("RLR_SMALL_BN64", "1")):
+        bn = 64
+    return bn
+
+
+def launch_record(kind, M, N, K, m_tiles, sms, conv, bmn=False, cluster=(1, 1)):
+    """One implicit-GEMM launch: FLOP = 2 M N K (useful work, masked rows excluded) and L2 operand bytes = what the CTAs' TMA
+    loads read, every CTA its own A and B tile per 64-deep k-block; an operand shared by the CTAs of a cluster is fetched once
+    per cluster (``cluster`` = CTAs along M sharing B, along N sharing A)."""
+    bn = pick_bn(N, m_tiles, sms, conv)
+    n_tiles = -(-N // bn)
+    kb = -(-K // BK)
+    ctas = m_tiles * n_tiles
+    cm, cn = cluster
+    a_bytes = ctas * kb * BM * BK * 2 / cn
+    b_bytes = ctas * kb * bn * BK * 2 / cm
+    return {"kind": kind, "M": M, "N": N, "K": K, "bn": bn, "grid": (m_tiles, n_tiles), "bmn": bmn,
+            "flop": 2.0 * M * N * K, "l2_bytes": a_bytes + b_bytes}
+
+
+def install_recorder(ext, sms, log):
+    """Wrap the extension's conv / GEMM entry points so every call appends its launch record to ``log``; ``advance_cursor``
+    (called once at the end of every training step) appends a step delimiter."""
+    orig = {n: getattr(ext, n) for n in ("conv_bf16", "conv_bf16_strided", "gemm_bf16", "stem_gemm_bf16", "advance_cursor")}
+
+    def conv_bf16(x, w, out, NB, planes, dh, *a):
+        wtap = a[-2]
+        Ho, Wo, Cout, Cin = out.shape[1], out.shape[2], out.shape[3], x.shape[3]
+        log.append(launch_record("dgrad" if wtap else "fwd", NB * Ho * Wo, Cout, len(dh) * Cin, conv_tiles(NB, Ho, Wo), sms, True,
+                                 bool(wtap)))
+        return orig["conv_bf16"](x, w, out, NB, planes, dh, *a)
+
+    def conv_bf16_strided(x, w, out, dh, dw, bias, relu, acc, wtap, T, in_s, out_s, ph, pw):
+        NB, Cin, Cout = x.shape[0], x.shape[3], out.shape[3]
+        Ho, Wo = out.shape[1] // out_s, out.shape[2] // out_s
+        log.append(launch_record("dgrad-s2-plane" if wtap else "fwd-s2", NB * Ho * Wo, Cout, len(dh) * Cin, conv_tiles(NB, Ho, Wo),
+                                 sms, True, bool(wtap)))
+        return orig["conv_bf16_strided"](x, w, out, dh, dw, bias, relu, acc, wtap, T, in_s, out_s, ph, pw)
+
+    def gemm_bf16(A, B, out, *a, **k):
+        M, K, N = A.shape[0], A.shape[1], B.shape[0]
+        log.append(launch_record("gemm", M, N, K, -(-M // BM), sms, False))
+        return orig["gemm_bf16"](A, B, out, *a, **k)
+
+    def stem_gemm_bf16(A, W, out, *a, **k):
+        M, N = A.shape[0], W.shape[0]
+        log.append(launch_record("stem", M, N, W.shape[1], -(-M // BM), sms, False))
+        return orig["stem_gemm_bf16"](A, W, out, *a, **k)
+
+    def advance_cursor(*a, **k):
+        log.append(None)
+        return orig["advance_cursor"](*a, **k)
+
+    for n, f in (("conv_bf16", conv_bf16), ("conv_bf16_strided", conv_bf16_strided), ("gemm_bf16", gemm_bf16),
+                 ("stem_gemm_bf16", stem_gemm_bf16), ("advance_cursor", advance_cursor)):
+        setattr(ext, n, f)
+    return orig
+
+
+def one_step_launches(log):
+    """Launch records of the first complete full-batch step in the log (an eager warm-up step before the graph is captured):
+    the first step whose first launch has the most rows."""
+    steps, cur = [], []
+    for r in log:
+        if r is None:
+            steps.append(cur)
+            cur = []
+        else:
+            cur.append(r)
+    steps = [s for s in steps if s]
+    if not steps:
+        raise RuntimeError("no training step was recorded")
+    top = max(s[0]["M"] for s in steps)
+    return next(s for s in steps if s[0]["M"] == top)
+
+
+def gpu_info():
+    q = "name,power.limit,clocks.max.sm"
+    try:
+        out = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True,
+                             timeout=30).stdout.strip().splitlines()
+        return out[0] if out else "unknown"
+    except Exception as e:  # noqa: BLE001
+        return f"nvidia-smi unavailable ({type(e).__name__})"
+
+
+def short_name(name):
+    n = name.split("(")[0].replace("void ", "").strip()
+    return n.split("rlr::")[-1]
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--out", default="profile_out")
+    ap.add_argument("--replays", type=int, default=20)
+    ap.add_argument("--bs", type=int, default=256)
+    ap.add_argument("--train_size", type=int, default=50000)
+    a = ap.parse_args()
+
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    from rlr_b200 import ops
+    from rlr_b200.engine import FLEngine
+    from rlr_b200.options import make_args
+    from rlr_b200.parallel import init_distributed
+
+    if not torch.cuda.is_available():
+        raise SystemExit("profile_step.py measures on the GPU; no CUDA device is visible")
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    log = []
+    install_recorder(ops.ext(), sms, log)
+    ctx = init_distributed(None, None)
+    args = make_args(data="cifar10", model="resnet18", num_agents=1, agents_in_flight=0, local_ep=2, bs=a.bs, aggr="avg",
+                     robustLR_threshold=0, num_corrupt=0, poison_frac=0.0, agent_frac=1.0, pattern_type="plus",
+                     synthetic=a.train_size, synthetic_val=1000, snap=10 ** 9, rounds=10 ** 9, log_dir="", trainer="auto",
+                     backend="auto", dtype="bf16", seed=0)
+    eng = FLEngine(args, ctx=ctx, verbose=False)
+    eng.run_round(1)                                   # captures the step graphs (and records one eager step's launches)
+    eng.run_round(2)
+    torch.cuda.synchronize()
+    launches = one_step_launches(log)
+    tr = eng.trainer
+    graphs = [g for k, g in tr._graphs.items() if k[0] == a.bs and not k[3]]
+    if not graphs:
+        raise RuntimeError("no captured full-batch step graph")
+    graph = graphs[0]
+    for _ in range(3):
+        tr.cursor.zero_()
+        graph.replay()
+    torch.cuda.synchronize()
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    ev0.record()
+    for _ in range(a.replays):
+        tr.cursor.zero_()                              # every replay reads the same valid sample indices
+        graph.replay()
+    ev1.record()
+    torch.cuda.synchronize()
+    step_ms_unprofiled = ev0.elapsed_time(ev1) / a.replays
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(a.replays):
+            tr.cursor.zero_()
+            graph.replay()
+        torch.cuda.synchronize()
+    with tempfile.TemporaryDirectory() as td:
+        path = os.path.join(td, "trace.json")
+        prof.export_chrome_trace(path)
+        trace = json.load(open(path))
+    kernels = [e for e in trace.get("traceEvents", []) if e.get("cat") == "kernel"]
+    gpu = gpu_info()
+    eng.close()
+
+    per_name = collections.defaultdict(lambda: [0, 0.0])
+    per_shape = collections.defaultdict(lambda: [0, 0.0])       # (name, grid) of the GEMM kernel
+    for e in kernels:
+        nm = short_name(e["name"])
+        per_name[nm][0] += 1
+        per_name[nm][1] += float(e["dur"])
+        if nm.startswith(KERNEL):
+            g = tuple(e.get("args", {}).get("grid", [0, 0, 0])[:2])
+            per_shape[(nm, g)][0] += 1
+            per_shape[(nm, g)][1] += float(e["dur"])
+    total_us = sum(v[1] for v in per_name.values()) / a.replays
+
+    # launch records -> traced GEMM kernels, matched by tile width, B layout (template arguments 1 and 3) and grid
+    by_grid = collections.defaultdict(list)
+    for r in launches:
+        by_grid[(r["bn"], r["bmn"], tuple(r["grid"]))].append(r)
+    shape_rows = []
+    for (nm, g), (cnt, us) in sorted(per_shape.items(), key=lambda kv: -kv[1][1]):
+        calls = cnt / a.replays
+        targs = [t.strip() for t in nm.split("<", 1)[1].rstrip(">").split(",")]
+        recs = by_grid.get((int(targs[0]), targs[2] == "true", g), [])
+        flop = sum(r["flop"] for r in recs)
+        l2 = sum(r["l2_bytes"] for r in recs)
+        kinds = sorted({f'{r["kind"]} M{r["M"]} N{r["N"]} K{r["K"]}' for r in recs})
+        us_step = us / a.replays
+        shape_rows.append({"kernel": nm, "grid": list(g), "calls_per_step": calls, "us_per_step": us_step,
+                           "matched_launches": len(recs), "launches": kinds, "gflop": flop / 1e9, "l2_mb": l2 / 1e6,
+                           "tflops": (flop / (us_step * 1e-6) / 1e12) if (recs and us_step and len(recs) == round(calls)) else None,
+                           "l2_tb_s": (l2 / (us_step * 1e-6) / 1e12) if (recs and us_step and len(recs) == round(calls)) else None})
+    rows = []
+    for nm, (cnt, us) in sorted(per_name.items(), key=lambda kv: -kv[1][1]):
+        us_step = us / a.replays
+        rows.append({"kernel": nm, "calls_per_step": cnt / a.replays, "us_per_step": us_step, "share": us_step / total_us})
+    gemm_us = sum(r["us_per_step"] for r in rows if r["kernel"].startswith(KERNEL))
+    gemm_flop = sum(r["flop"] for r in launches)
+    res = {"gpu": gpu, "replays": a.replays, "batch": a.bs, "step_ms_unprofiled": step_ms_unprofiled,
+           "kernel_us_per_step": total_us, "gemm_kernel_us_per_step": gemm_us, "gemm_kernel_share": gemm_us / total_us,
+           "gemm_gflop_per_step": gemm_flop / 1e9, "gemm_tflops": gemm_flop / (gemm_us * 1e-6) / 1e12 if gemm_us else None,
+           "conv_cluster": os.environ.get("RLR_CONV_CLUSTER", "default"), "kernels": rows, "gemm_shapes": shape_rows}
+    os.makedirs(a.out, exist_ok=True)
+    with open(os.path.join(a.out, "profile_step.json"), "w") as f:
+        json.dump(res, f, indent=1)
+    md = [f"GPU: {gpu} (name, power limit, max SM clock)  ",
+          f"Step (batch {a.bs}, graph replay, profiler off): {step_ms_unprofiled:.3f} ms; summed kernel time {total_us / 1e3:.3f} ms.  ",
+          f"`{KERNEL}` (all instantiations): {gemm_us:.0f} us/step = {100 * gemm_us / total_us:.1f} % of kernel time, "
+          f"{gemm_flop / 1e9:.0f} GFLOP/step, {res['gemm_tflops'] or 0:.0f} TFLOP/s.",
+          "", "| kernel | calls/step | us/step | share |", "|---|---:|---:|---:|"]
+    md += [f'| `{r["kernel"]}` | {r["calls_per_step"]:.0f} | {r["us_per_step"]:.1f} | {100 * r["share"]:.1f} % |' for r in rows]
+    md += ["", f"`{KERNEL}` by launch grid (m-tiles x n-tiles):", "",
+           "| instantiation | grid | calls/step | us/step | launches | GFLOP | L2 operand MB | TFLOP/s | L2 TB/s |",
+           "|---|---|---:|---:|---|---:|---:|---:|---:|"]
+    for r in shape_rows:
+        tf = f'{r["tflops"]:.0f}' if r["tflops"] else "-"
+        bw = f'{r["l2_tb_s"]:.1f}' if r["l2_tb_s"] else "-"
+        md.append(f'| `{r["kernel"].replace(KERNEL, "")}` | {r["grid"][0]}x{r["grid"][1]} | {r["calls_per_step"]:.0f} | '
+                  f'{r["us_per_step"]:.1f} | {"; ".join(r["launches"]) or "-"} | {r["gflop"]:.1f} | {r["l2_mb"]:.0f} | {tf} | {bw} |')
+    with open(os.path.join(a.out, "profile_step.md"), "w") as f:
+        f.write("\n".join(md) + "\n")
+    print("\n".join(md))
+
+
+if __name__ == "__main__":
+    main()

@@ -11,7 +11,8 @@ Flat layout (one buffer per role: params ``w``, grads ``g``, momentum ``m``):
     [ param_0 | pad | param_1 | pad | ... | (n_vote) | bn running stats ... | pad (n_total) ]
 
 Every tensor starts at a multiple of 64 elements.  Coordinates ``< n_vote`` take part in the sign vote / robust
-aggregation; BatchNorm running statistics live behind ``n_vote`` and are plainly averaged (SURVEY.md quirk 13).
+aggregation; BatchNorm running statistics live behind ``n_vote`` and are plainly averaged (SURVEY.md quirk 13).  GroupNorm
+(op ``gn``) has no running state: a model without BatchNorm has ``n_total == n_vote``, every coordinate is voted on.
 Because parameters already live in one vector, the reference's ``parameters_to_vector`` / ``vector_to_parameters``
 round trips (src/federated.py:59,66,72; src/agent.py:35,56-63; src/aggregation.py:38-40) disappear.
 
@@ -34,7 +35,7 @@ TOTAL_ALIGN = 4096
 
 @dataclass
 class Node:
-    op: str                     # conv | bn | relu | maxpool | avgpool | flatten | dropout | linear | save | add
+    op: str                     # conv | bn | gn | relu | maxpool | avgpool | flatten | dropout | linear | save | add
     name: str = ""
     inp: str = "x"
     out: str = "x"
@@ -47,7 +48,7 @@ class ParamInfo:
     shape: tuple        # storage shape (OHWI for conv weights)
     offset: int
     numel: int
-    kind: str           # conv_w | linear_w | bias | bn_w | bn_b | bn_mean | bn_var
+    kind: str           # conv_w | linear_w | bias | bn_w | bn_b | bn_mean | bn_var | gn_w | gn_b
     node: int
 
 
@@ -84,6 +85,10 @@ class FlatLayout:
             elif nd.op == "bn":
                 add(self.params, nd.name + ".weight", (a["c"],), "bn_w", i)
                 add(self.params, nd.name + ".bias", (a["c"],), "bn_b", i)
+            elif nd.op == "gn":         # torch.nn.GroupNorm(groups, c, eps, affine=True): per-channel affine, no buffers
+                assert a["c"] % a["groups"] == 0, f"{nd.name}: {a['groups']} groups do not divide {a['c']} channels"
+                add(self.params, nd.name + ".weight", (a["c"],), "gn_w", i)
+                add(self.params, nd.name + ".bias", (a["c"],), "gn_b", i)
         self.n_params = sum(p.numel for p in self.params)        # true parameter count (reference n_model_params)
         self.n_vote = _ceil(off, TOTAL_ALIGN)
         off = self.n_vote
@@ -117,7 +122,7 @@ class FlatLayout:
             elif p.kind == "bias":
                 bound = 1.0 / math.sqrt(fan_in[p.node])
                 v.uniform_(-bound, bound, generator=gen)
-            elif p.kind == "bn_w":
+            elif p.kind in ("bn_w", "gn_w"):
                 v.fill_(1.0)
             else:
                 v.zero_()
@@ -230,6 +235,10 @@ class GraphNet(nn.Module):
                 rm, rv = self._bufs[nd.name + ".running_mean"], self._bufs[nd.name + ".running_var"]
                 t = F.batch_norm(t, rm, rv, self.P(nd.name + ".weight"), self.P(nd.name + ".bias"),
                                  self.training, a.get("momentum", 0.1), a.get("eps", 1e-5))
+            elif nd.op == "gn":
+                # fp32 statistics and affine whatever the compute dtype (the bf16 torch trainer), result cast back
+                t = F.group_norm(t.float(), a["groups"], self.P(nd.name + ".weight"), self.P(nd.name + ".bias"),
+                                 a.get("eps", 1e-5)).to(cd)
             elif nd.op == "relu":
                 t = F.relu(t)
             elif nd.op == "maxpool":

@@ -7,6 +7,7 @@ per-tensor optimizer state, no zero_grad (every gradient is overwritten).  The p
 
     conv(+bias)(+ReLU)            conv -> per-channel sum / sum^2 (BatchNorm statistics) in the GEMM epilogue
     BN(batch stats) + residual add + ReLU in one pass; BN backward in two (reduce, apply) passes
+    GroupNorm + residual add + ReLU in one kernel (per-sample statistics, no running state); its backward in one kernel + ordered sum
     avg-pool + flatten + linear head + softmax cross-entropy
 
 Each primitive has two back-ends selected per op in ``self.impl``: ``"sm100"`` -- the hand-written wgmma/TMA
@@ -60,7 +61,7 @@ def dropout_stream_base(seed: int, agent_id: int, rnd: int) -> int:
 
 
 def native_supported(layout: FlatLayout) -> bool:
-    return all(nd.op in ("conv", "bn", "relu", "maxpool", "avgpool", "flatten", "dropout", "linear", "save", "add")
+    return all(nd.op in ("conv", "bn", "gn", "relu", "maxpool", "avgpool", "flatten", "dropout", "linear", "save", "add")
                for nd in layout.nodes)
 
 
@@ -149,9 +150,9 @@ class NativeNet:
                 op.saved["want_stats"] = want_stats
                 op.y = new_out(nd.out, op.out_shape)
                 plan.append(op)
-            elif nd.op == "bn":
+            elif nd.op in ("bn", "gn"):
                 shp = shape[nd.inp]
-                op = _Op("bn", node=i, name=nd.name, attrs=a, x=src, in_shape=shp, out_shape=shp)
+                op = _Op(nd.op, node=i, name=nd.name, attrs=a, x=src, in_shape=shp, out_shape=shp)
                 j, nx = next_same_slot(i, nd.out)
                 if nx is not None and nx.op == "relu":
                     op.relu = True
@@ -167,7 +168,7 @@ class NativeNet:
                 other = alias.get(tid(a["other"]), tid(a["other"]))
                 op = pending_bn.pop(i, None)
                 if op is None:
-                    raise NotImplementedError("add without a preceding BatchNorm is not used by any model in the zoo")
+                    raise NotImplementedError("add without a preceding BatchNorm / GroupNorm is not used by any model in the zoo")
                 op.res = other
                 j, nx = next_same_slot(i, nd.out)
                 if nx is not None and nx.op == "relu":
@@ -273,6 +274,8 @@ class NativeNet:
             op.saved["mean_rstd"] = torch.zeros(2, c, dtype=torch.float32, device=dev)
             off += 2 * c
         for op in self.plan:
+            if op.kind == "gn":        # per-sample (mean, rstd) of every group for the backward pass; GroupNorm has no statistics arena
+                op.saved["mean_rstd"] = torch.zeros(B, 2, op.attrs["groups"], dtype=torch.float32, device=dev)
             if op.kind == "maxpool":
                 op.saved["idx"] = torch.empty((B, *op.out_shape), dtype=torch.uint8, device=dev)
                 if "drop" in op.saved and self.impl["pool"] != "sm100":
@@ -280,7 +283,7 @@ class NativeNet:
             if op.kind == "dropout":
                 op.saved["mask"] = torch.empty((B, *op.out_shape), dtype=torch.uint8, device=dev)
         self._bn_src = {}
-        # Side branch of a residual block with a projection shortcut (1x1 conv + BatchNorm on the block input): independent of the main
+        # Side branch of a residual block with a projection shortcut (1x1 conv + BatchNorm / GroupNorm on the block input): independent of the main
         # path until the fused bn2 + add, so in the forward pass it runs on a second stream forked where the block input is ready --
         # in the captured step graph a parallel branch whose small kernels fill the tails of the main path's conv waves.
         for i, op in enumerate(self.plan):
@@ -289,7 +292,7 @@ class NativeNet:
             nxt = self.plan[i + 1] if i + 1 < len(self.plan) else None
             first = next((q for q in self.plan[:i] if q.x == op.x and q is not op), None)            # the block's conv1 reads the same input
             join = next((q for q in self.plan[i + 1:] if nxt is not None and q.res == nxt.y), None)  # the fused bn2 + add
-            if nxt is None or nxt.kind != "bn" or nxt.x != op.y or first is None or join is None:
+            if nxt is None or nxt.kind not in ("bn", "gn") or nxt.x != op.y or first is None or join is None:
                 continue
             first.saved["fork_before"] = True
             op.saved["side_branch"] = nxt.saved["side_branch"] = True
@@ -391,7 +394,7 @@ class NativeNet:
             if branch and op.saved.get("fork_before"):
                 cur.wait_stream(self._branch_stream)
             if branch and op.saved.get("side_branch"):
-                if op.kind == "bn":
+                if op.kind in ("bn", "gn"):
                     self._branch_stream.wait_stream(cur)
                 with torch.cuda.stream(self._branch_stream):
                     getattr(self, "_bwd_" + op.kind)(op, B)
@@ -500,6 +503,20 @@ class NativeNet:
         ops.bn_bwd(dy, y, x, gamma, op.saved["mean_rstd"], op.saved["dsum"], dx, dres,
                    self.pg[op.name + ".weight"], self.pg[op.name + ".bias"], op.relu, self.impl["bn"], zero_dsum=False,
                    beta=self.pw[op.name + ".bias"])
+
+    # ---- group norm (+ residual + relu): same computation in training and evaluation -----------------------------------
+    # (the BatchNorm back-end key ``impl["bn"]`` selects the back-end of every normalisation layer)
+    def _fwd_gn(self, op, B, train):
+        a = op.attrs
+        res = self.T(op.res, B) if op.res is not None else None
+        ops.gn_fwd(self.T(op.x, B), self.T(op.y, B), res, self.pw[op.name + ".weight"], self.pw[op.name + ".bias"],
+                   op.saved["mean_rstd"][:B], a["groups"], a.get("eps", 1e-5), op.relu, self.impl["bn"])
+
+    def _bwd_gn(self, op, B):
+        dres = self.G(op.res, B) if op.res is not None else None
+        ops.gn_bwd(self.G(op.y, B), self.T(op.y, B), self.T(op.x, B), self.pw[op.name + ".weight"], op.saved["mean_rstd"][:B],
+                   self.G(op.x, B), dres, self.pg[op.name + ".weight"], self.pg[op.name + ".bias"], op.attrs["groups"], op.relu,
+                   self.impl["bn"], zero=False)
 
     # ---- pooling ---------------------------------------------------------------------------------------------------
     def _drop(self, op, train=True):
@@ -710,7 +727,8 @@ class NativeTrainer:
 
     @torch.no_grad()
     def eval_forward(self, w):
-        """Eval-mode forward of parameters ``w`` through the native executor (running BN statistics, no dropout)."""
+        """Eval-mode forward of parameters ``w`` through the native executor (running BN statistics, no dropout; GroupNorm layers
+        normalise exactly as in training)."""
         key = w.data_ptr()
         if key not in self._eval_nets:
             net = NativeNet(self.layout, self.device, self.bs, self.net.impl, seed=self.args.seed)

@@ -486,4 +486,4 @@ def eval_metrics(logits, labels, loss_sum, confusion):
 
 
 from .nn import (avgpool_bwd, avgpool_fwd, bn_bwd, bn_fwd, conv2d_dgrad_sm100, conv2d_fwd_sm100, conv2d_wgrad_sm100, conv_supported,  # noqa: E402,F401
-                 dropout_bwd, dropout_fwd, linear_bwd, linear_fused_dropout_ok, linear_fwd, maxpool2_bwd, maxpool2_fwd, relu_bwd_, scratch, stem_geometry, STAT_SLOTS)
+                 dropout_bwd, dropout_fwd, gn_bwd, gn_fwd, linear_bwd, linear_fused_dropout_ok, linear_fwd, maxpool2_bwd, maxpool2_fwd, relu_bwd_, scratch, stem_geometry, STAT_SLOTS)

@@ -120,6 +120,15 @@ cudaError_t launch_bn_bwd_reduce(const __nv_bfloat16* dy, const __nv_bfloat16* y
 cudaError_t launch_bn_bwd_apply(const __nv_bfloat16* dy, const __nv_bfloat16* y, const __nv_bfloat16* x, const float* gamma,
                                 const float* mean_rstd, const float* dsum, __nv_bfloat16* dx, __nv_bfloat16* dres, float* dgamma,
                                 float* dbeta, long long M, int C, int relu, int num_sms, cudaStream_t st, const float* beta = nullptr, int nslots = 1);
+// ---- groupnorm.cu: GroupNorm (torch.nn.GroupNorm(G, C, eps) semantics) on x[B][HW][C], C % 8 == 0, G | C ----------------
+// y = act((x - mean_ng) * rstd_ng * gamma_c + beta_c [+ res]); mean_rstd [B][2][G] (mean, rstd) for the backward pass
+cudaError_t launch_gn_fwd(const __nv_bfloat16* x, const __nv_bfloat16* res, __nv_bfloat16* y, const float* gamma, const float* beta,
+                          float* mean_rstd, int B, int HW, int C, int G, float eps, int relu, int num_sms, cudaStream_t st);
+// dz = dy * [y > 0] (relu) ; dres = dz (if non-null) ; dx = rstd * (dz*gamma - s_a/M - xhat * s_b/M) ;
+// dgamma += sum dz * xhat, dbeta += sum dz (per-sample partials added in sample order)
+cudaError_t launch_gn_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* y, const __nv_bfloat16* x, const float* gamma,
+                          const float* mean_rstd, __nv_bfloat16* dx, __nv_bfloat16* dres, float* dgamma, float* dbeta, int B, int HW,
+                          int C, int G, int relu, int num_sms, cudaStream_t st);
 // scale != 1: the output went through fused dropout (mask = y > 0 covers ReLU and dropout together)
 cudaError_t launch_relu_bwd(__nv_bfloat16* dy, const __nv_bfloat16* y, long long n, int num_sms, cudaStream_t st, float scale = 1.0f);
 // drop_p > 0: dropout fused into the pooling kernel (Philox keep-mask of the pooled element, recomputed by the backward kernel; no mask tensor)

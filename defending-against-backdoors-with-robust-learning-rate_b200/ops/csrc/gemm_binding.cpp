@@ -267,6 +267,29 @@ void bn_bwd_recompute(at::Tensor dy, at::Tensor x, at::Tensor gamma, at::Tensor 
                                    (float*)dgamma.data_ptr(), (float*)dbeta.data_ptr(), M, C, 2, num_sms(), cur_stream(),
                                    (const float*)beta.data_ptr(), nslots), "bn_bwd_apply(recompute)");
 }
+// GroupNorm on x [B,H,W,C]: gamma / beta fp32 [C]; mean_rstd fp32 [B,2,groups] (written here, read by gn_bwd)
+void gn_fwd(at::Tensor x, c10::optional<at::Tensor> res, at::Tensor y, at::Tensor gamma, at::Tensor beta, at::Tensor mean_rstd, int64_t groups,
+            double eps, bool relu) {
+    c10::cuda::CUDAGuard g(x.device());
+    TORCH_CHECK(x.dim() == 4 && y.sizes() == x.sizes() && (!res.has_value() || !res->defined() || res->sizes() == x.sizes()), "gn_fwd: shapes");
+    const int B = x.size(0), HW = x.size(1) * x.size(2), C = x.size(3);
+    TORCH_CHECK(gamma.numel() == C && beta.numel() == C && mean_rstd.numel() == (int64_t)B * 2 * groups, "gn_fwd: gamma/beta [C], mean_rstd [B,2,groups]");
+    check(rlr::launch_gn_fwd(bf(x), bfo(res), bfm(y), f32(gamma), f32(beta), f32(mean_rstd), B, HW, C, (int)groups, (float)eps, relu, num_sms(),
+                             cur_stream()), "gn_fwd");
+}
+// dgamma / dbeta (fp32 [C], slices of the flat gradient) are ADDED into; y is read only when relu
+void gn_bwd(at::Tensor dy, c10::optional<at::Tensor> y, at::Tensor x, at::Tensor gamma, at::Tensor mean_rstd, at::Tensor dx,
+            c10::optional<at::Tensor> dres, at::Tensor dgamma, at::Tensor dbeta, int64_t groups, bool relu) {
+    c10::cuda::CUDAGuard g(x.device());
+    TORCH_CHECK(x.dim() == 4 && dy.sizes() == x.sizes() && dx.sizes() == x.sizes(), "gn_bwd: shapes");
+    TORCH_CHECK(!relu || (y.has_value() && y->defined() && y->sizes() == x.sizes()), "gn_bwd: relu needs the forward output y");
+    TORCH_CHECK(!dres.has_value() || !dres->defined() || dres->sizes() == x.sizes(), "gn_bwd: dres shape");
+    const int B = x.size(0), HW = x.size(1) * x.size(2), C = x.size(3);
+    TORCH_CHECK(gamma.numel() == C && dgamma.numel() == C && dbeta.numel() == C && mean_rstd.numel() == (int64_t)B * 2 * groups,
+                "gn_bwd: gamma/dgamma/dbeta [C], mean_rstd [B,2,groups]");
+    check(rlr::launch_gn_bwd(bf(dy), relu ? bf(*y) : nullptr, bf(x), f32(gamma), f32(mean_rstd), bfm(dx), const_cast<__nv_bfloat16*>(bfo(dres)),
+                             f32(dgamma), f32(dbeta), B, HW, C, (int)groups, relu, num_sms(), cur_stream()), "gn_bwd");
+}
 void relu_bwd(at::Tensor dy, at::Tensor y, double scale) {
     c10::cuda::CUDAGuard g(dy.device());
     check(rlr::launch_relu_bwd(bfm(dy), bf(y), dy.numel(), num_sms(), cur_stream(), (float)scale), "relu_bwd");
@@ -386,6 +409,8 @@ void register_gemm_bindings(py::module_& m) {
     m.def("bn_apply", &bn_apply);
     m.def("bn_bwd", &bn_bwd);
     m.def("bn_bwd_recompute", &bn_bwd_recompute);
+    m.def("gn_fwd", &gn_fwd);
+    m.def("gn_bwd", &gn_bwd);
     m.def("relu_bwd", &relu_bwd, py::arg("dy"), py::arg("y"), py::arg("scale") = 1.0);
     m.def("maxpool2_fwd", &maxpool2_fwd, py::arg("x"), py::arg("y"), py::arg("idx"), py::arg("drop_p") = 0.0, py::arg("drop_seed") = 0,
           py::arg("drop_step") = py::none(), py::arg("drop_stream") = 0);

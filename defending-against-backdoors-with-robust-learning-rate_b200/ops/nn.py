@@ -7,6 +7,7 @@ Reference call sites these primitives replace (SURVEY.md 2.4 rows K2-K8): the ``
 BatchNorm / residual / average-pool primitives serve ResNet-18 and VGG-11, which the reference does not have."""
 from __future__ import annotations
 
+import math
 import os
 
 import torch
@@ -385,6 +386,71 @@ def bn_bwd(dy, y, x, gamma, mean_rstd, dsum, dx, dres, dgamma, dbeta, relu, impl
     M = dz.shape[0]
     dbeta.copy_(s0); dgamma.copy_(s1)
     dx.copy_((gamma * mean_rstd[1] * (dz - s0 / M - xhat * s1 / M)).reshape(dx.shape))
+
+
+# =====================================================================================================================
+# group norm (+ residual + relu)
+# =====================================================================================================================
+def gn_supported(x, groups):
+    """Shapes the GroupNorm kernels (groupnorm.cu) take: NHWC, C % 8 == 0, ``groups`` divides C, at most 2048 channels per group
+    rounded up to whole 8-channel vectors."""
+    C = x.shape[-1]
+    cpg = C // groups if groups > 0 and C % groups == 0 else 0
+    return x.dim() == 4 and C % 8 == 0 and cpg > 0 and (8 // math.gcd(8, cpg)) * cpg <= 2048
+
+
+def gn_fwd(x, y, res, gamma, beta, mean_rstd, groups, eps, relu, impl):
+    """y[B,H,W,C] = [ReLU]((x - mean_ng) * rstd_ng * gamma_c + beta_c [+ res]) with torch.nn.GroupNorm(groups, C, eps) statistics
+    (per sample and group over H x W x C/groups, biased variance); ``mean_rstd`` [B,2,groups] fp32 receives mean / rstd for
+    ``gn_bwd``.  Training and evaluation compute the same thing (no running state)."""
+    if impl == "sm100":
+        if gn_supported(x, groups):
+            _ext().gn_fwd(x, res, y, gamma, beta, mean_rstd, int(groups), float(eps), bool(relu))
+            return
+        _fallback("gn_fwd", f"shape={tuple(x.shape)} groups={groups}")
+    B, C = x.shape[0], x.shape[-1]
+    xg = x.float().reshape(B, -1, groups, C // groups)                               # [B, HW, G, C/G]
+    mean = xg.mean((1, 3))
+    var = xg.var((1, 3), unbiased=False)
+    rstd = torch.rsqrt(var + eps)
+    mean_rstd[:, 0].copy_(mean); mean_rstd[:, 1].copy_(rstd)
+    out = ((xg - mean[:, None, :, None]) * rstd[:, None, :, None]).reshape(B, -1, C) * gamma + beta
+    if res is not None:
+        out = out + res.float().reshape(B, -1, C)
+    if relu:
+        out = out.clamp_min(0)
+    y.copy_(out.reshape(y.shape))
+
+
+def gn_bwd(dy, y, x, gamma, mean_rstd, dx, dres, dgamma, dbeta, groups, relu, impl, zero=True):
+    """Backward of ``gn_fwd``: dz = dy * [y > 0] (relu) ; dres = dz (residual) ; dx = rstd * (dz*gamma - s_a/M - xhat * s_b/M) with
+    s_a = sum dz*gamma, s_b = sum dz*gamma*xhat per (sample, group) and M = H*W*C/groups ; dgamma = sum dz*xhat, dbeta = sum dz.
+    ``zero=False``: dgamma / dbeta are added into (the native plan's flat gradient is zeroed once per step)."""
+    if zero:
+        _zero(dgamma)
+        _zero(dbeta)
+    if impl == "sm100":
+        if gn_supported(x, groups):
+            _ext().gn_bwd(dy, y if relu else None, x, gamma, mean_rstd, dx, dres, dgamma, dbeta, int(groups), bool(relu))
+            return
+        _fallback("gn_bwd", f"shape={tuple(x.shape)} groups={groups}")
+    B, C = x.shape[0], x.shape[-1]
+    G, cpg = groups, C // groups
+    dz = dy.float().reshape(B, -1, C)
+    if relu:
+        dz = dz * (y.float().reshape(B, -1, C) > 0)
+    if dres is not None:
+        dres.copy_(dz.reshape(dres.shape))
+    mean, rstd = mean_rstd[:, 0], mean_rstd[:, 1]                                    # [B, G]
+    xhat = ((x.float().reshape(B, -1, G, cpg) - mean[:, None, :, None]) * rstd[:, None, :, None]).reshape(B, -1, C)
+    dgamma.add_((dz * xhat).sum((0, 1)))
+    dbeta.add_(dz.sum((0, 1)))
+    dzg = (dz * gamma).reshape(B, -1, G, cpg)
+    M = dzg.shape[1] * cpg
+    s_a = dzg.sum((1, 3))[:, None, :, None]
+    s_b = (dzg * xhat.reshape(B, -1, G, cpg)).sum((1, 3))[:, None, :, None]
+    d = rstd[:, None, :, None] * (dzg - s_a / M - xhat.reshape(B, -1, G, cpg) * s_b / M)
+    dx.copy_(d.reshape(dx.shape))
 
 
 def relu_bwd_(dy, y, impl, scale=1.0):

@@ -14,7 +14,7 @@ import torch
 DATASETS = ("fmnist", "fedemnist", "cifar10")
 AGGREGATORS = ("avg", "comed", "sign")
 PATTERNS = ("plus", "square", "copyright", "apple")
-MODELS = ("auto", "cnn_mnist", "cnn_cifar", "resnet18", "resnet34", "vgg11", "vgg16")
+MODELS = ("auto", "cnn_mnist", "cnn_cifar", "resnet18", "resnet34", "vgg11", "vgg16", "resnet18_gn", "resnet34_gn", "vgg11_gn", "vgg16_gn")
 
 
 def _default_device():

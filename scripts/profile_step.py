@@ -1,6 +1,8 @@
 """Per-kernel profile of one training step of the bench.py workload (ResNet-18, CIFAR shape, batch 256, one GPU).
 
-    python scripts/profile_step.py [--out DIR] [--replays N] [--bs 256]
+    python scripts/profile_step.py [--out DIR] [--replays N] [--bs 256] [--model resnet18]
+
+``--model`` profiles another zoo model in the same configuration (e.g. ``resnet18_gn``).
 
 Builds the engine exactly as ``bench.py`` does, runs one warm-up round (which captures the training-step CUDA graph), then
 replays the captured full-batch step ``--replays`` times under ``torch.profiler`` with CUDA activities.  The kernels inside the
@@ -144,6 +146,7 @@ def main():
     ap.add_argument("--replays", type=int, default=20)
     ap.add_argument("--bs", type=int, default=256)
     ap.add_argument("--train_size", type=int, default=50000)
+    ap.add_argument("--model", default="resnet18")
     a = ap.parse_args()
 
     import torch
@@ -159,7 +162,7 @@ def main():
     log = []
     install_recorder(ops.ext(), sms, log)
     ctx = init_distributed(None, None)
-    args = make_args(data="cifar10", model="resnet18", num_agents=1, agents_in_flight=0, local_ep=2, bs=a.bs, aggr="avg",
+    args = make_args(data="cifar10", model=a.model, num_agents=1, agents_in_flight=0, local_ep=2, bs=a.bs, aggr="avg",
                      robustLR_threshold=0, num_corrupt=0, poison_frac=0.0, agent_frac=1.0, pattern_type="plus",
                      synthetic=a.train_size, synthetic_val=1000, snap=10 ** 9, rounds=10 ** 9, log_dir="", trainer="auto",
                      backend="auto", dtype="bf16", seed=0)
@@ -233,7 +236,7 @@ def main():
         rows.append({"kernel": nm, "calls_per_step": cnt / a.replays, "us_per_step": us_step, "share": us_step / total_us})
     gemm_us = sum(r["us_per_step"] for r in rows if r["kernel"].startswith(KERNEL))
     gemm_flop = sum(r["flop"] for r in launches)
-    res = {"gpu": gpu, "replays": a.replays, "batch": a.bs, "step_ms_unprofiled": step_ms_unprofiled,
+    res = {"gpu": gpu, "model": a.model, "replays": a.replays, "batch": a.bs, "step_ms_unprofiled": step_ms_unprofiled,
            "kernel_us_per_step": total_us, "gemm_kernel_us_per_step": gemm_us, "gemm_kernel_share": gemm_us / total_us,
            "gemm_gflop_per_step": gemm_flop / 1e9, "gemm_tflops": gemm_flop / (gemm_us * 1e-6) / 1e12 if gemm_us else None,
            "conv_cluster": os.environ.get("RLR_CONV_CLUSTER", "default"), "kernels": rows, "gemm_shapes": shape_rows}
@@ -241,6 +244,7 @@ def main():
     with open(os.path.join(a.out, "profile_step.json"), "w") as f:
         json.dump(res, f, indent=1)
     md = [f"GPU: {gpu} (name, power limit, max SM clock)  ",
+          f"Model: {a.model}  ",
           f"Step (batch {a.bs}, graph replay, profiler off): {step_ms_unprofiled:.3f} ms; summed kernel time {total_us / 1e3:.3f} ms.  ",
           f"`{KERNEL}` (all instantiations): {gemm_us:.0f} us/step = {100 * gemm_us / total_us:.1f} % of kernel time, "
           f"{gemm_flop / 1e9:.0f} GFLOP/step, {res['gemm_tflops'] or 0:.0f} TFLOP/s.",

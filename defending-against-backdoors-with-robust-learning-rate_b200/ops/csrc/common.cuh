@@ -104,6 +104,50 @@ __global__ void __launch_bounds__(256) ordered_sum_cols_kernel(T* __restrict__ o
     if (warp == 0 && col < n) out[col] += s;
 }
 
+// Same sums again, for few columns (the BatchNorm / GroupNorm statistics: 2C <= 2048 columns of 256-528 parts).  There the staged
+// kernel runs on 4-32 CTAs and its chain is load latency, then warp 0's additions, then the next load: this one spreads the columns
+// over 4x more CTAs (8 columns each) and double-buffers 256-part chunks, so the loads of chunk k + 1 are in flight while lanes 0-7
+// of warp 0 add chunk k in part order.  Additions and rounding are those of ordered_sum_kernel.
+template <typename T>
+__global__ void __launch_bounds__(256) ordered_sum_narrow_kernel(T* __restrict__ out, const T* __restrict__ part, int nparts, long long n) {
+    constexpr int kCols = 8, kRows = 256 * 8 / kCols, kPerThread = kRows * kCols / 256;
+    __shared__ T tile[2][kRows][kCols];
+    pdl_wait();
+    pdl_trigger();
+    const int c = threadIdx.x % kCols, r0 = threadIdx.x / kCols;          // element q of a thread: part row r0 + 32 q, column c
+    const long long col = (long long)blockIdx.x * kCols + c;
+    const int nchunks = (nparts + kRows - 1) / kRows;
+    T v[kPerThread];
+    auto load = [&](int chunk) {
+#pragma unroll
+        for (int q = 0; q < kPerThread; ++q) {
+            const int j = chunk * kRows + r0 + (256 / kCols) * q;
+            v[q] = (j < nparts && col < n) ? part[(size_t)j * n + col] : T(0);
+        }
+    };
+    auto stage = [&](int buf) {
+#pragma unroll
+        for (int q = 0; q < kPerThread; ++q) tile[buf][r0 + (256 / kCols) * q][c] = v[q];
+    };
+    load(0);
+    stage(0);
+    __syncthreads();
+    T s = T(0);
+    for (int k = 0; k < nchunks; ++k) {
+        if (k + 1 < nchunks) load(k + 1);
+        if (threadIdx.x < kCols) {
+            const int rows = nparts - k * kRows < kRows ? nparts - k * kRows : kRows;
+            int r = 0;
+            if (k == 0) { s = tile[0][0][threadIdx.x]; r = 1; }
+#pragma unroll 8
+            for (; r < rows; ++r) s += tile[k & 1][r][threadIdx.x];
+        }
+        if (k + 1 < nchunks) stage((k + 1) & 1);
+        __syncthreads();
+    }
+    if (threadIdx.x < kCols && col < n) out[col] += s;
+}
+
 __device__ __forceinline__ unsigned long long gtimer() {     // nanosecond timer common to all SMs
     unsigned long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -260,6 +304,8 @@ __device__ __forceinline__ uint32_t dropout_keep8(const DropSpec& d, long long q
 
 template <typename T>
 inline cudaError_t launch_ordered_sum(T* out, const T* part, int nparts, long long n, cudaStream_t st) {
+    if (nparts >= 16 && n <= 2048)
+        return launch_kernel(ordered_sum_narrow_kernel<T>, dim3((unsigned)((n + 7) / 8)), dim3(256), (size_t)0, st, out, part, nparts, n);
     if (nparts >= 16)
         return launch_kernel(ordered_sum_cols_kernel<T>, dim3((unsigned)((n + 31) / 32)), dim3(256), (size_t)0, st, out, part, nparts, n);
     long long blocks = (n + 255) / 256;

@@ -11,14 +11,14 @@
 namespace rlr {
 
 struct bf8 { float v[8]; };
-__device__ __forceinline__ bf8 load8(const __nv_bfloat16* p) {
-    const uint4 u = *reinterpret_cast<const uint4*>(p);
+__device__ __forceinline__ bf8 unpack8(const uint4& u) {
     const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
     bf8 r;
 #pragma unroll
     for (int i = 0; i < 4; ++i) { const float2 f = __bfloat1622float2(h[i]); r.v[2 * i] = f.x; r.v[2 * i + 1] = f.y; }
     return r;
 }
+__device__ __forceinline__ bf8 load8(const __nv_bfloat16* p) { return unpack8(*reinterpret_cast<const uint4*>(p)); }
 __device__ __forceinline__ void store8(__nv_bfloat16* p, const bf8& r) {
     uint4 u;
     u.x = pack_bf16x2(r.v[0], r.v[1]); u.y = pack_bf16x2(r.v[2], r.v[3]);
@@ -36,8 +36,11 @@ static inline bool chan_ok(int C) { return C >= 8 && C <= 2048 && (C % 8) == 0 &
 // per-channel reductions:  out[0][c] += sum_r a(r,c),  out[1][c] += sum_r b(r,c)
 // MODE 0: a = x, b = x^2 (forward statistics)     MODE 1: a = dz, b = dz * xhat (backward)
 // ---------------------------------------------------------------------------------------------------------------------
-template <int MODE, bool kRecompute = false>
-__global__ void __launch_bounds__(256, MODE == 0 ? 4 : 3) channel_reduce_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy,
+// U rows per thread and iteration, all loads issued before the first use.  The grid (and so the partial-sum layout) is fixed by the
+// launchers at kCtasPerSm CTAs per SM; U and the register cap are chosen per residency so that every thread keeps as many 16-byte
+// loads in flight as its registers allow.  U never changes a thread's rows or their order of addition.
+template <int MODE, bool kRecompute, int U, int kCtasPerSm>
+__global__ void __launch_bounds__(256, kCtasPerSm) channel_reduce_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy,
                                                                const __nv_bfloat16* __restrict__ y, const float* __restrict__ mean_rstd,
                                                                float* __restrict__ part /*[gridDim.x][ncols] partial sums*/, long long M, int C, int relu,
                                                                const float* __restrict__ gamma = nullptr, const float* __restrict__ beta = nullptr,
@@ -60,9 +63,6 @@ __global__ void __launch_bounds__(256, MODE == 0 ? 4 : 3) channel_reduce_kernel(
             for (int i = 0; i < 8; ++i) { msc[i] = gamma[cg * 8 + i] * rs[i]; msh[i] = beta[cg * 8 + i] - mu[i] * msc[i]; }
         }
     }
-    // U rows per iteration with every load issued before the first use: one 16-byte load per thread in flight leaves the kernel
-    // far below the HBM roofline
-    constexpr int U = MODE == 0 ? 4 : 2;
     const long long stride = (long long)gridDim.x * rpi;
     for (long long r0 = (long long)blockIdx.x * rpi + ry; r0 < M; r0 += stride * U) {
         uint4 xr[U], dr[U], yr[U];
@@ -131,8 +131,10 @@ cudaError_t launch_channel_stats(const __nv_bfloat16* x, long long M, int C, flo
     const int rpi = 256 / (C / 8);
     const int grid = rows_grid(M, rpi * 8, num_sms, nslots >= 4 ? 4 : 2), ncols = only_sum ? C : 2 * C;
     Scratch part((size_t)grid * ncols * sizeof(float), st);
-    RLR_CUDA_CHECK(launch_kernel(channel_reduce_kernel<0, false>, dim3(grid), dim3(256), (size_t)rpi * 2 * C * sizeof(float), st, x, nullptr,
-                                 nullptr, nullptr, part.as<float>(), M, C, 0, nullptr, nullptr, only_sum ? C : 0));
+    const size_t smem = (size_t)rpi * 2 * C * sizeof(float);
+    auto kernel = nslots >= 4 ? channel_reduce_kernel<0, false, 4, 4> : channel_reduce_kernel<0, false, 8, 2>;
+    RLR_CUDA_CHECK(launch_kernel(kernel, dim3(grid), dim3(256), smem, st, x, nullptr, nullptr, nullptr, part.as<float>(), M, C, 0, nullptr,
+                                 nullptr, only_sum ? C : 0));
     return launch_ordered_sum(stats, part.as<float>(), grid, (long long)ncols, st);
 }
 cudaError_t launch_bn_bwd_reduce(const __nv_bfloat16* dy, const __nv_bfloat16* y, const __nv_bfloat16* x, const float* mean_rstd,
@@ -140,15 +142,16 @@ cudaError_t launch_bn_bwd_reduce(const __nv_bfloat16* dy, const __nv_bfloat16* y
                                  const float* beta, int nslots) {
     if (!chan_ok(C) || (relu == 2 && (!gamma || !beta)) || (relu == 1 && !y) || nslots < 1) return cudaErrorInvalidValue;
     const int rpi = 256 / (C / 8);
-    const int grid = rows_grid(M, rpi * 8, num_sms, nslots >= 3 ? 3 : 2);
+    const bool three = nslots >= 3;
+    const int grid = rows_grid(M, rpi * 8, num_sms, three ? 3 : 2);
     const size_t smem = (size_t)rpi * 2 * C * sizeof(float);
     Scratch part((size_t)grid * 2 * C * sizeof(float), st);
     if (relu == 2)
-        RLR_CUDA_CHECK(launch_kernel(channel_reduce_kernel<1, true>, dim3(grid), dim3(256), smem, st, x, dy, y, mean_rstd, part.as<float>(), M, C,
-                                     relu, gamma, beta, 0));
+        RLR_CUDA_CHECK(launch_kernel(three ? channel_reduce_kernel<1, true, 2, 3> : channel_reduce_kernel<1, true, 4, 2>, dim3(grid), dim3(256), smem,
+                                     st, x, dy, y, mean_rstd, part.as<float>(), M, C, relu, gamma, beta, 0));
     else
-        RLR_CUDA_CHECK(launch_kernel(channel_reduce_kernel<1, false>, dim3(grid), dim3(256), smem, st, x, dy, y, mean_rstd, part.as<float>(), M, C,
-                                     relu, nullptr, nullptr, 0));
+        RLR_CUDA_CHECK(launch_kernel(three ? channel_reduce_kernel<1, false, 2, 3> : channel_reduce_kernel<1, false, 4, 2>, dim3(grid), dim3(256), smem,
+                                     st, x, dy, y, mean_rstd, part.as<float>(), M, C, relu, nullptr, nullptr, 0));
     return launch_ordered_sum(dsum, part.as<float>(), grid, 2LL * C, st);
 }
 
@@ -177,28 +180,49 @@ cudaError_t launch_bn_finalize(const float* stats, int slots, float* mean_rstd, 
     return cudaGetLastError();
 }
 
-// fin.mode 0: mean/rstd are given.  1 (training): derive them from the raw per-channel sums `fin.stats` ([slots][2][C]) in every
-// thread (16 loads + rsqrt), CTA 0 also stores mean/rstd for the backward pass and updates the running statistics -- this replaces
-// the separate bn_finalize launch.  2 (evaluation): derive them from the running statistics.
+// fin.mode 0: mean/rstd are given.  1 (training): derive them from the raw per-channel sums `fin.stats` ([slots][2][C]); CTA 0 also
+// stores mean/rstd for the backward pass and updates the running statistics -- this replaces the separate bn_finalize launch.
+// 2 (evaluation): derive them from the running statistics.
 struct BnFinalize {
     int mode;
     const float* stats; int slots;
     float count, eps, momentum;
     float* running_mean; float* running_var;
 };
-template <int U, int kMinBlocks>
-__global__ void __launch_bounds__(256, kMinBlocks) bn_apply_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ res,
+
+// The two BatchNorm apply passes are elementwise once their per-channel constants are fixed, and stream 3-5 bytes of HBM per byte of
+// arithmetic input, so they are organised for memory-level parallelism:
+//  - every CTA derives the per-channel constants ONCE into shared memory (one thread per channel), then each thread copies its 8;
+//  - the grid is the resident one (kApplyCtasPerSm / kBwdCtasPerSm CTAs per SM, the __launch_bounds__ register caps) and every
+//    thread keeps U independent 16-byte loads per tensor in flight;
+//  - the rows are walked as 4 KB tiles of rpi rows (256 threads x 16 bytes) from the END of the tensor backwards: the pass that read
+//    the same tensors just before (channel statistics forward, the backward reduction backward) walked them forwards, so the tail it
+//    read last is what is still in L2 when this pass starts.
+// Traversal and unrolling do not touch the per-element and per-channel expressions, so the results are bit-identical to a one-row-
+// at-a-time loop in any order.
+constexpr int kApplyU = 4, kApplyCtasPerSm = 3;
+constexpr int kBwdU = 4, kBwdCtasPerSm = 2;
+
+// Tile t of the reversed walk, rows [(nt - 1 - t) * rpi, +rpi); `ok` is false past the end (t >= nt, or a row of the ragged last tile).
+__device__ __forceinline__ long long rev_tile_row(int t, int nt, int rpi, int ry, long long M, bool& ok) {
+    const long long r = (long long)(nt - 1 - t) * rpi + ry;
+    ok = t < nt && r < M;
+    return r;
+}
+static inline int apply_grid(long long M, int rpi, int U, int num_sms, int per_sm) {
+    const long long nt = (M + rpi - 1) / rpi;
+    return rows_grid(nt, U, num_sms, per_sm);
+}
+
+template <int U>
+__global__ void __launch_bounds__(256, kApplyCtasPerSm) bn_apply_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ res,
                                                          __nv_bfloat16* __restrict__ y, const float* __restrict__ gamma,
                                                          const float* __restrict__ beta, float* __restrict__ mean_rstd,
                                                          long long M, int C, int relu, BnFinalize fin) {
+    extern __shared__ float2 apply_cst[];     // [C] (scale, shift)
     pdl_wait();
     pdl_trigger();
-    const int tpr = C / 8, rpi = 256 / tpr;
-    const int cg = threadIdx.x % tpr, ry = threadIdx.x / tpr;
-    float sc[8], sh[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const int c = cg * 8 + i;
+    for (int c = threadIdx.x; c < C; c += blockDim.x) {
         float mean, rstd;
         if (fin.mode == 1) {
             float s1 = 0.f, s2 = 0.f;
@@ -206,7 +230,7 @@ __global__ void __launch_bounds__(256, kMinBlocks) bn_apply_kernel(const __nv_bf
             mean = s1 / fin.count;
             const float var = fmaxf(s2 / fin.count - mean * mean, 0.f);
             rstd = rsqrtf(var + fin.eps);
-            if (blockIdx.x == 0 && ry == 0) {
+            if (blockIdx.x == 0) {
                 mean_rstd[c] = mean; mean_rstd[C + c] = rstd;
                 fin.running_mean[c] = (1.f - fin.momentum) * fin.running_mean[c] + fin.momentum * mean;
                 const float unbiased = fin.count > 1.f ? var * fin.count / (fin.count - 1.f) : var;
@@ -217,25 +241,33 @@ __global__ void __launch_bounds__(256, kMinBlocks) bn_apply_kernel(const __nv_bf
         } else {
             mean = mean_rstd[c]; rstd = mean_rstd[C + c];
         }
-        sc[i] = gamma[c] * rstd;
-        sh[i] = beta[c] - mean * sc[i];
+        const float scale = gamma[c] * rstd;
+        apply_cst[c] = make_float2(scale, beta[c] - mean * scale);
     }
-    // U rows per thread in flight (all loads issued before the first use): one 16-byte load per thread and iteration leaves the kernel
-    // latency-bound (32 KB in flight per SM)
-    const long long stride = (long long)gridDim.x * rpi;
-    for (long long r0 = (long long)blockIdx.x * rpi + ry; r0 < M; r0 += stride * U) {
+    __syncthreads();
+    const int tpr = C / 8, rpi = 256 / tpr;
+    const int cg = threadIdx.x % tpr, ry = threadIdx.x / tpr;
+    float sc[8], sh[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { const float2 k = apply_cst[cg * 8 + i]; sc[i] = k.x; sh[i] = k.y; }
+    const int nt = (int)((M + rpi - 1) / rpi), G = gridDim.x;
+    for (int t0 = blockIdx.x; t0 < nt; t0 += G * U) {
         uint4 xr[U], rr[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-            const long long r = r0 + u * stride;
-            const size_t off = (size_t)(r < M ? r : r0) * C + cg * 8;
-            xr[u] = *reinterpret_cast<const uint4*>(x + off);
-            if (res) rr[u] = *reinterpret_cast<const uint4*>(res + off);
+            bool ok;
+            const long long r = rev_tile_row(t0 + u * G, nt, rpi, ry, M, ok);
+            if (ok) {
+                const size_t off = (size_t)r * C + cg * 8;
+                xr[u] = *reinterpret_cast<const uint4*>(x + off);
+                if (res) rr[u] = *reinterpret_cast<const uint4*>(res + off);
+            }
         }
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-            const long long r = r0 + u * stride;
-            if (r >= M) continue;
+            bool ok;
+            const long long r = rev_tile_row(t0 + u * G, nt, rpi, ry, M, ok);
+            if (!ok) continue;
             const __nv_bfloat162* xh = reinterpret_cast<const __nv_bfloat162*>(&xr[u]);
             const __nv_bfloat162* rh = reinterpret_cast<const __nv_bfloat162*>(&rr[u]);
             bf8 v;
@@ -256,68 +288,67 @@ cudaError_t launch_bn_apply(const __nv_bfloat16* x, const __nv_bfloat16* res, __
     if (!chan_ok(C)) return cudaErrorInvalidValue;
     const int rpi = 256 / (C / 8);
     BnFinalize fin{fin_mode, stats, slots, count, eps, momentum, running_mean, running_var};
-    // rows per thread in flight: 1 (default) | 4 (RLR_BN_UNROLL=4)
-    static const int unroll = [] { const char* e = getenv("RLR_BN_UNROLL"); return e ? atoi(e) : 1; }();
-    // RLR_BN_OCC=1: register caps that let one more CTA per SM be resident (more loads in flight through occupancy instead of unrolling)
-    static const int occ = [] { const char* e = getenv("RLR_BN_OCC"); return e ? atoi(e) : 0; }();
-    if (unroll <= 1 && occ)
-        return launch_kernel(bn_apply_kernel<1, 6>, dim3(rows_grid(M, rpi * 4, num_sms, 12)), dim3(256), (size_t)0, st, x, res, y, gamma, beta, mean_rstd,
-                             M, C, relu, fin);
-    if (unroll <= 1)
-        return launch_kernel(bn_apply_kernel<1, 1>, dim3(rows_grid(M, rpi * 4, num_sms, 8)), dim3(256), (size_t)0, st, x, res, y, gamma, beta, mean_rstd, M,
-                             C, relu, fin);
-    return launch_kernel(bn_apply_kernel<4, 1>, dim3(rows_grid(M, rpi * 4, num_sms, 6)), dim3(256), (size_t)0, st, x, res, y, gamma, beta, mean_rstd, M, C,
-                         relu, fin);
+    return launch_kernel(bn_apply_kernel<kApplyU>, dim3(apply_grid(M, rpi, kApplyU, num_sms, kApplyCtasPerSm)), dim3(256),
+                         (size_t)C * sizeof(float2), st, x, res, y, gamma, beta, mean_rstd, M, C, relu, fin);
 }
 
-template <bool kRecompute, int U, int kMinBlocks = 1>
-__global__ void __launch_bounds__(256, kMinBlocks) bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ y,
+template <bool kRecompute, int U>
+__global__ void __launch_bounds__(256, kBwdCtasPerSm) bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ y,
                                                              const __nv_bfloat16* __restrict__ x, const float* __restrict__ gamma,
                                                              const float* __restrict__ mean_rstd, const float* __restrict__ dsum,
                                                              __nv_bfloat16* __restrict__ dx, __nv_bfloat16* __restrict__ dres,
                                                              float* dgamma, float* dbeta, long long M, int C, int relu,
                                                              const float* __restrict__ beta = nullptr, int nslots = 1) {
+    extern __shared__ float bwd_cst[];        // [6][C]: mean, rstd, g = gamma * rstd, k1, k2, msh
     pdl_wait();
     pdl_trigger();
+    const float invM = 1.0f / (float)M;
+    for (int c = threadIdx.x; c < C; c += blockDim.x) {
+        const float mu = mean_rstd[c], rs = mean_rstd[C + c], g = gamma[c] * rs;
+        float s0 = 0.f, s1 = 0.f;
+        for (int k = 0; k < nslots; ++k) { s0 += dsum[(size_t)k * 2 * C + c]; s1 += dsum[(size_t)k * 2 * C + C + c]; }
+        const float k1 = s0 * invM, k2 = s1 * invM;
+        bwd_cst[c] = mu; bwd_cst[C + c] = rs; bwd_cst[2 * C + c] = g; bwd_cst[3 * C + c] = k1; bwd_cst[4 * C + c] = k2;
+        bwd_cst[5 * C + c] = kRecompute ? beta[c] - mu * g : 0.f;     // g = gamma * rstd is bn_apply's scale, msh its shift
+        if (blockIdx.x == 0) { dbeta[c] = k1 * (float)M; dgamma[c] = k2 * (float)M; }
+    }
+    __syncthreads();
     const int tpr = C / 8, rpi = 256 / tpr;
     const int cg = threadIdx.x % tpr, ry = threadIdx.x / tpr;
     float mu[8], rs[8], g[8], k1[8], k2[8], msh[8];
-    const float invM = 1.0f / (float)M;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
         const int c = cg * 8 + i;
-        mu[i] = mean_rstd[c]; rs[i] = mean_rstd[C + c]; g[i] = gamma[c] * rs[i];
-        float s0 = 0.f, s1 = 0.f;
-        for (int k = 0; k < nslots; ++k) { s0 += dsum[(size_t)k * 2 * C + c]; s1 += dsum[(size_t)k * 2 * C + C + c]; }
-        k1[i] = s0 * invM; k2[i] = s1 * invM;
-        msh[i] = kRecompute ? beta[c] - mu[i] * g[i] : 0.f;     // g = gamma * rstd is bn_apply's scale, msh its shift
+        mu[i] = bwd_cst[c]; rs[i] = bwd_cst[C + c]; g[i] = bwd_cst[2 * C + c]; k1[i] = bwd_cst[3 * C + c]; k2[i] = bwd_cst[4 * C + c];
+        msh[i] = bwd_cst[5 * C + c];
     }
-    if (blockIdx.x == 0 && ry == 0) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) { dbeta[cg * 8 + i] = k1[i] * (float)M; dgamma[cg * 8 + i] = k2[i] * (float)M; }
-    }
-    // U rows per thread in flight (see bn_apply_kernel)
-    const long long stride = (long long)gridDim.x * rpi;
-    for (long long r0 = (long long)blockIdx.x * rpi + ry; r0 < M; r0 += stride * U) {
-        bf8 dzv[U], xvv[U], yvv[U];
+    const bool need_y = !kRecompute && relu;
+    const int nt = (int)((M + rpi - 1) / rpi), G = gridDim.x;
+    for (int t0 = blockIdx.x; t0 < nt; t0 += G * U) {
+        uint4 dr[U], xr[U], yr[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-            const long long r = r0 + u * stride;
-            const size_t off = (size_t)(r < M ? r : r0) * C + cg * 8;
-            dzv[u] = load8(dy + off);
-            xvv[u] = load8(x + off);
-            if (!kRecompute && relu) yvv[u] = load8(y + off);
+            bool ok;
+            const long long r = rev_tile_row(t0 + u * G, nt, rpi, ry, M, ok);
+            if (ok) {
+                const size_t off = (size_t)r * C + cg * 8;
+                dr[u] = *reinterpret_cast<const uint4*>(dy + off);
+                xr[u] = *reinterpret_cast<const uint4*>(x + off);
+                if (need_y) yr[u] = *reinterpret_cast<const uint4*>(y + off);
+            }
         }
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-            const long long r = r0 + u * stride;
-            if (r >= M) continue;
+            bool ok;
+            const long long r = rev_tile_row(t0 + u * G, nt, rpi, ry, M, ok);
+            if (!ok) continue;
             const size_t off = (size_t)r * C + cg * 8;
-            bf8 dz = dzv[u];
-            const bf8 xv = xvv[u];
-            if (!kRecompute && relu) {
+            bf8 dz = unpack8(dr[u]);
+            const bf8 xv = unpack8(xr[u]);
+            if (need_y) {
+                const bf8 yv = unpack8(yr[u]);
 #pragma unroll
-                for (int i = 0; i < 8; ++i) dz.v[i] = yvv[u].v[i] > 0.f ? dz.v[i] : 0.f;
+                for (int i = 0; i < 8; ++i) dz.v[i] = yv.v[i] > 0.f ? dz.v[i] : 0.f;
             } else if (kRecompute) {
 #pragma unroll
                 for (int i = 0; i < 8; ++i) dz.v[i] = (xv.v[i] * g[i] + msh[i]) > 0.f ? dz.v[i] : 0.f;
@@ -335,28 +366,12 @@ cudaError_t launch_bn_bwd_apply(const __nv_bfloat16* dy, const __nv_bfloat16* y,
                                 float* dbeta, long long M, int C, int relu, int num_sms, cudaStream_t st, const float* beta, int nslots) {
     if (!chan_ok(C) || (relu == 2 && !beta) || (relu == 1 && !y) || nslots < 1) return cudaErrorInvalidValue;
     const int rpi = 256 / (C / 8);
-    const int grid = rows_grid(M, rpi * 4, num_sms, 8);
-    static const int unroll = [] { const char* e = getenv("RLR_BN_UNROLL"); return e ? atoi(e) : 1; }();     // see launch_bn_apply
-    if (unroll > 1) {
-        if (relu == 2)
-            return launch_kernel(bn_bwd_apply_kernel<true, 2>, dim3(grid), dim3(256), (size_t)0, st, dy, y, x, gamma, mean_rstd, dsum, dx, dres, dgamma,
-                                 dbeta, M, C, relu, beta, nslots);
-        return launch_kernel(bn_bwd_apply_kernel<false, 2>, dim3(grid), dim3(256), (size_t)0, st, dy, y, x, gamma, mean_rstd, dsum, dx, dres, dgamma, dbeta,
-                             M, C, relu, nullptr, nslots);
-    }
-    static const int occ = [] { const char* e = getenv("RLR_BN_OCC"); return e ? atoi(e) : 0; }();       // see launch_bn_apply
-    if (occ) {
-        const int grid2 = rows_grid(M, rpi * 4, num_sms, 12);
-        if (relu == 2)
-            return launch_kernel(bn_bwd_apply_kernel<true, 1, 4>, dim3(grid2), dim3(256), (size_t)0, st, dy, y, x, gamma, mean_rstd, dsum, dx, dres, dgamma,
-                                 dbeta, M, C, relu, beta, nslots);
-        return launch_kernel(bn_bwd_apply_kernel<false, 1, 4>, dim3(grid2), dim3(256), (size_t)0, st, dy, y, x, gamma, mean_rstd, dsum, dx, dres, dgamma,
-                             dbeta, M, C, relu, nullptr, nslots);
-    }
+    const dim3 grid(apply_grid(M, rpi, kBwdU, num_sms, kBwdCtasPerSm));
+    const size_t smem = (size_t)6 * C * sizeof(float);
     if (relu == 2)
-        return launch_kernel(bn_bwd_apply_kernel<true, 1>, dim3(grid), dim3(256), (size_t)0, st, dy, y, x, gamma, mean_rstd, dsum, dx, dres, dgamma, dbeta, M,
+        return launch_kernel(bn_bwd_apply_kernel<true, kBwdU>, grid, dim3(256), smem, st, dy, y, x, gamma, mean_rstd, dsum, dx, dres, dgamma, dbeta, M,
                              C, relu, beta, nslots);
-    return launch_kernel(bn_bwd_apply_kernel<false, 1>, dim3(grid), dim3(256), (size_t)0, st, dy, y, x, gamma, mean_rstd, dsum, dx, dres, dgamma, dbeta, M, C,
+    return launch_kernel(bn_bwd_apply_kernel<false, kBwdU>, grid, dim3(256), smem, st, dy, y, x, gamma, mean_rstd, dsum, dx, dres, dgamma, dbeta, M, C,
                          relu, nullptr, nslots);
 }
 

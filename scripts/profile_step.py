@@ -2,7 +2,8 @@
 
     python scripts/profile_step.py [--out DIR] [--replays N] [--bs 256] [--model resnet18]
 
-``--model`` profiles another zoo model in the same configuration (e.g. ``resnet18_gn``).
+``--model`` profiles another zoo model in the same configuration (e.g. ``resnet18_gn``).  ``--bn_reps`` sets the launches per call
+of the BatchNorm isolation and copy-reference measurements.
 
 Builds the engine exactly as ``bench.py`` does, runs one warm-up round (which captures the training-step CUDA graph), then
 replays the captured full-batch step ``--replays`` times under ``torch.profiler`` with CUDA activities.  The kernels inside the
@@ -11,6 +12,11 @@ microseconds per step, share of the step and, for the implicit-GEMM conv / GEMM 
 TFLOP/s per launch shape.  FLOP and bytes come from the launch shapes (``launch_record`` below), recorded by wrapping the
 extension's conv / GEMM entry points during the warm-up round.  The card's name, power limit and maximum SM clock are read in
 the same run (read-only nvidia-smi query).
+
+The BatchNorm family (statistics, apply, backward reduction, backward apply and the ordered sums of their partials) gets a table
+of its own, per launch shape: M, C, mode, the HBM bytes each pass must move and the achieved TB/s in the step; then the same calls
+replayed one at a time outside the graph (no concurrent side-stream kernels), and a device-to-device copy of the same bytes in the
+same session as the attainable bandwidth on that card at its power limit.
 """
 from __future__ import annotations
 
@@ -108,6 +114,185 @@ def install_recorder(ext, sms, log):
     return orig
 
 
+BN_KERNELS = ("channel_reduce_kernel", "bn_apply_kernel", "bn_bwd_apply_kernel", "ordered_sum")
+
+
+def bn_record(kind, x, C, relu=False, res=False, dres=False, recompute=False):
+    """One BatchNorm entry-point call: kind 'stats' | 'apply' | 'bwd' (reduction + apply), its shape, mode and HBM bytes per pass
+    (bf16 activations, E bytes each): statistics read x; apply reads x (and the residual) and writes y; the backward reduction reads
+    dy, x (and y for the mask unless it is recomputed from x); the backward apply reads the same and writes dx (and the residual
+    gradient)."""
+    M = x.numel() // C
+    E = 2 * M * C
+    mode = "+".join(m for m, on in (("relu", relu), ("res", res or dres), ("recompute", recompute)) if on) or "plain"
+    if kind == "stats":
+        passes = {"stats": E}
+    elif kind == "apply":
+        passes = {"apply": E * (3 if res else 2)}
+    else:
+        reads = E * (2 if recompute or not relu else 3)
+        passes = {"bwd_reduce": reads, "bwd_apply": reads + E * (2 if dres else 1)}
+    return {"kind": "bn-" + kind, "M": M, "C": C, "mode": mode, "relu": relu, "res": res, "dres": dres, "recompute": recompute,
+            "passes": passes}
+
+
+def install_bn_recorder(ext, log):
+    """Wrap the BatchNorm entry points like install_recorder does the GEMMs; ``advance_cursor`` appends a step delimiter."""
+    orig = {n: getattr(ext, n) for n in ("channel_stats", "bn_apply", "bn_bwd", "bn_bwd_recompute", "advance_cursor")}
+
+    def channel_stats(x, stats):
+        log.append(bn_record("stats", x, x.shape[-1]))
+        return orig["channel_stats"](x, stats)
+
+    def bn_apply(x, res, y, *a):
+        if a[4] == 1:                                                    # training (fin_mode 1); evaluation is not in the step
+            log.append(bn_record("apply", x, x.shape[-1], relu=bool(a[3]), res=res is not None))
+        return orig["bn_apply"](x, res, y, *a)
+
+    def bn_bwd(dy, y, x, gamma, mr, dsum, dx, dres, *a):
+        log.append(bn_record("bwd", x, x.shape[-1], relu=bool(a[2]), dres=dres is not None))
+        return orig["bn_bwd"](dy, y, x, gamma, mr, dsum, dx, dres, *a)
+
+    def bn_bwd_recompute(dy, x, *a):
+        log.append(bn_record("bwd", x, x.shape[-1], relu=True, recompute=True))
+        return orig["bn_bwd_recompute"](dy, x, *a)
+
+    def advance_cursor(*a, **k):
+        log.append(None)
+        return orig["advance_cursor"](*a, **k)
+
+    for n, f in (("channel_stats", channel_stats), ("bn_apply", bn_apply), ("bn_bwd", bn_bwd), ("bn_bwd_recompute", bn_bwd_recompute),
+                 ("advance_cursor", advance_cursor)):
+        setattr(ext, n, f)
+    return orig
+
+
+def bn_signature(r):
+    return (r["kind"], r["M"], r["C"], r["mode"])
+
+
+def _replay_bn_call(ext, r, dev, torch):
+    """Fresh tensors of the recorded shape; returns a closure that issues that one call (the same launches as in the step)."""
+    M, C = r["M"], r["C"]
+    g = torch.Generator(dev).manual_seed(M + C)
+    t = lambda: torch.randn(M, C, device=dev, generator=g).to(torch.bfloat16)  # noqa: E731
+    gamma, beta = torch.rand(C, device=dev) + 0.5, torch.randn(C, device=dev) * 0.1
+    mr = torch.stack([torch.zeros(C, device=dev), torch.ones(C, device=dev)])
+    if r["kind"] == "bn-stats":
+        x, stats = t(), torch.zeros(1, 2, C, device=dev)
+        return lambda: ext.channel_stats(x, stats)
+    if r["kind"] == "bn-apply":
+        x, res, y = t(), (t() if r["res"] else None), t()
+        stats = torch.stack([torch.zeros(C, device=dev), torch.full((C,), float(M), device=dev)])[None] * 1.0
+        rm, rv = torch.zeros(C, device=dev), torch.ones(C, device=dev)
+        return lambda: ext.bn_apply(x, res, y, gamma, beta, mr, r["relu"], 1, stats, float(M), 1e-5, 0.1, rm, rv)
+    dy, x, y, dx = t(), t(), t(), t()
+    dres = t() if r["dres"] else None
+    dsum, dg, db = torch.zeros(1, 2, C, device=dev), torch.zeros(C, device=dev), torch.zeros(C, device=dev)
+    if r["recompute"]:
+        return lambda: ext.bn_bwd_recompute(dy, x, gamma, beta, mr, dsum, dx, dg, db, True)
+    return lambda: ext.bn_bwd(dy, y, x, gamma, mr, dsum, dx, dres, dg, db, r["relu"], True)
+
+
+def _trace_kernels(prof):
+    with tempfile.TemporaryDirectory() as td:
+        path = os.path.join(td, "trace.json")
+        prof.export_chrome_trace(path)
+        trace = json.load(open(path))
+    return [e for e in trace.get("traceEvents", []) if e.get("cat") == "kernel"]
+
+
+def _pass_of(name):
+    if name.startswith("bn_apply_kernel"):
+        return "apply"
+    if name.startswith("bn_bwd_apply_kernel"):
+        return "bwd_apply"
+    if name.startswith("channel_reduce_kernel"):
+        return "stats" if name.startswith("channel_reduce_kernel<0") else "bwd_reduce"
+    return "sum"
+
+
+def isolate_bn(ext, sigs, reps, dev):
+    """Every distinct BatchNorm call of the step replayed alone (no concurrent side-stream kernels), ``reps`` times under the
+    profiler: per kernel (name, grid) its microseconds per call.  The same (name, grid) keys identify the launches in the step trace."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    out = {}
+    for sig, r in sigs.items():
+        call = _replay_bn_call(ext, r, dev, torch)
+        for _ in range(3):
+            call()
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(reps):
+                call()
+            torch.cuda.synchronize()
+        per = collections.defaultdict(float)
+        for e in _trace_kernels(prof):
+            nm = short_name(e["name"])
+            if nm.startswith(BN_KERNELS):
+                per[(nm, tuple(e.get("args", {}).get("grid", [0, 0, 0])[:1]))] += float(e["dur"]) / reps
+        out[sig] = dict(per)
+    return out
+
+
+def copy_reference(nbytes_list, reps, dev):
+    """Device-to-device copy moving the same bytes (half read, half written): microseconds per copy, CUDA events."""
+    import torch
+    res = {}
+    for nb in sorted(set(nbytes_list)):
+        n = max(1, nb // 4)                                      # bf16 elements per side: nb / 2 bytes read + nb / 2 written
+        src, dst = torch.ones(n, device=dev, dtype=torch.bfloat16), torch.empty(n, device=dev, dtype=torch.bfloat16)
+        for _ in range(3):
+            dst.copy_(src)
+        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        ev0.record()
+        for _ in range(reps):
+            dst.copy_(src)
+        ev1.record()
+        torch.cuda.synchronize()
+        res[nb] = ev0.elapsed_time(ev1) * 1e3 / reps
+    return res
+
+
+def bn_tables(bn_launches, kernels, replays, ext, dev, reps):
+    """Per launch shape of the BatchNorm family: bytes, in-step microseconds and TB/s, the same launch alone, and a copy of the same
+    bytes.  Rows are (kernel, grid) keys, as for the GEMM table; a key's launches are the step's calls that produce it."""
+    counts = collections.Counter(bn_signature(r) for r in bn_launches)
+    sigs = {bn_signature(r): r for r in bn_launches}
+    iso = isolate_bn(ext, sigs, reps, dev)
+    step = collections.defaultdict(lambda: [0, 0.0])
+    for e in kernels:
+        nm = short_name(e["name"])
+        if nm.startswith(BN_KERNELS):
+            k = (nm, tuple(e.get("args", {}).get("grid", [0, 0, 0])[:1]))
+            step[k][0] += 1
+            step[k][1] += float(e["dur"])
+    rows = []
+    for key, (cnt, us) in sorted(step.items(), key=lambda kv: -kv[1][1]):
+        owners = [(s, n) for s, n in counts.items() if key in iso.get(s, {})]
+        if not owners:                                           # an ordered sum of a non-BatchNorm user (weight gradients, loss)
+            continue
+        p = _pass_of(key[0])
+        per_launch = [(n, sigs[s]["passes"].get(p, 0)) for s, n in owners]       # the ordered sums: microseconds only
+        nbytes = sum(n * b for n, b in per_launch)
+        iso_us = sum(n * iso[s][key] for s, n in owners)
+        calls, us_step = cnt / replays, us / replays
+        matched = round(calls) == sum(n for _, n in owners)
+        rows.append({"kernel": key[0], "grid": key[1][0], "pass": p, "calls_per_step": calls, "us_per_step": us_step,
+                     "launches": sorted(f"{s[0][3:]} M{s[1]} C{s[2]} {s[3]} x{n}" for s, n in owners), "mb": nbytes / 1e6,
+                     "tb_s": nbytes / (us_step * 1e-6) / 1e12 if (matched and nbytes and us_step) else None,
+                     "iso_us": iso_us, "iso_tb_s": nbytes / (iso_us * 1e-6) / 1e12 if (nbytes and iso_us) else None,
+                     "_per_launch": per_launch})
+    cref = copy_reference([b for r in rows for _, b in r["_per_launch"] if b], reps, dev)
+    for r in rows:
+        cu = sum(n * cref[b] for n, b in r.pop("_per_launch") if b)
+        r["copy_us"] = cu or None
+        r["copy_tb_s"] = r["mb"] * 1e6 / (cu * 1e-6) / 1e12 if cu else None
+    return rows
+
+
 def one_step_launches(log):
     """Launch records of the first complete full-batch step in the log (an eager warm-up step before the graph is captured):
     the first step whose first launch has the most rows."""
@@ -147,6 +332,7 @@ def main():
     ap.add_argument("--bs", type=int, default=256)
     ap.add_argument("--train_size", type=int, default=50000)
     ap.add_argument("--model", default="resnet18")
+    ap.add_argument("--bn_reps", type=int, default=20, help="launches per BatchNorm call in the isolation and copy measurements")
     a = ap.parse_args()
 
     import torch
@@ -161,6 +347,8 @@ def main():
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     log = []
     install_recorder(ops.ext(), sms, log)
+    bn_log = []
+    install_bn_recorder(ops.ext(), bn_log)
     ctx = init_distributed(None, None)
     args = make_args(data="cifar10", model=a.model, num_agents=1, agents_in_flight=0, local_ep=2, bs=a.bs, aggr="avg",
                      robustLR_threshold=0, num_corrupt=0, poison_frac=0.0, agent_frac=1.0, pattern_type="plus",
@@ -193,12 +381,10 @@ def main():
             tr.cursor.zero_()
             graph.replay()
         torch.cuda.synchronize()
-    with tempfile.TemporaryDirectory() as td:
-        path = os.path.join(td, "trace.json")
-        prof.export_chrome_trace(path)
-        trace = json.load(open(path))
-    kernels = [e for e in trace.get("traceEvents", []) if e.get("cat") == "kernel"]
+    kernels = _trace_kernels(prof)
     gpu = gpu_info()
+    bn_launches = [r for r in one_step_launches(bn_log)] if any(bn_log) else []
+    bn_rows = bn_tables(bn_launches, kernels, a.replays, ops.ext(), torch.device("cuda", 0), a.bn_reps) if bn_launches else []
     eng.close()
 
     per_name = collections.defaultdict(lambda: [0, 0.0])
@@ -239,7 +425,8 @@ def main():
     res = {"gpu": gpu, "model": a.model, "replays": a.replays, "batch": a.bs, "step_ms_unprofiled": step_ms_unprofiled,
            "kernel_us_per_step": total_us, "gemm_kernel_us_per_step": gemm_us, "gemm_kernel_share": gemm_us / total_us,
            "gemm_gflop_per_step": gemm_flop / 1e9, "gemm_tflops": gemm_flop / (gemm_us * 1e-6) / 1e12 if gemm_us else None,
-           "conv_cluster": os.environ.get("RLR_CONV_CLUSTER", "default"), "kernels": rows, "gemm_shapes": shape_rows}
+           "conv_cluster": os.environ.get("RLR_CONV_CLUSTER", "default"), "kernels": rows, "gemm_shapes": shape_rows,
+           "bn_shapes": bn_rows}
     os.makedirs(a.out, exist_ok=True)
     with open(os.path.join(a.out, "profile_step.json"), "w") as f:
         json.dump(res, f, indent=1)
@@ -258,6 +445,26 @@ def main():
         bw = f'{r["l2_tb_s"]:.1f}' if r["l2_tb_s"] else "-"
         md.append(f'| `{r["kernel"].replace(KERNEL, "")}` | {r["grid"][0]}x{r["grid"][1]} | {r["calls_per_step"]:.0f} | '
                   f'{r["us_per_step"]:.1f} | {"; ".join(r["launches"]) or "-"} | {r["gflop"]:.1f} | {r["l2_mb"]:.0f} | {tf} | {bw} |')
+    if bn_rows:
+        fam = sum(r["us_per_step"] for r in bn_rows)
+        md += ["", f"BatchNorm family by launch shape (kernel, grid): {fam:.1f} us/step in the step. MB = HBM bytes the pass must move "
+               "(bf16 activations; the ordered sums of the partials: time only). *alone* = the same launches replayed one at a time "
+               "outside the graph; *copy* = a device-to-device copy of the same bytes in this session.", "",
+               "| kernel | grid | pass | calls/step | us/step | launches | MB | TB/s | alone us | alone TB/s | copy us | copy TB/s |",
+               "|---|---:|---|---:|---:|---|---:|---:|---:|---:|---:|---:|"]
+        f1 = lambda v, d=1: f"{v:.{d}f}" if v else "-"  # noqa: E731
+        for r in bn_rows:
+            md.append(f'| `{r["kernel"]}` | {r["grid"]} | {r["pass"]} | {r["calls_per_step"]:.0f} | {r["us_per_step"]:.1f} | '
+                      f'{"; ".join(r["launches"])} | {f1(r["mb"], 0)} | {f1(r["tb_s"], 2)} | {r["iso_us"]:.1f} | {f1(r["iso_tb_s"], 2)} | '
+                      f'{f1(r["copy_us"])} | {f1(r["copy_tb_s"], 2)} |')
+        by_pass = collections.defaultdict(lambda: [0.0, 0.0, 0.0])
+        for r in bn_rows:
+            by_pass[r["pass"]][0] += r["us_per_step"]
+            by_pass[r["pass"]][1] += r["iso_us"]
+            by_pass[r["pass"]][2] += r["mb"]
+        md += ["", "| pass | us/step in the step | us/step alone | MB/step | TB/s in the step | TB/s alone |", "|---|---:|---:|---:|---:|---:|"]
+        for p, (us, iso_us, mb) in by_pass.items():
+            md.append(f"| {p} | {us:.1f} | {iso_us:.1f} | {mb:.0f} | {f1(mb / us if mb else 0, 2)} | {f1(mb / iso_us if mb else 0, 2)} |")
     with open(os.path.join(a.out, "profile_step.md"), "w") as f:
         f.write("\n".join(md) + "\n")
     print("\n".join(md))

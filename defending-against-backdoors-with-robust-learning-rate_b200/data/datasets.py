@@ -88,9 +88,10 @@ class DeviceDataset:
         return torch.unique(self.targets)
 
     # -- batches -------------------------------------------------------------------------------
-    def batch(self, idxs: torch.Tensor, dtype=torch.float32, channels_last=False):
-        """Normalised batch for sample indices ``idxs``: ``(x, y)``; x is NCHW (or NHWC if channels_last)."""
-        x = ops.gather_normalize(self.data, idxs, self.meta.mean, self.meta.std, dtype=dtype, nhwc=channels_last)
+    def batch(self, idxs: torch.Tensor, dtype=torch.float32, channels_last=False, augment=None):
+        """Normalised batch for sample indices ``idxs``: ``(x, y)``; x is NCHW (or NHWC if channels_last).  ``augment``: an
+        ``ops.Augment`` whose ``start`` is the epoch position of ``idxs[0]`` (training batches only)."""
+        x = ops.gather_normalize(self.data, idxs, self.meta.mean, self.meta.std, dtype=dtype, nhwc=channels_last, augment=augment)
         return x, self.targets[idxs]
 
     def __getitem__(self, i):

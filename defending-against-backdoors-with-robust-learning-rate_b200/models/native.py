@@ -601,6 +601,9 @@ class NativeTrainer:
         # tiny-K first layer: the batch-assembly kernel writes the stem convolution's im2col matrix directly (gather_im2col)
         self.stem = self.net.stem_geometry()
         self.xA = torch.zeros(self.bs * self.stem[2] * self.stem[3], 64, dtype=ACT, device=device) if self.stem else None
+        # training augmentation (--crop_pad / --hflip): the Philox stream word of the current epoch, set before the graphs replay
+        self.aug_stream = torch.zeros(1, dtype=torch.int64, device=device)
+        self.aug = ops.training_augment(args, self.aug_stream)
         self._graphs = {}
         self._eval_nets = {}
         self.bcast = None             # round hand-off source (parallel.FusedAggregator) once attach_broadcast() was called
@@ -643,11 +646,11 @@ class NativeTrainer:
             k, pad, Ho, Wo = self.stem
             xin = self.xA[:B * Ho * Wo]
             ops.gather_im2col(dataset.data, self.perm, meta.mean, meta.std, k, pad, xin, cursor=self.cursor, targets=dataset.targets,
-                              out_labels=self.y, batch=B)
+                              out_labels=self.y, batch=B, augment=self.aug)
         else:
             xin = self.x[:B]
             ops.gather_normalize(dataset.data, self.perm, meta.mean, meta.std, out=xin, nhwc=True, cursor=self.cursor,
-                                 targets=dataset.targets, out_labels=self.y, batch=B)
+                                 targets=dataset.targets, out_labels=self.y, batch=B, augment=self.aug)
         logits = self.net.forward_raw(xin, True)                              # bf16 [B,classes], in the head's activation buffer
         _, dl = ops.softmax_xent(logits, self.y[:B], True, self.loss_sum, dlogits=self.net.dlogits_buffer(B))
         self.net.backward(dl)
@@ -702,6 +705,8 @@ class NativeTrainer:
         for ep in range(args.local_ep):
             idx = agent.epoch_indices(args.seed, rnd, ep)
             self.perm[:n].copy_(idx)
+            if self.aug is not None:
+                self.aug_stream.fill_(ops.augment_stream(args.seed, agent.id, rnd, ep))
             self.cursor.zero_()
             for b in range(n // bs):
                 is_first = fused and ep == 0 and b == 0

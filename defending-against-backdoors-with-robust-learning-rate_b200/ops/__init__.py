@@ -14,7 +14,9 @@ from __future__ import annotations
 import importlib.util
 import os
 import threading
+from typing import NamedTuple
 
+import numpy as np
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -124,13 +126,96 @@ def _i32(x, device):
 # =====================================================================================================================
 # data path
 # =====================================================================================================================
+_M32, _M64 = 2 ** 32 - 1, 2 ** 64 - 1
+
+
+def philox4x32(ctr, stream, key):
+    """Philox4x32-10 (Salmon et al., SC'11) with the packing of ``struct Philox`` in ops/csrc/common.cuh: counter words
+    ``(ctr lo, ctr hi, stream lo, stream hi)``, key words ``(key lo, key hi)``.  ``ctr``: an integer or an integer array (uint64
+    values); ``stream`` / ``key``: integers.  Returns the four output words as uint32 arrays of ``ctr``'s shape."""
+    ctr = np.asarray(ctr).astype(np.uint64)
+    stream, key = int(stream) & _M64, int(key) & _M64
+    m32 = np.uint64(_M32)
+    c0, c1 = ctr & m32, ctr >> np.uint64(32)
+    c2, c3 = np.full_like(ctr, stream & _M32), np.full_like(ctr, stream >> 32)
+    a, b = np.uint64(key & _M32), np.uint64(key >> 32)
+    for _ in range(10):
+        p0, p1 = c0 * np.uint64(0xD2511F53), c2 * np.uint64(0xCD9E8D57)       # 32 x 32 -> 64 bit, exact in uint64
+        c0, c1, c2, c3 = (p1 >> np.uint64(32)) ^ c1 ^ a, p1 & m32, (p0 >> np.uint64(32)) ^ c3 ^ b, p0 & m32
+        a, b = (a + np.uint64(0x9E3779B9)) & m32, (b + np.uint64(0xBB67AE85)) & m32
+    return tuple(w.astype(np.uint32) for w in (c0, c1, c2, c3))
+
+
+_AUGMENT_TAG = 0x6A09E667F3BCC908       # domain tag: keeps augmentation streams apart from every other Philox stream
+
+
+def augment_stream(seed: int, agent_id: int, rnd: int, epoch: int) -> int:
+    """Philox stream word of the training augmentation of (agent, round, local epoch): a splitmix64 hash in the style of
+    ``models.native.dropout_stream_base``.  It does not depend on the rank, trainer or world size, so an agent draws the same
+    crops wherever and alongside whatever it is trained.  Kept below 2^63 so it fits the device int64 word."""
+    z = (int(seed) * 0x9E3779B97F4A7C15 + (int(agent_id) + 1) * 0xBF58476D1CE4E5B9 + (int(rnd) + 1) * 0x94D049BB133111EB
+         + (int(epoch) + 1) * 0xD6E8FEB86659FD93 + _AUGMENT_TAG) & _M64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _M64
+    return (z ^ (z >> 31)) & (2 ** 63 - 1)
+
+
+class Augment(NamedTuple):
+    """Training augmentation of a gathered batch: ``RandomCrop(H x W, padding=pad, fill=0)`` then ``RandomHorizontalFlip()`` (when
+    ``flip``) of the raw images, before normalisation.  Sample b of a batch is at position p = (cursor, or ``start`` without a
+    cursor) + b of the epoch order and draws ``u = philox4x32(p, stream, seed)``: crop offsets ``u.x % (2 pad + 1)``,
+    ``u.y % (2 pad + 1)``, flip ``u.z & 1``.  ``stream``: one-element int64 tensor on the data's device holding the epoch's
+    ``augment_stream`` (the kernels read it at run time, so captured graphs follow it from epoch to epoch)."""
+    pad: int
+    flip: bool
+    seed: int
+    stream: torch.Tensor
+    start: int = 0
+
+
+def training_augment(args, stream):
+    """The ``Augment`` of the engine flags ``--crop_pad`` / ``--hflip`` over the trainer's stream word; None when both are off."""
+    pad, flip = int(getattr(args, "crop_pad", 0)), bool(getattr(args, "hflip", False))
+    return Augment(pad, flip, int(args.seed), stream) if (pad or flip) else None
+
+
+def augment_draws(aug: Augment, positions):
+    """``(oy, ox, flip)`` int64 tensors of the samples at ``positions`` (the host statement of ``augment_draw``, common.cuh)."""
+    u = philox4x32(np.asarray(positions, dtype=np.int64), int(aug.stream), aug.seed)
+    n = 2 * int(aug.pad) + 1
+    flip = (u[2] & 1).astype(np.int64) if aug.flip else np.zeros(len(u[2]), dtype=np.int64)
+    return (torch.from_numpy((u[0] % n).astype(np.int64)), torch.from_numpy((u[1] % n).astype(np.int64)), torch.from_numpy(flip))
+
+
+def augment_raw(x, aug: Augment, pos0: int):
+    """Cropped / flipped raw images ``[B,H,W,C]`` of the batch at positions ``pos0 ..`` (the CPU path of the augmented gathers):
+    ``aug[b,h,w] = x[b, h + oy - pad, w' + ox - pad]`` with ``w' = W-1-w`` when flipped, and 0 outside the image."""
+    B, H, W, _ = x.shape
+    oy, ox, fl = augment_draws(aug, pos0 + np.arange(B))
+    P = int(aug.pad)
+    xp = torch.nn.functional.pad(x, (0, 0, P, P, P, P))
+    w = torch.arange(W)
+    rows = torch.arange(H)[None, :] + oy[:, None]                                             # [B,H] in padded coordinates
+    cols = torch.where(fl[:, None].bool(), W - 1 - w[None, :], w[None, :]) + ox[:, None]      # [B,W]
+    return xp[torch.arange(B)[:, None, None], rows[:, :, None], cols[:, None, :]]
+
+
+def _augment_args(aug):
+    """Trailing (crop pad, flip, seed, stream word, start) arguments of the gather bindings."""
+    if aug is None:
+        return 0, False, 0, None, 0
+    seed = int(aug.seed) & _M64
+    return int(aug.pad), bool(aug.flip), seed - 2 ** 64 if seed >= 2 ** 63 else seed, aug.stream, int(aug.start)
+
+
 def gather_normalize(data, idxs, mean, std, dtype=torch.float32, nhwc=False, c_pad=None, out=None,
-                     cursor=None, targets=None, out_labels=None, batch=None):
+                     cursor=None, targets=None, out_labels=None, batch=None, augment=None):
     """``normalize(data[idxs])``: raw NHWC uint8/float pixels -> fp32/bf16 batch (SURVEY.md K1).
 
     ``data`` [N,H,W,C]; ``idxs`` int64 sample indices (with ``cursor``: a device int32 offset into ``idxs`` so a CUDA
     graph can replay the launch over successive batches; ``batch`` = batch size then).  Output NCHW, or NHWC padded to
     ``c_pad`` channels when ``nhwc``.  Same arithmetic as ``ToTensor`` + ``Normalize`` (src/utils.py:101,112-115).
+    ``augment``: an ``Augment`` -- the raw images are randomly cropped / flipped before normalisation.
     """
     N, H, W, C = data.shape
     B = int(batch if batch is not None else idxs.shape[0])
@@ -140,11 +225,13 @@ def gather_normalize(data, idxs, mean, std, dtype=torch.float32, nhwc=False, c_p
         out = torch.empty(shape, dtype=dtype, device=data.device)
     if data.is_cuda:
         ext().gather_normalize(data, idxs, cursor, targets, out, out_labels, B, c_pad, not nhwc,
-                               [float(m) for m in mean], [float(s) for s in std])
+                               [float(m) for m in mean], [float(s) for s in std], *_augment_args(augment))
         return out
     off = int(cursor.item()) if cursor is not None else 0
     sel = idxs[off:off + B]
     x = data[sel].to(torch.float32)
+    if augment is not None:
+        x = augment_raw(x, augment, off if cursor is not None else augment.start)
     if data.dtype == torch.uint8:
         x = x / 255.0
     x = (x - torch.tensor(mean, dtype=torch.float32)) / torch.tensor(std, dtype=torch.float32)
@@ -159,20 +246,23 @@ def gather_normalize(data, idxs, mean, std, dtype=torch.float32, nhwc=False, c_p
     return out
 
 
-def gather_im2col(data, idxs, mean, std, k, pad, out, cursor=None, targets=None, out_labels=None, batch=None):
+def gather_im2col(data, idxs, mean, std, k, pad, out, cursor=None, targets=None, out_labels=None, batch=None, augment=None):
     """Batch assembly fused with the first layer's im2col (SURVEY.md K1+K2, tiny-K stems: C*k*k <= 64): row (b, ho, wo) of ``out``
     [B*Ho*Wo, 64] (bf16) is the k x k x C patch of the normalised image around that output pixel in (tap, channel) order, zero
-    padded -- the A operand of the stem convolution as a single-k-block wgmma GEMM.  Same cursor / label contract as
-    ``gather_normalize``."""
+    padded -- the A operand of the stem convolution as a single-k-block wgmma GEMM.  Same cursor / label / ``augment`` contract as
+    ``gather_normalize``; the convolution's zero padding lies outside the augmented image and stays 0."""
     N, H, W, C = data.shape
     B = int(batch if batch is not None else idxs.shape[0])
     Ho, Wo = H + 2 * pad - k + 1, W + 2 * pad - k + 1
     if data.is_cuda:
-        ext().gather_im2col(data, idxs, cursor, targets, out, out_labels, B, int(k), int(pad), [float(m) for m in mean], [float(s) for s in std])
+        ext().gather_im2col(data, idxs, cursor, targets, out, out_labels, B, int(k), int(pad), [float(m) for m in mean], [float(s) for s in std],
+                            *_augment_args(augment))
         return out
     off = int(cursor.item()) if cursor is not None else 0
     sel = idxs[off:off + B]
     x = data[sel].to(torch.float32)
+    if augment is not None:
+        x = augment_raw(x, augment, off if cursor is not None else augment.start)
     if data.dtype == torch.uint8:
         x = x / 255.0
     x = (x - torch.tensor(mean, dtype=torch.float32)) / torch.tensor(std, dtype=torch.float32)          # [B,H,W,C]

@@ -85,13 +85,23 @@ void update_sqnorm(at::Tensor w_agent_ptrs, int64_t w_global_ptr, int64_t n, at:
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// training augmentation of the gathers: crop pad, flip, Philox key and the device int64 stream word (needed when either is on)
+inline const long long* aug_stream_ptr(const c10::optional<at::Tensor>& stream, int64_t crop_pad, bool flip) {
+    if (crop_pad == 0 && !flip) return nullptr;
+    TORCH_CHECK(stream.has_value() && stream->defined() && stream->is_cuda() && stream->scalar_type() == at::kLong,
+                "augmentation needs a CUDA int64 stream word");
+    return reinterpret_cast<const long long*>(stream->data_ptr());
+}
+
 void gather_normalize(at::Tensor data, at::Tensor idx, c10::optional<at::Tensor> cursor, c10::optional<at::Tensor> targets,
                       at::Tensor out, c10::optional<at::Tensor> out_labels, int64_t B, int64_t c_pad, bool nchw,
-                      std::vector<double> mean, std::vector<double> stdv) {
+                      std::vector<double> mean, std::vector<double> stdv, int64_t crop_pad, bool flip, int64_t seed,
+                      c10::optional<at::Tensor> aug_stream, int64_t start) {
     CHECK_CUDA(data); CHECK_CUDA(idx); CHECK_CUDA(out);
     TORCH_CHECK(data.dim() == 4 && idx.scalar_type() == at::kLong);
     const int H = data.size(1), W = data.size(2), C = data.size(3);
     TORCH_CHECK((int)mean.size() == C && (int)stdv.size() == C);
+    TORCH_CHECK(crop_pad >= 0 && crop_pad < H && crop_pad < W, "crop_pad must lie in [0, image side)");
     const int in_is_float = data.scalar_type() == at::kFloat;
     TORCH_CHECK(in_is_float || data.scalar_type() == at::kByte, "dataset must be uint8 or float32");
     const int out_kind = out.scalar_type() == at::kFloat ? 0 : 1;
@@ -103,16 +113,19 @@ void gather_normalize(at::Tensor data, at::Tensor idx, c10::optional<at::Tensor>
     check(rlr::launch_gather_normalize(data.data_ptr(), in_is_float, idx.data_ptr<int64_t>(), ptr_or_null<const int>(cursor),
                                        ptr_or_null<const int64_t>(targets), out.data_ptr(), out_kind,
                                        ptr_or_null<int64_t>(out_labels), (int)B, H, W, C, (int)c_pad, nchw ? 1 : 0, mu, sd,
-                                       cur_stream()), "gather_normalize");
+                                       (int)crop_pad, flip ? 1 : 0, (long long)seed, aug_stream_ptr(aug_stream, crop_pad, flip),
+                                       (long long)start, cur_stream()), "gather_normalize");
 }
 
 // gather + normalise + im2col: A[B*Ho*Wo][64] (bf16) for a k x k / pad stem convolution over data[N,H,W,C]  (C*k*k <= 64)
 void gather_im2col(at::Tensor data, at::Tensor idx, c10::optional<at::Tensor> cursor, c10::optional<at::Tensor> targets, at::Tensor A,
-                   c10::optional<at::Tensor> out_labels, int64_t B, int64_t k, int64_t pad, std::vector<double> mean, std::vector<double> stdv) {
+                   c10::optional<at::Tensor> out_labels, int64_t B, int64_t k, int64_t pad, std::vector<double> mean, std::vector<double> stdv,
+                   int64_t crop_pad, bool flip, int64_t seed, c10::optional<at::Tensor> aug_stream, int64_t start) {
     CHECK_CUDA(data); CHECK_CUDA(idx); CHECK_CUDA(A);
     TORCH_CHECK(data.dim() == 4 && idx.scalar_type() == at::kLong && A.scalar_type() == at::kBFloat16);
     const int H = data.size(1), W = data.size(2), C = data.size(3);
     TORCH_CHECK((int)mean.size() == C && (int)stdv.size() == C && C * k * k <= 64);
+    TORCH_CHECK(crop_pad >= 0 && crop_pad < H && crop_pad < W, "crop_pad must lie in [0, image side)");
     const int in_is_float = data.scalar_type() == at::kFloat;
     TORCH_CHECK(in_is_float || data.scalar_type() == at::kByte, "dataset must be uint8 or float32");
     const int64_t Ho = H + 2 * pad - k + 1, Wo = W + 2 * pad - k + 1;
@@ -122,7 +135,8 @@ void gather_im2col(at::Tensor data, at::Tensor idx, c10::optional<at::Tensor> cu
     c10::cuda::CUDAGuard guard(data.device());
     check(rlr::launch_gather_im2col(data.data_ptr(), in_is_float, idx.data_ptr<int64_t>(), ptr_or_null<const int>(cursor),
                                     ptr_or_null<const int64_t>(targets), reinterpret_cast<__nv_bfloat16*>(A.data_ptr()),
-                                    ptr_or_null<int64_t>(out_labels), (int)B, H, W, C, (int)k, (int)pad, mu, sd, cur_stream()), "gather_im2col");
+                                    ptr_or_null<int64_t>(out_labels), (int)B, H, W, C, (int)k, (int)pad, mu, sd, (int)crop_pad, flip ? 1 : 0,
+                                    (long long)seed, aug_stream_ptr(aug_stream, crop_pad, flip), (long long)start, cur_stream()), "gather_im2col");
 }
 
 void stamp_pixels(at::Tensor data, at::Tensor sel, at::Tensor rows, at::Tensor cols, at::Tensor vals, int64_t mode) {

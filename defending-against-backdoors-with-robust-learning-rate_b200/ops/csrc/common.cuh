@@ -286,6 +286,23 @@ __device__ __forceinline__ float4 philox_normal4(const Philox& ph, uint64_t ctr,
     return make_float4(r0 * c0, r0 * s0, r1 * c1, r1 * s1);
 }
 
+// ---- training augmentation (RandomCrop(padding = pad, fill 0) + RandomHorizontalFlip) ----------------------------------------------
+// The sample at position p of an agent's epoch order (cursor + b, not its dataset index) draws u = Philox(seed)(p, *stream), where
+// *stream is a device word the trainer sets once per epoch (ops.augment_stream).  Augmented pixel (h, w) reads stored pixel
+// (h + oy - pad, w' + ox - pad), w' = W-1-w when flipped, and stored value 0 outside the image.  ops.philox4x32 is the host twin.
+struct AugSpec {
+    const long long* stream;
+    unsigned long long seed;
+    long long start;                 // position of batch row 0 when no cursor is given
+    int pad, flip;
+};
+struct AugDraw { int oy, ox, flip; };
+__device__ __forceinline__ AugDraw augment_draw(const AugSpec& a, long long pos) {
+    const uint4 u = Philox(a.seed)((uint64_t)pos, (uint64_t)*a.stream);
+    const uint32_t n = 2u * (uint32_t)a.pad + 1u;
+    return {(int)(u.x % n), (int)(u.y % n), a.flip ? (int)(u.z & 1u) : 0};
+}
+
 // ---- fused dropout --------------------------------------------------------------------------------------------------------------
 // Keep-mask of a tensor viewed as a flat array of elements: the 8 elements [8 q, 8 q + 8) share ONE Philox4x32-10 call keyed by
 // (seed; counter q, stream = (step << 20) ^ node), 16 random bits per element, keep iff bits >= p * 65536.  Every kernel that produces

@@ -19,36 +19,50 @@ bool pdl_enabled() {
 
 // ------------------------------------------------------------------------------------------------------------
 // batch = normalize(dataset[perm[cursor : cursor+B]])   (uint8/float NHWC  ->  fp32/bf16, NCHW or padded NHWC)
+// AUG: the raw image is random-cropped / flipped first (augment_draw, common.cuh); AUG = false is the plain gather, and the
+// launchers pick it whenever crop pad and flip are both off, so un-augmented batches keep exactly the arithmetic they always had.
 // ------------------------------------------------------------------------------------------------------------
-template <typename TIn, typename TOut>
+template <typename TIn, typename TOut, bool AUG>
 __global__ void gather_normalize_kernel(const TIn* __restrict__ data, const int64_t* __restrict__ idx,
                                         const int* __restrict__ cursor, const int64_t* __restrict__ targets,
-                                        TOut* __restrict__ out, int64_t* __restrict__ out_labels, int B, int HW, int C,
-                                        int c_pad, int nchw, float4 mean, float4 inv_std, float in_scale) {
+                                        TOut* __restrict__ out, int64_t* __restrict__ out_labels, int B, int H, int W, int C,
+                                        int c_pad, int nchw, float4 mean, float4 inv_std, float in_scale, AugSpec aug) {
+    const int HW = H * W;
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= B * HW) return;
     const int b = t / HW, px = t - b * HW;
     const int64_t src = idx[(cursor ? *cursor : 0) + b];
     if (px == 0 && out_labels) out_labels[b] = targets[src];
     const TIn* in = data + (src * HW + px) * C;
+    bool inside = true;
+    if constexpr (AUG) {
+        const AugDraw d = augment_draw(aug, (cursor ? (long long)*cursor : aug.start) + b);
+        const int h = px / W, w = px - h * W;
+        const int sh = h + d.oy - aug.pad, sw = (d.flip ? W - 1 - w : w) + d.ox - aug.pad;
+        inside = sh >= 0 && sh < H && sw >= 0 && sw < W;
+        in = data + (src * HW + (inside ? sh * W + sw : 0)) * C;
+    }
+    auto raw = [&](int c) { return (AUG && !inside) ? 0.f : (float)in[c]; };
     const float mu[4] = {mean.x, mean.y, mean.z, mean.w};
     const float is[4] = {inv_std.x, inv_std.y, inv_std.z, inv_std.w};
     if (nchw) {
         for (int c = 0; c < C; ++c)
-            out[((int64_t)b * C + c) * HW + px] = (TOut)(((float)in[c] * in_scale - mu[c]) * is[c]);
+            out[((int64_t)b * C + c) * HW + px] = (TOut)((raw(c) * in_scale - mu[c]) * is[c]);
     } else {
         TOut* o = out + ((int64_t)b * HW + px) * c_pad;
-        for (int c = 0; c < C; ++c) o[c] = (TOut)(((float)in[c] * in_scale - mu[c]) * is[c]);
+        for (int c = 0; c < C; ++c) o[c] = (TOut)((raw(c) * in_scale - mu[c]) * is[c]);
         for (int c = C; c < c_pad; ++c) o[c] = (TOut)0.f;
     }
 }
 
 // Padded NHWC output (c_pad % 8 == 0, bf16): c_pad/8 threads per pixel, one 16-byte store each -> fully coalesced rows.
-template <typename TIn>
+template <typename TIn, bool AUG>
 __global__ void __launch_bounds__(256) gather_normalize_padded_kernel(const TIn* __restrict__ data, const int64_t* __restrict__ idx,
                                                                         const int* __restrict__ cursor, const int64_t* __restrict__ targets,
                                                                         __nv_bfloat16* __restrict__ out, int64_t* __restrict__ out_labels, int B,
-                                                                        int HW, int C, int c_pad, float4 mean, float4 inv_std, float in_scale) {
+                                                                        int H, int W, int C, int c_pad, float4 mean, float4 inv_std, float in_scale,
+                                                                        AugSpec aug) {
+    const int HW = H * W;
     const int cpp = c_pad >> 3;                                  // chunks per pixel
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)B * HW * cpp) return;
@@ -60,10 +74,18 @@ __global__ void __launch_bounds__(256) gather_normalize_padded_kernel(const TIn*
     uint4 v = make_uint4(0, 0, 0, 0);
     if (chunk == 0) {
         const TIn* in = data + (src * HW + px) * C;
+        bool inside = true;
+        if constexpr (AUG) {
+            const AugDraw d = augment_draw(aug, (cursor ? (long long)*cursor : aug.start) + b);
+            const int h = px / W, w = px - h * W;
+            const int sh = h + d.oy - aug.pad, sw = (d.flip ? W - 1 - w : w) + d.ox - aug.pad;
+            inside = sh >= 0 && sh < H && sw >= 0 && sw < W;
+            in = data + (src * HW + (inside ? sh * W + sw : 0)) * C;
+        }
         const float mu[4] = {mean.x, mean.y, mean.z, mean.w};
         const float is[4] = {inv_std.x, inv_std.y, inv_std.z, inv_std.w};
         float f[4] = {0.f, 0.f, 0.f, 0.f};
-        for (int c = 0; c < C; ++c) f[c] = ((float)in[c] * in_scale - mu[c]) * is[c];
+        for (int c = 0; c < C; ++c) f[c] = (((AUG && !inside) ? 0.f : (float)in[c]) * in_scale - mu[c]) * is[c];
         v.x = pack_bf16x2(f[0], f[1]); v.y = pack_bf16x2(f[2], f[3]);
     }
     *reinterpret_cast<uint4*>(out + pix * c_pad + chunk * 8) = v;
@@ -78,11 +100,14 @@ __global__ void __launch_bounds__(256) gather_normalize_padded_kernel(const TIn*
 // coalesced row reads per block and fully coalesced 128-byte row writes (a first version gathered bytes straight from global
 // memory: 67 us per 256-image batch, L1-wavefront bound; this one streams at the store rate).
 // CT / KT > 0: channel count / filter size known at compile time (index arithmetic becomes multiply-shift); 0 = run-time values.
-template <typename TIn, int CT, int KT>
+// AUG: the tile holds rows of the cropped / flipped image -- only the source coordinate of the staging loop moves, crop-padding
+// pixels are stored value 0 normalised (-mean/std), and the convolution's own zero border stays 0.
+template <typename TIn, int CT, int KT, bool AUG>
 __global__ void __launch_bounds__(256) gather_im2col_kernel(const TIn* __restrict__ data, const int64_t* __restrict__ idx,
                                                               const int* __restrict__ cursor, const int64_t* __restrict__ targets,
                                                               __nv_bfloat16* __restrict__ A, int64_t* __restrict__ out_labels, int B, int H, int W,
-                                                              int C_rt, int k_rt, int pad, int Ho, int Wo, float4 mean, float4 inv_std, float in_scale) {
+                                                              int C_rt, int k_rt, int pad, int Ho, int Wo, float4 mean, float4 inv_std, float in_scale,
+                                                              AugSpec aug) {
     extern __shared__ float tile[];                               // [k][W + 2 pad][C] normalised input rows, zero outside the image
     const int C = CT > 0 ? CT : C_rt, k = KT > 0 ? KT : k_rt;
     const int ho = blockIdx.x, b = blockIdx.y;
@@ -92,6 +117,13 @@ __global__ void __launch_bounds__(256) gather_im2col_kernel(const TIn* __restric
     const float mu[4] = {mean.x, mean.y, mean.z, mean.w};
     const float is[4] = {inv_std.x, inv_std.y, inv_std.z, inv_std.w};
     const TIn* img = data + src * (int64_t)H * W * C;
+    AugDraw d{0, 0, 0};
+    if constexpr (AUG) {            // one draw per block: in every warp the Philox rounds doubled the kernel's instruction count
+        __shared__ AugDraw sdraw;
+        if (threadIdx.x == 0) sdraw = augment_draw(aug, (cursor ? (long long)*cursor : aug.start) + b);
+        __syncthreads();
+        d = sdraw;
+    }
     for (int i = threadIdx.x; i < k * Wp * C; i += blockDim.x) {
         const int dy = i / (Wp * C), r = i - dy * (Wp * C);
         const int wp = r / C, ch = r - wp * C;
@@ -100,7 +132,13 @@ __global__ void __launch_bounds__(256) gather_im2col_kernel(const TIn* __restric
         if (hh >= 0 && hh < H && ww >= 0 && ww < W) {
             const float m = ch == 0 ? mu[0] : ch == 1 ? mu[1] : ch == 2 ? mu[2] : mu[3];
             const float s_ = ch == 0 ? is[0] : ch == 1 ? is[1] : ch == 2 ? is[2] : is[3];
-            v = ((float)img[(hh * W + ww) * C + ch] * in_scale - m) * s_;
+            if constexpr (AUG) {
+                const int sh = hh + d.oy - aug.pad, sw = (d.flip ? W - 1 - ww : ww) + d.ox - aug.pad;
+                const float x = (sh >= 0 && sh < H && sw >= 0 && sw < W) ? (float)img[(sh * W + sw) * C + ch] : 0.f;
+                v = (x * in_scale - m) * s_;
+            } else {
+                v = ((float)img[(hh * W + ww) * C + ch] * in_scale - m) * s_;
+            }
         }
         tile[i] = v;
     }
@@ -124,10 +162,18 @@ __global__ void __launch_bounds__(256) gather_im2col_kernel(const TIn* __restric
     }
 }
 
+static inline bool make_aug(AugSpec& a, int H, int W, int crop_pad, int flip, long long seed, const long long* stream, long long start) {
+    a = AugSpec{stream, (unsigned long long)seed, start, crop_pad, flip ? 1 : 0};
+    return crop_pad >= 0 && crop_pad < H && crop_pad < W && (!(crop_pad > 0 || flip) || stream);
+}
+
 cudaError_t launch_gather_im2col(const void* data, int in_is_float, const int64_t* idx, const int* cursor, const int64_t* targets,
                                  __nv_bfloat16* A, int64_t* out_labels, int B, int H, int W, int C, int k, int pad, const float* mean,
-                                 const float* stdv, cudaStream_t st) {
+                                 const float* stdv, int crop_pad, int flip, long long seed, const long long* aug_stream, long long start,
+                                 cudaStream_t st) {
     if (C > 4 || B <= 0 || k * k * C > 64) return cudaErrorInvalidValue;
+    AugSpec aug;
+    if (!make_aug(aug, H, W, crop_pad, flip, seed, aug_stream, start)) return cudaErrorInvalidValue;
     float mu[4] = {0, 0, 0, 0}, is[4] = {1, 1, 1, 1};
     for (int c = 0; c < C; ++c) { mu[c] = mean[c]; is[c] = 1.0f / stdv[c]; }
     const float4 m4 = make_float4(mu[0], mu[1], mu[2], mu[3]), s4 = make_float4(is[0], is[1], is[2], is[3]);
@@ -136,7 +182,15 @@ cudaError_t launch_gather_im2col(const void* data, int in_is_float, const int64_
     const size_t smem = (size_t)k * (W + 2 * pad) * C * sizeof(float);
     if (smem > 40 * 1024) return cudaErrorInvalidValue;
     const int threads = Wo * 8 >= 256 ? 256 : ((Wo * 8 + 31) / 32) * 32;
-#define RLR_GI(TI, CT, KT, SC) gather_im2col_kernel<TI, CT, KT><<<grid, threads, smem, st>>>((const TI*)data, idx, cursor, targets, A, out_labels, B, H, W, C, k, pad, Ho, Wo, m4, s4, SC)
+#define RLR_GI(TI, CT, KT, SC)                                                                                                        \
+    do {                                                                                                                               \
+        if (crop_pad > 0 || flip)                                                                                                      \
+            gather_im2col_kernel<TI, CT, KT, true><<<grid, threads, smem, st>>>((const TI*)data, idx, cursor, targets, A, out_labels,  \
+                                                                                B, H, W, C, k, pad, Ho, Wo, m4, s4, SC, aug);          \
+        else                                                                                                                           \
+            gather_im2col_kernel<TI, CT, KT, false><<<grid, threads, smem, st>>>((const TI*)data, idx, cursor, targets, A, out_labels, \
+                                                                                 B, H, W, C, k, pad, Ho, Wo, m4, s4, SC, aug);         \
+    } while (0)
     if (in_is_float) {
         if (C == 1 && k == 3) RLR_GI(float, 1, 3, 1.0f); else if (C == 3 && k == 3) RLR_GI(float, 3, 3, 1.0f); else RLR_GI(float, 0, 0, 1.0f);
     } else {
@@ -150,8 +204,12 @@ cudaError_t launch_gather_im2col(const void* data, int in_is_float, const int64_
 cudaError_t launch_gather_normalize(const void* data, int in_is_float, const int64_t* idx, const int* cursor,
                                     const int64_t* targets, void* out, int out_kind, int64_t* out_labels, int B, int H,
                                     int W, int C, int c_pad, int nchw, const float* mean, const float* stdv,
+                                    int crop_pad, int flip, long long seed, const long long* aug_stream, long long start,
                                     cudaStream_t st) {
     if (C > 4 || B <= 0) return cudaErrorInvalidValue;
+    AugSpec aug;
+    if (!make_aug(aug, H, W, crop_pad, flip, seed, aug_stream, start)) return cudaErrorInvalidValue;
+    const bool on = crop_pad > 0 || flip;
     float mu[4] = {0, 0, 0, 0}, is[4] = {1, 1, 1, 1};
     for (int c = 0; c < C; ++c) { mu[c] = mean[c]; is[c] = 1.0f / stdv[c]; }
     const float4 m4 = make_float4(mu[0], mu[1], mu[2], mu[3]), s4 = make_float4(is[0], is[1], is[2], is[3]);
@@ -160,13 +218,23 @@ cudaError_t launch_gather_normalize(const void* data, int in_is_float, const int
     if (!nchw && out_kind == 1 && c_pad > C && c_pad % 8 == 0) {      // channel-padded bf16 NHWC (stem input of the wgmma conv)
         const long long tot = (long long)total * (c_pad / 8);
         const int nb = (int)((tot + 255) / 256);
-        if (in_is_float) gather_normalize_padded_kernel<float><<<nb, 256, 0, st>>>((const float*)data, idx, cursor, targets, (__nv_bfloat16*)out, out_labels, B, HW, C, c_pad, m4, s4, sc);
-        else gather_normalize_padded_kernel<uint8_t><<<nb, 256, 0, st>>>((const uint8_t*)data, idx, cursor, targets, (__nv_bfloat16*)out, out_labels, B, HW, C, c_pad, m4, s4, sc);
+#define RLR_GP(TI, A_)                                                                                                                 \
+        gather_normalize_padded_kernel<TI, A_><<<nb, 256, 0, st>>>((const TI*)data, idx, cursor, targets, (__nv_bfloat16*)out,        \
+                                                                    out_labels, B, H, W, C, c_pad, m4, s4, sc, aug)
+        if (in_is_float) { if (on) RLR_GP(float, true); else RLR_GP(float, false); }
+        else             { if (on) RLR_GP(uint8_t, true); else RLR_GP(uint8_t, false); }
+#undef RLR_GP
         return cudaGetLastError();
     }
-#define RLR_GN(TI, TO)                                                                                          \
-    gather_normalize_kernel<TI, TO><<<blocks, threads, 0, st>>>((const TI*)data, idx, cursor, targets, (TO*)out, \
-                                                                 out_labels, B, HW, C, c_pad, nchw, m4, s4, sc)
+#define RLR_GN(TI, TO)                                                                                                    \
+    do {                                                                                                                  \
+        if (on) gather_normalize_kernel<TI, TO, true><<<blocks, threads, 0, st>>>((const TI*)data, idx, cursor, targets,  \
+                                                                                   (TO*)out, out_labels, B, H, W, C,      \
+                                                                                   c_pad, nchw, m4, s4, sc, aug);         \
+        else gather_normalize_kernel<TI, TO, false><<<blocks, threads, 0, st>>>((const TI*)data, idx, cursor, targets,    \
+                                                                                 (TO*)out, out_labels, B, H, W, C,        \
+                                                                                 c_pad, nchw, m4, s4, sc, aug);           \
+    } while (0)
     if (in_is_float) { if (out_kind == 0) RLR_GN(float, float); else RLR_GN(float, __nv_bfloat16); }
     else             { if (out_kind == 0) RLR_GN(uint8_t, float); else RLR_GN(uint8_t, __nv_bfloat16); }
 #undef RLR_GN

@@ -42,14 +42,18 @@ cudaError_t launch_update_sqnorm(const float* const* w_agents, const float* w_gl
 
 // ---- data path ---------------------------------------------------------------------------------------
 // out_kind: 0 fp32, 1 bf16.  nchw: output layout NCHW (Cpad ignored) else NHWC with channels padded to c_pad.
+// Both gathers: crop_pad > 0 or flip turns on the training augmentation (AugSpec, common.cuh): sample b of the batch is drawn
+// at position (cursor ? *cursor : start) + b from the Philox stream word *aug_stream under key seed.
 cudaError_t launch_gather_normalize(const void* data, int in_is_float, const int64_t* idx, const int* cursor,
                                     const int64_t* targets, void* out, int out_kind, int64_t* out_labels, int B, int H,
                                     int W, int C, int c_pad, int nchw, const float* mean, const float* stdv,
+                                    int crop_pad, int flip, long long seed, const long long* aug_stream, long long start,
                                     cudaStream_t st);
 // gather + normalise + im2col for the stem conv (C*k*k <= 64): A[B*Ho*Wo][64] bf16, (tap, channel) column order, zero padded
 cudaError_t launch_gather_im2col(const void* data, int in_is_float, const int64_t* idx, const int* cursor, const int64_t* targets,
                                  __nv_bfloat16* A, int64_t* out_labels, int B, int H, int W, int C, int k, int pad, const float* mean,
-                                 const float* stdv, cudaStream_t st);
+                                 const float* stdv, int crop_pad, int flip, long long seed, const long long* aug_stream, long long start,
+                                 cudaStream_t st);
 cudaError_t launch_stamp_pixels(void* data, int is_float, const int64_t* sel, int S, const int* rows, const int* cols,
                                 const float* vals, int P, int H, int W, int C, int mode, cudaStream_t st);
 cudaError_t launch_advance_cursor(int* cursor, int delta, long long* step /*optional: += 1*/, cudaStream_t st);

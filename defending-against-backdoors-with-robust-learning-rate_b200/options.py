@@ -85,6 +85,11 @@ def build_parser() -> argparse.ArgumentParser:
                    help="clip each update to L2 norm --clip on the server (reference clip_updates, dead code there)")
     p.add_argument("--no_graphs", action="store_true", help="do not capture the local step in CUDA graphs")
     p.add_argument("--profile_phases", action="store_true", help="print per-phase CUDA-event timings every round")
+    p.add_argument("--crop_pad", type=int, default=0,
+                   help="training augmentation: pad each image by this many zero pixels and take a random crop of the image size "
+                        "(torchvision RandomCrop(padding=P); the CIFAR-10 recipe is 4; 0 = off).  Local training only")
+    p.add_argument("--hflip", action="store_true",
+                   help="training augmentation: mirror each image left-right with probability 1/2 (local training only)")
     return p
 
 
@@ -99,6 +104,11 @@ def finalize_args(args: argparse.Namespace) -> argparse.Namespace:
         raise ValueError(f"unknown --aggr {args.aggr!r}; expected one of {AGGREGATORS}")
     if args.data not in DATASETS:
         raise ValueError(f"unknown --data {args.data!r}; expected one of {DATASETS}")
+    from .data.datasets import DATASET_META
+    meta = DATASET_META[args.data]
+    side = min(meta.height, meta.width)
+    if not 0 <= args.crop_pad < side:
+        raise ValueError(f"--crop_pad {args.crop_pad} must lie in [0, {side}) for --data {args.data} ({meta.height}x{meta.width} images)")
     return args
 
 
@@ -135,4 +145,5 @@ def print_exp_details(args) -> None:
     print(f"    Poison Frac: {args.poison_frac}")
     print(f"    Clip: {args.clip}")
     print(f"    Model / dtype / trainer / backend: {args.model} / {args.dtype} / {args.trainer} / {args.backend}")
+    print(f"    Crop pad / hflip: {args.crop_pad} / {args.hflip}")
     print("======================================")

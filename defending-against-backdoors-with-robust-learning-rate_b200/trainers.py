@@ -42,6 +42,9 @@ class TorchTrainer:
         self.max_shard = max_shard
         self._graphs = {}
         self._w0 = None
+        # training augmentation (--crop_pad / --hflip): the Philox stream word of the current epoch, set before the graphs replay
+        self.aug_stream = torch.zeros(1, dtype=torch.int64, device=device)
+        self.aug = ops.training_augment(args, self.aug_stream)
         if cuda:
             torch.backends.cudnn.benchmark = True
             self.perm = torch.zeros(max(1, max_shard), dtype=torch.int64, device=device)
@@ -61,7 +64,7 @@ class TorchTrainer:
     def _graph_body(self, dataset, B, w0):
         meta = dataset.meta
         ops.gather_normalize(dataset.data, self.perm, meta.mean, meta.std, out=self.x[:B], cursor=self.cursor,
-                             targets=dataset.targets, out_labels=self.y, batch=B)
+                             targets=dataset.targets, out_labels=self.y, batch=B, augment=self.aug)
         ops.ext().advance_cursor(self.cursor, B)
         self._step(self.x[:B], self.y[:B], w0)
 
@@ -107,6 +110,8 @@ class TorchTrainer:
         torch.manual_seed(_agent_round_seed(args.seed, agent.id, rnd))
         for ep in range(args.local_ep):
             idx = agent.epoch_indices(args.seed, rnd, ep)
+            if self.aug is not None:
+                self.aug_stream.fill_(ops.augment_stream(args.seed, agent.id, rnd, ep))
             if graphs:
                 self.perm[:n].copy_(idx)
                 self.cursor.zero_()
@@ -117,7 +122,8 @@ class TorchTrainer:
                 steps += (n + bs - 1) // bs
             else:
                 for start in range(0, n, bs):
-                    x, y = dataset.batch(idx[start:start + bs], dtype=torch.float32)
+                    aug = self.aug._replace(start=start) if self.aug is not None else None
+                    x, y = dataset.batch(idx[start:start + bs], dtype=torch.float32, augment=aug)
                     self._step(x, y, w_global)
                     steps += 1
         if out.data_ptr() != self.w.data_ptr():

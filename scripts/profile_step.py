@@ -332,6 +332,8 @@ def main():
     ap.add_argument("--bs", type=int, default=256)
     ap.add_argument("--train_size", type=int, default=50000)
     ap.add_argument("--model", default="resnet18")
+    ap.add_argument("--crop_pad", type=int, default=0, help="training augmentation of the profiled step (engine flag --crop_pad)")
+    ap.add_argument("--hflip", action="store_true", help="training augmentation of the profiled step (engine flag --hflip)")
     ap.add_argument("--bn_reps", type=int, default=20, help="launches per BatchNorm call in the isolation and copy measurements")
     a = ap.parse_args()
 
@@ -353,7 +355,7 @@ def main():
     args = make_args(data="cifar10", model=a.model, num_agents=1, agents_in_flight=0, local_ep=2, bs=a.bs, aggr="avg",
                      robustLR_threshold=0, num_corrupt=0, poison_frac=0.0, agent_frac=1.0, pattern_type="plus",
                      synthetic=a.train_size, synthetic_val=1000, snap=10 ** 9, rounds=10 ** 9, log_dir="", trainer="auto",
-                     backend="auto", dtype="bf16", seed=0)
+                     backend="auto", dtype="bf16", seed=0, crop_pad=a.crop_pad, hflip=a.hflip)
     eng = FLEngine(args, ctx=ctx, verbose=False)
     eng.run_round(1)                                   # captures the step graphs (and records one eager step's launches)
     eng.run_round(2)
@@ -422,7 +424,7 @@ def main():
         rows.append({"kernel": nm, "calls_per_step": cnt / a.replays, "us_per_step": us_step, "share": us_step / total_us})
     gemm_us = sum(r["us_per_step"] for r in rows if r["kernel"].startswith(KERNEL))
     gemm_flop = sum(r["flop"] for r in launches)
-    res = {"gpu": gpu, "model": a.model, "replays": a.replays, "batch": a.bs, "step_ms_unprofiled": step_ms_unprofiled,
+    res = {"gpu": gpu, "model": a.model, "crop_pad": a.crop_pad, "hflip": a.hflip, "replays": a.replays, "batch": a.bs, "step_ms_unprofiled": step_ms_unprofiled,
            "kernel_us_per_step": total_us, "gemm_kernel_us_per_step": gemm_us, "gemm_kernel_share": gemm_us / total_us,
            "gemm_gflop_per_step": gemm_flop / 1e9, "gemm_tflops": gemm_flop / (gemm_us * 1e-6) / 1e12 if gemm_us else None,
            "conv_cluster": os.environ.get("RLR_CONV_CLUSTER", "default"), "kernels": rows, "gemm_shapes": shape_rows,
@@ -431,7 +433,7 @@ def main():
     with open(os.path.join(a.out, "profile_step.json"), "w") as f:
         json.dump(res, f, indent=1)
     md = [f"GPU: {gpu} (name, power limit, max SM clock)  ",
-          f"Model: {a.model}  ",
+          f"Model: {a.model}, crop pad {a.crop_pad}, hflip {a.hflip}  ",
           f"Step (batch {a.bs}, graph replay, profiler off): {step_ms_unprofiled:.3f} ms; summed kernel time {total_us / 1e3:.3f} ms.  ",
           f"`{KERNEL}` (all instantiations): {gemm_us:.0f} us/step = {100 * gemm_us / total_us:.1f} % of kernel time, "
           f"{gemm_flop / 1e9:.0f} GFLOP/step, {res['gemm_tflops'] or 0:.0f} TFLOP/s.",

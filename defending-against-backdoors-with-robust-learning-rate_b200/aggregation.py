@@ -17,6 +17,12 @@ from . import ops
 from .models.graph import GraphNet
 
 
+def server_opt_spec(args):
+    """``ops.ServerOptState`` keyword arguments of the ``--server_opt*`` flags."""
+    return dict(kind=getattr(args, "server_opt", "sgd"), beta1=getattr(args, "server_beta1", 0.9),
+                beta2=getattr(args, "server_beta2", 0.99), tau=getattr(args, "server_tau", 1e-3))
+
+
 class Aggregation:
     def __init__(self, agent_data_sizes, n_params, poisoned_val, args, writer=None, layout=None, fused=None):
         self.agent_data_sizes = agent_data_sizes
@@ -29,6 +35,7 @@ class Aggregation:
         self.fused = fused            # parallel.FusedAggregator or None (pure in-process use)
         self.cum_net_mov = 0.0
         self.last_flipped = 0
+        self.opt = None               # full-length server optimizer state of the in-process form (allocated on first use)
 
     # ---- the server step ------------------------------------------------------------------------------------
     def aggregate_updates(self, w_global, agent_params, cur_round, n_vote=None):
@@ -40,10 +47,12 @@ class Aggregation:
         scales = self._clip_scales(ops.update_norms(w_global, ws, nv)) if self._server_clip else None
         prev = w_global.clone() if self.args.diagnostics else None
         flipped = torch.zeros(1, dtype=torch.int64, device=w_global.device)
+        if self.opt is None:
+            self.opt = ops.ServerOptState(n=w_global.numel(), device=w_global.device, **server_opt_spec(self.args))
         ops.fused_aggregate(w_global, ws, weights, self.args.aggr, self.args.robustLR_threshold, self.server_lr,
                             self.args.noise * self.args.clip, self.args.seed, cur_round,
                             n_vote if n_vote is not None else (self.layout.n_vote if self.layout else None),
-                            scales, out=w_global, flipped=flipped)
+                            scales, out=w_global, flipped=flipped, opt=self.opt)
         self.last_flipped = flipped
         if self.args.diagnostics:
             self.plot_norms(dict(zip(ids, ops.update_norms(prev, ws, nv).tolist())), cur_round)

@@ -24,14 +24,14 @@ import numpy as np
 import torch
 
 from .agent import Agent
-from .aggregation import Aggregation
+from .aggregation import Aggregation, server_opt_spec
 from .data import distribute_data, get_datasets, make_poisoned_val
 from .data.datasets import DeviceDataset, h5_to_device_dataset, load_fedemnist_client
 from .models import get_layout
 from .options import print_exp_details
 from .parallel import FusedAggregator, init_distributed
 from .trainers import make_trainer
-from .utils import MetricLogger, PhaseTimer, get_loss_n_accuracy, load_checkpoint, save_checkpoint
+from .utils import MetricLogger, PhaseTimer, get_loss_n_accuracy, load_checkpoint, restore_server_opt, save_checkpoint
 
 
 class FLEngine:
@@ -86,7 +86,8 @@ class FLEngine:
         if backend == "auto" and ctx.is_dist and ctx.backend == "gloo":
             backend = "gloo"
         self.fused = FusedAggregator(ctx, self.layout.n_total, self.layout.n_vote, max_slots, backend,
-                                     transport=getattr(args, "agg_transport", "auto"))
+                                     transport=getattr(args, "agg_transport", "auto"), server_opt=server_opt_spec(args),
+                                     n_part=self.n_part)
         init = torch.zeros(self.layout.n_total, dtype=torch.float32)
         self.layout.init_(init, args.seed)
         self.fused.w_global.copy_(init.to(dev))
@@ -131,6 +132,7 @@ class FLEngine:
         self._stream_src = None
         if args.resume:
             ck = load_checkpoint(args.resume, self.w_global, self.layout)
+            restore_server_opt(ck, self.fused)
             self.start_round = ck["round"] + 1
             self.cum_poison_acc_mean = ck["extra"].get("cum_poison_acc_mean", 0.0)
         ctx.barrier()
@@ -314,9 +316,12 @@ class FLEngine:
                 print({k: round(v, 3) for k, v in rec.items() if k.startswith("ms_")})
             self.logger.record(rnd, **rec)
             history.append({"round": rnd, **rec})
-            if args.checkpoint and self.ctx.is_main and ((args.ckpt_every and rnd % args.ckpt_every == 0) or rnd == rounds):
-                save_checkpoint(args.checkpoint, self.global_params(), rnd, args, self.layout,
-                                {"cum_poison_acc_mean": self.cum_poison_acc_mean})
+            if args.checkpoint and ((args.ckpt_every and rnd % args.ckpt_every == 0) or rnd == rounds):
+                state = self.fused.server_opt_state()      # every rank takes part: each holds one slice on the fused multi-GPU path
+                if self.ctx.is_main:
+                    so = None if state is None else {**self.fused.opt.hparams, "m": state[0], "v": state[1]}
+                    save_checkpoint(args.checkpoint, self.global_params(), rnd, args, self.layout,
+                                    {"cum_poison_acc_mean": self.cum_poison_acc_mean}, so)
         if self.verbose:
             print("Training has finished!")
         return history

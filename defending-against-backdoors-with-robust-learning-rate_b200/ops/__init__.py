@@ -27,6 +27,7 @@ _lock = threading.Lock()
 
 MODE_IDS = {"avg": 0, "comed": 1, "sign": 2}
 MAX_FUSED_AGENTS = 1024   # kMaxAgents of ops/csrc/aggregate.cu (participant tables of the fused kernel)
+SERVER_OPTS = {"sgd": 0, "momentum": 1, "adagrad": 2, "adam": 3, "yogi": 4}   # AggParams::opt of ops/csrc/aggregate.cu
 
 
 class _Counter:
@@ -303,12 +304,81 @@ def stamp_pixels(data, sel, rows, cols, vals, mode):
 # =====================================================================================================================
 # server step
 # =====================================================================================================================
+class ServerOptState:
+    """Server optimizer (``--server_opt``) and its state over coordinates ``[base, base + n)`` of the flat vector.
+
+    ``m`` (every kind but sgd) starts at 0 and ``v`` (adagrad / adam / yogi) at ``tau**2``; both are fp32 and rounded once per round.
+    sgd holds no state.  The update rules are in ``server_opt_step``."""
+
+    def __init__(self, kind="sgd", n=0, beta1=0.9, beta2=0.99, tau=1e-3, device="cpu", base=0):
+        if kind not in SERVER_OPTS:
+            raise ValueError(f"unknown server optimizer {kind!r}; expected one of {tuple(SERVER_OPTS)}")
+        self.kind, self.beta1, self.beta2, self.tau, self.base = kind, float(beta1), float(beta2), float(tau), int(base)
+        self.m = torch.zeros(n, dtype=torch.float32, device=device) if kind != "sgd" else None
+        self.v = torch.full((n,), self.tau * self.tau, dtype=torch.float32, device=device) if kind in ("adagrad", "adam", "yogi") else None
+
+    @property
+    def hparams(self):
+        return {"server_opt": self.kind, "beta1": self.beta1, "beta2": self.beta2, "tau": self.tau}
+
+
+def server_opt_step(d, opt):
+    """fp64 server optimizer on the pseudo-gradient ``d`` of coordinates ``[opt.base, opt.base + len(d))`` (Reddi et al., Adaptive
+    Federated Optimization, Algorithm 2, without bias correction; FedAvgM for momentum).  Returns the step that the server lr
+    scales; the new state is rounded into ``opt.m`` / ``opt.v`` while the step uses the unrounded fp64 values.  Also the statement
+    of the kernel's epilogue (``server_step`` in ops/csrc/aggregate.cu)."""
+    b1, b2 = opt.beta1, opt.beta2
+    m0 = opt.m[: d.numel()]
+    if opt.kind == "momentum":
+        m1 = b1 * m0.double() + d
+        m0.copy_(m1)
+        return m1
+    m1 = b1 * m0.double() + (1.0 - b1) * d
+    v0, d2 = opt.v[: d.numel()].double(), d * d
+    if opt.kind == "adagrad":
+        v1 = v0 + d2
+    elif opt.kind == "adam":
+        v1 = b2 * v0 + (1.0 - b2) * d2
+    elif opt.kind == "yogi":
+        v1 = v0 - (1.0 - b2) * d2 * torch.sign(v0 - d2)
+    else:
+        raise ValueError(opt.kind)
+    m0.copy_(m1)
+    opt.v[: d.numel()].copy_(v1)
+    return m1 / (v1.sqrt() + opt.tau)
+
+
+def _server_update(g, agg, signs, mean_tail, theta, server_lr, n_vote, opt):
+    """RLR flip + server step (sgd, or ``opt``'s optimizer) on the voted coordinates, plain weighted mean behind ``n_vote``."""
+    n = g.numel()
+    lr = torch.full_like(g, float(server_lr))
+    flipped = 0
+    neg = None
+    if theta > 0:
+        neg = signs.abs() < theta
+        neg[n_vote:] = False
+        lr[neg] = -float(server_lr)
+        flipped = int(neg.sum())
+    if opt is None or opt.kind == "sgd":
+        new = g + lr * agg
+    else:
+        if opt.base != 0:
+            raise ValueError("the fp64 server step needs the full-length optimizer state (base 0)")
+        d = agg[:n_vote] if neg is None else torch.where(neg[:n_vote], -agg[:n_vote], agg[:n_vote])
+        new = g.clone()
+        new[:n_vote] = g[:n_vote] + float(server_lr) * server_opt_step(d, opt)
+    if n_vote < n:
+        new[n_vote:] = g[n_vote:] + mean_tail[n_vote:]
+    return new.float(), flipped
+
+
 def aggregate_oracle(w_global, w_agents, weights, mode="avg", theta=0, server_lr=1.0, noise=None, n_vote=None,
-                     scales=None):
+                     scales=None, opt=None):
     """fp64 PyTorch statement of the server step (reference src/aggregation.py:19-75).
 
     ``w_agents``: list of local parameter vectors; updates are ``w_k - w_global``.  ``noise``: optional pre-sampled
     noise vector (added to the aggregate BEFORE the lr multiply).  Coordinates ``>= n_vote`` get a plain weighted mean.
+    ``opt``: optional ``ServerOptState`` (full length); its state is updated in place.
     Returns ``(new_global_fp32, n_flipped)``.
     """
     g = w_global.double()
@@ -331,17 +401,7 @@ def aggregate_oracle(w_global, w_agents, weights, mode="avg", theta=0, server_lr
         raise ValueError(mode)
     if noise is not None:
         agg = agg + noise.double()
-    lr = torch.full_like(g, float(server_lr))
-    flipped = 0
-    if theta > 0:
-        neg = signs.abs() < theta
-        neg[n_vote:] = False
-        lr[neg] = -float(server_lr)
-        flipped = int(neg.sum())
-    new = g + lr * agg
-    if n_vote < n:
-        new[n_vote:] = g[n_vote:] + mean_raw[n_vote:]
-    return new.float(), flipped
+    return _server_update(g, agg, signs, mean_raw, theta, server_lr, n_vote, opt)
 
 
 def aggregate_partials(w_global, w_local_agents, local_weights, n_vote=None, scales=None):
@@ -362,7 +422,8 @@ def aggregate_partials(w_global, w_local_agents, local_weights, n_vote=None, sca
     return vote, wsum
 
 
-def aggregate_from_partials(w_global, vote, wsum, total_weight, mode="avg", theta=0, server_lr=1.0, noise=None, n_vote=None):
+def aggregate_from_partials(w_global, vote, wsum, total_weight, mode="avg", theta=0, server_lr=1.0, noise=None, n_vote=None,
+                            opt=None):
     """Finish the server step from globally reduced partials (same formulas and order as ``aggregate_oracle``; avg / sign only)."""
     if mode not in ("avg", "sign"):
         raise ValueError(f"aggregate_from_partials: mode {mode!r} is not additive (coordinate median needs every update)")
@@ -374,17 +435,7 @@ def aggregate_from_partials(w_global, vote, wsum, total_weight, mode="avg", thet
     agg = mean.clone() if mode == "avg" else torch.sign(signs)
     if noise is not None:
         agg = agg + noise.double()
-    lr = torch.full_like(g, float(server_lr))
-    flipped = 0
-    if theta > 0:
-        neg = signs.abs() < theta
-        neg[n_vote:] = False
-        lr[neg] = -float(server_lr)
-        flipped = int(neg.sum())
-    new = g + lr * agg
-    if n_vote < n:
-        new[n_vote:] = g[n_vote:] + mean[n_vote:]
-    return new.float(), flipped
+    return _server_update(g, agg, signs, mean, theta, server_lr, n_vote, opt)
 
 
 class PtrTable:
@@ -396,12 +447,13 @@ class PtrTable:
 
 
 def fused_aggregate(w_global, w_agents, weights, mode="avg", theta=0, server_lr=1.0, noise_std=0.0, seed=0,
-                    noise_stream=0, n_vote=None, scales=None, out=None, out_bf16=None, flipped=None):
+                    noise_stream=0, n_vote=None, scales=None, out=None, out_bf16=None, flipped=None, opt=None):
     """Single-process fused server step: ``out <- w_global + lr ⊙ agg({w_k - w_global})`` in one kernel.
 
     On CUDA this launches ``fused_aggregate_kernel`` (ops/csrc/aggregate.cu); on CPU it runs the fp64 oracle (with
-    torch-sampled noise).  ``out`` may alias ``w_global``.  Returns the tensor written.  The multi-GPU variant (peer
-    pointers, multicast stores, in-kernel barriers) is driven by ``parallel.fused_agg.FusedAggregator``.
+    torch-sampled noise).  ``out`` may alias ``w_global``.  ``opt``: optional full-length ``ServerOptState``, updated in place.
+    Returns the tensor written.  The multi-GPU variant (peer pointers, multicast stores, in-kernel barriers) is driven by
+    ``parallel.fused_agg.FusedAggregator``.
     """
     n = w_global.numel()
     n_vote = n if n_vote is None else int(n_vote)
@@ -412,7 +464,7 @@ def fused_aggregate(w_global, w_agents, weights, mode="avg", theta=0, server_lr=
             gen = torch.Generator().manual_seed(int(seed) * 1000003 + int(noise_stream))
             noise = torch.randn(n, generator=gen, dtype=torch.float64) * noise_std
             noise[n_vote:] = 0
-        new, nflip = aggregate_oracle(w_global, w_agents, weights, mode, theta, server_lr, noise, n_vote, scales)
+        new, nflip = aggregate_oracle(w_global, w_agents, weights, mode, theta, server_lr, noise, n_vote, scales, opt)
         out.copy_(new)
         if out_bf16 is not None:
             out_bf16.copy_(new.to(torch.bfloat16))
@@ -429,7 +481,7 @@ def fused_aggregate(w_global, w_agents, weights, mode="avg", theta=0, server_lr=
             gen = torch.Generator(device=dev).manual_seed(int(seed) * 1000003 + int(noise_stream))
             noise = torch.randn(n, generator=gen, dtype=torch.float64, device=dev) * noise_std
             noise[n_vote:] = 0
-        new, nflip = aggregate_oracle(w_global, w_agents, weights, mode, theta, server_lr, noise, n_vote, scales)
+        new, nflip = aggregate_oracle(w_global, w_agents, weights, mode, theta, server_lr, noise, n_vote, scales, opt)
         out.copy_(new)
         if out_bf16 is not None:
             out_bf16.copy_(new.to(torch.bfloat16))
@@ -446,8 +498,16 @@ def fused_aggregate(w_global, w_agents, weights, mode="avg", theta=0, server_lr=
     sc = torch.as_tensor(scales, dtype=torch.float32).to(dev) if scales is not None else None
     ext().fused_aggregate(agents.tensor, wt, sc, float(sum(float(x) for x in weights)), w_global.data_ptr(), outs.tensor,
                           outs_b.tensor if outs_b else None, False, 0, n, n_vote, MODE_IDS[mode], int(theta),
-                          float(server_lr), float(noise_std), int(seed), int(noise_stream), flipped, None, None, 0, 1, 0)
+                          float(server_lr), float(noise_std), int(seed), int(noise_stream), flipped, None, None, 0, 1, 0,
+                          False, *opt_launch_args(opt))
     return out
+
+
+def opt_launch_args(opt):
+    """The server optimizer arguments of the ``fused_aggregate`` binding: (opt, beta1, beta2, tau, opt_m, opt_v, state_base)."""
+    if opt is None or opt.kind == "sgd":
+        return 0, 0.0, 0.0, 0.0, None, None, 0
+    return SERVER_OPTS[opt.kind], opt.beta1, opt.beta2, opt.tau, opt.m, opt.v, opt.base
 
 
 def update_norms(w_global, w_agents, n=None):

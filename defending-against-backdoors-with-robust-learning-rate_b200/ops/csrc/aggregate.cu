@@ -5,7 +5,9 @@
 //     (Robust Learning Rate; reference src/aggregation.py:48-54),
 //   * aggregates: data-size-weighted mean (:57-64) | lower coordinate median (:66-69) | sign majority (:71-75),
 //   * adds optional Gaussian noise (in-kernel Philox; :34-35) BEFORE the lr multiply, like the reference,
-//   * applies the server step  w_g' = w_g + lr * agg  (:38-40) in fp64 then rounds to fp32,
+//   * applies the server step  w_g' = w_g + lr * agg  (:38-40) in fp64 then rounds to fp32 -- or, with --server_opt, the server
+//     optimizer (FedAvgM momentum, FedAdagrad, FedAdam, FedYogi) on the pseudo-gradient ±agg, its fp32 state m, v read and
+//     written in the same pass (state index i - state_base: a rank keeps only its own slice on the fused multi-GPU path),
 //   * and writes w_g' (+ its bf16 GEMM-operand shadow) to every GPU: one NVLS `multimem.st` per 16 bytes when a
 //     multicast mapping exists, else one P2P store per peer.  This store IS the next round's broadcast
 //     (reference src/federated.py:72).
@@ -150,12 +152,36 @@ __device__ __forceinline__ void agg_epilogue(const AggParams& p, AggShared& sh, 
 }
 
 // ---- one coordinate: noise, RLR flip, server step -----------------------------------------------------------------------------
-__device__ __forceinline__ float server_step(const AggParams& p, float g, double agg, int s, float nz, unsigned long long& flipped) {
+// The server optimizers (Reddi et al., Adaptive Federated Optimization, Algorithm 2, no bias correction; FedAvgM for momentum) act on
+// the pseudo-gradient d = ±(agg + noise).  m and v are this coordinate's state: read and rounded back to fp32 here, while the new
+// weight uses this round's unrounded fp64 values.  sgd keeps the exact expression of the plain step.
+enum : int { kOptSgd = 0, kOptMomentum = 1, kOptAdagrad = 2, kOptAdam = 3, kOptYogi = 4 };
+
+__device__ __forceinline__ float server_step(const AggParams& p, float g, double agg, int s, float nz, unsigned long long& flipped,
+                                             float& m, float& v, bool stateful = true) {
     const double a = agg + (double)nz;
     const bool keep = (p.theta <= 0) || (abs(s) >= p.theta);
     flipped += keep ? 0 : 1;
-    const double lr = keep ? (double)p.server_lr : -(double)p.server_lr;
-    return (float)((double)g + lr * a);
+    if (!stateful || p.opt == kOptSgd) {
+        const double lr = keep ? (double)p.server_lr : -(double)p.server_lr;
+        return (float)((double)g + lr * a);
+    }
+    const double d = keep ? a : -a;
+    double m1, step;
+    if (p.opt == kOptMomentum) {
+        m1 = p.beta1 * (double)m + d;
+        step = m1;
+    } else {
+        m1 = p.beta1 * (double)m + (1.0 - p.beta1) * d;
+        const double v0 = (double)v, d2 = d * d;
+        const double v1 = p.opt == kOptAdagrad ? v0 + d2
+                        : p.opt == kOptAdam    ? p.beta2 * v0 + (1.0 - p.beta2) * d2
+                                               : v0 - (1.0 - p.beta2) * d2 * (double)((v0 > d2) - (v0 < d2));   // yogi
+        v = (float)v1;
+        step = m1 / (sqrt(v1) + p.tau);
+    }
+    m = (float)m1;
+    return (float)((double)g + (double)p.server_lr * step);
 }
 
 __device__ __forceinline__ void store4(const AggParams& p, long long i, const float (&out)[4]) {
@@ -174,9 +200,12 @@ __device__ __forceinline__ void store4(const AggParams& p, long long i, const fl
 
 // =================================================================================================================================
 // vector path: four coordinates per thread.  MODE 0 avg, 1 comed (KT = 1..8 participants, compile time), 2 sign.
+// OPT: a server optimizer with state (float4 loads / stores of m, v).  A compile-time switch here: with a run-time one the sgd build of
+// the K = 8 median spills at ptxas's 64-register choice.  The stateful builds are allowed 2 CTAs per SM so ptxas keeps their fp64 step
+// (~80 registers) out of local memory.
 // =================================================================================================================================
-template <int MODE, int KT>
-__global__ void __launch_bounds__(kAggThreads) fused_aggregate_kernel(AggParams p) {
+template <int MODE, int KT, bool OPT>
+__global__ void __launch_bounds__(kAggThreads, OPT ? 2 : 0) fused_aggregate_kernel(AggParams p) {
     __shared__ AggShared sh;
     const int K = KT > 0 ? KT : p.K;
     agg_prologue(p, sh, K);
@@ -233,9 +262,15 @@ __global__ void __launch_bounds__(kAggThreads) fused_aggregate_kernel(AggParams 
                 const float4 z = philox_normal4(ph, (uint64_t)(i >> 2), p.noise_stream);
                 nz[0] = z.x * p.noise_std; nz[1] = z.y * p.noise_std; nz[2] = z.z * p.noise_std; nz[3] = z.w * p.noise_std;
             }
+            float4 m4 = make_float4(0.f, 0.f, 0.f, 0.f), v4 = m4;
+            if (OPT) m4 = ld_f4(p.opt_m + (i - p.state_base));
+            if (OPT && p.opt_v) v4 = ld_f4(p.opt_v + (i - p.state_base));
+            float m[4] = {m4.x, m4.y, m4.z, m4.w}, v[4] = {v4.x, v4.y, v4.z, v4.w};
 #pragma unroll
             for (int c = 0; c < 4; ++c)   // avg keeps its fp64 mean; comed / sign values are exact in fp32
-                out[c] = server_step(p, g[c], (MODE == 0) ? acc[c] * inv_total : (double)agg[c], s[c], nz[c], flipped);
+                out[c] = server_step(p, g[c], (MODE == 0) ? acc[c] * inv_total : (double)agg[c], s[c], nz[c], flipped, m[c], v[c], OPT);
+            if (OPT) st_f4(p.opt_m + (i - p.state_base), make_float4(m[0], m[1], m[2], m[3]));
+            if (OPT && p.opt_v) st_f4(p.opt_v + (i - p.state_base), make_float4(v[0], v[1], v[2], v[3]));
         }
         store4(p, i, out);
     }
@@ -323,7 +358,12 @@ __global__ void __launch_bounds__(NT > 0 ? kAggThreads : kSelThreads) fused_aggr
                     const int c = (int)(i & 3);
                     nz = (c == 0 ? z.x : c == 1 ? z.y : c == 2 ? z.z : z.w) * p.noise_std;
                 }
-                out = server_step(p, g, (double)med, s, nz, flipped);
+                float* const mp = p.opt_m ? p.opt_m + (i - p.state_base) : nullptr;
+                float* const vp = p.opt_v ? p.opt_v + (i - p.state_base) : nullptr;
+                float m = mp ? *mp : 0.f, v = vp ? *vp : 0.f;
+                out = server_step(p, g, (double)med, s, nz, flipped, m, v);
+                if (mp) *mp = m;
+                if (vp) *vp = v;
             }
         }
         // regroup: lanes 4j .. 4j+3 -> one 16-byte store by lane 4j
@@ -339,7 +379,8 @@ __global__ void __launch_bounds__(NT > 0 ? kAggThreads : kSelThreads) fused_aggr
 
 template <int MODE, int KT>
 static cudaError_t launch_vec(const AggParams& p, int grid, cudaStream_t st) {
-    fused_aggregate_kernel<MODE, KT><<<grid, kAggThreads, 0, st>>>(p);
+    if (p.opt == kOptSgd) fused_aggregate_kernel<MODE, KT, false><<<grid, kAggThreads, 0, st>>>(p);
+    else fused_aggregate_kernel<MODE, KT, true><<<grid, kAggThreads, 0, st>>>(p);
     return cudaGetLastError();
 }
 template <int NT>
@@ -353,6 +394,8 @@ int aggregate_max_agents() { return kMaxAgents; }
 cudaError_t launch_fused_aggregate(const AggParams& p, int num_sms, cudaStream_t st) {
     if (p.K < 1 || p.K > kMaxAgents) return cudaErrorInvalidValue;
     if (((p.end - p.begin) & 3) || (p.begin & 3) || (p.n_vote & 3)) return cudaErrorInvalidValue;
+    if (p.opt < kOptSgd || p.opt > kOptYogi || (p.state_base & 3) || p.state_base > p.begin) return cudaErrorInvalidValue;
+    if ((p.opt != kOptSgd && !p.opt_m) || (p.opt >= kOptAdagrad && !p.opt_v)) return cudaErrorInvalidValue;
     const long long n = p.end - p.begin;
     const bool scalar = p.mode == 1 && p.K > 8;
     const long long per_block = scalar ? (p.K > 64 ? kSelThreads : kAggThreads) : 4LL * kAggThreads;

@@ -32,7 +32,9 @@ void fused_aggregate(at::Tensor w_agent_ptrs, at::Tensor weights, c10::optional<
                      bool use_multimem, int64_t begin, int64_t end, int64_t n_vote, int64_t mode, int64_t theta,
                      double server_lr, double noise_std, int64_t seed, int64_t noise_stream,
                      c10::optional<at::Tensor> flipped, c10::optional<at::Tensor> flag_ptrs,
-                     c10::optional<at::Tensor> local_sync, int64_t rank, int64_t world, int64_t epoch, bool handoff) {
+                     c10::optional<at::Tensor> local_sync, int64_t rank, int64_t world, int64_t epoch, bool handoff,
+                     int64_t opt, double beta1, double beta2, double tau, c10::optional<at::Tensor> opt_m, c10::optional<at::Tensor> opt_v,
+                     int64_t state_base) {
     CHECK_CUDA(w_agent_ptrs); CHECK_CUDA(weights); CHECK_CUDA(out_ptrs);
     TORCH_CHECK(w_agent_ptrs.scalar_type() == at::kLong && out_ptrs.scalar_type() == at::kLong, "pointer tables must be int64");
     TORCH_CHECK(weights.scalar_type() == at::kDouble, "weights must be float64");
@@ -58,6 +60,17 @@ void fused_aggregate(at::Tensor w_agent_ptrs, at::Tensor weights, c10::optional<
     p.rank = (int)rank; p.world = (int)world; p.epoch = (uint32_t)epoch;
     p.handoff = handoff ? 1 : 0;
     TORCH_CHECK(world <= 1 || (p.flag_ptrs && p.local_sync), "multi-GPU aggregation needs flag_ptrs and local_sync");
+    // server optimizer state: fp32 on the launch device, covering [state_base, end)
+    for (const auto* t : {&opt_m, &opt_v}) {
+        if (!t->has_value() || !(*t)->defined()) continue;
+        CHECK_CUDA(**t);
+        TORCH_CHECK((*t)->scalar_type() == at::kFloat && (*t)->device() == w_agent_ptrs.device(), "optimizer state must be float32 on the launch device");
+        TORCH_CHECK(state_base <= begin && state_base + (*t)->numel() >= end, "optimizer state does not cover the coordinate slice");
+    }
+    p.opt = (int)opt; p.beta1 = beta1; p.beta2 = beta2; p.tau = tau;
+    p.opt_m = ptr_or_null<float>(opt_m);
+    p.opt_v = ptr_or_null<float>(opt_v);
+    p.state_base = state_base;
     check(rlr::launch_fused_aggregate(p, num_sms(), cur_stream()), "fused_aggregate");
 }
 
@@ -285,7 +298,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("w_global_ptr"), py::arg("out_ptrs"), py::arg("out_bf16_ptrs"), py::arg("use_multimem"), py::arg("begin"), py::arg("end"),
           py::arg("n_vote"), py::arg("mode"), py::arg("theta"), py::arg("server_lr"), py::arg("noise_std"), py::arg("seed"),
           py::arg("noise_stream"), py::arg("flipped"), py::arg("flag_ptrs"), py::arg("local_sync"), py::arg("rank"), py::arg("world"),
-          py::arg("epoch"), py::arg("handoff") = false);
+          py::arg("epoch"), py::arg("handoff") = false, py::arg("opt") = 0, py::arg("beta1") = 0.0, py::arg("beta2") = 0.0,
+          py::arg("tau") = 0.0, py::arg("opt_m") = py::none(), py::arg("opt_v") = py::none(), py::arg("state_base") = 0);
     m.def("aggregate_max_agents", &rlr::aggregate_max_agents);
     m.def("acquire_slices", &acquire_slices);
     m.def("update_sqnorm", &update_sqnorm);

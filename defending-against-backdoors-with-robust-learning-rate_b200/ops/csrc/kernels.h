@@ -31,6 +31,12 @@ struct AggParams {
     int rank, world;
     uint32_t epoch;                 // monotonically increasing per call
     int handoff;                    // 1: publish this rank's slice in the peers' ready words (flag slot 2*world + rank) instead of the barrier-out
+    // server optimizer applied to the voted coordinates (0 sgd, 1 momentum, 2 adagrad, 3 adam, 4 yogi); state fp32, indexed by i - state_base
+    int opt;
+    double beta1, beta2, tau;
+    float* opt_m;                   // first moment (every optimizer but sgd) or nullptr
+    float* opt_v;                   // second moment (adagrad / adam / yogi) or nullptr
+    long long state_base;           // coordinate of opt_m[0] / opt_v[0] (multiple of 4; = begin when the state is sharded)
 };
 cudaError_t launch_fused_aggregate(const AggParams& p, int num_sms, cudaStream_t st);
 int aggregate_max_agents();         // capacity of the kernel's participant tables

@@ -3,7 +3,8 @@
 Same flag names, types and defaults as the reference (src/options.py:4-74) so existing command lines
 (src/runner.sh:12-38) keep working, plus engine flags that have no reference counterpart
 (``--model --dtype --backend --synthetic --seed --checkpoint ...``).  ``finalize_args`` applies the
-reference's post-parse fix-up ``server_lr = server_lr if aggr == 'sign' else 1.0`` (src/federated.py:23).
+reference's post-parse fix-up ``server_lr = server_lr if aggr == 'sign' else 1.0`` (src/federated.py:23) to the plain
+sgd server step; with ``--server_opt`` other than sgd, ``--server_lr`` is the optimizer's step size for every aggregator.
 """
 from __future__ import annotations
 
@@ -13,6 +14,7 @@ import torch
 
 DATASETS = ("fmnist", "fedemnist", "cifar10")
 AGGREGATORS = ("avg", "comed", "sign")
+SERVER_OPTS = ("sgd", "momentum", "adagrad", "adam", "yogi")
 PATTERNS = ("plus", "square", "copyright", "apple")
 MODELS = ("auto", "cnn_mnist", "cnn_cifar", "resnet18", "resnet34", "vgg11", "vgg16", "resnet18_gn", "resnet34_gn", "vgg11_gn", "vgg16_gn")
 
@@ -35,7 +37,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--bs", type=int, default=256, help="local batch size: B")
     p.add_argument("--client_lr", type=float, default=0.1, help="clients' learning rate")
     p.add_argument("--client_moment", type=float, default=0.9, help="clients' momentum")
-    p.add_argument("--server_lr", type=float, default=1, help="server learning rate (only honoured for aggr=sign)")
+    p.add_argument("--server_lr", type=float, default=1,
+                   help="server learning rate (with --server_opt sgd only honoured for aggr=sign)")
     p.add_argument("--base_class", type=int, default=5, help="base class of the backdoor attack")
     p.add_argument("--target_class", type=int, default=7, help="target class of the backdoor attack")
     p.add_argument("--poison_frac", type=float, default=0.0, help="fraction of base-class samples a corrupt agent poisons")
@@ -90,13 +93,27 @@ def build_parser() -> argparse.ArgumentParser:
                         "(torchvision RandomCrop(padding=P); the CIFAR-10 recipe is 4; 0 = off).  Local training only")
     p.add_argument("--hflip", action="store_true",
                    help="training augmentation: mirror each image left-right with probability 1/2 (local training only)")
+    p.add_argument("--server_opt", type=str, default="sgd", choices=SERVER_OPTS,
+                   help="server optimizer on the (RLR-signed) aggregate: sgd = w + server_lr * agg (reference); momentum = FedAvgM; "
+                        "adagrad / adam / yogi = FedAdagrad / FedAdam / FedYogi (Reddi et al. 2021, no bias correction)")
+    p.add_argument("--server_beta1", type=float, default=0.9, help="server optimizer first-moment decay, in [0, 1)")
+    p.add_argument("--server_beta2", type=float, default=0.99, help="adam / yogi second-moment decay, in [0, 1)")
+    p.add_argument("--server_tau", type=float, default=1e-3, help="adagrad / adam / yogi adaptivity tau > 0 (v starts at tau^2)")
     return p
 
 
 def finalize_args(args: argparse.Namespace) -> argparse.Namespace:
     """Post-parse normalisation shared by the CLI and programmatic users."""
-    # reference src/federated.py:23 -- server_lr is forced to 1 unless sign aggregation is used
-    args.server_lr = args.server_lr if args.aggr == "sign" else 1.0
+    # reference src/federated.py:23 -- server_lr is forced to 1 unless sign aggregation is used (plain sgd server step only)
+    if getattr(args, "server_opt", "sgd") == "sgd":
+        args.server_lr = args.server_lr if args.aggr == "sign" else 1.0
+    if getattr(args, "server_opt", "sgd") not in SERVER_OPTS:
+        raise ValueError(f"unknown --server_opt {args.server_opt!r}; expected one of {SERVER_OPTS}")
+    for name in ("server_beta1", "server_beta2"):
+        if not 0.0 <= getattr(args, name, 0.0) < 1.0:
+            raise ValueError(f"--{name} {getattr(args, name)} must lie in [0, 1)")
+    if not getattr(args, "server_tau", 1.0) > 0:
+        raise ValueError(f"--server_tau {args.server_tau} must be > 0")
     if args.model == "auto":
         args.model = "cnn_cifar" if args.data == "cifar10" else "cnn_mnist"
     if args.aggr not in AGGREGATORS:
@@ -146,4 +163,6 @@ def print_exp_details(args) -> None:
     print(f"    Clip: {args.clip}")
     print(f"    Model / dtype / trainer / backend: {args.model} / {args.dtype} / {args.trainer} / {args.backend}")
     print(f"    Crop pad / hflip: {args.crop_pad} / {args.hflip}")
+    if getattr(args, "server_opt", "sgd") != "sgd":
+        print(f"    Server optimizer (beta1 / beta2 / tau): {args.server_opt} ({args.server_beta1} / {args.server_beta2} / {args.server_tau})")
     print("======================================")

@@ -28,6 +28,10 @@ queued right behind it waits for the remaining slices, so the first-layer GEMM o
 
 With ``backend in {nccl, gloo}`` (the baseline transport) the slots are all-gathered and the same kernel runs on the
 gathered copies locally; on CPU it runs the fp64 oracle.
+
+Server optimizer state (``--server_opt`` other than sgd; ``ops.ServerOptState``) lives in ordinary device memory, allocated once:
+on the fused multi-GPU path rank r keeps only the state of its slice [begin, end) -- it is the only rank that ever steps those
+coordinates -- and with every other transport each rank keeps the full vector (identical on all ranks).
 """
 from __future__ import annotations
 
@@ -41,7 +45,9 @@ FLAG_BYTES = 4096
 
 class FusedAggregator:
     def __init__(self, ctx, n_total: int, n_vote: int, max_slots: int, backend: str = "auto", with_bf16: bool = True,
-                 transport: str = "auto"):
+                 transport: str = "auto", server_opt=None, n_part: int | None = None):
+        """``server_opt``: optional ``dict(kind=..., beta1=..., beta2=..., tau=...)``; ``n_part``: participants per round (default
+        every slot), which fixes whether the fused multi-GPU kernel or the gather fallback runs, and so the state layout."""
         self.ctx = ctx
         # nccl / gloo back-ends: "gather" all-gathers every participant's parameters and runs the kernel on the copies (any
         # aggregator); "reduce" all-reduces per-coordinate partial sums (vote, weighted update sum) -- O(N) instead of O(K N)
@@ -100,6 +106,14 @@ class FusedAggregator:
             self.per = per
             self.begin = min(n, ctx.rank * per)
             self.end = min(n, self.begin + per)
+        n_part = self.max_slots * ctx.world if n_part is None else int(n_part)
+        self.sharded = use_symm and n_part <= ops.MAX_FUSED_AGENTS
+        so = dict(server_opt or {})
+        kind = so.pop("kind", "sgd")
+        if self.sharded:
+            self.opt = ops.ServerOptState(kind, self.end - self.begin, device=dev, base=self.begin, **so)
+        else:
+            self.opt = ops.ServerOptState(kind, n, device=dev, **so)
 
     # ---- hand-off fused with the next round's first GEMM -------------------------------------------------------------------
     def enable_handoff(self):
@@ -146,7 +160,11 @@ class FusedAggregator:
         ctx, dev = self.ctx, self.ctx.device
         self.flipped.zero_()
         self.flipped_is_partial = False
-        if self.backend == "fused" and ctx.is_dist and n_part <= ops.MAX_FUSED_AGENTS:
+        fused_p2p = self.backend == "fused" and ctx.is_dist and n_part <= ops.MAX_FUSED_AGENTS
+        if self.opt.kind != "sgd" and fused_p2p != self.sharded:
+            raise ValueError(f"{n_part} participants: the server optimizer state was laid out for the "
+                             f"{'fused multi-GPU' if self.sharded else 'gather'} path")
+        if fused_p2p:
             self.flipped_is_partial = True
             self.epoch += 1
             wt = torch.as_tensor(weights, dtype=torch.float64).to(dev)
@@ -156,7 +174,7 @@ class FusedAggregator:
                 self.out_ptrs.tensor, self.out_bf16_ptrs.tensor if self.out_bf16_ptrs else None, self.use_multimem,
                 self.begin, self.end, self.n_vote, ops.MODE_IDS[mode], int(theta), float(server_lr), float(noise_std),
                 int(seed), int(rnd), self.flipped, self.flag_ptrs.tensor, self.local_sync, ctx.rank, ctx.world, self.epoch,
-                bool(self.handoff))
+                bool(self.handoff), *ops.opt_launch_args(self.opt))
             if self.handoff:
                 self.epoch_dev.fill_(self.epoch)      # what the next round's consumers wait for (stream-ordered before their graphs)
             return
@@ -172,7 +190,7 @@ class FusedAggregator:
         else:
             agents = [self.slots[j] for j in range(n_part)]
         ops.fused_aggregate(self.w_global, agents, weights, mode, theta, server_lr, noise_std, seed, rnd, self.n_vote,
-                            scales, out=self.w_global, out_bf16=self.w_bf16, flipped=self.flipped)
+                            scales, out=self.w_global, out_bf16=self.w_bf16, flipped=self.flipped, opt=self.opt)
 
     def _aggregate_reduce(self, weights, mode, theta, server_lr, noise_std, seed, rnd, scales):
         """All-reduce transport: every rank folds its local participants into (vote, weighted sum), two all_reduce calls make them
@@ -191,11 +209,36 @@ class FusedAggregator:
             noise = (torch.randn(self.n, generator=gen, dtype=torch.float64) * noise_std).to(self.w_global.device)
             noise[self.n_vote:] = 0
         new, nflip = ops.aggregate_from_partials(self.w_global, vote, wsum, sum(float(x) for x in weights), mode, theta, server_lr,
-                                                 noise, self.n_vote)
+                                                 noise, self.n_vote, self.opt)
         self.w_global.copy_(new)
         if self.w_bf16 is not None:
             self.w_bf16.copy_(new.to(torch.bfloat16))
         self.flipped += nflip
+
+    def server_opt_state(self):
+        """Full-length fp32 copies ``(m, v)`` of the server optimizer state on every rank (``v`` is None for momentum), or None for
+        sgd.  Collective on the fused multi-GPU path, where each rank contributes its slice."""
+        opt = self.opt
+        if opt.kind == "sgd":
+            return None
+        full = []
+        for t in (opt.m, opt.v):
+            if t is None:
+                full.append(None)
+            elif not self.sharded:
+                full.append(t.clone())
+            else:
+                part = torch.zeros(self.per, dtype=t.dtype, device=t.device)
+                part[: t.numel()] = t
+                full.append(self.ctx.all_gather(part).view(-1)[: self.n].clone())
+        return tuple(full)
+
+    def load_server_opt_state(self, m, v):
+        """Set the state from full-length vectors (this rank's slice of them on the fused multi-GPU path)."""
+        lo, hi = (self.begin, self.end) if self.sharded else (0, self.n)
+        for dst, src in ((self.opt.m, m), (self.opt.v, v)):
+            if dst is not None:
+                dst.copy_(src[lo:hi].to(dst.device))
 
     def gather_participants(self, n_part: int):
         """Every participant's flat parameter vector on THIS rank (list of ``n_part`` tensors; remote slots are copied through an

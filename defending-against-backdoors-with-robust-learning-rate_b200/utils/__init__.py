@@ -2,7 +2,7 @@
 from .evaluate import get_loss_n_accuracy
 from .logging import MetricLogger
 from .timers import PhaseTimer
-from .checkpoint import save_checkpoint, load_checkpoint
+from .checkpoint import save_checkpoint, load_checkpoint, restore_server_opt
 
 
 
@@ -19,4 +19,4 @@ def __getattr__(name):
     raise AttributeError(name)
 
 
-__all__ = ["get_loss_n_accuracy", "MetricLogger", "PhaseTimer", "save_checkpoint", "load_checkpoint"]
+__all__ = ["get_loss_n_accuracy", "MetricLogger", "PhaseTimer", "save_checkpoint", "load_checkpoint", "restore_server_opt"]

@@ -3,6 +3,8 @@
 ``aggregate_updates`` = Robust-LR sign vote + {FedAvg | coordinate median | sign majority} + optional noise + server
 step, executed by ONE fused kernel over the flat parameter vector (``ops.fused_aggregate`` in-process, or
 ``parallel.FusedAggregator`` across GPUs) instead of the reference's ~30 elementwise fp64 passes (SURVEY.md 2.4b).
+With ``--select krum | multikrum`` a selection stage runs first: the participants' pairwise update distances
+(``ops.pairwise_sqdist``), Krum scores on the host (``ops.krum_select``), and only the admitted participants enter the step.
 The reference's dead / disabled pieces are available behind flags: ``clip_updates`` (``--server_clip``) and the
 diagnostics ``plot_norms`` / ``comp_diag_fisher`` / ``plot_sign_agreement`` (``--diagnostics``), the latter with the
 reference's latent bugs fixed (model built on the right device; Fisher uses log-probabilities -- SURVEY.md quirk 7).
@@ -35,6 +37,8 @@ class Aggregation:
         self.fused = fused            # parallel.FusedAggregator or None (pure in-process use)
         self.cum_net_mov = 0.0
         self.last_flipped = 0
+        self.last_admitted = None     # agent ids admitted by --select in the last round
+        self.last_select = None       # the Select/* scalars of the last round
         self.opt = None               # full-length server optimizer state of the in-process form (allocated on first use)
 
     # ---- the server step ------------------------------------------------------------------------------------
@@ -42,9 +46,16 @@ class Aggregation:
         """In-process form: ``agent_params`` = {agent_id: flat local parameters}.  Updates ``w_global`` in place."""
         ids = list(agent_params.keys())
         ws = [agent_params[i] for i in ids]
-        weights = [float(self.agent_data_sizes[i]) for i in ids]
         nv = n_vote if n_vote is not None else (self.layout.n_vote if self.layout else None)
         scales = self._clip_scales(ops.update_norms(w_global, ws, nv)) if self._server_clip else None
+        all_ids, all_ws = ids, ws
+        if self._select:
+            D = ops.pairwise_sqdist(ws, nv if nv is not None else w_global.numel(), w_global if scales is not None else None, scales)
+            keep = self._admit(D, ids, cur_round)
+            if len(keep) < len(ids):
+                ids, ws = [ids[j] for j in keep], [ws[j] for j in keep]
+                scales = scales[torch.as_tensor(keep, device=scales.device)] if scales is not None else None
+        weights = [float(self.agent_data_sizes[i]) for i in ids]
         prev = w_global.clone() if self.args.diagnostics else None
         flipped = torch.zeros(1, dtype=torch.int64, device=w_global.device)
         if self.opt is None:
@@ -55,8 +66,8 @@ class Aggregation:
                             scales, out=w_global, flipped=flipped, opt=self.opt)
         self.last_flipped = flipped
         if self.args.diagnostics:
-            self.plot_norms(dict(zip(ids, ops.update_norms(prev, ws, nv).tolist())), cur_round)
-            self.plot_sign_agreement(prev, w_global, ws, ids, cur_round)
+            self.plot_norms(dict(zip(all_ids, ops.update_norms(prev, all_ws, nv).tolist())), cur_round)
+            self.plot_sign_agreement(prev, w_global, ws, ids, cur_round)     # the vote that happened: admitted participants only
         return
 
     def aggregate_slots(self, participants, cur_round):
@@ -69,19 +80,44 @@ class Aggregation:
             norms = self.fused.update_norms(len(participants))
         if self._server_clip:
             scales = self._clip_scales(norms)
-        if diag:   # the sign-agreement analysis needs the pre-step global parameters and every participant's parameters
+        keep, copies = None, None
+        if self._select:
+            # on the gather transport both passes read the same all-gathered copies (one all_gather per round)
+            copies = self.fused.gather_participants(len(participants)) if self.fused.gathers(len(participants)) else None
+            keep = self._admit(self.fused.pairwise_sqdist(len(participants), scales, copies), participants, cur_round)
+        if diag:   # the sign-agreement analysis needs the pre-step global parameters and every admitted participant's parameters
             prev = self.fused.w_global.clone()
             ws = [w.clone() for w in self.fused.gather_participants(len(participants))]
+            voters = participants
+            if keep is not None:
+                ws, voters = [ws[j] for j in keep], [participants[j] for j in keep]
         self.fused.aggregate(weights, self.args.aggr, self.args.robustLR_threshold, self.server_lr,
-                             self.args.noise * self.args.clip, self.args.seed, cur_round, scales)
+                             self.args.noise * self.args.clip, self.args.seed, cur_round, scales, members=keep, participants=copies)
         self.last_flipped = self.fused.flipped
         if diag:
             self.plot_norms(dict(zip(participants, norms.tolist())), cur_round)
-            self.plot_sign_agreement(prev, self.fused.w_global, ws, participants, cur_round)
+            self.plot_sign_agreement(prev, self.fused.w_global, ws, voters, cur_round)
 
     @property
     def _server_clip(self):
         return bool(getattr(self.args, "server_clip", False)) and self.args.clip > 0
+
+    @property
+    def _select(self):
+        return getattr(self.args, "select", "none") != "none"
+
+    def _admit(self, D, ids, cur_round):
+        """Krum / Multi-Krum admission from the pairwise distances ``D`` of the participants ``ids``: the admitted positions
+        (ascending).  Records ``last_admitted`` and logs how many corrupt participants (ids < num_corrupt) came and got through."""
+        keep = ops.krum_select(D, ids, self.args.select_f, self.args.select_m)
+        self.last_admitted = [ids[j] for j in keep]
+        nc = self.args.num_corrupt
+        self.last_select = {"Select/Corrupt_Participants": sum(1 for i in ids if i < nc),
+                            "Select/Corrupt_Admitted": sum(1 for i in self.last_admitted if i < nc)}
+        if self.writer is not None:
+            for k, v in self.last_select.items():
+                self.writer.add_scalar(k, v, cur_round)
+        return keep
 
     def _clip_scales(self, norms):
         """reference ``clip_updates`` (src/aggregation.py:77-81): update /= max(1, ||update||/clip)."""

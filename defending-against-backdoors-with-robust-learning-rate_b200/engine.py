@@ -311,6 +311,9 @@ class FLEngine:
             loss, flipped = self.round_result()
             rec["train_loss"] = loss / max(1, info["steps"])
             rec["frac_flipped"] = flipped / max(1, self.layout.n_params)
+            if self.aggregator.last_select is not None:
+                rec["select_corrupt_participants"] = self.aggregator.last_select["Select/Corrupt_Participants"]
+                rec["select_corrupt_admitted"] = self.aggregator.last_select["Select/Corrupt_Admitted"]
             rec.update({f"ms_{k}": v for k, v in self.timer.elapsed().items()})
             if args.profile_phases and self.verbose:
                 print({k: round(v, 3) for k, v in rec.items() if k.startswith("ms_")})

@@ -525,6 +525,69 @@ def update_norms(w_global, w_agents, n=None):
 
 
 # =====================================================================================================================
+# participant selection (Krum / Multi-Krum, Blanchard et al. 2017)
+# =====================================================================================================================
+def sqdist_statement(w_agents, lo, hi, w_global=None, scales=None):
+    """fp64 statement of the pairwise squared distances over coordinates ``[lo, hi)``: ``D[i][j] = sum_c (x_i[c] - x_j[c])^2`` with
+    ``x_k = w_k`` (no scales: ``w_global`` cancels) or ``x_k = (w_k - w_global) * scales[k]``.  Symmetric, zero diagonal."""
+    K = len(w_agents)
+    dev = w_agents[0].device
+    D = torch.zeros(K, K, dtype=torch.float64, device=dev)
+    sc = torch.as_tensor(scales, dtype=torch.float32).to(dev).double()[:, None] if scales is not None else None
+    step = max(4, (1 << 24) // max(1, K))                 # coordinates per pass: K * step fp64 values
+    for c in range(lo, hi, step):
+        e = min(hi, c + step)
+        x = torch.stack([w[c:e] for w in w_agents]).double()
+        if sc is not None:
+            x = (x - w_global[c:e].double()) * sc
+        for i in range(K - 1):
+            D[i, i + 1:] += ((x[i + 1:] - x[i]) ** 2).sum(1)
+    return D + D.T
+
+
+def pairwise_sqdist(w_agents, n_vote, w_global=None, scales=None):
+    """K x K float64 squared distances between the participants' updates over the voted coordinates ``[0, n_vote)`` (the BatchNorm
+    running statistics behind ``n_vote`` do not count).  ``scales`` (server clipping) need ``w_global``; without them the updates'
+    differences are the parameters' differences.  On CUDA this launches ``pairwise_sqdist_kernel`` (ops/csrc/select.cu); on CPU, and
+    for more participants than the kernel's tables hold (recorded as a library fall-through), it evaluates ``sqdist_statement``."""
+    nv = w_agents[0].numel() if n_vote is None else int(n_vote)
+    if scales is not None and w_global is None:
+        raise ValueError("pairwise_sqdist: scales need w_global")
+    if not w_agents[0].is_cuda:
+        return sqdist_statement(w_agents, 0, nv, w_global, scales)
+    dev = w_agents[0].device
+    if len(w_agents) > MAX_FUSED_AGENTS:
+        note_fallback("pairwise_sqdist", f"K={len(w_agents)} > {MAX_FUSED_AGENTS}")
+        return sqdist_statement(w_agents, 0, nv, w_global, scales)
+    assert nv % 4 == 0, "flat buffers are padded to multiples of 4"
+    for w in w_agents:
+        assert w.is_cuda and w.dtype == torch.float32 and w.is_contiguous() and w.numel() >= nv
+    tab = PtrTable([w.data_ptr() for w in w_agents], dev, w_agents)
+    sc = torch.as_tensor(scales, dtype=torch.float32).to(dev) if scales is not None else None
+    out = torch.empty(len(w_agents), len(w_agents), dtype=torch.float64, device=dev)
+    ext().pairwise_sqdist(tab.tensor, w_global.data_ptr() if sc is not None else 0, sc, 0, nv, out, None, None, 0, 1, 0)
+    return out
+
+
+def krum_select(D, ids, f, m):
+    """Krum / Multi-Krum admission on the host, in fp64: ``score_i`` = the sum of the ``K - f - 2`` smallest ``D[i][j]`` (``j != i``),
+    added in ascending order; the ``m`` lowest scores are admitted (one-shot Multi-Krum; Krum is ``m = 1``), ties to the lower id in
+    ``ids``.  A NaN distance counts as +inf.  Returns the admitted positions (indices into ``ids``) in ascending order, so every rank
+    and every placement of the participants admits the same agents."""
+    d = np.nan_to_num(torch.as_tensor(D).detach().double().cpu().numpy(), nan=np.inf)
+    K = d.shape[0]
+    nb = K - int(f) - 2
+    if K < 2 * int(f) + 3 or nb < 1:
+        raise ValueError(f"Krum needs K >= 2f + 3 participants (K={K}, f={f})")
+    if not 1 <= int(m) <= K:
+        raise ValueError(f"Multi-Krum keeps m in [1, K] (m={m}, K={K})")
+    others = np.sort(d[~np.eye(K, dtype=bool)].reshape(K, K - 1), axis=1)[:, :nb]
+    scores = np.cumsum(others, axis=1)[:, -1].tolist()       # cumsum adds sequentially: the ascending order of the statement
+    order = sorted(range(K), key=lambda i: (scores[i], ids[i]))
+    return sorted(order[: int(m)])
+
+
+# =====================================================================================================================
 # optimiser over flat buffers
 # =====================================================================================================================
 def round_init(w_global, w_local=None, w_bf16=None, mom=None):

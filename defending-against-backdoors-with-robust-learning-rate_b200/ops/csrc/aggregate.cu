@@ -86,16 +86,6 @@ __device__ __forceinline__ float from_ordered_bits(uint32_t o) {
     return __uint_as_float((o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o);
 }
 
-// Cross-GPU barrier executed by the first `world` threads of ONE block.
-__device__ __forceinline__ void xgpu_barrier(uint32_t* const* flag_ptrs, int slot_base, int rank, int world, uint32_t epoch) {
-    const int t = threadIdx.x;
-    if (t < world) {
-        st_release_sys(flag_ptrs[t] + slot_base + rank, epoch);           // tell peer t "rank is here"
-        const uint32_t* mine = flag_ptrs[rank] + slot_base + t;           // wait for peer t
-        while ((int32_t)(ld_acquire_sys(mine) - epoch) < 0) { __nanosleep(64); }
-    }
-}
-
 struct AggShared {
     const float* w[kMaxAgents];
     double wt[kMaxAgents];

@@ -256,6 +256,16 @@ __device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
     return v;
 }
 
+// Cross-GPU barrier executed by the first `world` threads of ONE block (aggregate.cu, select.cu).
+__device__ __forceinline__ void xgpu_barrier(uint32_t* const* flag_ptrs, int slot_base, int rank, int world, uint32_t epoch) {
+    const int t = threadIdx.x;
+    if (t < world) {
+        st_release_sys(flag_ptrs[t] + slot_base + rank, epoch);           // tell peer t "rank is here"
+        const uint32_t* mine = flag_ptrs[rank] + slot_base + t;           // wait for peer t
+        while ((int32_t)(ld_acquire_sys(mine) - epoch) < 0) { __nanosleep(64); }
+    }
+}
+
 // ---- Philox4x32-10 counter RNG (Salmon et al.), used for dropout masks and server noise ---------------
 struct Philox {
     uint32_t k0, k1;

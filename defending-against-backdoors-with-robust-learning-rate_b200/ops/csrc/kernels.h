@@ -46,6 +46,22 @@ cudaError_t launch_acquire_slices(const uint32_t* ready, int first, int last, co
 cudaError_t launch_update_sqnorm(const float* const* w_agents, const float* w_global, long long n, int K, double* out,
                                  int num_sms, cudaStream_t st);
 
+// ---- participant selection (Krum / Multi-Krum): pairwise squared distances of the participants' updates ----------------------------
+// out[i][j] = sum_{begin <= c < end} (x_i[c] - x_j[c])^2 in fp64 ([K][K], symmetric, zero diagonal), x_k = w_k without scales and
+// x_k = (w_k - w_global) * scales[k] with them.  Fixed-order sums, no atomics: bitwise reproducible.
+struct DistParams {
+    const float* const* w_agents;   // [K] device pointers (local or peer-mapped)
+    const float* w_global;          // only read with scales
+    const float* scales;            // [K] server clipping scales or nullptr
+    long long begin, end;           // coordinate range (multiples of 4), already clipped to [0, n_vote)
+    int K;
+    uint32_t* const* flag_ptrs;     // world > 1: the aggregation's barrier-in words and intra-GPU ready flag (ops/csrc/aggregate.cu)
+    uint32_t* local_sync;
+    int rank, world;
+    uint32_t epoch;
+};
+cudaError_t launch_pairwise_sqdist(const DistParams& p, double* out, int num_sms, cudaStream_t st);
+
 // ---- data path ---------------------------------------------------------------------------------------
 // out_kind: 0 fp32, 1 bf16.  nchw: output layout NCHW (Cpad ignored) else NHWC with channels padded to c_pad.
 // Both gathers: crop_pad > 0 or flip turns on the training augmentation (AugSpec, common.cuh): sample b of the batch is drawn

@@ -9,12 +9,14 @@ sgd server step; with ``--server_opt`` other than sgd, ``--server_lr`` is the op
 from __future__ import annotations
 
 import argparse
+import math
 
 import torch
 
 DATASETS = ("fmnist", "fedemnist", "cifar10")
 AGGREGATORS = ("avg", "comed", "sign")
 SERVER_OPTS = ("sgd", "momentum", "adagrad", "adam", "yogi")
+SELECTIONS = ("none", "krum", "multikrum")
 PATTERNS = ("plus", "square", "copyright", "apple")
 MODELS = ("auto", "cnn_mnist", "cnn_cifar", "resnet18", "resnet34", "vgg11", "vgg16", "resnet18_gn", "resnet34_gn", "vgg11_gn", "vgg16_gn")
 
@@ -99,6 +101,13 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--server_beta1", type=float, default=0.9, help="server optimizer first-moment decay, in [0, 1)")
     p.add_argument("--server_beta2", type=float, default=0.99, help="adam / yogi second-moment decay, in [0, 1)")
     p.add_argument("--server_tau", type=float, default=1e-3, help="adagrad / adam / yogi adaptivity tau > 0 (v starts at tau^2)")
+    p.add_argument("--select", type=str, default="none", choices=SELECTIONS,
+                   help="participant selection before the --aggr rule (Blanchard et al. 2017): krum admits the participant whose update "
+                        "is closest to its K-F-2 nearest neighbours; multikrum the M best such scores.  Rejected participants take no "
+                        "part in the round (vote, rule, BatchNorm mean, noise, server optimizer)")
+    p.add_argument("--select_f", type=int, default=-1,
+                   help="Byzantine participants the selection assumes (-1 = ceil(num_corrupt * K / num_agents), K participants per round)")
+    p.add_argument("--select_m", type=int, default=0, help="participants multikrum admits (0 = K - F; krum admits 1)")
     return p
 
 
@@ -126,7 +135,39 @@ def finalize_args(args: argparse.Namespace) -> argparse.Namespace:
     side = min(meta.height, meta.width)
     if not 0 <= args.crop_pad < side:
         raise ValueError(f"--crop_pad {args.crop_pad} must lie in [0, {side}) for --data {args.data} ({meta.height}x{meta.width} images)")
+    _finalize_select(args)
     return args
+
+
+def _finalize_select(args) -> None:
+    """Validate ``--select`` and resolve its defaults in place: ``select_f`` = F, ``select_m`` = M (1 for krum)."""
+    select = getattr(args, "select", "none")
+    if select not in SELECTIONS:
+        raise ValueError(f"unknown --select {select!r}; expected one of {SELECTIONS}")
+    if select == "none":
+        if getattr(args, "select_f", -1) != -1 or getattr(args, "select_m", 0) != 0:
+            raise ValueError("--select_f / --select_m need --select krum or multikrum")
+        return
+    K = max(1, math.floor(args.num_agents * args.agent_frac))
+    f = args.select_f
+    if f < -1:
+        raise ValueError(f"--select_f {f} must be >= 0 (or -1 for the default)")
+    if f == -1:
+        f = math.ceil(args.num_corrupt * K / args.num_agents)
+    if K < 2 * f + 3:
+        raise ValueError(f"--select {select} needs K >= 2F + 3 participants per round (K={K}, F={f})")
+    m = args.select_m
+    if select == "krum":
+        if m not in (0, 1):
+            raise ValueError(f"--select krum admits one participant; --select_m {m} needs --select multikrum")
+        m = 1
+    elif m == 0:
+        m = K - f
+    if not 1 <= m <= K:
+        raise ValueError(f"--select_m {m} must lie in [1, K={K}]")
+    if args.robustLR_threshold > m:
+        raise ValueError(f"--robustLR_threshold {args.robustLR_threshold} > {m} admitted participants would flip every coordinate")
+    args.select_f, args.select_m = f, m
 
 
 def args_parser(argv=None) -> argparse.Namespace:
@@ -165,4 +206,6 @@ def print_exp_details(args) -> None:
     print(f"    Crop pad / hflip: {args.crop_pad} / {args.hflip}")
     if getattr(args, "server_opt", "sgd") != "sgd":
         print(f"    Server optimizer (beta1 / beta2 / tau): {args.server_opt} ({args.server_beta1} / {args.server_beta2} / {args.server_tau})")
+    if getattr(args, "select", "none") != "none":
+        print(f"    Selection (F / M): {args.select} ({args.select_f} / {args.select_m})")
     print("======================================")

@@ -153,11 +153,54 @@ class FusedAggregator:
             self._tables[n_part] = ops.PtrTable(ptrs, self.ctx.device)
         return self._tables[n_part]
 
-    def aggregate(self, weights, mode, theta, server_lr, noise_std=0.0, seed=0, rnd=0, scales=None):
-        """Aggregate the first ``len(weights)`` participants (participant j lives in ``slot_owner(j)``) and update
-        ``w_global`` on every rank.  Returns nothing; ``self.flipped`` accumulates the flipped-coordinate count."""
+    def gathers(self, n_part: int) -> bool:
+        """True when a round of ``n_part`` participants runs on all-gathered copies of the participants (the nccl / gloo transports,
+        and more participants than the fused kernel's tables hold).  Selection then gathers once (``gather_participants``) and hands the
+        copies to both ``pairwise_sqdist`` and ``aggregate``."""
+        return self.ctx.is_dist and not (self.backend == "fused" and n_part <= ops.MAX_FUSED_AGENTS)
+
+    def pairwise_sqdist(self, n_part: int, scales=None, participants=None):
+        """K x K float64 squared distances between the round's ``n_part`` participants' updates over ``[0, n_vote)`` (Krum / Multi-Krum
+        selection), identical on every rank.  Call it after the slots are final and before ``aggregate`` of the same round.
+
+        Fused multi-GPU path: each rank runs ``pairwise_sqdist_kernel`` over its coordinate slice of the peer-mapped participant slots,
+        behind the aggregation kernel's barrier-in (an epoch of its own), and the ranks all_gather their partial matrices and add them in
+        rank order.  Gather transport and single process: the same kernel over ``participants`` (every participant's parameters on
+        this rank, as ``gather_participants`` returns them; gathered here when not given).  The reduce transport never holds cross-rank
+        pairs, so selection always takes the gather transport, as the coordinate median does."""
+        ctx, dev = self.ctx, self.ctx.device
+        if self.backend == "fused" and ctx.is_dist and n_part <= ops.MAX_FUSED_AGENTS:
+            if scales is not None:
+                self.acquire()                       # the clipped distances read this rank's w_global
+            self.epoch += 1
+            part = torch.empty(n_part, n_part, dtype=torch.float64, device=dev)
+            sc = torch.as_tensor(scales, dtype=torch.float32).to(dev) if scales is not None else None
+            ops.ext().pairwise_sqdist(self._agent_table(n_part).tensor, self.w_global.data_ptr() if sc is not None else 0, sc,
+                                      self.begin, max(self.begin, min(self.end, self.n_vote)), part, self.flag_ptrs.tensor,
+                                      self.local_sync, ctx.rank, ctx.world, self.epoch)
+            parts = ctx.all_gather(part)                                 # [world, K, K]
+            D = parts[0].clone()
+            for r in range(1, ctx.world):
+                D += parts[r]
+            return D
+        agents = self._participants(n_part, participants)
+        return ops.pairwise_sqdist(agents, self.n_vote, self.w_global if scales is not None else None, scales)
+
+    def aggregate(self, weights, mode, theta, server_lr, noise_std=0.0, seed=0, rnd=0, scales=None, members=None, participants=None):
+        """Aggregate the round's ``len(weights)`` participants (participant j lives in ``slot_owner(j)``; ``weights`` and ``scales`` are
+        per participant) and update ``w_global`` on every rank.  ``members``: positions of the participants admitted by selection
+        (ascending); only they enter the vote, the rule, the BatchNorm mean and the server step.  ``participants``: copies from
+        ``gather_participants`` for the gather transport (gathered here when not given).  Returns nothing; ``self.flipped`` accumulates
+        the flipped-coordinate count."""
         n_part = len(weights)
         ctx, dev = self.ctx, self.ctx.device
+        if members is not None and [int(j) for j in members] == list(range(n_part)):
+            members = None                           # everyone admitted: exactly the unselected launch
+        if members is not None:
+            idx = [int(j) for j in members]
+            weights = [weights[j] for j in idx]
+            if scales is not None:
+                scales = scales[torch.as_tensor(idx, device=scales.device)] if torch.is_tensor(scales) else [scales[j] for j in idx]
         self.flipped.zero_()
         self.flipped_is_partial = False
         fused_p2p = self.backend == "fused" and ctx.is_dist and n_part <= ops.MAX_FUSED_AGENTS
@@ -169,8 +212,10 @@ class FusedAggregator:
             self.epoch += 1
             wt = torch.as_tensor(weights, dtype=torch.float64).to(dev)
             sc = torch.as_tensor(scales, dtype=torch.float32).to(dev) if scales is not None else None
+            table = self._agent_table(n_part) if members is None else ops.PtrTable(
+                [self.buf.peer_ptr(r, self.off_slots + 4 * self.n * s) for r, s in map(self.slot_owner, idx)], dev)
             ops.ext().fused_aggregate(
-                self._agent_table(n_part).tensor, wt, sc, float(sum(float(x) for x in weights)), self.w_global.data_ptr(),
+                table.tensor, wt, sc, float(sum(float(x) for x in weights)), self.w_global.data_ptr(),
                 self.out_ptrs.tensor, self.out_bf16_ptrs.tensor if self.out_bf16_ptrs else None, self.use_multimem,
                 self.begin, self.end, self.n_vote, ops.MODE_IDS[mode], int(theta), float(server_lr), float(noise_std),
                 int(seed), int(rnd), self.flipped, self.flag_ptrs.tensor, self.local_sync, ctx.rank, ctx.world, self.epoch,
@@ -179,16 +224,13 @@ class FusedAggregator:
                 self.epoch_dev.fill_(self.epoch)      # what the next round's consumers wait for (stream-ordered before their graphs)
             return
         # ---- baseline transports / single process ------------------------------------------------------------------
-        if ctx.is_dist and self.transport == "reduce" and mode in ("avg", "sign"):
+        if ctx.is_dist and self.transport == "reduce" and mode in ("avg", "sign") and members is None:
             self._aggregate_reduce(weights, mode, theta, server_lr, noise_std, seed, rnd, scales)
             return
         # gather participant params, run the kernel locally
-        if ctx.is_dist:
-            mine = torch.stack(self.slots, 0)                       # [max_slots, n]
-            allp = ctx.all_gather(mine)                             # [world, max_slots, n]
-            agents = [allp[j % ctx.world, j // ctx.world] for j in range(n_part)]
-        else:
-            agents = [self.slots[j] for j in range(n_part)]
+        agents = self._participants(n_part, participants)
+        if members is not None:
+            agents = [agents[j] for j in idx]
         ops.fused_aggregate(self.w_global, agents, weights, mode, theta, server_lr, noise_std, seed, rnd, self.n_vote,
                             scales, out=self.w_global, out_bf16=self.w_bf16, flipped=self.flipped, opt=self.opt)
 
@@ -242,12 +284,20 @@ class FusedAggregator:
 
     def gather_participants(self, n_part: int):
         """Every participant's flat parameter vector on THIS rank (list of ``n_part`` tensors; remote slots are copied through an
-        all_gather).  Off the hot path: used by the ``--diagnostics`` analyses and by bench.py's post-run aggregation check."""
+        all_gather).  The gather transport's input, and the copies the ``--diagnostics`` analyses and bench.py's post-run aggregation
+        check read."""
         ctx = self.ctx
         if not ctx.is_dist:
             return [self.slots[j] for j in range(n_part)]
         allp = ctx.all_gather(torch.stack(self.slots, 0))            # [world, max_slots, n]
         return [allp[j % ctx.world, j // ctx.world] for j in range(n_part)]
+
+    def _participants(self, n_part: int, participants):
+        if participants is None:
+            return self.gather_participants(n_part)
+        if len(participants) != n_part:
+            raise ValueError(f"{len(participants)} participant copies for {n_part} participants")
+        return list(participants)
 
     def update_norms(self, n_part: int):
         """||w_j - w_global|| for every participant (float64 [n_part]), computed where the slot lives."""

@@ -37,33 +37,42 @@ class Aggregation:
         self.fused = fused            # parallel.FusedAggregator or None (pure in-process use)
         self.cum_net_mov = 0.0
         self.last_flipped = 0
-        self.last_admitted = None     # agent ids admitted by --select in the last round
+        self.last_admitted = None     # agent ids admitted by --select (and trusted by --aggr fltrust) in the last round
         self.last_select = None       # the Select/* scalars of the last round
+        self.last_trust = None        # the Trust/* scalars of the last round (--aggr fltrust)
         self.opt = None               # full-length server optimizer state of the in-process form (allocated on first use)
 
     # ---- the server step ------------------------------------------------------------------------------------
-    def aggregate_updates(self, w_global, agent_params, cur_round, n_vote=None):
-        """In-process form: ``agent_params`` = {agent_id: flat local parameters}.  Updates ``w_global`` in place."""
+    def aggregate_updates(self, w_global, agent_params, cur_round, n_vote=None, root_params=None):
+        """In-process form: ``agent_params`` = {agent_id: flat local parameters}.  Updates ``w_global`` in place.  ``root_params``:
+        the server's root-trained parameters, needed by ``--aggr fltrust``."""
         ids = list(agent_params.keys())
         ws = [agent_params[i] for i in ids]
         nv = n_vote if n_vote is not None else (self.layout.n_vote if self.layout else None)
         scales = self._clip_scales(ops.update_norms(w_global, ws, nv)) if self._server_clip else None
         all_ids, all_ws = ids, ws
+        keep, total = None, None
         if self._select:
             D = ops.pairwise_sqdist(ws, nv if nv is not None else w_global.numel(), w_global if scales is not None else None, scales)
             keep = self._admit(D, ids, cur_round)
-            if len(keep) < len(ids):
-                ids, ws = [ids[j] for j in keep], [ws[j] for j in keep]
-                scales = scales[torch.as_tensor(keep, device=scales.device)] if scales is not None else None
-        weights = [float(self.agent_data_sizes[i]) for i in ids]
+        if self._fltrust:
+            if root_params is None:
+                raise ValueError("--aggr fltrust needs the server's root parameters (root_params)")
+            stats = ops.trust_stats(ws, root_params, w_global, nv)
+            keep, weights, scales, total = self._trust(stats, ids, keep, cur_round)
+        else:
+            weights = [float(self.agent_data_sizes[i]) for i in ids]
+        if keep is not None and len(keep) < len(ids):
+            ids, ws, weights = [ids[j] for j in keep], [ws[j] for j in keep], [weights[j] for j in keep]
+            scales = scales[torch.as_tensor(keep, device=scales.device)] if scales is not None else None
         prev = w_global.clone() if self.args.diagnostics else None
         flipped = torch.zeros(1, dtype=torch.int64, device=w_global.device)
         if self.opt is None:
             self.opt = ops.ServerOptState(n=w_global.numel(), device=w_global.device, **server_opt_spec(self.args))
-        ops.fused_aggregate(w_global, ws, weights, self.args.aggr, self.args.robustLR_threshold, self.server_lr,
+        ops.fused_aggregate(w_global, ws, weights, self._mode, self.args.robustLR_threshold, self.server_lr,
                             self.args.noise * self.args.clip, self.args.seed, cur_round,
                             n_vote if n_vote is not None else (self.layout.n_vote if self.layout else None),
-                            scales, out=w_global, flipped=flipped, opt=self.opt)
+                            scales, out=w_global, flipped=flipped, opt=self.opt, total_weight=total)
         self.last_flipped = flipped
         if self.args.diagnostics:
             self.plot_norms(dict(zip(all_ids, ops.update_norms(prev, all_ws, nv).tolist())), cur_round)
@@ -71,28 +80,36 @@ class Aggregation:
         return
 
     def aggregate_slots(self, participants, cur_round):
-        """Engine form: participant j's parameters live in ``fused.slot_owner(j)``; updates every rank's global."""
+        """Engine form: participant j's parameters live in ``fused.slot_owner(j)``; updates every rank's global.  Under
+        ``--aggr fltrust`` the server's root job is position ``len(participants)``."""
+        K = len(participants)
         weights = [float(self.agent_data_sizes[i]) for i in participants]
         scales = None
         norms = None
+        total = None
         diag = bool(self.args.diagnostics)
         if self._server_clip or diag:
-            norms = self.fused.update_norms(len(participants))
+            norms = self.fused.update_norms(K)
         if self._server_clip:
             scales = self._clip_scales(norms)
-        keep, copies = None, None
+        keep, copies, gathered = None, None, None
+        if (self._select or self._fltrust) and self.fused.gathers(K):
+            # on the gather transport every pass reads the same all-gathered copies (one all_gather per round; the root job included)
+            gathered = self.fused.gather_participants(K + 1 if self._fltrust else K)
+            copies = gathered[:K]
         if self._select:
-            # on the gather transport both passes read the same all-gathered copies (one all_gather per round)
-            copies = self.fused.gather_participants(len(participants)) if self.fused.gathers(len(participants)) else None
-            keep = self._admit(self.fused.pairwise_sqdist(len(participants), scales, copies), participants, cur_round)
+            keep = self._admit(self.fused.pairwise_sqdist(K, scales, copies), participants, cur_round)
+        if self._fltrust:
+            keep, weights, scales, total = self._trust(self.fused.trust_stats(K, K, gathered), participants, keep, cur_round)
         if diag:   # the sign-agreement analysis needs the pre-step global parameters and every admitted participant's parameters
             prev = self.fused.w_global.clone()
-            ws = [w.clone() for w in self.fused.gather_participants(len(participants))]
+            ws = [w.clone() for w in self.fused.gather_participants(K)]
             voters = participants
             if keep is not None:
                 ws, voters = [ws[j] for j in keep], [participants[j] for j in keep]
-        self.fused.aggregate(weights, self.args.aggr, self.args.robustLR_threshold, self.server_lr,
-                             self.args.noise * self.args.clip, self.args.seed, cur_round, scales, members=keep, participants=copies)
+        self.fused.aggregate(weights, self._mode, self.args.robustLR_threshold, self.server_lr,
+                             self.args.noise * self.args.clip, self.args.seed, cur_round, scales, members=keep, participants=copies,
+                             total_weight=total)
         self.last_flipped = self.fused.flipped
         if diag:
             self.plot_norms(dict(zip(participants, norms.tolist())), cur_round)
@@ -118,6 +135,44 @@ class Aggregation:
             for k, v in self.last_select.items():
                 self.writer.add_scalar(k, v, cur_round)
         return keep
+
+    @property
+    def _fltrust(self):
+        return self.args.aggr == "fltrust"
+
+    @property
+    def _mode(self):
+        """The aggregate kernel's rule: FLTrust is its weighted mean with trust weights and per-participant scales."""
+        return "avg" if self._fltrust else self.args.aggr
+
+    def _trust(self, stats, ids, keep, cur_round):
+        """FLTrust admission from the statistics ``stats`` (``ops.trust_statement``'s layout) of the participants ``ids``, among the
+        positions ``keep`` that selection admitted (all when None).  Returns ``(members, weights, scales, total_weight)`` for the step:
+        the trusted positions (TS > 0) with weights TS, scales s and total weight sum TS -- or, when nobody is trusted, every candidate
+        with weight 0 and total weight 1, so the aggregate is 0 (plus noise) and the round still runs its one aggregate launch.
+        Records ``last_admitted`` and logs the mean trust of honest (ids >= num_corrupt) and corrupt participants."""
+        K = len(ids)
+        s = stats.detach().double().cpu()
+        ts, scales, _ = ops.fltrust_weights(s[:K], s[K:2 * K], s[2 * K])
+        cand = list(range(K)) if keep is None else [int(j) for j in keep]
+        members = [j for j in cand if ts[j] > 0]
+        weights = [float(ts[j]) for j in range(K)]
+        total = sum(weights[j] for j in members)
+        if not members:
+            members, total = cand, 1.0
+            weights = [0.0] * K
+        self.last_admitted = [ids[j] for j in cand if ts[j] > 0]
+        nc = self.args.num_corrupt
+        honest = [float(ts[j]) for j in cand if ids[j] >= nc]
+        corrupt = [float(ts[j]) for j in cand if ids[j] < nc]
+        self.last_trust = {"Trust/Avg_Honest": sum(honest) / len(honest) if honest else None,
+                           "Trust/Avg_Corrupt": sum(corrupt) / len(corrupt) if corrupt else None,
+                           "Trust/Admitted": len(self.last_admitted)}
+        if self.writer is not None:
+            for k, v in self.last_trust.items():
+                if v is not None:
+                    self.writer.add_scalar(k, v, cur_round)
+        return members, weights, scales, total
 
     def _clip_scales(self, norms):
         """reference ``clip_updates`` (src/aggregation.py:77-81): update /= max(1, ||update||/clip)."""

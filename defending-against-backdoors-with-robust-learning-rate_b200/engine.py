@@ -34,6 +34,21 @@ from .trainers import make_trainer
 from .utils import MetricLogger, PhaseTimer, get_loss_n_accuracy, load_checkpoint, restore_server_opt, save_checkpoint
 
 
+_ROOT_SET_TAG = 0x464C5472           # "FLTr": keeps the root-set draw apart from every other stream seeded by --seed
+
+
+def draw_root_set(n_train: int, excluded, size: int, seed: int):
+    """FLTrust's root set: ``size`` distinct training-sample indices drawn uniformly without replacement from ``[0, n_train)`` minus
+    ``excluded`` (the poisoned samples), seeded by ``seed`` alone -- every rank, and a resumed run, draws the same set.  Ascending
+    int64 array; raises ValueError when fewer than ``size`` samples are eligible."""
+    keep = np.ones(int(n_train), dtype=bool)
+    keep[np.asarray(list(excluded), dtype=np.int64)] = False
+    pool = np.flatnonzero(keep)
+    if not 1 <= size <= pool.size:
+        raise ValueError(f"--root_size {size}: only {pool.size} of {n_train} training samples are unpoisoned")
+    return np.sort(np.random.default_rng([int(seed), _ROOT_SET_TAG]).choice(pool, int(size), replace=False)).astype(np.int64)
+
+
 class FLEngine:
     def __init__(self, args, ctx=None, datasets=None, verbose=True):
         self.args = args
@@ -75,9 +90,16 @@ class FLEngine:
                 self.agents.append(Agent(_id, args, self.train_dataset, groups[_id], seed=args.seed))
         for a in self.agents:
             self.agent_data_sizes[a.id] = a.n_data
+        # ---- FLTrust: the server's root job, an agent (id num_agents, never corrupt) on a clean sample of the training set -----------
+        self.root_agent = None
+        if args.aggr == "fltrust":
+            poisoned = [i for a in self.agents for i in a.poisoned_idxs]      # poisoning is in place on the shared dataset
+            root = draw_root_set(len(self.train_dataset), poisoned, args.root_size, args.seed)
+            self.root_agent = Agent(args.num_agents, args, self.train_dataset, root.tolist(), seed=args.seed)
         self.n_part = max(1, math.floor(args.num_agents * args.agent_frac))
-        max_slots = (self.n_part + ctx.world - 1) // ctx.world
-        max_shard = max(a.n_data for a in self.agents)
+        n_jobs = self.n_part + (1 if self.root_agent is not None else 0)   # the root job is position n_part of every round
+        max_slots = (n_jobs + ctx.world - 1) // ctx.world
+        max_shard = max(a.n_data for a in self._jobs())
 
         # ---- parameters: flat, symmetric ---------------------------------------------------------------------
         backend = args.backend
@@ -137,6 +159,10 @@ class FLEngine:
             self.cum_poison_acc_mean = ck["extra"].get("cum_poison_acc_mean", 0.0)
         ctx.barrier()
 
+    def _jobs(self):
+        """Every agent this engine may train: the clients, then the FLTrust root job."""
+        return self.agents + ([self.root_agent] if self.root_agent is not None else [])
+
     # ---- sampling (src/federated.py:68; seeded here) ---------------------------------------------------------
     def sample_agents(self, rnd: int):
         rs = np.random.RandomState((self.args.seed * 1_000_003 + rnd) % (2 ** 31))
@@ -173,12 +199,12 @@ class FLEngine:
         self._stream_src = {}
         dev = self.ctx.device
         pin = (lambda t: t.cpu().pin_memory()) if dev.type == "cuda" else (lambda t: t.cpu().clone())
-        total, n_max = 0, max(a.n_data for a in self.agents)
+        total, n_max = 0, max(a.n_data for a in self._jobs())
         ref = self.agents[0].dataset
         # one staging dataset per in-flight trainer: trainer i always trains out of buffer i, so its CUDA graphs keep their addresses
         self._stream_bufs = [DeviceDataset(ref.name, torch.zeros((n_max, *ref.data.shape[1:]), dtype=ref.data.dtype, device=dev),
                                            torch.zeros(n_max, dtype=torch.int64, device=dev)) for _ in self.trainers]
-        for a in self.agents:
+        for a in self._jobs():
             x, y = a.dataset.data[a.idxs].contiguous(), a.dataset.targets[a.idxs].contiguous()
             self._stream_src[a.id] = (pin(x), pin(y))
             a.dataset = self._stream_bufs[0]                         # re-pointed to its trainer's buffer right before training
@@ -213,25 +239,31 @@ class FLEngine:
                 cur = torch.cuda.current_stream(ctx.device)
                 for st_ in self.streams:
                     st_.wait_stream(cur)                                 # w_global of this round is ready
+        jobs = [self.agents[aid] for aid in chosen]
+        if self.root_agent is not None:
+            jobs.append(self.root_agent)                                 # position len(chosen): trained like any agent
         k = 0
-        for j, aid in enumerate(chosen):
+        for j, agent in enumerate(jobs):
             r, s = fused.slot_owner(j)
             if r != ctx.rank:
                 continue
-            agent = self.agents[aid]
+            client = agent is not self.root_agent                        # the loss and step count describe the clients
             if concurrent:
                 i = k % len(self.trainers)
                 with (torch.cuda.stream(self.streams[i]) if self.streams is not None else contextlib.nullcontext()):
                     if stream_inputs:
                         h2d += self._upload_shard(agent, self._stream_bufs[i])     # on stream i: ordered after trainer i's previous agent
                     st = agent.local_train(self.trainers[i], self.w_global, fused.slots[s], rnd)
-                    self._loss_parts[i] += st["loss_sum"]
+                    if client:
+                        self._loss_parts[i] += st["loss_sum"]
             else:
                 if stream_inputs:
                     h2d += self._upload_shard(agent)
                 st = agent.local_train(self.trainer, self.w_global, fused.slots[s], rnd)
-                self.round_loss += st["loss_sum"]
-            steps += st["steps"]
+                if client:
+                    self.round_loss += st["loss_sum"]
+            if client:
+                steps += st["steps"]
             k += 1
         if concurrent:
             if self.streams is not None:
@@ -314,6 +346,10 @@ class FLEngine:
             if self.aggregator.last_select is not None:
                 rec["select_corrupt_participants"] = self.aggregator.last_select["Select/Corrupt_Participants"]
                 rec["select_corrupt_admitted"] = self.aggregator.last_select["Select/Corrupt_Admitted"]
+            if self.aggregator.last_trust is not None:
+                rec["trust_avg_honest"] = self.aggregator.last_trust["Trust/Avg_Honest"]
+                rec["trust_avg_corrupt"] = self.aggregator.last_trust["Trust/Avg_Corrupt"]
+                rec["trust_admitted"] = self.aggregator.last_trust["Trust/Admitted"]
             rec.update({f"ms_{k}": v for k, v in self.timer.elapsed().items()})
             if args.profile_phases and self.verbose:
                 print({k: round(v, 3) for k, v in rec.items() if k.startswith("ms_")})

@@ -12,6 +12,7 @@ The reference has no operator layer at all (SURVEY.md 2.4): each row of that tab
 from __future__ import annotations
 
 import importlib.util
+import math
 import os
 import threading
 from typing import NamedTuple
@@ -373,12 +374,13 @@ def _server_update(g, agg, signs, mean_tail, theta, server_lr, n_vote, opt):
 
 
 def aggregate_oracle(w_global, w_agents, weights, mode="avg", theta=0, server_lr=1.0, noise=None, n_vote=None,
-                     scales=None, opt=None):
+                     scales=None, opt=None, total_weight=None):
     """fp64 PyTorch statement of the server step (reference src/aggregation.py:19-75).
 
     ``w_agents``: list of local parameter vectors; updates are ``w_k - w_global``.  ``noise``: optional pre-sampled
     noise vector (added to the aggregate BEFORE the lr multiply).  Coordinates ``>= n_vote`` get a plain weighted mean.
-    ``opt``: optional ``ServerOptState`` (full length); its state is updated in place.
+    ``opt``: optional ``ServerOptState`` (full length); its state is updated in place.  ``total_weight``: the weighted mean's
+    denominator (default ``sum(weights)``).
     Returns ``(new_global_fp32, n_flipped)``.
     """
     g = w_global.double()
@@ -386,10 +388,11 @@ def aggregate_oracle(w_global, w_agents, weights, mode="avg", theta=0, server_lr
     n_vote = n if n_vote is None else int(n_vote)
     ups = [(w.double() - g) for w in w_agents]
     wt = torch.as_tensor(weights, dtype=torch.float64, device=g.device)
-    mean_raw = sum(w_ * u for w_, u in zip(wt, ups)) / wt.sum()     # tail coordinates (BatchNorm statistics) are never clip-scaled
+    tot = wt.sum() if total_weight is None else float(total_weight)
+    mean_raw = sum(w_ * u for w_, u in zip(wt, ups)) / tot     # tail coordinates (BatchNorm statistics) are never clip-scaled
     if scales is not None:
         ups = [u * float(s) for u, s in zip(ups, scales)]
-    mean = sum(w_ * u for w_, u in zip(wt, ups)) / wt.sum()
+    mean = sum(w_ * u for w_, u in zip(wt, ups)) / tot
     signs = sum(torch.sign(u) for u in ups)
     if mode == "avg":
         agg = mean.clone()
@@ -447,11 +450,12 @@ class PtrTable:
 
 
 def fused_aggregate(w_global, w_agents, weights, mode="avg", theta=0, server_lr=1.0, noise_std=0.0, seed=0,
-                    noise_stream=0, n_vote=None, scales=None, out=None, out_bf16=None, flipped=None, opt=None):
+                    noise_stream=0, n_vote=None, scales=None, out=None, out_bf16=None, flipped=None, opt=None, total_weight=None):
     """Single-process fused server step: ``out <- w_global + lr ⊙ agg({w_k - w_global})`` in one kernel.
 
     On CUDA this launches ``fused_aggregate_kernel`` (ops/csrc/aggregate.cu); on CPU it runs the fp64 oracle (with
     torch-sampled noise).  ``out`` may alias ``w_global``.  ``opt``: optional full-length ``ServerOptState``, updated in place.
+    ``total_weight``: the weighted mean's denominator (default ``sum(weights)``; FLTrust passes 1 when every weight is 0).
     Returns the tensor written.  The multi-GPU variant (peer pointers, multicast stores, in-kernel barriers) is driven by
     ``parallel.fused_agg.FusedAggregator``.
     """
@@ -464,7 +468,8 @@ def fused_aggregate(w_global, w_agents, weights, mode="avg", theta=0, server_lr=
             gen = torch.Generator().manual_seed(int(seed) * 1000003 + int(noise_stream))
             noise = torch.randn(n, generator=gen, dtype=torch.float64) * noise_std
             noise[n_vote:] = 0
-        new, nflip = aggregate_oracle(w_global, w_agents, weights, mode, theta, server_lr, noise, n_vote, scales, opt)
+        new, nflip = aggregate_oracle(w_global, w_agents, weights, mode, theta, server_lr, noise, n_vote, scales, opt,
+                                      total_weight)
         out.copy_(new)
         if out_bf16 is not None:
             out_bf16.copy_(new.to(torch.bfloat16))
@@ -481,7 +486,8 @@ def fused_aggregate(w_global, w_agents, weights, mode="avg", theta=0, server_lr=
             gen = torch.Generator(device=dev).manual_seed(int(seed) * 1000003 + int(noise_stream))
             noise = torch.randn(n, generator=gen, dtype=torch.float64, device=dev) * noise_std
             noise[n_vote:] = 0
-        new, nflip = aggregate_oracle(w_global, w_agents, weights, mode, theta, server_lr, noise, n_vote, scales, opt)
+        new, nflip = aggregate_oracle(w_global, w_agents, weights, mode, theta, server_lr, noise, n_vote, scales, opt,
+                                      total_weight)
         out.copy_(new)
         if out_bf16 is not None:
             out_bf16.copy_(new.to(torch.bfloat16))
@@ -496,7 +502,8 @@ def fused_aggregate(w_global, w_agents, weights, mode="avg", theta=0, server_lr=
     outs_b = PtrTable([out_bf16.data_ptr()], dev) if out_bf16 is not None else None
     wt = torch.as_tensor(weights, dtype=torch.float64).to(dev)
     sc = torch.as_tensor(scales, dtype=torch.float32).to(dev) if scales is not None else None
-    ext().fused_aggregate(agents.tensor, wt, sc, float(sum(float(x) for x in weights)), w_global.data_ptr(), outs.tensor,
+    tot = float(sum(float(x) for x in weights)) if total_weight is None else float(total_weight)
+    ext().fused_aggregate(agents.tensor, wt, sc, tot, w_global.data_ptr(), outs.tensor,
                           outs_b.tensor if outs_b else None, False, 0, n, n_vote, MODE_IDS[mode], int(theta),
                           float(server_lr), float(noise_std), int(seed), int(noise_stream), flipped, None, None, 0, 1, 0,
                           False, *opt_launch_args(opt))
@@ -585,6 +592,70 @@ def krum_select(D, ids, f, m):
     scores = np.cumsum(others, axis=1)[:, -1].tolist()       # cumsum adds sequentially: the ascending order of the statement
     order = sorted(range(K), key=lambda i: (scores[i], ids[i]))
     return sorted(order[: int(m)])
+
+
+# =====================================================================================================================
+# FLTrust (Cao, Fang, Liu, Gong, NDSS 2021): trust scores against the server's root update
+# =====================================================================================================================
+def trust_statement(w_agents, w_ref, w_global, lo, hi):
+    """fp64 statement of the FLTrust statistics over coordinates ``[lo, hi)``: a float64 ``[2K + 1]`` tensor holding
+    ``d_k = sum_c Δk[c] Δ0[c]`` (K values), ``q_k = sum_c Δk[c]^2`` (K values) and ``q0 = sum_c Δ0[c]^2``, with ``Δk = w_k - w_global``
+    and ``Δ0 = w_ref - w_global``."""
+    K = len(w_agents)
+    dev = w_global.device
+    out = torch.zeros(2 * K + 1, dtype=torch.float64, device=dev)
+    step = max(4, (1 << 24) // max(1, K))                 # coordinates per pass: K * step fp64 values
+    for c in range(lo, hi, step):
+        e = min(hi, c + step)
+        g = w_global[c:e].double()
+        x = torch.stack([w[c:e] for w in w_agents]).double() - g
+        d0 = w_ref[c:e].double() - g
+        out[:K] += x @ d0
+        out[K:2 * K] += (x * x).sum(1)
+        out[2 * K] += (d0 * d0).sum()
+    return out
+
+
+def trust_stats(w_agents, w_ref, w_global, n_vote=None):
+    """FLTrust statistics (``trust_statement``'s layout) of the participants ``w_agents`` against the root parameters ``w_ref`` over the
+    voted coordinates ``[0, n_vote)`` (the BatchNorm running statistics behind ``n_vote`` do not count).  On CUDA this launches
+    ``trust_stats_kernel`` (ops/csrc/trust.cu); on CPU, and for more participants than the kernel's tables hold (recorded as a library
+    fall-through), it evaluates ``trust_statement``."""
+    nv = w_global.numel() if n_vote is None else int(n_vote)
+    if not w_global.is_cuda:
+        return trust_statement(w_agents, w_ref, w_global, 0, nv)
+    dev = w_global.device
+    if len(w_agents) > MAX_FUSED_AGENTS:
+        note_fallback("trust_stats", f"K={len(w_agents)} > {MAX_FUSED_AGENTS}")
+        return trust_statement(w_agents, w_ref, w_global, 0, nv)
+    assert nv % 4 == 0, "flat buffers are padded to multiples of 4"
+    for w in (*w_agents, w_ref, w_global):
+        assert w.is_cuda and w.dtype == torch.float32 and w.is_contiguous() and w.numel() >= nv
+    tab = PtrTable([w.data_ptr() for w in w_agents], dev, w_agents)
+    out = torch.empty(2 * len(w_agents) + 1, dtype=torch.float64, device=dev)
+    ext().trust_stats(tab.tensor, w_ref.data_ptr(), w_global.data_ptr(), 0, nv, out, None, None, 0, 1, 0)
+    return out
+
+
+def fltrust_weights(d, q, q0):
+    """FLTrust trust scores and rescaling on the host, in fp64, shared by every path: ``TS_k = max(0, d_k / sqrt(q_k q0))`` (0 when
+    ``q_k`` or ``q0`` is 0, or the cosine is NaN) and ``s_k = fp32(sqrt(q0 / q_k))`` (1 when ``q_k = 0``), which rescales update k to
+    the root update's norm.  Returns ``(TS float64 [K], s float32 [K], admitted positions)``: the positions with ``TS > 0``,
+    ascending."""
+    d = np.asarray(torch.as_tensor(d).detach().double().cpu().numpy(), dtype=np.float64).reshape(-1)
+    q = np.asarray(torch.as_tensor(q).detach().double().cpu().numpy(), dtype=np.float64).reshape(-1)
+    q0 = float(q0)
+    K = d.shape[0]
+    ts = np.zeros(K, dtype=np.float64)
+    sc = np.ones(K, dtype=np.float32)
+    for k in range(K):
+        qk = float(q[k])
+        if qk > 0 and q0 > 0:
+            c = float(d[k]) / math.sqrt(qk * q0)
+            ts[k] = c if c > 0 else 0.0             # NaN -> 0
+        if qk > 0:
+            sc[k] = np.float32(math.sqrt(q0 / qk))
+    return torch.from_numpy(ts), torch.from_numpy(sc), [k for k in range(K) if ts[k] > 0]
 
 
 # =====================================================================================================================

@@ -124,6 +124,28 @@ void pairwise_sqdist(at::Tensor w_agent_ptrs, int64_t w_global_ptr, c10::optiona
     check(rlr::launch_pairwise_sqdist(p, out.data_ptr<double>(), num_sms(), cur_stream()), "pairwise_sqdist");
 }
 
+// FLTrust statistics over coordinates [begin, end): fp64 [2K + 1] = (Δk.Δ0 for every k, |Δk|^2 for every k, |Δ0|^2), Δk = w_k - w_global,
+// Δ0 = w_ref - w_global.  world > 1: the fused multi-GPU form, which first runs the aggregation's barrier-in at `epoch`.
+void trust_stats(at::Tensor w_agent_ptrs, int64_t w_ref_ptr, int64_t w_global_ptr, int64_t begin, int64_t end, at::Tensor out,
+                 c10::optional<at::Tensor> flag_ptrs, c10::optional<at::Tensor> local_sync, int64_t rank, int64_t world, int64_t epoch) {
+    CHECK_CUDA(w_agent_ptrs); CHECK_CUDA(out);
+    TORCH_CHECK(w_agent_ptrs.scalar_type() == at::kLong, "pointer table must be int64");
+    const int64_t K = w_agent_ptrs.numel();
+    TORCH_CHECK(out.scalar_type() == at::kDouble && out.numel() == 2 * K + 1, "out must be a float64 [2K + 1] tensor");
+    TORCH_CHECK(w_ref_ptr && w_global_ptr, "trust_stats needs w_ref and w_global");
+    c10::cuda::CUDAGuard guard(out.device());
+    rlr::TrustParams p{};
+    p.w_agents = reinterpret_cast<const float* const*>(w_agent_ptrs.data_ptr());
+    p.w_ref = reinterpret_cast<const float*>(w_ref_ptr);
+    p.w_global = reinterpret_cast<const float*>(w_global_ptr);
+    p.begin = begin; p.end = end;
+    p.K = (int)K;
+    p.flag_ptrs = ptr_or_null<uint32_t* const>(flag_ptrs);
+    p.local_sync = ptr_or_null<uint32_t>(local_sync);
+    p.rank = (int)rank; p.world = (int)world; p.epoch = (uint32_t)epoch;
+    check(rlr::launch_trust_stats(p, out.data_ptr<double>(), num_sms(), cur_stream()), "trust_stats");
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // training augmentation of the gathers: crop pad, flip, Philox key and the device int64 stream word (needed when either is on)
 inline const long long* aug_stream_ptr(const c10::optional<at::Tensor>& stream, int64_t crop_pad, bool flip) {
@@ -331,6 +353,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("acquire_slices", &acquire_slices);
     m.def("update_sqnorm", &update_sqnorm);
     m.def("pairwise_sqdist", &pairwise_sqdist);
+    m.def("trust_stats", &trust_stats);
     m.def("gather_normalize", &gather_normalize);
     m.def("gather_im2col", &gather_im2col);
     m.def("stamp_pixels", &stamp_pixels);

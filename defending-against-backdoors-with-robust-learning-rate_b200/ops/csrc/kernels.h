@@ -62,6 +62,22 @@ struct DistParams {
 };
 cudaError_t launch_pairwise_sqdist(const DistParams& p, double* out, int num_sms, cudaStream_t st);
 
+// ---- FLTrust: each participant's update against the server's root update Δ0 = w_ref - w_global -----------------------------------------
+// out[k] = sum_c Δk[c] Δ0[c], out[K + k] = sum_c Δk[c]^2, out[2K] = sum_c Δ0[c]^2 over [begin, end), fp64 [2K + 1], Δk = w_k - w_global.
+// Fixed-order sums, no atomics: bitwise reproducible.
+struct TrustParams {
+    const float* const* w_agents;   // [K] device pointers (local or peer-mapped)
+    const float* w_ref;             // the root job's parameters (local or peer-mapped)
+    const float* w_global;          // this rank's global parameters
+    long long begin, end;           // coordinate range (multiples of 4), already clipped to [0, n_vote)
+    int K;
+    uint32_t* const* flag_ptrs;     // world > 1: the aggregation's barrier-in words and intra-GPU ready flag (ops/csrc/aggregate.cu)
+    uint32_t* local_sync;
+    int rank, world;
+    uint32_t epoch;
+};
+cudaError_t launch_trust_stats(const TrustParams& p, double* out, int num_sms, cudaStream_t st);
+
 // ---- data path ---------------------------------------------------------------------------------------
 // out_kind: 0 fp32, 1 bf16.  nchw: output layout NCHW (Cpad ignored) else NHWC with channels padded to c_pad.
 // Both gathers: crop_pad > 0 or flip turns on the training augmentation (AugSpec, common.cuh): sample b of the batch is drawn

@@ -14,7 +14,8 @@ import math
 import torch
 
 DATASETS = ("fmnist", "fedemnist", "cifar10")
-AGGREGATORS = ("avg", "comed", "sign")
+AGGREGATORS = ("avg", "comed", "sign", "fltrust")
+ROOT_SIZE = 100                  # FLTrust root set: the paper's 100 clean samples
 SERVER_OPTS = ("sgd", "momentum", "adagrad", "adam", "yogi")
 SELECTIONS = ("none", "krum", "multikrum")
 PATTERNS = ("plus", "square", "copyright", "apple")
@@ -34,7 +35,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--agent_frac", type=float, default=1, help="fraction of agents per round: C")
     p.add_argument("--num_corrupt", type=int, default=0, help="number of corrupt agents (ids 0..n-1)")
     p.add_argument("--rounds", type=int, default=200, help="number of communication rounds: R")
-    p.add_argument("--aggr", type=str, default="avg", help="aggregation rule: avg | comed | sign")
+    p.add_argument("--aggr", type=str, default="avg",
+                   help="aggregation rule: avg | comed | sign | fltrust (trust-weighted mean against a server-trained root update)")
     p.add_argument("--local_ep", type=int, default=2, help="number of local epochs: E")
     p.add_argument("--bs", type=int, default=256, help="local batch size: B")
     p.add_argument("--client_lr", type=float, default=0.1, help="clients' learning rate")
@@ -108,6 +110,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--select_f", type=int, default=-1,
                    help="Byzantine participants the selection assumes (-1 = ceil(num_corrupt * K / num_agents), K participants per round)")
     p.add_argument("--select_m", type=int, default=0, help="participants multikrum admits (0 = K - F; krum admits 1)")
+    p.add_argument("--root_size", type=int, default=None,
+                   help=f"--aggr fltrust: clean training samples the server trains its root update on each round (default {ROOT_SIZE}); "
+                        "drawn once from --seed, never a poisoned sample")
     return p
 
 
@@ -136,7 +141,24 @@ def finalize_args(args: argparse.Namespace) -> argparse.Namespace:
     if not 0 <= args.crop_pad < side:
         raise ValueError(f"--crop_pad {args.crop_pad} must lie in [0, {side}) for --data {args.data} ({meta.height}x{meta.width} images)")
     _finalize_select(args)
+    _finalize_fltrust(args)
     return args
+
+
+def _finalize_fltrust(args) -> None:
+    """Validate the FLTrust flags and resolve ``root_size`` in place (``ROOT_SIZE`` by default under ``--aggr fltrust``)."""
+    root_size = getattr(args, "root_size", None)
+    if args.aggr != "fltrust":
+        if root_size is not None:
+            raise ValueError("--root_size needs --aggr fltrust")
+        return
+    if getattr(args, "server_clip", False):
+        raise ValueError("--server_clip does not combine with --aggr fltrust, which rescales every update to the root update's norm")
+    if root_size is None:
+        root_size = ROOT_SIZE
+    if root_size < 1:
+        raise ValueError(f"--root_size {root_size} must be >= 1")
+    args.root_size = int(root_size)
 
 
 def _finalize_select(args) -> None:
@@ -208,4 +230,6 @@ def print_exp_details(args) -> None:
         print(f"    Server optimizer (beta1 / beta2 / tau): {args.server_opt} ({args.server_beta1} / {args.server_beta2} / {args.server_tau})")
     if getattr(args, "select", "none") != "none":
         print(f"    Selection (F / M): {args.select} ({args.select_f} / {args.select_m})")
+    if args.aggr == "fltrust":
+        print(f"    Root set: {args.root_size}")
     print("======================================")

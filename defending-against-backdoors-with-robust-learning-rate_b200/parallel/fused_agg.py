@@ -186,12 +186,45 @@ class FusedAggregator:
         agents = self._participants(n_part, participants)
         return ops.pairwise_sqdist(agents, self.n_vote, self.w_global if scales is not None else None, scales)
 
-    def aggregate(self, weights, mode, theta, server_lr, noise_std=0.0, seed=0, rnd=0, scales=None, members=None, participants=None):
+    def trust_stats(self, n_part: int, ref: int, participants=None):
+        """FLTrust statistics (``ops.trust_statement``'s float64 ``[2 n_part + 1]`` layout) of the round's ``n_part`` participants against
+        the root job at position ``ref`` (its parameters live in ``slot_owner(ref)``) over ``[0, n_vote)``, identical on every rank.
+        Call it after the slots are final and before ``aggregate`` of the same round.
+
+        Fused multi-GPU path: each rank runs ``trust_stats_kernel`` over its coordinate slice of the peer-mapped slots, behind the
+        aggregation kernel's barrier-in (an epoch of its own), and the ranks all_gather their partials and add them in rank order.  The
+        pass reads ``w_global``, so it first acquires the broadcast slices of a fused hand-off.  Gather transport and single process:
+        the same kernel over ``participants`` (``gather_participants(max(n_part, ref + 1))``'s copies, indexed by position; gathered
+        here when not given).  The reduce transport never holds a participant and the root on one rank, so the trust pass always takes
+        the gather transport; the step that follows then gathers too whenever it leaves a participant out (``members``), and forms the
+        same weighted mean from all-reduced partials when every participant is trusted or none is."""
+        ctx, dev = self.ctx, self.ctx.device
+        if self.backend == "fused" and ctx.is_dist and n_part <= ops.MAX_FUSED_AGENTS:
+            self.acquire()
+            self.epoch += 1
+            part = torch.empty(2 * n_part + 1, dtype=torch.float64, device=dev)
+            owner, slot = self.slot_owner(ref)
+            ops.ext().trust_stats(self._agent_table(n_part).tensor, self.buf.peer_ptr(owner, self.off_slots + 4 * self.n * slot),
+                                  self.w_global.data_ptr(), self.begin, max(self.begin, min(self.end, self.n_vote)), part,
+                                  self.flag_ptrs.tensor, self.local_sync, ctx.rank, ctx.world, self.epoch)
+            parts = ctx.all_gather(part)                                 # [world, 2 n_part + 1]
+            out = parts[0].clone()
+            for r in range(1, ctx.world):
+                out += parts[r]
+            return out
+        copies = participants if participants is not None else self.gather_participants(max(n_part, ref + 1))
+        if len(copies) <= max(n_part - 1, ref):
+            raise ValueError(f"{len(copies)} participant copies for {n_part} participants and the root job at position {ref}")
+        return ops.trust_stats(list(copies[:n_part]), copies[ref], self.w_global, self.n_vote)
+
+    def aggregate(self, weights, mode, theta, server_lr, noise_std=0.0, seed=0, rnd=0, scales=None, members=None, participants=None,
+                  total_weight=None):
         """Aggregate the round's ``len(weights)`` participants (participant j lives in ``slot_owner(j)``; ``weights`` and ``scales`` are
         per participant) and update ``w_global`` on every rank.  ``members``: positions of the participants admitted by selection
         (ascending); only they enter the vote, the rule, the BatchNorm mean and the server step.  ``participants``: copies from
-        ``gather_participants`` for the gather transport (gathered here when not given).  Returns nothing; ``self.flipped`` accumulates
-        the flipped-coordinate count."""
+        ``gather_participants`` for the gather transport (gathered here when not given).  ``total_weight``: the weighted mean's
+        denominator (default: the members' summed weights).  Returns nothing; ``self.flipped`` accumulates the flipped-coordinate
+        count."""
         n_part = len(weights)
         ctx, dev = self.ctx, self.ctx.device
         if members is not None and [int(j) for j in members] == list(range(n_part)):
@@ -201,6 +234,7 @@ class FusedAggregator:
             weights = [weights[j] for j in idx]
             if scales is not None:
                 scales = scales[torch.as_tensor(idx, device=scales.device)] if torch.is_tensor(scales) else [scales[j] for j in idx]
+        total = float(sum(float(x) for x in weights)) if total_weight is None else float(total_weight)
         self.flipped.zero_()
         self.flipped_is_partial = False
         fused_p2p = self.backend == "fused" and ctx.is_dist and n_part <= ops.MAX_FUSED_AGENTS
@@ -215,7 +249,7 @@ class FusedAggregator:
             table = self._agent_table(n_part) if members is None else ops.PtrTable(
                 [self.buf.peer_ptr(r, self.off_slots + 4 * self.n * s) for r, s in map(self.slot_owner, idx)], dev)
             ops.ext().fused_aggregate(
-                table.tensor, wt, sc, float(sum(float(x) for x in weights)), self.w_global.data_ptr(),
+                table.tensor, wt, sc, total, self.w_global.data_ptr(),
                 self.out_ptrs.tensor, self.out_bf16_ptrs.tensor if self.out_bf16_ptrs else None, self.use_multimem,
                 self.begin, self.end, self.n_vote, ops.MODE_IDS[mode], int(theta), float(server_lr), float(noise_std),
                 int(seed), int(rnd), self.flipped, self.flag_ptrs.tensor, self.local_sync, ctx.rank, ctx.world, self.epoch,
@@ -225,16 +259,16 @@ class FusedAggregator:
             return
         # ---- baseline transports / single process ------------------------------------------------------------------
         if ctx.is_dist and self.transport == "reduce" and mode in ("avg", "sign") and members is None:
-            self._aggregate_reduce(weights, mode, theta, server_lr, noise_std, seed, rnd, scales)
+            self._aggregate_reduce(weights, mode, theta, server_lr, noise_std, seed, rnd, scales, total)
             return
         # gather participant params, run the kernel locally
         agents = self._participants(n_part, participants)
         if members is not None:
             agents = [agents[j] for j in idx]
         ops.fused_aggregate(self.w_global, agents, weights, mode, theta, server_lr, noise_std, seed, rnd, self.n_vote,
-                            scales, out=self.w_global, out_bf16=self.w_bf16, flipped=self.flipped, opt=self.opt)
+                            scales, out=self.w_global, out_bf16=self.w_bf16, flipped=self.flipped, opt=self.opt, total_weight=total)
 
-    def _aggregate_reduce(self, weights, mode, theta, server_lr, noise_std, seed, rnd, scales):
+    def _aggregate_reduce(self, weights, mode, theta, server_lr, noise_std, seed, rnd, scales, total_weight):
         """All-reduce transport: every rank folds its local participants into (vote, weighted sum), two all_reduce calls make them
         global, and every rank finishes the identical server step locally (ops.aggregate_from_partials).  The noise vector is
         drawn from a torch generator seeded like the CPU oracle on every rank (same stream everywhere; it is NOT the Philox
@@ -250,7 +284,7 @@ class FusedAggregator:
             gen = torch.Generator().manual_seed(int(seed) * 1000003 + int(rnd))
             noise = (torch.randn(self.n, generator=gen, dtype=torch.float64) * noise_std).to(self.w_global.device)
             noise[self.n_vote:] = 0
-        new, nflip = ops.aggregate_from_partials(self.w_global, vote, wsum, sum(float(x) for x in weights), mode, theta, server_lr,
+        new, nflip = ops.aggregate_from_partials(self.w_global, vote, wsum, total_weight, mode, theta, server_lr,
                                                  noise, self.n_vote, self.opt)
         self.w_global.copy_(new)
         if self.w_bf16 is not None:

@@ -17,6 +17,8 @@
 //   warp 9 = second TMA producer for the B tiles.
 // * 4-stage (BN=64) / 3-stage (BN=128) smem ring with full/empty mbarriers; a stage is released once the wgmma group that read
 //   it has retired; two CTAs are resident per SM (<= 113 KB smem each) so one CTA's epilogue overlaps the other's mainloop.
+// * one-wave configuration (kOcc = 1, BN = 128): a grid that fits the SMs in a single wave has no second CTA to hide behind, so it
+//   runs one CTA per SM with a deep ring (6 x 32 KB) -- see pick_conv_tile.
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -37,8 +39,10 @@ constexpr int kEpiThreads = kConsumers;
 
 template <int BN, int kOcc = 2>
 struct TileCfg {
-    // two CTAs per SM: 4 x 24 KB / 3 x 32 KB ring; three CTAs per SM (kOcc = 3): 3 x 24 KB / 2 x 32 KB ring
-    static constexpr int kStages = kOcc == 3 ? (BN == 64 ? 3 : 2) : (BN == 64 ? 4 : 3);
+    // two CTAs per SM: 4 x 24 KB / 3 x 32 KB ring; three CTAs per SM (kOcc = 3): 3 x 24 KB / 2 x 32 KB ring;
+    // one CTA per SM (kOcc = 1, one-wave grids of the 128-wide tile): 6 x 32 KB ring
+    static_assert(kOcc != 1 || BN == 128, "the one-wave configuration exists for the 128-wide tile");
+    static constexpr int kStages = kOcc == 1 ? 6 : kOcc == 3 ? (BN == 64 ? 3 : 2) : (BN == 64 ? 4 : 3);
     static constexpr int kABytes = BM * BK * 2;
     static constexpr int kBBytes = BN * BK * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
@@ -48,14 +52,12 @@ struct TileCfg {
     static_assert(kStagingBytes + 2 * BN * 4 <= kRingBytes, "staging aliases the operand ring");
     static constexpr int kTailBytes = BN == 128 ? 2048 : 1024;   // barriers, row index (640 B) + the tile's bias values (BN floats)
     static constexpr int kSmemBytes = kRingBytes + 1024 /*align slack*/ + kTailBytes;
+    static_assert(kStages <= 8, "SharedTail holds eight barriers per array");
 };
 
 struct __align__(8) SharedTail {
-    uint64_t full[4];
-    uint64_t empty[4];
-    uint64_t pad0;
-    uint32_t pad1;
-    uint32_t pad2;
+    uint64_t full[8];
+    uint64_t empty[8];
     int row_index[BM];   // global output row of each tile row, -1 = masked
 };
 static_assert(sizeof(SharedTail) <= 640, "the bias slice starts 640 bytes into the tail");
@@ -387,20 +389,22 @@ static int conv_occ3() {
     return g_occ3;
 }
 
-// default (RLR_CONV_OCC3=0 disables): 64-wide tiles with a 3-stage ring at three CTAs per SM (three TMA producers / MMA issue threads per SM)
-template <int BN>
-static cudaError_t launch_bn_occ3(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const ConvGemmParams& p, int m_tiles,
-                                  cudaStream_t st) {
-    using Cfg = TileCfg<BN, 3>;
+// The configurations next to the two-CTA default, for launches whose statistics (if any) ride on the TMA-store epilogue:
+// kOcc = 3 (default for the 64-wide tile, RLR_CONV_OCC3=0 disables): a 3-stage ring at three CTAs per SM (three TMA producers / MMA
+// issue threads per SM); kOcc = 1: the one-wave configuration (pick_conv_tile).
+template <int BN, int kOcc>
+static cudaError_t launch_bn_occ(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const ConvGemmParams& p, int m_tiles,
+                                 cudaStream_t st) {
+    using Cfg = TileCfg<BN, kOcc>;
     static bool configured = false;
     if (!configured) {
-        RLR_CUDA_CHECK(cudaFuncSetAttribute(umma_conv_gemm_kernel<BN, false, false, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-        RLR_CUDA_CHECK(cudaFuncSetAttribute(umma_conv_gemm_kernel<BN, false, true, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+        RLR_CUDA_CHECK(cudaFuncSetAttribute(umma_conv_gemm_kernel<BN, false, false, kOcc>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+        RLR_CUDA_CHECK(cudaFuncSetAttribute(umma_conv_gemm_kernel<BN, false, true, kOcc>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
         configured = true;
     }
     dim3 grid(m_tiles, (p.N + BN - 1) / BN);
-    if (p.b_mn) return launch_kernel(umma_conv_gemm_kernel<BN, false, true, 3>, grid, dim3(kThreads), Cfg::kSmemBytes, st, tmA, tmB, tmC, p);
-    return launch_kernel(umma_conv_gemm_kernel<BN, false, false, 3>, grid, dim3(kThreads), Cfg::kSmemBytes, st, tmA, tmB, tmC, p);
+    if (p.b_mn) return launch_kernel(umma_conv_gemm_kernel<BN, false, true, kOcc>, grid, dim3(kThreads), Cfg::kSmemBytes, st, tmA, tmB, tmC, p);
+    return launch_kernel(umma_conv_gemm_kernel<BN, false, false, kOcc>, grid, dim3(kThreads), Cfg::kSmemBytes, st, tmA, tmB, tmC, p);
 }
 
 static int sm_count() {
@@ -454,12 +458,9 @@ static cudaError_t make_out_tmap(CUtensorMap* tmC, const ConvGemmParams& p) {
     return make_tmap_bf16(tmC, p.out, 2, d, s, b);
 }
 
-template <int BN>
-static cudaError_t launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvGemmParams& p_in, int m_tiles, cudaStream_t st) {
-    using Cfg = TileCfg<BN>;
-    ConvGemmParams p = p_in;
+// Epilogue and producer settings every launch of the kernel shares; tmC is written only when the TMA-store epilogue applies.
+static void finish_params(ConvGemmParams& p, CUtensorMap& tmC) {
     p.dbg = g_trace;
-    CUtensorMap tmC = tmA;                                       // dummy unless the TMA-store epilogue applies
     {   // slots used by the TMA-store epilogue's statistics (RLR_EPI_STAT_SLOTS; python reads the same variable for the prefix it reduces)
         static const int epi_slots = [] { const char* e = getenv("RLR_EPI_STAT_SLOTS"); int v = e ? atoi(e) : 2; return v < 1 ? 1 : (v > kStatSlots ? kStatSlots : v); }();
         p.stat_slots = epi_slots;
@@ -469,6 +470,12 @@ static cudaError_t launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, con
         p.tma_store = 1;
     if (g_split_prod < 0) { const char* e = getenv("RLR_SPLIT_PRODUCER"); g_split_prod = (e && atoi(e) == 0) ? 0 : 1; }   // default on
     p.split_prod = (g_split_prod && !p.b_src) ? 1 : 0;
+}
+
+template <int BN>
+static cudaError_t launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const ConvGemmParams& p, int m_tiles,
+                             cudaStream_t st) {
+    using Cfg = TileCfg<BN>;
     if (p.b_src && !p.stats && p.N <= BN) {
         // stem GEMM: ONE k-block per output tile, so a one-tile CTA is all fixed cost (set-up, the filter gather, a lone TMA round trip).
         // The persistent kernel builds the B tile once per SM, streams the A tiles through its ring and overlaps every tile's epilogue
@@ -482,7 +489,7 @@ static cudaError_t launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, con
         return launch_persistent_bn<BN>(tmA, tmB, p, m_tiles, persistent_sms(), st);
     // statistics ride on the TMA-store epilogue of the plain instantiation (runtime p.stats); without TMA stores: the kStats variant below
     if constexpr (BN == 64)
-        if ((!p.stats || p.tma_store) && conv_occ3() >= 1) return launch_bn_occ3<BN>(tmA, tmB, tmC, p, m_tiles, st);
+        if ((!p.stats || p.tma_store) && conv_occ3() >= 1) return launch_bn_occ<BN, 3>(tmA, tmB, tmC, p, m_tiles, st);
     static bool configured = false;
     if (!configured) {
         RLR_CUDA_CHECK(cudaFuncSetAttribute(umma_conv_gemm_kernel<BN, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
@@ -497,6 +504,30 @@ static cudaError_t launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, con
 }
 
 static int pick_bn(int N) { return (N % 128 == 0) ? 128 : 64; }
+
+static int g_one_wave = 1;
+void set_conv_one_wave(int on) { g_one_wave = on ? 1 : 0; }
+
+// Tile of an implicit-GEMM convolution over `px` output pixels (`m_tiles` 128-pixel boxes), Cout filters and `num_kb` k-blocks.
+// A 128-wide grid smaller than the SMs goes to the 64-wide tile so that every SM has work, but the N = 64 MMA is shared-memory
+// bound and reads 1.5x the L2 operand bytes.  So when the 128-wide grid still fills one wave -- at least 0.9 of the SMs -- it is
+// launched in the one-wave configuration (one CTA per SM, deep ring) instead: the 512-filter 3x3 layers of ResNet-18 at batch 256,
+// 32 x 4 = 128 CTAs on 132 SMs, run 1.4-1.6x faster launched alone (H100 SXM at 700 W, docs/PROFILE_H100.md).
+// One CTA per SM exposes the tile's prologue and epilogue, so the reduction has to be deep: launches of 4-16 k-blocks (1x1
+// shortcuts, stride-2 data-gradient parity planes) measured no gain and keep their tile.
+// `one_wave_ok`: the launch can run an instantiation the one-wave configuration is compiled for (launch_bn_occ).
+constexpr int kOneWaveMinKb = 24;
+struct ConvTile { int bn; bool one_wave; };
+static ConvTile pick_conv_tile(long long px, int m_tiles, int Cout, int num_kb, bool one_wave_ok) {
+    const int sms = sm_count();
+    if (g_one_wave && one_wave_ok && Cout % 128 == 0 && num_kb >= kOneWaveMinKb) {
+        const int ctas = m_tiles * (Cout / 128);
+        if (ctas <= sms && 10 * ctas >= 9 * sms) return {128, true};
+    }
+    const int bn = pick_bn(Cout);
+    if (bn == 128 && ((px + BM - 1) / BM) * (Cout / 128) < sms) return {64, false};
+    return {bn, false};
+}
 
 // Plain GEMM: out[M][ldc] (bf16) = A[M][K] * B[N][K]^T (+bias)(relu).  K % 64 == 0, N % 64 == 0.
 cudaError_t launch_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K, int lda, int ldb, int ldc,
@@ -524,7 +555,9 @@ cudaError_t launch_gemm_bf16(const void* A, const void* B, void* out, int M, int
     p.M = M; p.N = N; p.num_kb = K / BK; p.mode = 0; p.in_stride = 1; p.out_stride = 1;
     p.out = out; p.ldc = ldc; p.bias = bias; p.stats = stats; p.relu = relu; p.accumulate = accumulate;
     if (drop && drop->thr) p.drop = *drop;      // fused dropout lives in the epilogue
-    return bn == 128 ? launch_bn<128>(tmA, tmB, p, m_tiles, st) : launch_bn<64>(tmA, tmB, p, m_tiles, st);
+    CUtensorMap tmC = tmA;
+    finish_params(p, tmC);
+    return bn == 128 ? launch_bn<128>(tmA, tmB, tmC, p, m_tiles, st) : launch_bn<64>(tmA, tmB, tmC, p, m_tiles, st);
 }
 
 // Stem GEMM (tiny-K first layer): A is the im2col matrix [M][64] (gather_im2col), W the un-padded bf16 filter [N][ldw] with kvalid <= 64
@@ -548,7 +581,9 @@ cudaError_t launch_stem_gemm_bf16(const void* A, const void* W, void* out, int M
     p.out = out; p.ldc = N; p.bias = bias; p.stats = stats; p.relu = relu; p.accumulate = 0;
     p.b_src = reinterpret_cast<const __nv_bfloat16*>(W); p.b_ld = ldw; p.b_kvalid = kvalid;
     p.wait_flags = wait_flags; p.wait_lo = wait_lo; p.wait_hi = wait_hi; p.wait_epoch = wait_epoch;
-    return bn == 128 ? launch_bn<128>(tmA, tmA, p, m_tiles, st) : launch_bn<64>(tmA, tmA, p, m_tiles, st);   // tmB unused: B is gathered by the warp
+    CUtensorMap tmC = tmA;
+    finish_params(p, tmC);
+    return bn == 128 ? launch_bn<128>(tmA, tmA, tmC, p, m_tiles, st) : launch_bn<64>(tmA, tmA, tmC, p, m_tiles, st);   // tmB unused: B is gathered by the warp
 }
 
 static int pow2_ceil(int x) { int p = 1; while (p < x) p <<= 1; return p; }
@@ -562,13 +597,7 @@ cudaError_t launch_conv_bf16(const void* x, const void* w, void* out, int NB, in
     if (Cin % BK || Cout % 8 || ntaps < 1 || ntaps > 9) return cudaErrorInvalidValue;
     if (in_stride < 1 || in_stride > 2 || out_stride < 1 || out_stride > 2 || (in_stride > 1 && planes != 1)) return cudaErrorInvalidValue;
     if (wtap && (stats || Cout % 64)) return cudaErrorInvalidValue;   // MN-major filter path: whole 64-wide ci groups, no statistics
-    int bn = pick_bn(Cout);
     ConvGemmParams p{};
-    {   // few M tiles (deep layers at small batch / 4x4 maps): prefer the 64-wide tile so the grid covers all SMs
-        static const int small_bn64 = [] { const char* e = getenv("RLR_SMALL_BN64"); return e ? atoi(e) : 1; }();
-        const long long px = (long long)NB * Ho * Wo;
-        if (small_bn64 && bn == 128 && ((px + BM - 1) / BM) * (Cout / 128) < sm_count()) bn = 64;
-    }
     // output tile: TW x TH x TN = 128 output pixels, TW/TH powers of two covering the image
     int TW = pow2_ceil(Wo); if (TW > BM) TW = BM;
     int TH = pow2_ceil(Ho); if (TW * TH > BM) TH = BM / TW;
@@ -584,7 +613,10 @@ cudaError_t launch_conv_bf16(const void* x, const void* w, void* out, int NB, in
     p.in_stride = in_stride; p.out_stride = out_stride; p.out_ph = out_ph; p.out_pw = out_pw; p.OutH = Ho * out_stride; p.OutW = Wo * out_stride;
     for (int t = 0; t < ntaps; ++t) { p.dh[t] = (int8_t)dh[t]; p.dw[t] = (int8_t)dw[t]; p.dn[t] = dplane[t] * NB; }
     p.out = out; p.ldc = ldc; p.bias = bias; p.stats = stats; p.relu = relu; p.accumulate = accumulate;
-    CUtensorMap tmA, tmB;
+    CUtensorMap tmA, tmB, tmC{};
+    finish_params(p, tmC);
+    const ConvTile tile = pick_conv_tile((long long)NB * Ho * Wo, m_tiles, Cout, p.num_kb, !p.stats || p.tma_store);
+    const int bn = tile.bn;
     {
         const uint64_t d[4] = {(uint64_t)Cin, (uint64_t)Win, (uint64_t)Hin, (uint64_t)planes * NB};
         const uint64_t s[3] = {(uint64_t)Cin * 2, (uint64_t)Win * Cin * 2, (uint64_t)Hin * Win * Cin * 2};
@@ -607,7 +639,8 @@ cudaError_t launch_conv_bf16(const void* x, const void* w, void* out, int NB, in
         const uint32_t b[2] = {BK, (uint32_t)bn};
         RLR_CUDA_CHECK(make_tmap_bf16(&tmB, w, 2, d, s, b));
     }
-    return bn == 128 ? launch_bn<128>(tmA, tmB, p, m_tiles, st) : launch_bn<64>(tmA, tmB, p, m_tiles, st);
+    if (tile.one_wave) return launch_bn_occ<128, 1>(tmA, tmB, tmC, p, m_tiles, st);
+    return bn == 128 ? launch_bn<128>(tmA, tmB, tmC, p, m_tiles, st) : launch_bn<64>(tmA, tmB, tmC, p, m_tiles, st);
 }
 
 }  // namespace rlr

@@ -69,6 +69,8 @@ cudaError_t launch_gemm_splitk_bf16(const void* A, const void* B, void* out, flo
 void set_persistent_conv(int on);
 // three CTAs per SM: level 0 never, 1 (default) for the 64-wide tile (RLR_CONV_OCC3 env; higher levels select 1)
 void set_conv_occ3(int level);
+// one-wave conv tiles (default on, see pick_conv_tile in gemm.cu); off: every conv launches the two- / three-CTA configurations
+void set_conv_one_wave(int on);
 // per-CTA timeline buffer for the NEXT launches of the generic conv / GEMM kernel (nullptr = off); see ConvGemmParams::dbg
 void set_conv_tma_store(int on);           // epilogue via TMA tensor stores (default on; RLR_TMA_STORE=0)
 void set_conv_split_producer(int on);      // experiment: two TMA producer threads per CTA (RLR_SPLIT_PRODUCER env)

@@ -383,6 +383,7 @@ void register_gemm_bindings(py::module_& m) {
     m.def("set_persistent_conv", [](bool on) { rlr::set_persistent_conv(on ? 1 : 0); });
     m.def("set_pdl", [](bool on) { rlr::set_pdl(on ? 1 : 0); });
     m.def("set_conv_occ3", [](int64_t level) { rlr::set_conv_occ3((int)level); });
+    m.def("set_conv_one_wave", [](bool on) { rlr::set_conv_one_wave(on ? 1 : 0); });
     m.def("set_conv_tma_store", [](bool on) { rlr::set_conv_tma_store(on ? 1 : 0); });
     m.def("set_conv_split_producer", [](bool on) { rlr::set_conv_split_producer(on ? 1 : 0); });
     m.def("set_conv_trace", [](c10::optional<at::Tensor> buf) {   // int64 [CTAs * 8] timeline buffer for the next generic conv / GEMM launches

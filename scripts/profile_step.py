@@ -1,9 +1,10 @@
 """Per-kernel profile of one training step of the bench.py workload (ResNet-18, CIFAR shape, batch 256, one GPU).
 
-    python scripts/profile_step.py [--out DIR] [--replays N] [--bs 256] [--model resnet18]
+    python scripts/profile_step.py [--out DIR] [--replays N] [--bs 256] [--model resnet18] [--previous_tiles]
 
 ``--model`` profiles another zoo model in the same configuration (e.g. ``resnet18_gn``).  ``--bn_reps`` sets the launches per call
-of the BatchNorm isolation and copy-reference measurements.
+of the BatchNorm isolation and copy-reference measurements.  ``--previous_tiles`` profiles the step without the one-wave conv tiles
+(``set_conv_one_wave(False)``), for an A/B in one session.
 
 Builds the engine exactly as ``bench.py`` does, runs one warm-up round (which captures the training-step CUDA graph), then
 replays the captured full-batch step ``--replays`` times under ``torch.profiler`` with CUDA activities.  The kernels inside the
@@ -52,19 +53,27 @@ def conv_tiles(NB, Ho, Wo):
     return -(-Wo // TW) * -(-Ho // TH) * -(-NB // TN)
 
 
-def pick_bn(N, m_tiles, sms, conv):
-    """Tile width launch_conv_bf16 / launch_gemm_bf16 choose (RLR_SMALL_BN64 default on for convs)."""
+ONE_WAVE = True        # False: the tiles of set_conv_one_wave(False)
+
+
+def pick_bn(N, K, m_tiles, sms, conv, one_wave=None):
+    """Tile width launch_conv_bf16 (pick_conv_tile in gemm.cu) / launch_gemm_bf16 choose: 128 when it divides N, else 64; a 128-wide
+    conv grid smaller than the SMs goes to the 64-wide tile, unless it fills one wave (0.9 of the SMs) over at least 24 k-blocks."""
+    if conv and (ONE_WAVE if one_wave is None else one_wave) and N % 128 == 0 and -(-K // BK) >= 24:
+        ctas = m_tiles * (N // 128)
+        if ctas <= sms and 10 * ctas >= 9 * sms:
+            return 128
     bn = 128 if N % 128 == 0 else 64
-    if conv and bn == 128 and m_tiles * (N // 128) < sms and int(os.environ.get("RLR_SMALL_BN64", "1")):
+    if conv and bn == 128 and m_tiles * (N // 128) < sms:
         bn = 64
     return bn
 
 
-def launch_record(kind, M, N, K, m_tiles, sms, conv, bmn=False, cluster=(1, 1)):
+def launch_record(kind, M, N, K, m_tiles, sms, conv, bmn=False, cluster=(1, 1), one_wave=None):
     """One implicit-GEMM launch: FLOP = 2 M N K (useful work, masked rows excluded) and L2 operand bytes = what the CTAs' TMA
     loads read, every CTA its own A and B tile per 64-deep k-block; an operand shared by the CTAs of a cluster is fetched once
     per cluster (``cluster`` = CTAs along M sharing B, along N sharing A)."""
-    bn = pick_bn(N, m_tiles, sms, conv)
+    bn = pick_bn(N, K, m_tiles, sms, conv, one_wave)
     n_tiles = -(-N // bn)
     kb = -(-K // BK)
     ctas = m_tiles * n_tiles
@@ -334,6 +343,7 @@ def main():
     ap.add_argument("--model", default="resnet18")
     ap.add_argument("--crop_pad", type=int, default=0, help="training augmentation of the profiled step (engine flag --crop_pad)")
     ap.add_argument("--hflip", action="store_true", help="training augmentation of the profiled step (engine flag --hflip)")
+    ap.add_argument("--previous_tiles", action="store_true", help="profile without the one-wave conv tiles (set_conv_one_wave(False))")
     ap.add_argument("--bn_reps", type=int, default=20, help="launches per BatchNorm call in the isolation and copy measurements")
     a = ap.parse_args()
 
@@ -347,6 +357,10 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("profile_step.py measures on the GPU; no CUDA device is visible")
     sms = torch.cuda.get_device_properties(0).multi_processor_count
+    if a.previous_tiles:
+        global ONE_WAVE
+        ONE_WAVE = False
+        ops.ext().set_conv_one_wave(False)
     log = []
     install_recorder(ops.ext(), sms, log)
     bn_log = []
@@ -427,13 +441,13 @@ def main():
     res = {"gpu": gpu, "model": a.model, "crop_pad": a.crop_pad, "hflip": a.hflip, "replays": a.replays, "batch": a.bs, "step_ms_unprofiled": step_ms_unprofiled,
            "kernel_us_per_step": total_us, "gemm_kernel_us_per_step": gemm_us, "gemm_kernel_share": gemm_us / total_us,
            "gemm_gflop_per_step": gemm_flop / 1e9, "gemm_tflops": gemm_flop / (gemm_us * 1e-6) / 1e12 if gemm_us else None,
-           "conv_cluster": os.environ.get("RLR_CONV_CLUSTER", "default"), "kernels": rows, "gemm_shapes": shape_rows,
+           "conv_cluster": os.environ.get("RLR_CONV_CLUSTER", "default"), "one_wave_tiles": ONE_WAVE, "kernels": rows, "gemm_shapes": shape_rows,
            "bn_shapes": bn_rows}
     os.makedirs(a.out, exist_ok=True)
     with open(os.path.join(a.out, "profile_step.json"), "w") as f:
         json.dump(res, f, indent=1)
     md = [f"GPU: {gpu} (name, power limit, max SM clock)  ",
-          f"Model: {a.model}, crop pad {a.crop_pad}, hflip {a.hflip}  ",
+          f"Model: {a.model}, crop pad {a.crop_pad}, hflip {a.hflip}, one-wave conv tiles {'on' if ONE_WAVE else 'off'}  ",
           f"Step (batch {a.bs}, graph replay, profiler off): {step_ms_unprofiled:.3f} ms; summed kernel time {total_us / 1e3:.3f} ms.  ",
           f"`{KERNEL}` (all instantiations): {gemm_us:.0f} us/step = {100 * gemm_us / total_us:.1f} % of kernel time, "
           f"{gemm_flop / 1e9:.0f} GFLOP/step, {res['gemm_tflops'] or 0:.0f} TFLOP/s.",

@@ -49,19 +49,14 @@ class Aggregation:
         ids = list(agent_params.keys())
         ws = [agent_params[i] for i in ids]
         nv = n_vote if n_vote is not None else (self.layout.n_vote if self.layout else None)
-        scales = self._clip_scales(ops.update_norms(w_global, ws, nv)) if self._server_clip else None
+        if self._fltrust and root_params is None:
+            raise ValueError("--aggr fltrust needs the server's root parameters (root_params)")
+        clip = self._clip_scales(ops.update_norms(w_global, ws, nv)) if self._server_clip else None
         all_ids, all_ws = ids, ws
-        keep, total = None, None
-        if self._select:
-            D = ops.pairwise_sqdist(ws, nv if nv is not None else w_global.numel(), w_global if scales is not None else None, scales)
-            keep = self._admit(D, ids, cur_round)
-        if self._fltrust:
-            if root_params is None:
-                raise ValueError("--aggr fltrust needs the server's root parameters (root_params)")
-            stats = ops.trust_stats(ws, root_params, w_global, nv)
-            keep, weights, scales, total = self._trust(stats, ids, keep, cur_round)
-        else:
-            weights = [float(self.agent_data_sizes[i]) for i in ids]
+        distances = lambda: ops.pairwise_sqdist(ws, nv if nv is not None else w_global.numel(), w_global if clip is not None else None,
+                                                clip)
+        keep, weights, scales, total = self._admission(ids, clip, distances, lambda: ops.trust_stats(ws, root_params, w_global, nv),
+                                                       cur_round)
         if keep is not None and len(keep) < len(ids):
             ids, ws, weights = [ids[j] for j in keep], [ws[j] for j in keep], [weights[j] for j in keep]
             scales = scales[torch.as_tensor(keep, device=scales.device)] if scales is not None else None
@@ -83,24 +78,16 @@ class Aggregation:
         """Engine form: participant j's parameters live in ``fused.slot_owner(j)``; updates every rank's global.  Under
         ``--aggr fltrust`` the server's root job is position ``len(participants)``."""
         K = len(participants)
-        weights = [float(self.agent_data_sizes[i]) for i in participants]
-        scales = None
-        norms = None
-        total = None
         diag = bool(self.args.diagnostics)
-        if self._server_clip or diag:
-            norms = self.fused.update_norms(K)
-        if self._server_clip:
-            scales = self._clip_scales(norms)
-        keep, copies, gathered = None, None, None
+        norms = self.fused.update_norms(K) if self._server_clip or diag else None
+        clip = self._clip_scales(norms) if self._server_clip else None
+        copies, gathered = None, None
         if (self._select or self._fltrust) and self.fused.gathers(K):
             # on the gather transport every pass reads the same all-gathered copies (one all_gather per round; the root job included)
             gathered = self.fused.gather_participants(K + 1 if self._fltrust else K)
             copies = gathered[:K]
-        if self._select:
-            keep = self._admit(self.fused.pairwise_sqdist(K, scales, copies), participants, cur_round)
-        if self._fltrust:
-            keep, weights, scales, total = self._trust(self.fused.trust_stats(K, K, gathered), participants, keep, cur_round)
+        keep, weights, scales, total = self._admission(participants, clip, lambda: self.fused.pairwise_sqdist(K, clip, copies),
+                                                       lambda: self.fused.trust_stats(K, K, gathered), cur_round)
         if diag:   # the sign-agreement analysis needs the pre-step global parameters and every admitted participant's parameters
             prev = self.fused.w_global.clone()
             ws = [w.clone() for w in self.fused.gather_participants(K)]
@@ -122,6 +109,15 @@ class Aggregation:
     @property
     def _select(self):
         return getattr(self.args, "select", "none") != "none"
+
+    def _admission(self, ids, clip, distances, trust_stats, cur_round):
+        """Admission of the participants ``ids`` shared by both forms of the step: Krum / Multi-Krum on ``distances()`` (``--select``),
+        then FLTrust on ``trust_stats()`` (``--aggr fltrust``).  ``clip``: the server-clipping scales or None.  Returns
+        ``(members, weights, scales, total_weight)`` for the step: members None admits everyone; weights are per position in ``ids``."""
+        keep = self._admit(distances(), ids, cur_round) if self._select else None
+        if self._fltrust:
+            return self._trust(trust_stats(), ids, keep, cur_round)
+        return keep, [float(self.agent_data_sizes[i]) for i in ids], clip, None
 
     def _admit(self, D, ids, cur_round):
         """Krum / Multi-Krum admission from the pairwise distances ``D`` of the participants ``ids``: the admitted positions

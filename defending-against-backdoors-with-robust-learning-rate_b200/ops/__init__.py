@@ -462,27 +462,14 @@ def fused_aggregate(w_global, w_agents, weights, mode="avg", theta=0, server_lr=
     n = w_global.numel()
     n_vote = n if n_vote is None else int(n_vote)
     out = w_global if out is None else out
-    if not w_global.is_cuda:
-        noise = None
-        if noise_std > 0:
-            gen = torch.Generator().manual_seed(int(seed) * 1000003 + int(noise_stream))
-            noise = torch.randn(n, generator=gen, dtype=torch.float64) * noise_std
-            noise[n_vote:] = 0
-        new, nflip = aggregate_oracle(w_global, w_agents, weights, mode, theta, server_lr, noise, n_vote, scales, opt,
-                                      total_weight)
-        out.copy_(new)
-        if out_bf16 is not None:
-            out_bf16.copy_(new.to(torch.bfloat16))
-        if flipped is not None:
-            flipped += nflip
-        return out
     dev = w_global.device
-    if len(w_agents) > MAX_FUSED_AGENTS:
-        # more participants than the kernel's pointer / weight tables hold (1024): exact torch evaluation on the device (fp64, same
-        # semantics) -- recorded as a library fall-through
-        note_fallback("fused_aggregate", f"K={len(w_agents)} > {MAX_FUSED_AGENTS}")
+    if not w_global.is_cuda or len(w_agents) > MAX_FUSED_AGENTS:
+        if w_global.is_cuda:
+            # more participants than the kernel's pointer / weight tables hold (1024): exact torch evaluation on the device (fp64,
+            # same semantics) -- recorded as a library fall-through
+            note_fallback("fused_aggregate", f"K={len(w_agents)} > {MAX_FUSED_AGENTS}")
         noise = None
-        if noise_std > 0:
+        if noise_std > 0:     # a torch generator on the data's device: the CPU and the device fall-through draw different streams
             gen = torch.Generator(device=dev).manual_seed(int(seed) * 1000003 + int(noise_stream))
             noise = torch.randn(n, generator=gen, dtype=torch.float64, device=dev) * noise_std
             noise[n_vote:] = 0
@@ -524,11 +511,34 @@ def update_norms(w_global, w_agents, n=None):
     n = w_global.numel() if n is None else int(n)
     if not w_global.is_cuda:
         return torch.stack([(w[:n].double() - w_global[:n].double()).norm() for w in w_agents])
-    dev = w_global.device
+    # the trust pass with the root parameters at w_global: the root update is 0, so its q_k = ||w_k - w_global||^2 come out of the same
+    # fixed-order sums (bitwise reproducible) while w_global is read once per group of participants.  q_k depends on participant k
+    # alone, so chunks of the kernel's table size keep any number of participants on the device.
+    out = torch.empty(len(w_agents), dtype=torch.float64, device=w_global.device)
+    for c in range(0, len(w_agents), MAX_FUSED_AGENTS):
+        part = w_agents[c:c + MAX_FUSED_AGENTS]
+        torch.sqrt(trust_stats(part, w_global, w_global, n)[len(part):2 * len(part)], out=out[c:c + len(part)])
+    return out
+
+
+def _participant_pass(site, w_agents, others, nv, shape, statement, launch):
+    """Dispatch of a per-participant pass over the voted coordinates ``[0, nv)``: the fp64 ``statement()`` on CPU and, recorded as a
+    library fall-through at ``site``, for more participants than the kernels' tables hold; else ``launch(table, out)`` on the device
+    pointer table of ``w_agents`` and a float64 ``out`` of ``shape``, which it returns.  ``others``: further flat buffers the kernel
+    reads."""
+    if not w_agents[0].is_cuda:
+        return statement()
+    if len(w_agents) > MAX_FUSED_AGENTS:
+        note_fallback(site, f"K={len(w_agents)} > {MAX_FUSED_AGENTS}")
+        return statement()
+    assert nv % 4 == 0, "flat buffers are padded to multiples of 4"
+    for w in (*w_agents, *others):
+        assert w.is_cuda and w.dtype == torch.float32 and w.is_contiguous() and w.numel() >= nv
+    dev = w_agents[0].device
     tab = PtrTable([w.data_ptr() for w in w_agents], dev, w_agents)
-    out = torch.zeros(len(w_agents), dtype=torch.float64, device=dev)
-    ext().update_sqnorm(tab.tensor, w_global.data_ptr(), n, out)
-    return out.sqrt()
+    out = torch.empty(shape, dtype=torch.float64, device=dev)
+    launch(tab.tensor, out)
+    return out
 
 
 # =====================================================================================================================
@@ -560,20 +570,13 @@ def pairwise_sqdist(w_agents, n_vote, w_global=None, scales=None):
     nv = w_agents[0].numel() if n_vote is None else int(n_vote)
     if scales is not None and w_global is None:
         raise ValueError("pairwise_sqdist: scales need w_global")
-    if not w_agents[0].is_cuda:
-        return sqdist_statement(w_agents, 0, nv, w_global, scales)
-    dev = w_agents[0].device
-    if len(w_agents) > MAX_FUSED_AGENTS:
-        note_fallback("pairwise_sqdist", f"K={len(w_agents)} > {MAX_FUSED_AGENTS}")
-        return sqdist_statement(w_agents, 0, nv, w_global, scales)
-    assert nv % 4 == 0, "flat buffers are padded to multiples of 4"
-    for w in w_agents:
-        assert w.is_cuda and w.dtype == torch.float32 and w.is_contiguous() and w.numel() >= nv
-    tab = PtrTable([w.data_ptr() for w in w_agents], dev, w_agents)
-    sc = torch.as_tensor(scales, dtype=torch.float32).to(dev) if scales is not None else None
-    out = torch.empty(len(w_agents), len(w_agents), dtype=torch.float64, device=dev)
-    ext().pairwise_sqdist(tab.tensor, w_global.data_ptr() if sc is not None else 0, sc, 0, nv, out, None, None, 0, 1, 0)
-    return out
+
+    def launch(tab, out):
+        sc = torch.as_tensor(scales, dtype=torch.float32).to(out.device) if scales is not None else None
+        ext().pairwise_sqdist(tab, w_global.data_ptr() if sc is not None else 0, sc, 0, nv, out, None, None, 0, 1, 0)
+    K = len(w_agents)
+    return _participant_pass("pairwise_sqdist", w_agents, (), nv, (K, K), lambda: sqdist_statement(w_agents, 0, nv, w_global, scales),
+                             launch)
 
 
 def krum_select(D, ids, f, m):
@@ -622,19 +625,10 @@ def trust_stats(w_agents, w_ref, w_global, n_vote=None):
     ``trust_stats_kernel`` (ops/csrc/trust.cu); on CPU, and for more participants than the kernel's tables hold (recorded as a library
     fall-through), it evaluates ``trust_statement``."""
     nv = w_global.numel() if n_vote is None else int(n_vote)
-    if not w_global.is_cuda:
-        return trust_statement(w_agents, w_ref, w_global, 0, nv)
-    dev = w_global.device
-    if len(w_agents) > MAX_FUSED_AGENTS:
-        note_fallback("trust_stats", f"K={len(w_agents)} > {MAX_FUSED_AGENTS}")
-        return trust_statement(w_agents, w_ref, w_global, 0, nv)
-    assert nv % 4 == 0, "flat buffers are padded to multiples of 4"
-    for w in (*w_agents, w_ref, w_global):
-        assert w.is_cuda and w.dtype == torch.float32 and w.is_contiguous() and w.numel() >= nv
-    tab = PtrTable([w.data_ptr() for w in w_agents], dev, w_agents)
-    out = torch.empty(2 * len(w_agents) + 1, dtype=torch.float64, device=dev)
-    ext().trust_stats(tab.tensor, w_ref.data_ptr(), w_global.data_ptr(), 0, nv, out, None, None, 0, 1, 0)
-    return out
+    return _participant_pass("trust_stats", w_agents, (w_ref, w_global), nv, (2 * len(w_agents) + 1,),
+                             lambda: trust_statement(w_agents, w_ref, w_global, 0, nv),
+                             lambda tab, out: ext().trust_stats(tab, w_ref.data_ptr(), w_global.data_ptr(), 0, nv, out,
+                                                                None, None, 0, 1, 0))
 
 
 def fltrust_weights(d, q, q0):

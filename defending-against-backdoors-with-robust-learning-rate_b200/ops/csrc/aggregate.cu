@@ -101,17 +101,8 @@ __device__ __forceinline__ void agg_prologue(const AggParams& p, AggShared& sh, 
         sh.wt[k] = p.weights[k];
         sh.sc[k] = p.scales ? p.scales[k] : 1.0f;
     }
-    // barrier-in: every peer's local training has finished and its w_k is globally visible
-    if (p.world > 1) {
-        if (blockIdx.x == 0) {
-            xgpu_barrier(p.flag_ptrs, 0, p.rank, p.world, p.epoch);
-            __syncthreads();
-            if (threadIdx.x == 0) st_release_gpu(p.local_sync, p.epoch);
-        } else if (threadIdx.x == 0) {
-            while ((int32_t)(ld_acquire_gpu(p.local_sync) - p.epoch) < 0) { __nanosleep(32); }
-        }
-    }
-    __syncthreads();
+    // every peer's local training has finished and its w_k is globally visible
+    barrier_in(p.gate, blockIdx.x == 0);
 }
 
 // ---- epilogue: flipped counter, then barrier-out or slice publication ------------------------------------------------------------
@@ -120,22 +111,23 @@ __device__ __forceinline__ void agg_epilogue(const AggParams& p, AggShared& sh, 
         const unsigned long long tot = block_sum<unsigned long long>(flipped, sh.scratch);
         if (threadIdx.x == 0 && tot) atomicAdd(p.flipped, tot);
     }
-    if (p.world > 1) {
+    const Gate& g = p.gate;
+    if (g.world > 1) {
         __threadfence_system();                    // this thread's (multicast / peer) stores are ordered before the flag stores below
         __syncthreads();
         if (threadIdx.x == 0) {
-            const unsigned prev = atomicAdd(p.local_sync + 1, 1u);
+            const unsigned prev = atomicAdd(g.local_sync + 1, 1u);
             sh.last = (prev == gridDim.x - 1);
-            if (sh.last) { p.local_sync[1] = 0; }
+            if (sh.last) { g.local_sync[1] = 0; }
             __threadfence();
         }
         __syncthreads();
         if (sh.last) {                             // the last CTA of this GPU: every CTA's stores are fenced
             if (p.handoff) {
                 // publish "slice `rank` of round `epoch` has landed" to every peer (slot 2*world + rank of its flag words); nobody waits
-                if ((int)threadIdx.x < p.world) st_release_sys(p.flag_ptrs[threadIdx.x] + 2 * p.world + p.rank, p.epoch);
+                if ((int)threadIdx.x < g.world) st_release_sys(g.flag_ptrs[threadIdx.x] + 2 * g.world + g.rank, g.epoch);
             } else {
-                xgpu_barrier(p.flag_ptrs, p.world, p.rank, p.world, p.epoch);
+                xgpu_barrier(g.flag_ptrs, g.world, g.rank, g.world, g.epoch);
             }
         }
     }
@@ -382,7 +374,7 @@ static cudaError_t launch_net(const AggParams& p, int grid, cudaStream_t st) {
 int aggregate_max_agents() { return kMaxAgents; }
 
 cudaError_t launch_fused_aggregate(const AggParams& p, int num_sms, cudaStream_t st) {
-    if (p.K < 1 || p.K > kMaxAgents) return cudaErrorInvalidValue;
+    if (p.K < 1 || p.K > kMaxAgents || !gate_ok(p.gate)) return cudaErrorInvalidValue;
     if (((p.end - p.begin) & 3) || (p.begin & 3) || (p.n_vote & 3)) return cudaErrorInvalidValue;
     if (p.opt < kOptSgd || p.opt > kOptYogi || (p.state_base & 3) || p.state_base > p.begin) return cudaErrorInvalidValue;
     if ((p.opt != kOptSgd && !p.opt_m) || (p.opt >= kOptAdagrad && !p.opt_v)) return cudaErrorInvalidValue;
@@ -451,31 +443,6 @@ cudaError_t launch_acquire_slices(const uint32_t* ready, int first, int last, co
                                   long long tail_n, cudaStream_t st) {
     if (ready && !epoch) return cudaErrorInvalidValue;
     acquire_slices_kernel<<<1, 32, 0, st>>>(ready, first, last, epoch, tail_src, tail_dst, tail_n);
-    return cudaGetLastError();
-}
-
-// ---- per-agent update L2 norms  ||w_k - w_g||_2^2  (server clipping + the Norms/* diagnostics) -------------
-__global__ void __launch_bounds__(256) update_sqnorm_kernel(const float* const* w_agents, const float* w_global,
-                                                              long long n, double* out /*[K]*/) {
-    __shared__ double scratch[32];
-    const float* w = w_agents[blockIdx.y];
-    double acc = 0.0;
-    for (long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 4; i < n; i += (long long)gridDim.x * blockDim.x * 4) {
-        const float4 a = ld_f4(w + i), g = ld_f4(w_global + i);
-        const float d0 = a.x - g.x, d1 = a.y - g.y, d2 = a.z - g.z, d3 = a.w - g.w;
-        acc += (double)(d0 * d0 + d1 * d1) + (double)(d2 * d2 + d3 * d3);
-    }
-    const double tot = block_sum<double>(acc, scratch);
-    if (threadIdx.x == 0) atomicAdd(out + blockIdx.y, tot);
-}
-
-cudaError_t launch_update_sqnorm(const float* const* w_agents, const float* w_global, long long n, int K, double* out,
-                                 int num_sms, cudaStream_t st) {
-    if (n & 3) return cudaErrorInvalidValue;
-    RLR_CUDA_CHECK(cudaMemsetAsync(out, 0, sizeof(double) * K, st));
-    long long want = (n / 4 + 255) / 256;
-    int gx = (int)(want > num_sms * 4 ? num_sms * 4 : (want < 1 ? 1 : want));
-    update_sqnorm_kernel<<<dim3(gx, K), 256, 0, st>>>(w_agents, w_global, n, out);
     return cudaGetLastError();
 }
 

@@ -25,6 +25,11 @@ inline T* ptr_or_null(const c10::optional<at::Tensor>& t) {
     return t.has_value() && t->defined() ? reinterpret_cast<T*>(t->data_ptr()) : nullptr;
 }
 #define CHECK_CUDA(x) TORCH_CHECK((x).is_cuda() && (x).is_contiguous(), #x " must be a contiguous CUDA tensor")
+// the cross-GPU gate of a server-step launch: flag_ptrs / local_sync are only needed (and checked by the launchers) when world > 1
+inline rlr::Gate gate_of(const c10::optional<at::Tensor>& flag_ptrs, const c10::optional<at::Tensor>& local_sync, int64_t rank,
+                         int64_t world, int64_t epoch) {
+    return {ptr_or_null<uint32_t* const>(flag_ptrs), ptr_or_null<uint32_t>(local_sync), (int)rank, (int)world, (uint32_t)epoch};
+}
 
 // ---------------------------------------------------------------------------------------------------------------
 void fused_aggregate(at::Tensor w_agent_ptrs, at::Tensor weights, c10::optional<at::Tensor> scales, double total_weight,
@@ -55,11 +60,8 @@ void fused_aggregate(at::Tensor w_agent_ptrs, at::Tensor weights, c10::optional<
     p.server_lr = (float)server_lr; p.noise_std = (float)noise_std;
     p.seed = (uint64_t)seed; p.noise_stream = (uint64_t)noise_stream;
     p.flipped = ptr_or_null<unsigned long long>(flipped);
-    p.flag_ptrs = ptr_or_null<uint32_t* const>(flag_ptrs);
-    p.local_sync = ptr_or_null<uint32_t>(local_sync);
-    p.rank = (int)rank; p.world = (int)world; p.epoch = (uint32_t)epoch;
+    p.gate = gate_of(flag_ptrs, local_sync, rank, world, epoch);
     p.handoff = handoff ? 1 : 0;
-    TORCH_CHECK(world <= 1 || (p.flag_ptrs && p.local_sync), "multi-GPU aggregation needs flag_ptrs and local_sync");
     // server optimizer state: fp32 on the launch device, covering [state_base, end)
     for (const auto* t : {&opt_m, &opt_v}) {
         if (!t->has_value() || !(*t)->defined()) continue;
@@ -88,15 +90,6 @@ void acquire_slices(int64_t ready_ptr, int64_t first, int64_t last, c10::optiona
           "acquire_slices");
 }
 
-void update_sqnorm(at::Tensor w_agent_ptrs, int64_t w_global_ptr, int64_t n, at::Tensor out) {
-    CHECK_CUDA(w_agent_ptrs); CHECK_CUDA(out);
-    TORCH_CHECK(out.scalar_type() == at::kDouble && out.numel() >= w_agent_ptrs.numel());
-    c10::cuda::CUDAGuard guard(out.device());
-    check(rlr::launch_update_sqnorm(reinterpret_cast<const float* const*>(w_agent_ptrs.data_ptr()),
-                                    reinterpret_cast<const float*>(w_global_ptr), n, (int)w_agent_ptrs.numel(),
-                                    out.data_ptr<double>(), num_sms(), cur_stream()), "update_sqnorm");
-}
-
 // K x K fp64 squared distances of the participants' updates over coordinates [begin, end) (Krum / Multi-Krum selection).  w_global_ptr
 // is read only with scales.  world > 1: the fused multi-GPU form, which first runs the aggregation's barrier-in at `epoch`.
 void pairwise_sqdist(at::Tensor w_agent_ptrs, int64_t w_global_ptr, c10::optional<at::Tensor> scales, int64_t begin, int64_t end,
@@ -118,9 +111,7 @@ void pairwise_sqdist(at::Tensor w_agent_ptrs, int64_t w_global_ptr, c10::optiona
     p.scales = sc;
     p.begin = begin; p.end = end;
     p.K = (int)K;
-    p.flag_ptrs = ptr_or_null<uint32_t* const>(flag_ptrs);
-    p.local_sync = ptr_or_null<uint32_t>(local_sync);
-    p.rank = (int)rank; p.world = (int)world; p.epoch = (uint32_t)epoch;
+    p.gate = gate_of(flag_ptrs, local_sync, rank, world, epoch);
     check(rlr::launch_pairwise_sqdist(p, out.data_ptr<double>(), num_sms(), cur_stream()), "pairwise_sqdist");
 }
 
@@ -140,9 +131,7 @@ void trust_stats(at::Tensor w_agent_ptrs, int64_t w_ref_ptr, int64_t w_global_pt
     p.w_global = reinterpret_cast<const float*>(w_global_ptr);
     p.begin = begin; p.end = end;
     p.K = (int)K;
-    p.flag_ptrs = ptr_or_null<uint32_t* const>(flag_ptrs);
-    p.local_sync = ptr_or_null<uint32_t>(local_sync);
-    p.rank = (int)rank; p.world = (int)world; p.epoch = (uint32_t)epoch;
+    p.gate = gate_of(flag_ptrs, local_sync, rank, world, epoch);
     check(rlr::launch_trust_stats(p, out.data_ptr<double>(), num_sms(), cur_stream()), "trust_stats");
 }
 
@@ -351,7 +340,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("tau") = 0.0, py::arg("opt_m") = py::none(), py::arg("opt_v") = py::none(), py::arg("state_base") = 0);
     m.def("aggregate_max_agents", &rlr::aggregate_max_agents);
     m.def("acquire_slices", &acquire_slices);
-    m.def("update_sqnorm", &update_sqnorm);
     m.def("pairwise_sqdist", &pairwise_sqdist);
     m.def("trust_stats", &trust_stats);
     m.def("gather_normalize", &gather_normalize);

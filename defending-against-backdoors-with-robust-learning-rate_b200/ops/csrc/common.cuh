@@ -5,6 +5,7 @@
 #include <stdint.h>
 
 #include "dropspec.h"
+#include "kernels.h"
 
 #define RLR_CUDA_CHECK(expr)                                                                     \
     do {                                                                                         \
@@ -256,7 +257,7 @@ __device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
     return v;
 }
 
-// Cross-GPU barrier executed by the first `world` threads of ONE block (aggregate.cu, select.cu).
+// Cross-GPU barrier executed by the first `world` threads of ONE block (barrier_in below, the aggregate kernel's barrier-out).
 __device__ __forceinline__ void xgpu_barrier(uint32_t* const* flag_ptrs, int slot_base, int rank, int world, uint32_t epoch) {
     const int t = threadIdx.x;
     if (t < world) {
@@ -264,6 +265,34 @@ __device__ __forceinline__ void xgpu_barrier(uint32_t* const* flag_ptrs, int slo
         const uint32_t* mine = flag_ptrs[rank] + slot_base + t;           // wait for peer t
         while ((int32_t)(ld_acquire_sys(mine) - epoch) < 0) { __nanosleep(64); }
     }
+}
+
+// Barrier-in of the server step's passes (aggregate, distances, trust statistics) on the fused multi-GPU path: every rank's participant
+// slots are final before any peer slot is read.  Every thread calls it.  The `leader` CTA runs the cross-GPU barrier and then releases
+// the other CTAs of this GPU through the ready flag, so every CTA of the grid has to be resident (the launchers cap their grids).
+__device__ __forceinline__ void barrier_in(const Gate& g, bool leader) {
+    if (g.world > 1) {
+        if (leader) {
+            xgpu_barrier(g.flag_ptrs, 0, g.rank, g.world, g.epoch);
+            __syncthreads();
+            if (threadIdx.x == 0) st_release_gpu(g.local_sync, g.epoch);
+        } else if (threadIdx.x == 0) {
+            while ((int32_t)(ld_acquire_gpu(g.local_sync) - g.epoch) < 0) { __nanosleep(32); }
+        }
+    }
+    __syncthreads();
+}
+// Host check of a launch's gate: the multi-GPU form needs the flag words and the intra-GPU sync words.
+inline bool gate_ok(const Gate& g) { return g.world <= 1 || (g.flag_ptrs && g.local_sync); }
+
+// Coordinate splits of a participant pass: about two waves of CTAs, one wave when world > 1 (every CTA has to be resident while the
+// leader waits in barrier_in), at least 4096 coordinates per split, at most `max_splits` (a workspace bound), and at least one.
+inline long long coord_splits(long long len, long long ctas_per_split, long long resident, int world,
+                              long long max_splits = 1LL << 62) {
+    long long splits = (world > 1 ? resident : 2 * resident) / ctas_per_split;
+    splits = splits < len / 4096 ? splits : len / 4096;
+    splits = splits < max_splits ? splits : max_splits;
+    return splits < 1 ? 1 : splits;
 }
 
 // ---- Philox4x32-10 counter RNG (Salmon et al.), used for dropout masks and server noise ---------------

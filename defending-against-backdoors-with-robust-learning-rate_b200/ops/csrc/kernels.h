@@ -7,6 +7,15 @@
 
 namespace rlr {
 
+// Cross-GPU gate of the server step's launches (world > 1: the fused multi-GPU path).  The aggregate, distance and trust kernels open
+// with the barrier-in on it (barrier_in, common.cuh); the aggregate kernel also runs its barrier-out or hand-off on these words.
+struct Gate {
+    uint32_t* const* flag_ptrs;     // [world] peer-mapped signal words, 3*world per rank (in / out barrier, broadcast-ready words)
+    uint32_t* local_sync;           // [2] intra-GPU: ready flag, finished-CTA counter
+    int rank, world;
+    uint32_t epoch;                 // monotonically increasing per call
+};
+
 struct AggParams {
     const float* const* w_agents;   // [K] device pointers: each participant's flat params (local or peer-mapped)
     const double* weights;          // [K] data sizes n_k
@@ -26,11 +35,8 @@ struct AggParams {
     float noise_std;
     uint64_t seed, noise_stream;
     unsigned long long* flipped;    // optional counter of coordinates with negated lr
-    uint32_t* const* flag_ptrs;     // [world] peer-mapped signal words, 2*world per rank (in / out barrier)
-    uint32_t* local_sync;           // [2] intra-GPU: ready flag, finished-CTA counter
-    int rank, world;
-    uint32_t epoch;                 // monotonically increasing per call
-    int handoff;                    // 1: publish this rank's slice in the peers' ready words (flag slot 2*world + rank) instead of the barrier-out
+    Gate gate;
+    int handoff;                   // 1: publish this rank's slice in the peers' ready words (flag slot 2*world + rank) instead of the barrier-out
     // server optimizer applied to the voted coordinates (0 sgd, 1 momentum, 2 adagrad, 3 adam, 4 yogi); state fp32, indexed by i - state_base
     int opt;
     double beta1, beta2, tau;
@@ -43,8 +49,6 @@ int aggregate_max_agents();         // capacity of the kernel's participant tabl
 // consumer side of the hand-off: wait for ready words [first, last] >= epoch (ready may be null), then copy the BatchNorm-statistics tail
 cudaError_t launch_acquire_slices(const uint32_t* ready, int first, int last, const uint32_t* epoch, const float* tail_src, float* tail_dst,
                                   long long tail_n, cudaStream_t st);
-cudaError_t launch_update_sqnorm(const float* const* w_agents, const float* w_global, long long n, int K, double* out,
-                                 int num_sms, cudaStream_t st);
 
 // ---- participant selection (Krum / Multi-Krum): pairwise squared distances of the participants' updates ----------------------------
 // out[i][j] = sum_{begin <= c < end} (x_i[c] - x_j[c])^2 in fp64 ([K][K], symmetric, zero diagonal), x_k = w_k without scales and
@@ -55,10 +59,7 @@ struct DistParams {
     const float* scales;            // [K] server clipping scales or nullptr
     long long begin, end;           // coordinate range (multiples of 4), already clipped to [0, n_vote)
     int K;
-    uint32_t* const* flag_ptrs;     // world > 1: the aggregation's barrier-in words and intra-GPU ready flag (ops/csrc/aggregate.cu)
-    uint32_t* local_sync;
-    int rank, world;
-    uint32_t epoch;
+    Gate gate;                      // world > 1: the aggregation's barrier-in
 };
 cudaError_t launch_pairwise_sqdist(const DistParams& p, double* out, int num_sms, cudaStream_t st);
 
@@ -71,10 +72,7 @@ struct TrustParams {
     const float* w_global;          // this rank's global parameters
     long long begin, end;           // coordinate range (multiples of 4), already clipped to [0, n_vote)
     int K;
-    uint32_t* const* flag_ptrs;     // world > 1: the aggregation's barrier-in words and intra-GPU ready flag (ops/csrc/aggregate.cu)
-    uint32_t* local_sync;
-    int rank, world;
-    uint32_t epoch;
+    Gate gate;                      // world > 1: the aggregation's barrier-in
 };
 cudaError_t launch_trust_stats(const TrustParams& p, double* out, int num_sms, cudaStream_t st);
 

@@ -63,17 +63,7 @@ __global__ void __launch_bounds__(kDistThreads, 2) pairwise_sqdist_kernel(DistKe
         wp[q] = valid ? p.w_agents[k] : nullptr;
         scs[q] = valid && p.scales ? p.scales[k] : 1.0f;
     }
-    // barrier-in (fused multi-GPU path): every rank's slots are final before any peer slot is read
-    if (p.world > 1) {
-        if (blockIdx.x == 0 && blockIdx.y == 0) {
-            xgpu_barrier(p.flag_ptrs, 0, p.rank, p.world, p.epoch);
-            __syncthreads();
-            if (tid == 0) st_release_gpu(p.local_sync, p.epoch);
-        } else if (tid == 0) {
-            while ((int32_t)(ld_acquire_gpu(p.local_sync) - p.epoch) < 0) { __nanosleep(32); }
-        }
-    }
-    __syncthreads();
+    barrier_in(p.gate, blockIdx.x == 0 && blockIdx.y == 0);
 
     // this thread's pair block (bi, bj) and coordinate lane l
     const int NB = diag ? nbr * (nbr + 1) / 2 : nbr * nbc;
@@ -190,8 +180,7 @@ __global__ void __launch_bounds__(kDistThreads, 2) pairwise_sqdist_kernel(DistKe
 cudaError_t launch_pairwise_sqdist(const DistParams& p, double* out, int num_sms, cudaStream_t st) {
     if (p.K < 1 || p.K > kDistMaxAgents) return cudaErrorInvalidValue;
     if ((p.begin & 3) || (p.end & 3) || p.end < p.begin) return cudaErrorInvalidValue;
-    if (p.scales && !p.w_global) return cudaErrorInvalidValue;
-    if (p.world > 1 && (!p.flag_ptrs || !p.local_sync)) return cudaErrorInvalidValue;
+    if ((p.scales && !p.w_global) || !gate_ok(p.gate)) return cudaErrorInvalidValue;
     static int occ = 0;
     if (!occ) {
         RLR_CUDA_CHECK(cudaFuncSetAttribute(pairwise_sqdist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDistSmem));
@@ -204,12 +193,7 @@ cudaError_t launch_pairwise_sqdist(const DistParams& p, double* out, int num_sms
     const int tiles = kp.tiles_side * (kp.tiles_side + 1) / 2;
     const long long len = p.end - p.begin;
     const long long kk = (long long)p.K * p.K;
-    const long long resident = (long long)occ * num_sms;
-    long long splits = (p.world > 1 ? resident : 2 * resident) / tiles;
-    const long long by_len = len / 4096, by_ws = kMaxWorkspace / (kk * (long long)sizeof(double));
-    splits = splits < by_len ? splits : by_len;
-    splits = splits < by_ws ? splits : by_ws;
-    splits = splits < 1 ? 1 : splits;
+    const long long splits = coord_splits(len, tiles, (long long)occ * num_sms, p.gate.world, kMaxWorkspace / (kk * (long long)sizeof(double)));
     kp.span = ((len + splits - 1) / splits + 3) & ~3LL;
     Scratch ws((size_t)(splits * kk) * sizeof(double), st);
     kp.ws = ws.as<double>();

@@ -3,6 +3,7 @@
 // over the coordinates [begin, end).  The dot product is formed per coordinate: the Gram identity Δk.Δ0 = (|Δk|^2 + |Δ0|^2 -
 // |w_k - w_ref|^2) / 2 cancels catastrophically when the cosine is near 0, which is where the trust score's ReLU decides whether a
 // participant counts (and honest cosines are small in high dimension).
+// With w_ref = w_global (Δ0 = 0) the q_k are the squared update norms of server clipping and the Norms/* diagnostics (ops.update_norms).
 //
 // Work decomposition:
 //   grid.x  coordinate splits, sized so the grid covers about two waves (one wave on the fused multi-GPU path, where every CTA has to
@@ -40,17 +41,7 @@ __global__ void __launch_bounds__(kTrustThreads) trust_stats_kernel(TrustKernelP
 #pragma unroll
     for (int j = 0; j < kTrustGroup; ++j) wp[j] = j < nk ? p.w_agents[k0 + j] : nullptr;
 
-    // barrier-in (fused multi-GPU path): every rank's slots are final before any peer slot is read
-    if (p.world > 1) {
-        if (blockIdx.x == 0 && blockIdx.y == 0) {
-            xgpu_barrier(p.flag_ptrs, 0, p.rank, p.world, p.epoch);
-            __syncthreads();
-            if (tid == 0) st_release_gpu(p.local_sync, p.epoch);
-        } else if (tid == 0) {
-            while ((int32_t)(ld_acquire_gpu(p.local_sync) - p.epoch) < 0) { __nanosleep(32); }
-        }
-        __syncthreads();
-    }
+    barrier_in(p.gate, blockIdx.x == 0 && blockIdx.y == 0);
 
     double dd[kTrustGroup], qd[kTrustGroup], q0d = 0.0;
 #pragma unroll
@@ -117,8 +108,7 @@ __global__ void __launch_bounds__(kTrustThreads) trust_stats_kernel(TrustKernelP
 
 cudaError_t launch_trust_stats(const TrustParams& p, double* out, int num_sms, cudaStream_t st) {
     if (p.K < 1 || p.K > kTrustMaxAgents || !p.w_ref || !p.w_global) return cudaErrorInvalidValue;
-    if ((p.begin & 3) || (p.end & 3) || p.end < p.begin) return cudaErrorInvalidValue;
-    if (p.world > 1 && (!p.flag_ptrs || !p.local_sync)) return cudaErrorInvalidValue;
+    if ((p.begin & 3) || (p.end & 3) || p.end < p.begin || !gate_ok(p.gate)) return cudaErrorInvalidValue;
     static int occ = 0;
     if (!occ) {
         RLR_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, trust_stats_kernel, kTrustThreads, 0));
@@ -129,11 +119,7 @@ cudaError_t launch_trust_stats(const TrustParams& p, double* out, int num_sms, c
     const int groups = (p.K + kTrustGroup - 1) / kTrustGroup;
     const long long len = p.end - p.begin;
     const long long nvals = 2LL * p.K + 1;
-    const long long resident = (long long)occ * num_sms;
-    long long splits = (p.world > 1 ? resident : 2 * resident) / groups;
-    const long long by_len = len / 4096;
-    splits = splits < by_len ? splits : by_len;
-    splits = splits < 1 ? 1 : splits;
+    const long long splits = coord_splits(len, groups, (long long)occ * num_sms, p.gate.world);
     kp.span = ((len + splits - 1) / splits + 3) & ~3LL;
     Scratch ws((size_t)(splits * nvals) * sizeof(double), st);
     kp.ws = ws.as<double>();

@@ -35,6 +35,8 @@ coordinates -- and with every other transport each rank keeps the full vector (i
 """
 from __future__ import annotations
 
+from functools import partial
+
 import torch
 
 from .. import ops
@@ -157,7 +159,26 @@ class FusedAggregator:
         """True when a round of ``n_part`` participants runs on all-gathered copies of the participants (the nccl / gloo transports,
         and more participants than the fused kernel's tables hold).  Selection then gathers once (``gather_participants``) and hands the
         copies to both ``pairwise_sqdist`` and ``aggregate``."""
-        return self.ctx.is_dist and not (self.backend == "fused" and n_part <= ops.MAX_FUSED_AGENTS)
+        return self.ctx.is_dist and not self._p2p(n_part)
+
+    def _p2p(self, n_part: int) -> bool:
+        """True when a round of ``n_part`` participants runs on the fused multi-GPU path (peer-mapped slots, in-kernel barriers)."""
+        return self.backend == "fused" and self.ctx.is_dist and n_part <= ops.MAX_FUSED_AGENTS
+
+    def _fused_pass(self, shape, launch):
+        """A participant pass on the fused multi-GPU path: ``launch(begin, end, out, flag_ptrs, local_sync, rank, world, epoch)`` over
+        this rank's slice of ``[0, n_vote)`` into a float64 ``out`` of ``shape``, behind the aggregation kernel's barrier-in at an epoch
+        of its own; the ranks all_gather their partials and add them in rank order, so the result is identical on every rank."""
+        ctx = self.ctx
+        self.epoch += 1
+        part = torch.empty(shape, dtype=torch.float64, device=ctx.device)
+        launch(self.begin, max(self.begin, min(self.end, self.n_vote)), part, self.flag_ptrs.tensor, self.local_sync, ctx.rank, ctx.world,
+               self.epoch)
+        parts = ctx.all_gather(part)                                     # [world, *shape]
+        out = parts[0].clone()
+        for r in range(1, ctx.world):
+            out += parts[r]
+        return out
 
     def pairwise_sqdist(self, n_part: int, scales=None, participants=None):
         """K x K float64 squared distances between the round's ``n_part`` participants' updates over ``[0, n_vote)`` (Krum / Multi-Krum
@@ -168,21 +189,12 @@ class FusedAggregator:
         rank order.  Gather transport and single process: the same kernel over ``participants`` (every participant's parameters on
         this rank, as ``gather_participants`` returns them; gathered here when not given).  The reduce transport never holds cross-rank
         pairs, so selection always takes the gather transport, as the coordinate median does."""
-        ctx, dev = self.ctx, self.ctx.device
-        if self.backend == "fused" and ctx.is_dist and n_part <= ops.MAX_FUSED_AGENTS:
+        if self._p2p(n_part):
             if scales is not None:
                 self.acquire()                       # the clipped distances read this rank's w_global
-            self.epoch += 1
-            part = torch.empty(n_part, n_part, dtype=torch.float64, device=dev)
-            sc = torch.as_tensor(scales, dtype=torch.float32).to(dev) if scales is not None else None
-            ops.ext().pairwise_sqdist(self._agent_table(n_part).tensor, self.w_global.data_ptr() if sc is not None else 0, sc,
-                                      self.begin, max(self.begin, min(self.end, self.n_vote)), part, self.flag_ptrs.tensor,
-                                      self.local_sync, ctx.rank, ctx.world, self.epoch)
-            parts = ctx.all_gather(part)                                 # [world, K, K]
-            D = parts[0].clone()
-            for r in range(1, ctx.world):
-                D += parts[r]
-            return D
+            sc = torch.as_tensor(scales, dtype=torch.float32).to(self.ctx.device) if scales is not None else None
+            return self._fused_pass((n_part, n_part), partial(ops.ext().pairwise_sqdist, self._agent_table(n_part).tensor,
+                                                              self.w_global.data_ptr() if sc is not None else 0, sc))
         agents = self._participants(n_part, participants)
         return ops.pairwise_sqdist(agents, self.n_vote, self.w_global if scales is not None else None, scales)
 
@@ -198,20 +210,12 @@ class FusedAggregator:
         here when not given).  The reduce transport never holds a participant and the root on one rank, so the trust pass always takes
         the gather transport; the step that follows then gathers too whenever it leaves a participant out (``members``), and forms the
         same weighted mean from all-reduced partials when every participant is trusted or none is."""
-        ctx, dev = self.ctx, self.ctx.device
-        if self.backend == "fused" and ctx.is_dist and n_part <= ops.MAX_FUSED_AGENTS:
+        if self._p2p(n_part):
             self.acquire()
-            self.epoch += 1
-            part = torch.empty(2 * n_part + 1, dtype=torch.float64, device=dev)
             owner, slot = self.slot_owner(ref)
-            ops.ext().trust_stats(self._agent_table(n_part).tensor, self.buf.peer_ptr(owner, self.off_slots + 4 * self.n * slot),
-                                  self.w_global.data_ptr(), self.begin, max(self.begin, min(self.end, self.n_vote)), part,
-                                  self.flag_ptrs.tensor, self.local_sync, ctx.rank, ctx.world, self.epoch)
-            parts = ctx.all_gather(part)                                 # [world, 2 n_part + 1]
-            out = parts[0].clone()
-            for r in range(1, ctx.world):
-                out += parts[r]
-            return out
+            return self._fused_pass((2 * n_part + 1,), partial(ops.ext().trust_stats, self._agent_table(n_part).tensor,
+                                                               self.buf.peer_ptr(owner, self.off_slots + 4 * self.n * slot),
+                                                               self.w_global.data_ptr()))
         copies = participants if participants is not None else self.gather_participants(max(n_part, ref + 1))
         if len(copies) <= max(n_part - 1, ref):
             raise ValueError(f"{len(copies)} participant copies for {n_part} participants and the root job at position {ref}")
@@ -237,7 +241,7 @@ class FusedAggregator:
         total = float(sum(float(x) for x in weights)) if total_weight is None else float(total_weight)
         self.flipped.zero_()
         self.flipped_is_partial = False
-        fused_p2p = self.backend == "fused" and ctx.is_dist and n_part <= ops.MAX_FUSED_AGENTS
+        fused_p2p = self._p2p(n_part)
         if self.opt.kind != "sgd" and fused_p2p != self.sharded:
             raise ValueError(f"{n_part} participants: the server optimizer state was laid out for the "
                              f"{'fused multi-GPU' if self.sharded else 'gather'} path")

@@ -377,8 +377,8 @@ __global__ void __launch_bounds__(256) sgd_step_kernel(float* __restrict__ w, co
                                                          float* __restrict__ m, const float* __restrict__ w0,
                                                          __nv_bfloat16* __restrict__ wb, long long n4, float lr,
                                                          float momentum, float max_grad_norm,
-                                                         const double* __restrict__ g_sqnorm, double* d_sqnorm, long long n4_pgd,
-                                                         const float* __restrict__ w_in, int first) {
+                                                         const double* __restrict__ g_sqnorm, double* d_part /*[gridDim.x]*/,
+                                                         long long n4_pgd, const float* __restrict__ w_in, int first) {
     // first = 1: first local step of a round, fused with the round hand-off -- parameters are read from the broadcast buffer w_in
     // (= the round's global parameters) and the momentum is taken as zero (fresh optimizer every round, src/agent.py:37-38), so no
     // separate "w <- w_global, m <- 0" pass exists.  Coordinates >= n4_pgd (BatchNorm running statistics, already updated in w by
@@ -400,7 +400,7 @@ __global__ void __launch_bounds__(256) sgd_step_kernel(float* __restrict__ w, co
         wn.x = wv.x - lr * mn.x; wn.y = wv.y - lr * mn.y; wn.z = wv.z - lr * mn.z; wn.w = wv.w - lr * mn.w;
         st_f4(m + 4 * q, mn);
         st_f4(w + 4 * q, wn);
-        if (d_sqnorm) {
+        if (d_part) {
             // PGD radius is measured over the model parameters only ([0, n_pgd): the reference projects parameters_to_vector(),
             // src/agent.py:54-60); BatchNorm running statistics stored behind them never count and are never rescaled
             if (q < n4_pgd) {
@@ -412,9 +412,9 @@ __global__ void __launch_bounds__(256) sgd_step_kernel(float* __restrict__ w, co
             *reinterpret_cast<uint2*>(wb + 4 * q) = make_uint2(pack_bf16x2(wn.x, wn.y), pack_bf16x2(wn.z, wn.w));
         }
     }
-    if (d_sqnorm) {
+    if (d_part) {
         const double tot = block_sum<double>(dacc, scratch);
-        if (threadIdx.x == 0) atomicAdd(d_sqnorm, tot);
+        if (threadIdx.x == 0) d_part[blockIdx.x] = tot;
     }
 }
 cudaError_t launch_sgd_step(float* w, const float* g, float* m, const float* w0, __nv_bfloat16* w_bf16, long long n,
@@ -422,8 +422,18 @@ cudaError_t launch_sgd_step(float* w, const float* g, float* m, const float* w0,
                             int num_sms, cudaStream_t st, long long n_pgd, const float* w_in) {
     if ((n & 3) || (n_pgd & 3)) return cudaErrorInvalidValue;
     if (n_pgd <= 0 || n_pgd > n) n_pgd = n;
-    sgd_step_kernel<<<grid_for(n / 4, 256, num_sms, 4), 256, 0, st>>>(w, g, m, w0, w_bf16, n / 4, lr, momentum,
-                                                                       max_grad_norm, g_sqnorm, d_sqnorm, n_pgd / 4, w_in, w_in ? 1 : 0);
+    const int grid = grid_for(n / 4, 256, num_sms, 4);
+    auto step = [&](double* dp) {
+        sgd_step_kernel<<<grid, 256, 0, st>>>(w, g, m, w0, w_bf16, n / 4, lr, momentum, max_grad_norm, g_sqnorm, dp, n_pgd / 4,
+                                              w_in, w_in ? 1 : 0);
+        return cudaGetLastError();
+    };
+    if (!d_sqnorm) return step(nullptr);
+    // PGD: per-CTA ||w - w0||^2 partials, added into d_sqnorm in CTA order (as launch_sqnorm), so the radius pgd_project reads is
+    // the same sum on every run
+    Scratch part((size_t)grid * sizeof(double), st);
+    RLR_CUDA_CHECK(step(part.as<double>()));
+    RLR_CUDA_CHECK(launch_ordered_sum(d_sqnorm, part.as<double>(), grid, 1LL, st));
     return cudaGetLastError();
 }
 
@@ -474,7 +484,11 @@ __global__ void softmax_xent_kernel(const T* __restrict__ logits, const int64_t*
         for (int c = 0; c < C; ++c) { v[c] = __expf(v[c] - mx); se += v[c]; }
         const int y = (int)labels[b];
         const float inv = 1.0f / se;
-        loss = -(__logf(v[y] * inv + 1e-30f));
+        // -log p_y while p_y is far above underflow (the 1e-30 guard is then below rounding).  Below 2^-64 the label lies ~44 or more
+        // below the max, and -log(p_y + 1e-30) would saturate at 69.08 once p_y underflows: there the loss is the stable
+        // log(se) - (x_y - mx) of eval_metrics, from the label's logit itself
+        const float q = v[y] * inv + 1e-30f;
+        loss = q >= 0x1p-64f ? -(__logf(q)) : logf(se) - ((float)logits[(int64_t)b * C + y] - mx);
         ok = (arg == y);
         if (dlogits)
             for (int c = 0; c < C; ++c) dlogits[(int64_t)b * C + c] = (T)((v[c] * inv - (c == y ? 1.f : 0.f)) * grad_scale);
@@ -503,7 +517,7 @@ cudaError_t launch_softmax_xent(const void* logits, int kind, const int64_t* lab
 // host with .item() syncs, src/utils.py:144-152)
 template <typename T>
 __global__ void eval_metrics_kernel(const T* __restrict__ logits, const int64_t* __restrict__ labels, int B, int C,
-                                    double* loss_sum, long long* confusion) {
+                                    double* loss_part /*[gridDim.x]*/, long long* confusion) {
     __shared__ double scratch[32];
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     double loss = 0.0;
@@ -521,14 +535,18 @@ __global__ void eval_metrics_kernel(const T* __restrict__ logits, const int64_t*
         atomicAdd((unsigned long long*)(confusion + (int64_t)y * C + arg), 1ull);
     }
     const double tot = block_sum<double>(loss, scratch);
-    if (threadIdx.x == 0) atomicAdd(loss_sum, tot);
+    if (threadIdx.x == 0) loss_part[blockIdx.x] = tot;
 }
 cudaError_t launch_eval_metrics(const void* logits, int kind, const int64_t* labels, int B, int C, double* loss_sum,
                                 long long* confusion, cudaStream_t st) {
     if (B <= 0) return cudaSuccess;
     const int threads = 128, blocks = (B + threads - 1) / threads;
-    if (kind == 0) eval_metrics_kernel<float><<<blocks, threads, 0, st>>>((const float*)logits, labels, B, C, loss_sum, confusion);
-    else eval_metrics_kernel<__nv_bfloat16><<<blocks, threads, 0, st>>>((const __nv_bfloat16*)logits, labels, B, C, loss_sum, confusion);
+    Scratch part((size_t)blocks * sizeof(double), st);                // per-block loss sums, added into loss_sum in block order
+    double* lp = part.as<double>();
+    if (kind == 0) eval_metrics_kernel<float><<<blocks, threads, 0, st>>>((const float*)logits, labels, B, C, lp, confusion);
+    else eval_metrics_kernel<__nv_bfloat16><<<blocks, threads, 0, st>>>((const __nv_bfloat16*)logits, labels, B, C, lp, confusion);
+    RLR_CUDA_CHECK(cudaGetLastError());
+    RLR_CUDA_CHECK(launch_ordered_sum(loss_sum, lp, blocks, 1LL, st));
     return cudaGetLastError();
 }
 

@@ -5,6 +5,8 @@ step, executed by ONE fused kernel over the flat parameter vector (``ops.fused_a
 ``parallel.FusedAggregator`` across GPUs) instead of the reference's ~30 elementwise fp64 passes (SURVEY.md 2.4b).
 With ``--select krum | multikrum`` a selection stage runs first: the participants' pairwise update distances
 (``ops.pairwise_sqdist``), Krum scores on the host (``ops.krum_select``), and only the admitted participants enter the step.
+``--aggr fltrust`` and ``--aggr rfa`` are the same weighted-mean launch with weights from a per-participant pass: FLTrust's trust
+scores (``ops.trust_stats``) or RFA's smoothed Weiszfeld weights (``ops.rfa`` over ``ops.rfa_sqdist`` passes).
 The reference's dead / disabled pieces are available behind flags: ``clip_updates`` (``--server_clip``) and the
 diagnostics ``plot_norms`` / ``comp_diag_fisher`` / ``plot_sign_agreement`` (``--diagnostics``), the latter with the
 reference's latent bugs fixed (model built on the right device; Fisher uses log-probabilities -- SURVEY.md quirk 7).
@@ -40,6 +42,7 @@ class Aggregation:
         self.last_admitted = None     # agent ids admitted by --select (and trusted by --aggr fltrust) in the last round
         self.last_select = None       # the Select/* scalars of the last round
         self.last_trust = None        # the Trust/* scalars of the last round (--aggr fltrust)
+        self.last_rfa = None          # the RFA/* scalars of the last round (--aggr rfa)
         self.opt = None               # full-length server optimizer state of the in-process form (allocated on first use)
 
     # ---- the server step ------------------------------------------------------------------------------------
@@ -55,8 +58,11 @@ class Aggregation:
         all_ids, all_ws = ids, ws
         distances = lambda: ops.pairwise_sqdist(ws, nv if nv is not None else w_global.numel(), w_global if clip is not None else None,
                                                 clip)
+        rfa_pass = lambda b, members: ops.rfa_sqdist(
+            [ws[j] for j in members], b, nv, w_global if clip is not None else None,
+            clip[torch.as_tensor(members, device=clip.device)] if clip is not None else None)
         keep, weights, scales, total = self._admission(ids, clip, distances, lambda: ops.trust_stats(ws, root_params, w_global, nv),
-                                                       cur_round)
+                                                       rfa_pass, cur_round)
         if keep is not None and len(keep) < len(ids):
             ids, ws, weights = [ids[j] for j in keep], [ws[j] for j in keep], [weights[j] for j in keep]
             scales = scales[torch.as_tensor(keep, device=scales.device)] if scales is not None else None
@@ -82,12 +88,13 @@ class Aggregation:
         norms = self.fused.update_norms(K) if self._server_clip or diag else None
         clip = self._clip_scales(norms) if self._server_clip else None
         copies, gathered = None, None
-        if (self._select or self._fltrust) and self.fused.gathers(K):
+        if (self._select or self._fltrust or (self._rfa and self.args.rfa_iters > 0)) and self.fused.gathers(K):
             # on the gather transport every pass reads the same all-gathered copies (one all_gather per round; the root job included)
             gathered = self.fused.gather_participants(K + 1 if self._fltrust else K)
             copies = gathered[:K]
         keep, weights, scales, total = self._admission(participants, clip, lambda: self.fused.pairwise_sqdist(K, clip, copies),
-                                                       lambda: self.fused.trust_stats(K, K, gathered), cur_round)
+                                                       lambda: self.fused.trust_stats(K, K, gathered),
+                                                       lambda b, members: self.fused.rfa_sqdist(K, b, clip, members, copies), cur_round)
         if diag:   # the sign-agreement analysis needs the pre-step global parameters and every admitted participant's parameters
             prev = self.fused.w_global.clone()
             ws = [w.clone() for w in self.fused.gather_participants(K)]
@@ -110,14 +117,18 @@ class Aggregation:
     def _select(self):
         return getattr(self.args, "select", "none") != "none"
 
-    def _admission(self, ids, clip, distances, trust_stats, cur_round):
+    def _admission(self, ids, clip, distances, trust_stats, rfa_pass, cur_round):
         """Admission of the participants ``ids`` shared by both forms of the step: Krum / Multi-Krum on ``distances()`` (``--select``),
-        then FLTrust on ``trust_stats()`` (``--aggr fltrust``).  ``clip``: the server-clipping scales or None.  Returns
-        ``(members, weights, scales, total_weight)`` for the step: members None admits everyone; weights are per position in ``ids``."""
+        then FLTrust on ``trust_stats()`` (``--aggr fltrust``) or RFA's weights from ``rfa_pass(b, members)`` (``--aggr rfa``).  ``clip``:
+        the server-clipping scales or None.  Returns ``(members, weights, scales, total_weight)`` for the step: members None admits
+        everyone; weights are per position in ``ids``."""
         keep = self._admit(distances(), ids, cur_round) if self._select else None
         if self._fltrust:
             return self._trust(trust_stats(), ids, keep, cur_round)
-        return keep, [float(self.agent_data_sizes[i]) for i in ids], clip, None
+        weights = [float(self.agent_data_sizes[i]) for i in ids]
+        if self._rfa:
+            return self._rfa_weights(ids, keep, weights, clip, rfa_pass, cur_round)
+        return keep, weights, clip, None
 
     def _admit(self, D, ids, cur_round):
         """Krum / Multi-Krum admission from the pairwise distances ``D`` of the participants ``ids``: the admitted positions
@@ -137,9 +148,34 @@ class Aggregation:
         return self.args.aggr == "fltrust"
 
     @property
+    def _rfa(self):
+        return self.args.aggr == "rfa"
+
+    @property
     def _mode(self):
-        """The aggregate kernel's rule: FLTrust is its weighted mean with trust weights and per-participant scales."""
-        return "avg" if self._fltrust else self.args.aggr
+        """The aggregate kernel's rule: FLTrust is its weighted mean with trust weights and per-participant scales, RFA with its
+        Weiszfeld weights."""
+        return "avg" if self._fltrust or self._rfa else self.args.aggr
+
+    def _rfa_weights(self, ids, keep, weights, clip, rfa_pass, cur_round):
+        """RFA over the positions ``keep`` that selection admitted (all when None): ``--rfa_iters`` smoothed Weiszfeld passes
+        (``ops.rfa``) from the data sizes ``weights``, each pass ``rfa_pass(b, members)`` returning the members' squared distances to
+        their ``b``-weighted mean.  Nobody is dropped.  Returns ``(members, weights, scales, total_weight)`` for the step: the members'
+        weights replaced by the final beta and total weight sum beta (``--rfa_iters 0``: exactly the avg step's weights and total).
+        Logs the share of the weight that corrupt participants (ids < num_corrupt) hold."""
+        cand = list(range(len(ids))) if keep is None else [int(j) for j in keep]
+        T = int(self.args.rfa_iters)
+        beta, _ = ops.rfa([weights[j] for j in cand], lambda b: rfa_pass(b, cand), T, self.args.rfa_nu)
+        weights = list(weights)
+        for j, bj in zip(cand, beta):
+            weights[j] = bj
+        total = sum(beta)
+        nc = self.args.num_corrupt
+        self.last_rfa = {"RFA/Corrupt_Weight": sum(bj for j, bj in zip(cand, beta) if ids[j] < nc) / total, "RFA/Passes": T}
+        if self.writer is not None:
+            for k, v in self.last_rfa.items():
+                self.writer.add_scalar(k, v, cur_round)
+        return keep, weights, clip, total
 
     def _trust(self, stats, ids, keep, cur_round):
         """FLTrust admission from the statistics ``stats`` (``ops.trust_statement``'s layout) of the participants ``ids``, among the

@@ -350,6 +350,9 @@ class FLEngine:
                 rec["trust_avg_honest"] = self.aggregator.last_trust["Trust/Avg_Honest"]
                 rec["trust_avg_corrupt"] = self.aggregator.last_trust["Trust/Avg_Corrupt"]
                 rec["trust_admitted"] = self.aggregator.last_trust["Trust/Admitted"]
+            if self.aggregator.last_rfa is not None:
+                rec["rfa_corrupt_weight"] = self.aggregator.last_rfa["RFA/Corrupt_Weight"]
+                rec["rfa_passes"] = self.aggregator.last_rfa["RFA/Passes"]
             rec.update({f"ms_{k}": v for k, v in self.timer.elapsed().items()})
             if args.profile_phases and self.verbose:
                 print({k: round(v, 3) for k, v in rec.items() if k.startswith("ms_")})

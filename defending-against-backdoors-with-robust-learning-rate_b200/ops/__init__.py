@@ -653,6 +653,74 @@ def fltrust_weights(d, q, q0):
 
 
 # =====================================================================================================================
+# RFA (Pillutla, Kakade, Harchaoui, IEEE TSP 2022): the smoothed geometric median by Weiszfeld passes
+# =====================================================================================================================
+def rfa_statement(w_agents, b, lo, hi, w_global=None, scales=None):
+    """fp64 statement of the RFA distance pass over coordinates ``[lo, hi)``: a float64 ``[K]`` tensor of
+    ``d_k^2 = sum_c (x_k[c] - z[c])^2`` with ``z[c] = sum_j b_j x_j[c]`` (added in position order), ``x_k = w_k`` (no scales: ``w_global``
+    cancels because the ``b_j`` sum to 1) or ``x_k = (w_k - w_global) * scales[k]``."""
+    K = len(w_agents)
+    dev = w_agents[0].device
+    bt = torch.as_tensor(b, dtype=torch.float64).to(dev)
+    sc = torch.as_tensor(scales, dtype=torch.float32).to(dev).double()[:, None] if scales is not None else None
+    out = torch.zeros(K, dtype=torch.float64, device=dev)
+    step = max(4, (1 << 24) // max(1, K))                 # coordinates per pass: K * step fp64 values
+    for c in range(lo, hi, step):
+        e = min(hi, c + step)
+        x = torch.stack([w[c:e] for w in w_agents]).double()
+        if sc is not None:
+            x = (x - w_global[c:e].double()) * sc
+        z = bt[0] * x[0]
+        for j in range(1, K):
+            z = z + bt[j] * x[j]
+        out += ((x - z) ** 2).sum(1)
+    return out
+
+
+def rfa_sqdist(w_agents, b, n_vote=None, w_global=None, scales=None):
+    """float64 ``[K]`` squared distances of the participants' updates to their ``b``-weighted mean over the voted coordinates
+    ``[0, n_vote)`` (``rfa_statement``'s values; ``b`` sums to 1).  ``scales`` (server clipping) need ``w_global``.  On CUDA this launches
+    ``rfa_sqdist_kernel`` (ops/csrc/rfa.cu); on CPU, and for more participants than the kernel's tables hold (recorded as a library
+    fall-through), it evaluates ``rfa_statement``."""
+    nv = w_agents[0].numel() if n_vote is None else int(n_vote)
+    if scales is not None and w_global is None:
+        raise ValueError("rfa_sqdist: scales need w_global")
+
+    def launch(tab, out):
+        sc = torch.as_tensor(scales, dtype=torch.float32).to(out.device) if scales is not None else None
+        bt = torch.as_tensor(b, dtype=torch.float64).to(out.device)
+        ext().rfa_sqdist(tab, bt, w_global.data_ptr() if sc is not None else 0, sc, 0, nv, out, None, None, 0, 1, 0)
+    return _participant_pass("rfa_sqdist", w_agents, (w_global,) if scales is not None else (), nv, (len(w_agents),),
+                             lambda: rfa_statement(w_agents, b, 0, nv, w_global, scales), launch)
+
+
+def rfa_weights(alpha, d2, nu):
+    """One smoothed Weiszfeld re-weighting on the host, in fp64: ``beta_k = alpha_k / max(nu, d_k)`` with ``d_k = sqrt(d2_k)``.  Returns
+    float64 numpy ``[K]``."""
+    a = np.asarray(alpha, dtype=np.float64).reshape(-1)
+    d = np.sqrt(np.asarray(torch.as_tensor(d2).detach().double().cpu().numpy(), dtype=np.float64).reshape(-1))
+    return a / np.maximum(float(nu), d)
+
+
+def rfa(alpha, pass_fn, T, nu):
+    """RFA's smoothed Weiszfeld loop, shared by every form of the server step.  ``alpha``: the participants' data sizes; ``pass_fn(b)``:
+    the squared distances (float64 ``[K]``) of the updates to their ``b``-weighted mean, ``b`` a float64 numpy ``[K]`` summing to 1.
+    ``T`` passes of ``b = beta / sum(beta)``, ``beta = rfa_weights(alpha, pass_fn(b), nu)`` from ``beta = alpha``.  Returns
+    ``(beta, F)``: the final weights as a list of floats (``T = 0``: exactly ``alpha``) and, per pass, the objective
+    ``F(z) = sum_k alpha_k ||z - x_k||`` at that pass's weighted mean ``z``.  While every distance is >= ``nu``, F does not increase
+    from one pass to the next (the Weiszfeld property)."""
+    a = np.asarray([float(x) for x in alpha], dtype=np.float64)
+    beta = a.copy()
+    F = []
+    for _ in range(int(T)):
+        d2 = pass_fn(beta / beta.sum())
+        d = np.sqrt(np.asarray(torch.as_tensor(d2).detach().double().cpu().numpy(), dtype=np.float64).reshape(-1))
+        F.append(float(np.dot(a, d)))
+        beta = rfa_weights(a, d2, nu)
+    return [float(x) for x in beta], F
+
+
+# =====================================================================================================================
 # optimiser over flat buffers
 # =====================================================================================================================
 def round_init(w_global, w_local=None, w_bf16=None, mom=None):

@@ -135,6 +135,33 @@ void trust_stats(at::Tensor w_agent_ptrs, int64_t w_ref_ptr, int64_t w_global_pt
     check(rlr::launch_trust_stats(p, out.data_ptr<double>(), num_sms(), cur_stream()), "trust_stats");
 }
 
+// RFA: fp64 [K] squared distances of the participants' updates to their b-weighted mean over coordinates [begin, end).  w_global_ptr is
+// read only with scales.  world > 1: the fused multi-GPU form, which first runs the aggregation's barrier-in at `epoch`.
+void rfa_sqdist(at::Tensor w_agent_ptrs, at::Tensor b, int64_t w_global_ptr, c10::optional<at::Tensor> scales, int64_t begin, int64_t end,
+                at::Tensor out, c10::optional<at::Tensor> flag_ptrs, c10::optional<at::Tensor> local_sync, int64_t rank, int64_t world,
+                int64_t epoch) {
+    CHECK_CUDA(w_agent_ptrs); CHECK_CUDA(b); CHECK_CUDA(out);
+    TORCH_CHECK(w_agent_ptrs.scalar_type() == at::kLong, "pointer table must be int64");
+    const int64_t K = w_agent_ptrs.numel();
+    TORCH_CHECK(b.scalar_type() == at::kDouble && b.numel() == K, "b must be a float64 [K] tensor");
+    TORCH_CHECK(out.scalar_type() == at::kDouble && out.numel() == K, "out must be a float64 [K] tensor");
+    const float* sc = ptr_or_null<const float>(scales);
+    if (sc) {
+        CHECK_CUDA(*scales);
+        TORCH_CHECK(scales->scalar_type() == at::kFloat && scales->numel() == K && w_global_ptr, "scales: float32 [K], with w_global");
+    }
+    c10::cuda::CUDAGuard guard(out.device());
+    rlr::RfaParams p{};
+    p.w_agents = reinterpret_cast<const float* const*>(w_agent_ptrs.data_ptr());
+    p.b = b.data_ptr<double>();
+    p.w_global = reinterpret_cast<const float*>(w_global_ptr);
+    p.scales = sc;
+    p.begin = begin; p.end = end;
+    p.K = (int)K;
+    p.gate = gate_of(flag_ptrs, local_sync, rank, world, epoch);
+    check(rlr::launch_rfa_sqdist(p, out.data_ptr<double>(), num_sms(), cur_stream()), "rfa_sqdist");
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // training augmentation of the gathers: crop pad, flip, Philox key and the device int64 stream word (needed when either is on)
 inline const long long* aug_stream_ptr(const c10::optional<at::Tensor>& stream, int64_t crop_pad, bool flip) {
@@ -342,6 +369,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("acquire_slices", &acquire_slices);
     m.def("pairwise_sqdist", &pairwise_sqdist);
     m.def("trust_stats", &trust_stats);
+    m.def("rfa_sqdist", &rfa_sqdist);
     m.def("gather_normalize", &gather_normalize);
     m.def("gather_im2col", &gather_im2col);
     m.def("stamp_pixels", &stamp_pixels);

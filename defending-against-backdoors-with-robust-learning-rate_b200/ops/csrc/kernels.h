@@ -76,6 +76,20 @@ struct TrustParams {
 };
 cudaError_t launch_trust_stats(const TrustParams& p, double* out, int num_sms, cudaStream_t st);
 
+// ---- RFA (smoothed Weiszfeld geometric median): each participant's squared distance to the b-weighted mean of the updates -------------
+// out[k] = sum_{begin <= c < end} (x_k[c] - z[c])^2 in fp64 [K], z[c] = sum_j b[j] x_j[c] (sum_j b[j] = 1), x_k = w_k without scales and
+// x_k = (w_k - w_global) * scales[k] with them.  Fixed-order sums, no atomics: bitwise reproducible.
+struct RfaParams {
+    const float* const* w_agents;   // [K] device pointers (local or peer-mapped)
+    const double* b;                // [K] normalised weights
+    const float* w_global;          // only read with scales
+    const float* scales;            // [K] server clipping scales or nullptr
+    long long begin, end;           // coordinate range (multiples of 4), already clipped to [0, n_vote)
+    int K;
+    Gate gate;                      // world > 1: the aggregation's barrier-in
+};
+cudaError_t launch_rfa_sqdist(const RfaParams& p, double* out, int num_sms, cudaStream_t st);
+
 // ---- data path ---------------------------------------------------------------------------------------
 // out_kind: 0 fp32, 1 bf16.  nchw: output layout NCHW (Cpad ignored) else NHWC with channels padded to c_pad.
 // Both gathers: crop_pad > 0 or flip turns on the training augmentation (AugSpec, common.cuh): sample b of the batch is drawn

@@ -14,8 +14,10 @@ import math
 import torch
 
 DATASETS = ("fmnist", "fedemnist", "cifar10")
-AGGREGATORS = ("avg", "comed", "sign", "fltrust")
+AGGREGATORS = ("avg", "comed", "sign", "fltrust", "rfa")
 ROOT_SIZE = 100                  # FLTrust root set: the paper's 100 clean samples
+RFA_ITERS = 3                    # RFA: a few smoothed Weiszfeld passes per round
+RFA_NU = 1e-6                    # RFA smoothing: distances below nu count as nu
 SERVER_OPTS = ("sgd", "momentum", "adagrad", "adam", "yogi")
 SELECTIONS = ("none", "krum", "multikrum")
 PATTERNS = ("plus", "square", "copyright", "apple")
@@ -36,7 +38,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--num_corrupt", type=int, default=0, help="number of corrupt agents (ids 0..n-1)")
     p.add_argument("--rounds", type=int, default=200, help="number of communication rounds: R")
     p.add_argument("--aggr", type=str, default="avg",
-                   help="aggregation rule: avg | comed | sign | fltrust (trust-weighted mean against a server-trained root update)")
+                   help="aggregation rule: avg | comed | sign | fltrust (trust-weighted mean against a server-trained root update) | "
+                        "rfa (smoothed geometric median by Weiszfeld passes, Pillutla et al. 2022)")
     p.add_argument("--local_ep", type=int, default=2, help="number of local epochs: E")
     p.add_argument("--bs", type=int, default=256, help="local batch size: B")
     p.add_argument("--client_lr", type=float, default=0.1, help="clients' learning rate")
@@ -113,6 +116,12 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--root_size", type=int, default=None,
                    help=f"--aggr fltrust: clean training samples the server trains its root update on each round (default {ROOT_SIZE}); "
                         "drawn once from --seed, never a poisoned sample")
+    p.add_argument("--rfa_iters", type=int, default=None,
+                   help=f"--aggr rfa: smoothed Weiszfeld passes per round (default {RFA_ITERS}; 0 = the avg step).  Each pass reweights "
+                        "every participant by its data size over its distance to the current weighted mean; a fixed count keeps the "
+                        "cost per round fixed")
+    p.add_argument("--rfa_nu", type=float, default=None,
+                   help=f"--aggr rfa: smoothing nu > 0 of the Weiszfeld weights alpha_k / max(nu, d_k) (default {RFA_NU})")
     return p
 
 
@@ -142,7 +151,24 @@ def finalize_args(args: argparse.Namespace) -> argparse.Namespace:
         raise ValueError(f"--crop_pad {args.crop_pad} must lie in [0, {side}) for --data {args.data} ({meta.height}x{meta.width} images)")
     _finalize_select(args)
     _finalize_fltrust(args)
+    _finalize_rfa(args)
     return args
+
+
+def _finalize_rfa(args) -> None:
+    """Validate the RFA flags and resolve their defaults in place (``RFA_ITERS`` / ``RFA_NU`` under ``--aggr rfa``)."""
+    iters, nu = getattr(args, "rfa_iters", None), getattr(args, "rfa_nu", None)
+    if args.aggr != "rfa":
+        if iters is not None or nu is not None:
+            raise ValueError("--rfa_iters / --rfa_nu need --aggr rfa")
+        return
+    iters = RFA_ITERS if iters is None else iters
+    nu = RFA_NU if nu is None else nu
+    if int(iters) != iters or iters < 0:
+        raise ValueError(f"--rfa_iters {iters} must be an integer >= 0")
+    if not (nu > 0 and math.isfinite(nu)):
+        raise ValueError(f"--rfa_nu {nu} must be a finite number > 0")
+    args.rfa_iters, args.rfa_nu = int(iters), float(nu)
 
 
 def _finalize_fltrust(args) -> None:
@@ -232,4 +258,6 @@ def print_exp_details(args) -> None:
         print(f"    Selection (F / M): {args.select} ({args.select_f} / {args.select_m})")
     if args.aggr == "fltrust":
         print(f"    Root set: {args.root_size}")
+    if args.aggr == "rfa":
+        print(f"    RFA passes / nu: {args.rfa_iters} / {args.rfa_nu}")
     print("======================================")

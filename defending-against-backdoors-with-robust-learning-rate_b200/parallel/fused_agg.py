@@ -155,6 +155,10 @@ class FusedAggregator:
             self._tables[n_part] = ops.PtrTable(ptrs, self.ctx.device)
         return self._tables[n_part]
 
+    def _member_table(self, idx):
+        """Pointer table of the slots of the participants at positions ``idx`` (the admitted ones)."""
+        return ops.PtrTable([self.buf.peer_ptr(r, self.off_slots + 4 * self.n * s) for r, s in map(self.slot_owner, idx)], self.ctx.device)
+
     def gathers(self, n_part: int) -> bool:
         """True when a round of ``n_part`` participants runs on all-gathered copies of the participants (the nccl / gloo transports,
         and more participants than the fused kernel's tables hold).  Selection then gathers once (``gather_participants``) and hands the
@@ -221,6 +225,34 @@ class FusedAggregator:
             raise ValueError(f"{len(copies)} participant copies for {n_part} participants and the root job at position {ref}")
         return ops.trust_stats(list(copies[:n_part]), copies[ref], self.w_global, self.n_vote)
 
+    def rfa_sqdist(self, n_part: int, b, scales=None, members=None, participants=None):
+        """RFA distance pass (``ops.rfa_statement``): the float64 squared distances of the updates of the participants at positions
+        ``members`` (ascending; every one of the round's ``n_part`` when None) to their ``b``-weighted mean over ``[0, n_vote)``, identical
+        on every rank.  ``b`` is per member and sums to 1; ``scales`` (server clipping) is per participant.  Call it after the slots are
+        final and before ``aggregate`` of the same round.
+
+        Fused multi-GPU path: each rank runs ``rfa_sqdist_kernel`` over its coordinate slice of the peer-mapped slots of the members (the
+        pointer table ``aggregate(members=)`` uses), behind the aggregation kernel's barrier-in (an epoch of its own), and the ranks
+        all_gather their partials and add them in rank order.  With clipping the pass reads ``w_global``, so it first acquires the
+        broadcast slices of a fused hand-off.  Gather transport and single process: the same kernel over ``participants``
+        (``gather_participants``' copies; gathered here when not given).  The reduce transport never holds every participant on one rank,
+        so the passes take the gather transport, as the coordinate median does; the step that follows keeps every member and may still
+        all-reduce."""
+        idx = list(range(n_part)) if members is None else [int(j) for j in members]
+        if scales is not None:
+            scales = scales[torch.as_tensor(idx, device=scales.device)] if torch.is_tensor(scales) else [scales[j] for j in idx]
+        if self._p2p(n_part):
+            if scales is not None:
+                self.acquire()
+            dev = self.ctx.device
+            table = self._agent_table(n_part) if idx == list(range(n_part)) else self._member_table(idx)
+            bt = torch.as_tensor(b, dtype=torch.float64).to(dev)
+            sc = torch.as_tensor(scales, dtype=torch.float32).to(dev) if scales is not None else None
+            return self._fused_pass((len(idx),), partial(ops.ext().rfa_sqdist, table.tensor, bt,
+                                                         self.w_global.data_ptr() if sc is not None else 0, sc))
+        agents = self._participants(n_part, participants)
+        return ops.rfa_sqdist([agents[j] for j in idx], b, self.n_vote, self.w_global if scales is not None else None, scales)
+
     def aggregate(self, weights, mode, theta, server_lr, noise_std=0.0, seed=0, rnd=0, scales=None, members=None, participants=None,
                   total_weight=None):
         """Aggregate the round's ``len(weights)`` participants (participant j lives in ``slot_owner(j)``; ``weights`` and ``scales`` are
@@ -250,8 +282,7 @@ class FusedAggregator:
             self.epoch += 1
             wt = torch.as_tensor(weights, dtype=torch.float64).to(dev)
             sc = torch.as_tensor(scales, dtype=torch.float32).to(dev) if scales is not None else None
-            table = self._agent_table(n_part) if members is None else ops.PtrTable(
-                [self.buf.peer_ptr(r, self.off_slots + 4 * self.n * s) for r, s in map(self.slot_owner, idx)], dev)
+            table = self._agent_table(n_part) if members is None else self._member_table(idx)
             ops.ext().fused_aggregate(
                 table.tensor, wt, sc, total, self.w_global.data_ptr(),
                 self.out_ptrs.tensor, self.out_bf16_ptrs.tensor if self.out_bf16_ptrs else None, self.use_multimem,

@@ -6,7 +6,9 @@ step, executed by ONE fused kernel over the flat parameter vector (``ops.fused_a
 With ``--select krum | multikrum`` a selection stage runs first: the participants' pairwise update distances
 (``ops.pairwise_sqdist``), Krum scores on the host (``ops.krum_select``), and only the admitted participants enter the step.
 ``--aggr fltrust`` and ``--aggr rfa`` are the same weighted-mean launch with weights from a per-participant pass: FLTrust's trust
-scores (``ops.trust_stats``) or RFA's smoothed Weiszfeld weights (``ops.rfa`` over ``ops.rfa_sqdist`` passes).
+scores (``ops.trust_stats``) or RFA's smoothed Weiszfeld weights (``ops.rfa`` over ``ops.rfa_sqdist`` passes).  ``--aggr flame`` is
+that launch too: the Gram matrix of the updates (``ops.pairwise_gram``) gives FLAME's cosine clustering, median-norm clip scales and
+noise (``ops.flame_admit``), and the admitted participants' clipped updates are averaged with equal weights.
 The reference's dead / disabled pieces are available behind flags: ``clip_updates`` (``--server_clip``) and the
 diagnostics ``plot_norms`` / ``comp_diag_fisher`` / ``plot_sign_agreement`` (``--diagnostics``), the latter with the
 reference's latent bugs fixed (model built on the right device; Fisher uses log-probabilities -- SURVEY.md quirk 7).
@@ -43,6 +45,7 @@ class Aggregation:
         self.last_select = None       # the Select/* scalars of the last round
         self.last_trust = None        # the Trust/* scalars of the last round (--aggr fltrust)
         self.last_rfa = None          # the RFA/* scalars of the last round (--aggr rfa)
+        self.last_flame = None        # the FLAME/* scalars of the last round (--aggr flame)
         self.opt = None               # full-length server optimizer state of the in-process form (allocated on first use)
 
     # ---- the server step ------------------------------------------------------------------------------------
@@ -61,8 +64,10 @@ class Aggregation:
         rfa_pass = lambda b, members: ops.rfa_sqdist(
             [ws[j] for j in members], b, nv, w_global if clip is not None else None,
             clip[torch.as_tensor(members, device=clip.device)] if clip is not None else None)
-        keep, weights, scales, total = self._admission(ids, clip, distances, lambda: ops.trust_stats(ws, root_params, w_global, nv),
-                                                       rfa_pass, cur_round)
+        gram = lambda members: ops.pairwise_gram([ws[j] for j in members], w_global, nv)
+        keep, weights, scales, total, noise_std = self._admission(ids, clip, distances,
+                                                                  lambda: ops.trust_stats(ws, root_params, w_global, nv), rfa_pass, gram,
+                                                                  cur_round)
         if keep is not None and len(keep) < len(ids):
             ids, ws, weights = [ids[j] for j in keep], [ws[j] for j in keep], [weights[j] for j in keep]
             scales = scales[torch.as_tensor(keep, device=scales.device)] if scales is not None else None
@@ -70,8 +75,8 @@ class Aggregation:
         flipped = torch.zeros(1, dtype=torch.int64, device=w_global.device)
         if self.opt is None:
             self.opt = ops.ServerOptState(n=w_global.numel(), device=w_global.device, **server_opt_spec(self.args))
-        ops.fused_aggregate(w_global, ws, weights, self._mode, self.args.robustLR_threshold, self.server_lr,
-                            self.args.noise * self.args.clip, self.args.seed, cur_round,
+        ops.fused_aggregate(w_global, ws, weights, self._mode, self.args.robustLR_threshold, self.server_lr, noise_std, self.args.seed,
+                            cur_round,
                             n_vote if n_vote is not None else (self.layout.n_vote if self.layout else None),
                             scales, out=w_global, flipped=flipped, opt=self.opt, total_weight=total)
         self.last_flipped = flipped
@@ -88,22 +93,22 @@ class Aggregation:
         norms = self.fused.update_norms(K) if self._server_clip or diag else None
         clip = self._clip_scales(norms) if self._server_clip else None
         copies, gathered = None, None
-        if (self._select or self._fltrust or (self._rfa and self.args.rfa_iters > 0)) and self.fused.gathers(K):
+        if (self._select or self._fltrust or self._flame or (self._rfa and self.args.rfa_iters > 0)) and self.fused.gathers(K):
             # on the gather transport every pass reads the same all-gathered copies (one all_gather per round; the root job included)
             gathered = self.fused.gather_participants(K + 1 if self._fltrust else K)
             copies = gathered[:K]
-        keep, weights, scales, total = self._admission(participants, clip, lambda: self.fused.pairwise_sqdist(K, clip, copies),
-                                                       lambda: self.fused.trust_stats(K, K, gathered),
-                                                       lambda b, members: self.fused.rfa_sqdist(K, b, clip, members, copies), cur_round)
+        keep, weights, scales, total, noise_std = self._admission(
+            participants, clip, lambda: self.fused.pairwise_sqdist(K, clip, copies), lambda: self.fused.trust_stats(K, K, gathered),
+            lambda b, members: self.fused.rfa_sqdist(K, b, clip, members, copies),
+            lambda members: self.fused.pairwise_gram(K, members, copies), cur_round)
         if diag:   # the sign-agreement analysis needs the pre-step global parameters and every admitted participant's parameters
             prev = self.fused.w_global.clone()
             ws = [w.clone() for w in self.fused.gather_participants(K)]
             voters = participants
             if keep is not None:
                 ws, voters = [ws[j] for j in keep], [participants[j] for j in keep]
-        self.fused.aggregate(weights, self._mode, self.args.robustLR_threshold, self.server_lr,
-                             self.args.noise * self.args.clip, self.args.seed, cur_round, scales, members=keep, participants=copies,
-                             total_weight=total)
+        self.fused.aggregate(weights, self._mode, self.args.robustLR_threshold, self.server_lr, noise_std, self.args.seed, cur_round,
+                             scales, members=keep, participants=copies, total_weight=total)
         self.last_flipped = self.fused.flipped
         if diag:
             self.plot_norms(dict(zip(participants, norms.tolist())), cur_round)
@@ -117,18 +122,22 @@ class Aggregation:
     def _select(self):
         return getattr(self.args, "select", "none") != "none"
 
-    def _admission(self, ids, clip, distances, trust_stats, rfa_pass, cur_round):
+    def _admission(self, ids, clip, distances, trust_stats, rfa_pass, gram, cur_round):
         """Admission of the participants ``ids`` shared by both forms of the step: Krum / Multi-Krum on ``distances()`` (``--select``),
-        then FLTrust on ``trust_stats()`` (``--aggr fltrust``) or RFA's weights from ``rfa_pass(b, members)`` (``--aggr rfa``).  ``clip``:
-        the server-clipping scales or None.  Returns ``(members, weights, scales, total_weight)`` for the step: members None admits
-        everyone; weights are per position in ``ids``."""
+        then FLTrust on ``trust_stats()`` (``--aggr fltrust``), RFA's weights from ``rfa_pass(b, members)`` (``--aggr rfa``) or FLAME on
+        the Gram matrix ``gram(members)`` (``--aggr flame``).  ``clip``: the server-clipping scales or None.  Returns
+        ``(members, weights, scales, total_weight, noise_std)`` for the step: members None admits everyone; weights are per position in
+        ``ids``."""
         keep = self._admit(distances(), ids, cur_round) if self._select else None
+        noise_std = self.args.noise * self.args.clip
         if self._fltrust:
-            return self._trust(trust_stats(), ids, keep, cur_round)
+            return (*self._trust(trust_stats(), ids, keep, cur_round), noise_std)
+        if self._flame:
+            return self._flame_step(ids, keep, gram, cur_round)
         weights = [float(self.agent_data_sizes[i]) for i in ids]
         if self._rfa:
-            return self._rfa_weights(ids, keep, weights, clip, rfa_pass, cur_round)
-        return keep, weights, clip, None
+            return (*self._rfa_weights(ids, keep, weights, clip, rfa_pass, cur_round), noise_std)
+        return keep, weights, clip, None, noise_std
 
     def _admit(self, D, ids, cur_round):
         """Krum / Multi-Krum admission from the pairwise distances ``D`` of the participants ``ids``: the admitted positions
@@ -152,10 +161,39 @@ class Aggregation:
         return self.args.aggr == "rfa"
 
     @property
+    def _flame(self):
+        return self.args.aggr == "flame"
+
+    @property
     def _mode(self):
         """The aggregate kernel's rule: FLTrust is its weighted mean with trust weights and per-participant scales, RFA with its
-        Weiszfeld weights."""
-        return "avg" if self._fltrust or self._rfa else self.args.aggr
+        Weiszfeld weights, FLAME with equal weights and its clip scales."""
+        return "avg" if self._fltrust or self._rfa or self._flame else self.args.aggr
+
+    def _flame_step(self, ids, keep, gram, cur_round):
+        """FLAME over the positions ``keep`` that selection admitted (all when None): ``ops.flame_admit`` on ``gram(candidates)``.
+        Returns ``(members, weights, scales, total_weight, noise_std)`` for the step: the admitted positions with weight 1 each, total
+        weight their count, the clip scales and noise std ``flame_lambda * S`` -- or, when nobody is admitted, every candidate with weight 0
+        and total weight 1, so the aggregate is 0 plus noise.  Records ``last_admitted`` and logs the admitted count, the corrupt ones
+        among them (ids < num_corrupt), the clip bound S and the noise std."""
+        K = len(ids)
+        cand = list(range(K)) if keep is None else [int(j) for j in keep]
+        adm, sc, S, noise_std = ops.flame_admit(gram(cand), [ids[j] for j in cand], self.args.flame_lambda)
+        members = [cand[j] for j in adm]
+        scales = torch.ones(K, dtype=torch.float32)
+        scales[torch.as_tensor(cand, dtype=torch.int64)] = sc
+        weights, total = [1.0] * K, float(len(members))
+        self.last_admitted = [ids[j] for j in members]
+        if not members:
+            members, weights, total = cand, [0.0] * K, 1.0
+        nc = self.args.num_corrupt
+        self.last_flame = {"FLAME/Admitted": len(self.last_admitted),
+                           "FLAME/Corrupt_Admitted": sum(1 for i in self.last_admitted if i < nc),
+                           "FLAME/Clip_Bound": S, "FLAME/Noise_Std": noise_std}
+        if self.writer is not None:
+            for k, v in self.last_flame.items():
+                self.writer.add_scalar(k, v, cur_round)
+        return members, weights, scales, total, noise_std
 
     def _rfa_weights(self, ids, keep, weights, clip, rfa_pass, cur_round):
         """RFA over the positions ``keep`` that selection admitted (all when None): ``--rfa_iters`` smoothed Weiszfeld passes

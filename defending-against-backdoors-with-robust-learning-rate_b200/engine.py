@@ -353,6 +353,11 @@ class FLEngine:
             if self.aggregator.last_rfa is not None:
                 rec["rfa_corrupt_weight"] = self.aggregator.last_rfa["RFA/Corrupt_Weight"]
                 rec["rfa_passes"] = self.aggregator.last_rfa["RFA/Passes"]
+            if self.aggregator.last_flame is not None:
+                rec["flame_admitted"] = self.aggregator.last_flame["FLAME/Admitted"]
+                rec["flame_corrupt_admitted"] = self.aggregator.last_flame["FLAME/Corrupt_Admitted"]
+                rec["flame_clip_bound"] = self.aggregator.last_flame["FLAME/Clip_Bound"]
+                rec["flame_noise_std"] = self.aggregator.last_flame["FLAME/Noise_Std"]
             rec.update({f"ms_{k}": v for k, v in self.timer.elapsed().items()})
             if args.profile_phases and self.verbose:
                 print({k: round(v, 3) for k, v in rec.items() if k.startswith("ms_")})

@@ -721,6 +721,118 @@ def rfa(alpha, pass_fn, T, nu):
 
 
 # =====================================================================================================================
+# FLAME (Nguyen et al., USENIX Security 2022): cosine clustering, median-norm clipping and adaptive noise
+# =====================================================================================================================
+def gram_statement(w_agents, w_global, lo, hi):
+    """fp64 statement of the FLAME Gram pass over coordinates ``[lo, hi)``: a float64 ``[K][K]`` tensor of ``G[i][j] = sum_c Δi[c] Δj[c]``
+    with ``Δk = w_k - w_global``; the diagonal holds the squared update norms."""
+    K = len(w_agents)
+    dev = w_global.device
+    G = torch.zeros(K, K, dtype=torch.float64, device=dev)
+    step = max(4, (1 << 24) // max(1, K))                 # coordinates per pass: K * step fp64 values
+    for c in range(lo, hi, step):
+        e = min(hi, c + step)
+        x = torch.stack([w[c:e] for w in w_agents]).double() - w_global[c:e].double()
+        G += x @ x.T
+    return G
+
+
+def pairwise_gram(w_agents, w_global, n_vote=None):
+    """K x K float64 Gram matrix of the participants' updates ``w_k - w_global`` over the voted coordinates ``[0, n_vote)``
+    (``gram_statement``'s values; the BatchNorm running statistics behind ``n_vote`` do not count).  On CUDA this launches
+    ``pairwise_sqdist_kernel<true>`` (ops/csrc/select.cu); on CPU, and for more participants than the kernel's tables hold (recorded as a
+    library fall-through), it evaluates ``gram_statement``."""
+    nv = w_global.numel() if n_vote is None else int(n_vote)
+    K = len(w_agents)
+    return _participant_pass("pairwise_gram", w_agents, (w_global,), nv, (K, K), lambda: gram_statement(w_agents, w_global, 0, nv),
+                             lambda tab, out: ext().pairwise_gram(tab, w_global.data_ptr(), 0, nv, out, None, None, 0, 1, 0))
+
+
+def _first_cluster(d, m):
+    """Single linkage on the symmetric distances ``d`` (float64 ``[n][n]``, +inf allowed): the vertices of the first connected component
+    of at least ``m`` vertices in the graph of the edges ``d_ij <= h`` as ``h`` grows, all edges of one ``h`` taken together; [] when
+    ``n < m``.  Those components are the ones of the minimum spanning tree's edges ``<= h``, so this is Prim's tree (O(n^2) in numpy)
+    and a union-find over its ``n - 1`` edges."""
+    n = d.shape[0]
+    if n < m:
+        return []
+    if m <= 1:
+        return list(range(n))
+    in_tree = np.zeros(n, dtype=bool)
+    in_tree[0] = True
+    best, parent = d[0].copy(), np.zeros(n, dtype=np.int64)
+    edges = []
+    for _ in range(n - 1):
+        out = np.flatnonzero(~in_tree)
+        k = int(out[np.argmin(best[out])])
+        edges.append((float(best[k]), int(parent[k]), k))
+        in_tree[k] = True
+        closer = d[k] < best
+        parent[closer] = k
+        best[closer] = d[k][closer]
+    root, size = list(range(n)), [1] * n
+
+    def find(x):
+        while root[x] != x:
+            root[x] = root[root[x]]
+            x = root[x]
+        return x
+    edges.sort(key=lambda t: t[0])
+    i, hit = 0, None
+    while i < len(edges):
+        h = edges[i][0]
+        while i < len(edges) and edges[i][0] == h:
+            a, b = find(edges[i][1]), find(edges[i][2])
+            if a != b:
+                root[b] = a
+                size[a] += size[b]
+                if size[a] >= m:
+                    hit = a                # m > n / 2: at most one component ever reaches m
+            i += 1
+        if hit is not None:
+            r = find(hit)
+            return [k for k in range(n) if find(k) == r]
+    return []
+
+
+def flame_admit(G, ids, lam):
+    """FLAME's admission, clip bound and noise on the host, in fp64, shared by every form of the server step.  ``G``: the Gram matrix of
+    the candidates' updates (``gram_statement``'s layout); ``ids``: their agent ids; ``lam``: the noise factor lambda.
+
+    ``e_k = sqrt(G_kk)``; ``cos_ij = G_ij / sqrt(G_ii G_jj)`` clamped to [-1, 1] (0 when a norm is 0); ``d_ij = 1 - cos_ij`` (NaN counts
+    as +inf).  The admitted set is the first single-linkage cluster of at least ``m = K // 2 + 1`` candidates (``_first_cluster``) among
+    those whose ``e_k`` is finite -- HDBSCAN(min_cluster_size=m, min_samples=1, allow_single_cluster=True) on these distances.  The pairs
+    are read from the upper triangle in agent-id order, so the admitted ids do not depend on the candidates' positions.  The clip bound
+    ``S`` is the median of every candidate's ``e_k`` (numpy's: the mean of the middle two for even K; NaN sorts as +inf) and
+    ``s_k = fp32(min(1, S / e_k))`` (1 when ``e_k`` is 0 or NaN).  Returns ``(members, scales, S, noise_std)``: the admitted positions
+    (ascending, possibly none), float32 ``[K]`` scales, ``S`` and ``noise_std = lam * S``."""
+    g = np.asarray(torch.as_tensor(G).detach().double().cpu().numpy(), dtype=np.float64)
+    K = g.shape[0]
+    if g.shape != (K, K) or len(ids) != K:
+        raise ValueError(f"flame_admit: a {g.shape} Gram matrix for {len(ids)} candidates")
+    order = sorted(range(K), key=lambda k: ids[k])
+    g = g[np.ix_(order, order)]
+    g = np.triu(g) + np.triu(g, 1).T
+    q = np.diag(g).copy()
+    e = np.sqrt(q)
+    with np.errstate(all="ignore"):
+        nrm = np.sqrt(np.outer(q, q))
+        d = 1.0 - np.clip(np.where(nrm > 0, g / np.where(nrm > 0, nrm, 1.0), 0.0), -1.0, 1.0)
+    d[np.isnan(d)] = np.inf
+    ok = np.flatnonzero(np.isfinite(e))
+    cluster = _first_cluster(d[np.ix_(ok, ok)], K // 2 + 1)
+    members = sorted(order[int(ok[j])] for j in cluster)
+    e_pos = np.empty(K, dtype=np.float64)
+    e_pos[order] = e
+    S = float(np.median(np.where(np.isnan(e_pos), np.inf, e_pos)))
+    scales = np.ones(K, dtype=np.float32)
+    for k in range(K):
+        if e_pos[k] > 0:
+            scales[k] = np.float32(min(1.0, S / float(e_pos[k])))
+    return members, torch.from_numpy(scales), S, float(lam) * S
+
+
+# =====================================================================================================================
 # optimiser over flat buffers
 # =====================================================================================================================
 def round_init(w_global, w_local=None, w_bf16=None, mom=None):

@@ -115,6 +115,25 @@ void pairwise_sqdist(at::Tensor w_agent_ptrs, int64_t w_global_ptr, c10::optiona
     check(rlr::launch_pairwise_sqdist(p, out.data_ptr<double>(), num_sms(), cur_stream()), "pairwise_sqdist");
 }
 
+// FLAME: K x K fp64 Gram matrix of the participants' updates w_k - w_global over coordinates [begin, end), diagonal included.  world > 1:
+// the fused multi-GPU form, which first runs the aggregation's barrier-in at `epoch`.
+void pairwise_gram(at::Tensor w_agent_ptrs, int64_t w_global_ptr, int64_t begin, int64_t end, at::Tensor out,
+                   c10::optional<at::Tensor> flag_ptrs, c10::optional<at::Tensor> local_sync, int64_t rank, int64_t world, int64_t epoch) {
+    CHECK_CUDA(w_agent_ptrs); CHECK_CUDA(out);
+    TORCH_CHECK(w_agent_ptrs.scalar_type() == at::kLong, "pointer table must be int64");
+    const int64_t K = w_agent_ptrs.numel();
+    TORCH_CHECK(out.scalar_type() == at::kDouble && out.numel() == K * K, "out must be a float64 [K, K] tensor");
+    TORCH_CHECK(w_global_ptr, "pairwise_gram needs w_global");
+    c10::cuda::CUDAGuard guard(out.device());
+    rlr::DistParams p{};
+    p.w_agents = reinterpret_cast<const float* const*>(w_agent_ptrs.data_ptr());
+    p.w_global = reinterpret_cast<const float*>(w_global_ptr);
+    p.begin = begin; p.end = end;
+    p.K = (int)K;
+    p.gate = gate_of(flag_ptrs, local_sync, rank, world, epoch);
+    check(rlr::launch_pairwise_gram(p, out.data_ptr<double>(), num_sms(), cur_stream()), "pairwise_gram");
+}
+
 // FLTrust statistics over coordinates [begin, end): fp64 [2K + 1] = (Δk.Δ0 for every k, |Δk|^2 for every k, |Δ0|^2), Δk = w_k - w_global,
 // Δ0 = w_ref - w_global.  world > 1: the fused multi-GPU form, which first runs the aggregation's barrier-in at `epoch`.
 void trust_stats(at::Tensor w_agent_ptrs, int64_t w_ref_ptr, int64_t w_global_ptr, int64_t begin, int64_t end, at::Tensor out,
@@ -368,6 +387,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("aggregate_max_agents", &rlr::aggregate_max_agents);
     m.def("acquire_slices", &acquire_slices);
     m.def("pairwise_sqdist", &pairwise_sqdist);
+    m.def("pairwise_gram", &pairwise_gram);
     m.def("trust_stats", &trust_stats);
     m.def("rfa_sqdist", &rfa_sqdist);
     m.def("gather_normalize", &gather_normalize);

@@ -62,6 +62,9 @@ struct DistParams {
     Gate gate;                      // world > 1: the aggregation's barrier-in
 };
 cudaError_t launch_pairwise_sqdist(const DistParams& p, double* out, int num_sms, cudaStream_t st);
+// FLAME's Gram matrix of the updates: out[i][j] = sum_{begin <= c < end} Δi[c] Δj[c] in fp64 ([K][K], symmetric, diagonal = squared
+// update norms), Δk = w_k - w_global formed in fp32.  Same kernel, tiles and fixed-order sums as the distances; needs w_global, no scales.
+cudaError_t launch_pairwise_gram(const DistParams& p, double* out, int num_sms, cudaStream_t st);
 
 // ---- FLTrust: each participant's update against the server's root update Δ0 = w_ref - w_global -----------------------------------------
 // out[k] = sum_c Δk[c] Δ0[c], out[K + k] = sum_c Δk[c]^2, out[2K] = sum_c Δ0[c]^2 over [begin, end), fp64 [2K + 1], Δk = w_k - w_global.

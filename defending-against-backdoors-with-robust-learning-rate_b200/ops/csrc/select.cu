@@ -14,6 +14,10 @@
 // fp64.  Small tiles give each pair block several coordinate lanes; the lanes are added in lane order at the end.  Every (tile, split)
 // CTA writes its tile, mirrored, to its split's [K][K] workspace slot and launch_ordered_sum adds the slots in split order.  No atomics:
 // the matrix is bitwise identical from run to run.
+//
+// The same kernel with GRAM = true is FLAME's Gram pass: G[i][j] = sum_c Δi[c] Δj[c] with Δk = w_k - w_global formed per coordinate in
+// fp32 while staging, one FMA per pair and coordinate, and the diagonal (the squared update norms) kept.  Cosines are taken from G
+// directly: deriving them from D through (|a|^2 + |b|^2 - D) / 2 cancels near cos = 0, where honest high-dimensional updates sit.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -35,6 +39,7 @@ struct DistKernelParams {
     double* ws;                                         // [splits][K][K]
 };
 
+template <bool GRAM>
 __global__ void __launch_bounds__(kDistThreads, 2) pairwise_sqdist_kernel(DistKernelParams kp) {
     extern __shared__ float4 stage4[];
     float* const stage = reinterpret_cast<float*>(stage4);
@@ -103,7 +108,10 @@ __global__ void __launch_bounds__(kDistThreads, 2) pairwise_sqdist_kernel(DistKe
                 if (idx < P * G && g < ng && wp[q]) {
                     const long long i = cc + 4 * g;
                     v[u] = ld_f4(wp[q] + i);
-                    if (p.scales) {
+                    if (GRAM) {
+                        const float4 gg = ld_f4(p.w_global + i);
+                        v[u] = make_float4(v[u].x - gg.x, v[u].y - gg.y, v[u].z - gg.z, v[u].w - gg.w);
+                    } else if (p.scales) {
                         const float4 gg = ld_f4(p.w_global + i);
                         const float s = scs[q];
                         v[u] = make_float4((v[u].x - gg.x) * s, (v[u].y - gg.y) * s, (v[u].z - gg.z) * s, (v[u].w - gg.w) * s);
@@ -135,11 +143,18 @@ __global__ void __launch_bounds__(kDistThreads, 2) pairwise_sqdist_kernel(DistKe
                     const float4 x = cb[c * (RS >> 2) + g];
 #pragma unroll
                     for (int r = 0; r < 4; ++r) {
-                        float d;
-                        d = a[r].x - x.x; acc[r][c] = __fmaf_rn(d, d, acc[r][c]);
-                        d = a[r].y - x.y; acc[r][c] = __fmaf_rn(d, d, acc[r][c]);
-                        d = a[r].z - x.z; acc[r][c] = __fmaf_rn(d, d, acc[r][c]);
-                        d = a[r].w - x.w; acc[r][c] = __fmaf_rn(d, d, acc[r][c]);
+                        if (GRAM) {
+                            acc[r][c] = __fmaf_rn(a[r].x, x.x, acc[r][c]);
+                            acc[r][c] = __fmaf_rn(a[r].y, x.y, acc[r][c]);
+                            acc[r][c] = __fmaf_rn(a[r].z, x.z, acc[r][c]);
+                            acc[r][c] = __fmaf_rn(a[r].w, x.w, acc[r][c]);
+                        } else {
+                            float d;
+                            d = a[r].x - x.x; acc[r][c] = __fmaf_rn(d, d, acc[r][c]);
+                            d = a[r].y - x.y; acc[r][c] = __fmaf_rn(d, d, acc[r][c]);
+                            d = a[r].z - x.z; acc[r][c] = __fmaf_rn(d, d, acc[r][c]);
+                            d = a[r].w - x.w; acc[r][c] = __fmaf_rn(d, d, acc[r][c]);
+                        }
                     }
                 }
             }
@@ -168,7 +183,7 @@ __global__ void __launch_bounds__(kDistThreads, 2) pairwise_sqdist_kernel(DistKe
                 for (int ll = 1; ll < L; ++ll) v += red[(ll * NB + tid) * 16 + r * 4 + c];
                 const int i = r0 + 4 * bi + r, j = c0 + 4 * bj + c;
                 if (4 * bi + r < nr && 4 * bj + c < nc) {
-                    if (i == j) v = 0.0;
+                    if (!GRAM && i == j) v = 0.0;
                     out[(size_t)i * K + j] = v;
                     out[(size_t)j * K + i] = v;
                 }
@@ -177,14 +192,15 @@ __global__ void __launch_bounds__(kDistThreads, 2) pairwise_sqdist_kernel(DistKe
     }
 }
 
-cudaError_t launch_pairwise_sqdist(const DistParams& p, double* out, int num_sms, cudaStream_t st) {
+template <bool GRAM>
+static cudaError_t launch_pairwise(const DistParams& p, double* out, int num_sms, cudaStream_t st) {
     if (p.K < 1 || p.K > kDistMaxAgents) return cudaErrorInvalidValue;
     if ((p.begin & 3) || (p.end & 3) || p.end < p.begin) return cudaErrorInvalidValue;
-    if ((p.scales && !p.w_global) || !gate_ok(p.gate)) return cudaErrorInvalidValue;
+    if (((GRAM || p.scales) && !p.w_global) || (GRAM && p.scales) || !gate_ok(p.gate)) return cudaErrorInvalidValue;
     static int occ = 0;
     if (!occ) {
-        RLR_CUDA_CHECK(cudaFuncSetAttribute(pairwise_sqdist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDistSmem));
-        RLR_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pairwise_sqdist_kernel, kDistThreads, kDistSmem));
+        RLR_CUDA_CHECK(cudaFuncSetAttribute(pairwise_sqdist_kernel<GRAM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDistSmem));
+        RLR_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pairwise_sqdist_kernel<GRAM>, kDistThreads, kDistSmem));
         occ = occ < 1 ? 1 : occ;
     }
     DistKernelParams kp{};
@@ -198,9 +214,17 @@ cudaError_t launch_pairwise_sqdist(const DistParams& p, double* out, int num_sms
     Scratch ws((size_t)(splits * kk) * sizeof(double), st);
     kp.ws = ws.as<double>();
     RLR_CUDA_CHECK(cudaMemsetAsync(out, 0, (size_t)kk * sizeof(double), st));
-    pairwise_sqdist_kernel<<<dim3((unsigned)tiles, (unsigned)splits), kDistThreads, kDistSmem, st>>>(kp);
+    pairwise_sqdist_kernel<GRAM><<<dim3((unsigned)tiles, (unsigned)splits), kDistThreads, kDistSmem, st>>>(kp);
     RLR_CUDA_CHECK(cudaGetLastError());
     return launch_ordered_sum(out, kp.ws, (int)splits, kk, st);
+}
+
+cudaError_t launch_pairwise_sqdist(const DistParams& p, double* out, int num_sms, cudaStream_t st) {
+    return launch_pairwise<false>(p, out, num_sms, st);
+}
+
+cudaError_t launch_pairwise_gram(const DistParams& p, double* out, int num_sms, cudaStream_t st) {
+    return launch_pairwise<true>(p, out, num_sms, st);
 }
 
 }  // namespace rlr

@@ -14,10 +14,11 @@ import math
 import torch
 
 DATASETS = ("fmnist", "fedemnist", "cifar10")
-AGGREGATORS = ("avg", "comed", "sign", "fltrust", "rfa")
+AGGREGATORS = ("avg", "comed", "sign", "fltrust", "rfa", "flame")
 ROOT_SIZE = 100                  # FLTrust root set: the paper's 100 clean samples
 RFA_ITERS = 3                    # RFA: a few smoothed Weiszfeld passes per round
 RFA_NU = 1e-6                    # RFA smoothing: distances below nu count as nu
+FLAME_LAMBDA = 1e-3              # FLAME noise factor: the paper's value for image classification
 SERVER_OPTS = ("sgd", "momentum", "adagrad", "adam", "yogi")
 SELECTIONS = ("none", "krum", "multikrum")
 PATTERNS = ("plus", "square", "copyright", "apple")
@@ -39,7 +40,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--rounds", type=int, default=200, help="number of communication rounds: R")
     p.add_argument("--aggr", type=str, default="avg",
                    help="aggregation rule: avg | comed | sign | fltrust (trust-weighted mean against a server-trained root update) | "
-                        "rfa (smoothed geometric median by Weiszfeld passes, Pillutla et al. 2022)")
+                        "rfa (smoothed geometric median by Weiszfeld passes, Pillutla et al. 2022) | flame (cosine clustering, "
+                        "median-norm clipping and adaptive noise, Nguyen et al. 2022)")
     p.add_argument("--local_ep", type=int, default=2, help="number of local epochs: E")
     p.add_argument("--bs", type=int, default=256, help="local batch size: B")
     p.add_argument("--client_lr", type=float, default=0.1, help="clients' learning rate")
@@ -122,6 +124,9 @@ def build_parser() -> argparse.ArgumentParser:
                         "cost per round fixed")
     p.add_argument("--rfa_nu", type=float, default=None,
                    help=f"--aggr rfa: smoothing nu > 0 of the Weiszfeld weights alpha_k / max(nu, d_k) (default {RFA_NU})")
+    p.add_argument("--flame_lambda", type=float, default=None,
+                   help=f"--aggr flame: noise factor lambda >= 0; the round's Gaussian noise has std lambda * S, S the median update norm "
+                        f"the admitted updates are clipped to (default {FLAME_LAMBDA})")
     return p
 
 
@@ -152,7 +157,31 @@ def finalize_args(args: argparse.Namespace) -> argparse.Namespace:
     _finalize_select(args)
     _finalize_fltrust(args)
     _finalize_rfa(args)
+    _finalize_flame(args)
     return args
+
+
+def _finalize_flame(args) -> None:
+    """Validate the FLAME flags and resolve ``flame_lambda`` in place (``FLAME_LAMBDA`` by default under ``--aggr flame``)."""
+    lam = getattr(args, "flame_lambda", None)
+    if args.aggr != "flame":
+        if lam is not None:
+            raise ValueError("--flame_lambda needs --aggr flame")
+        return
+    lam = FLAME_LAMBDA if lam is None else lam
+    if not (math.isfinite(lam) and lam >= 0):
+        raise ValueError(f"--flame_lambda {lam} must be a finite number >= 0")
+    if getattr(args, "server_clip", False):
+        raise ValueError("--server_clip does not combine with --aggr flame, which clips every update to the round's median norm")
+    if args.noise > 0:
+        raise ValueError("--noise does not combine with --aggr flame, which adds noise of std --flame_lambda times the clip bound")
+    # FLAME admits at least floor(K'/2) + 1 of the K' candidates whenever their norms are finite: the fewest voters it guarantees
+    K = max(1, math.floor(args.num_agents * args.agent_frac))
+    cand = args.select_m if getattr(args, "select", "none") != "none" else K
+    if args.robustLR_threshold > cand // 2 + 1:
+        raise ValueError(f"--robustLR_threshold {args.robustLR_threshold} > {cand // 2 + 1}, the fewest participants --aggr flame admits "
+                         f"of {cand}, could flip every coordinate")
+    args.flame_lambda = float(lam)
 
 
 def _finalize_rfa(args) -> None:
@@ -260,4 +289,6 @@ def print_exp_details(args) -> None:
         print(f"    Root set: {args.root_size}")
     if args.aggr == "rfa":
         print(f"    RFA passes / nu: {args.rfa_iters} / {args.rfa_nu}")
+    if args.aggr == "flame":
+        print(f"    FLAME lambda: {args.flame_lambda}")
     print("======================================")

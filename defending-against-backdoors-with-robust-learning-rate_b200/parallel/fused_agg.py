@@ -253,6 +253,25 @@ class FusedAggregator:
         agents = self._participants(n_part, participants)
         return ops.rfa_sqdist([agents[j] for j in idx], b, self.n_vote, self.w_global if scales is not None else None, scales)
 
+    def pairwise_gram(self, n_part: int, members=None, participants=None):
+        """FLAME Gram pass (``ops.gram_statement``): the float64 Gram matrix of the updates ``w_j - w_global`` of the participants at
+        positions ``members`` (ascending; every one of the round's ``n_part`` when None) over ``[0, n_vote)``, identical on every rank.
+        Call it after the slots are final and before ``aggregate`` of the same round.
+
+        Fused multi-GPU path: each rank runs ``pairwise_sqdist_kernel<true>`` over its coordinate slice of the peer-mapped slots of the
+        members, behind the aggregation kernel's barrier-in (an epoch of its own), and the ranks all_gather their partial matrices and add
+        them in rank order.  The pass reads ``w_global``, so it first acquires the broadcast slices of a fused hand-off.  Gather transport
+        and single process: the same kernel over ``participants`` (``gather_participants``' copies; gathered here when not given).  The
+        reduce transport never holds cross-rank pairs, so the pass takes the gather transport, as Krum's does; the step that follows
+        forms the mean from all-reduced partials when everyone is admitted."""
+        idx = list(range(n_part)) if members is None else [int(j) for j in members]
+        if self._p2p(n_part):
+            self.acquire()
+            table = self._agent_table(n_part) if idx == list(range(n_part)) else self._member_table(idx)
+            return self._fused_pass((len(idx), len(idx)), partial(ops.ext().pairwise_gram, table.tensor, self.w_global.data_ptr()))
+        agents = self._participants(n_part, participants)
+        return ops.pairwise_gram([agents[j] for j in idx], self.w_global, self.n_vote)
+
     def aggregate(self, weights, mode, theta, server_lr, noise_std=0.0, seed=0, rnd=0, scales=None, members=None, participants=None,
                   total_weight=None):
         """Aggregate the round's ``len(weights)`` participants (participant j lives in ``slot_owner(j)``; ``weights`` and ``scales`` are

@@ -23,6 +23,7 @@ import random
 import numpy as np
 import torch
 
+from . import ops
 from .agent import Agent
 from .aggregation import Aggregation, server_opt_spec
 from .data import distribute_data, get_datasets, make_poisoned_val
@@ -152,11 +153,30 @@ class FLEngine:
         self.cum_poison_acc_mean = 0.0
         self.start_round = 1
         self._stream_src = None
+        # ---- model-poisoning attackers (DESIGN.md section 3): boost factor, and Neurotoxin's state -------------------------
+        # w_prev = the global parameters at the start of the previous round; the mask words and |M| are rewritten in place every round,
+        # so the corrupt agents' captured graphs stay valid
+        self.attack_boost = float(getattr(args, "attack_boost", 1.0))
+        p = float(getattr(args, "attack_neurotoxin", 0.0))
+        self.neurotoxin_k = math.floor(p * self.layout.n_params) if p > 0 else None
+        self.last_masked_coords = None
+        if self.neurotoxin_k is not None:
+            nv = self.layout.n_vote
+            self.w_prev = torch.zeros(nv, dtype=torch.float32, device=dev)
+            self.attack_mask = torch.zeros(ops.mask_words(nv), dtype=torch.int32, device=dev)
+            self.masked_coords = torch.zeros(1, dtype=torch.int64, device=dev)
+            self._have_prev = False
         if args.resume:
             ck = load_checkpoint(args.resume, self.w_global, self.layout)
             restore_server_opt(ck, self.fused)
             self.start_round = ck["round"] + 1
             self.cum_poison_acc_mean = ck["extra"].get("cum_poison_acc_mean", 0.0)
+            if self.neurotoxin_k is not None:
+                w_prev = ck["extra"].get("neurotoxin_w_prev")
+                if w_prev is None:
+                    raise ValueError("checkpoint has no Neurotoxin state (w_prev), but this run uses --attack_neurotoxin")
+                self.w_prev.copy_(w_prev.to(dev))
+                self._have_prev = True
         ctx.barrier()
 
     def _jobs(self):
@@ -231,6 +251,9 @@ class FLEngine:
         steps = 0
         h2d = 0
         self.timer.start("local_train")
+        mask = self._neurotoxin_mask() if self.neurotoxin_k is not None else None
+        for t in self.trainers:
+            t.attack_mask = mask
         concurrent = len(self.trainers) > 1
         if concurrent:
             for part in self._loss_parts:
@@ -254,12 +277,14 @@ class FLEngine:
                     if stream_inputs:
                         h2d += self._upload_shard(agent, self._stream_bufs[i])     # on stream i: ordered after trainer i's previous agent
                     st = agent.local_train(self.trainers[i], self.w_global, fused.slots[s], rnd)
+                    self._boost(agent, fused.slots[s])
                     if client:
                         self._loss_parts[i] += st["loss_sum"]
             else:
                 if stream_inputs:
                     h2d += self._upload_shard(agent)
                 st = agent.local_train(self.trainer, self.w_global, fused.slots[s], rnd)
+                self._boost(agent, fused.slots[s])
                 if client:
                     self.round_loss += st["loss_sum"]
             if client:
@@ -277,6 +302,25 @@ class FLEngine:
         self.timer.stop("aggregate")
         return {"chosen": chosen, "steps": steps, "h2d_bytes": h2d}
 
+    def _neurotoxin_mask(self):
+        """Start of a round with Neurotoxin on: the mask of the last global update ``w_global - w_prev`` (the top-k coordinates by
+        magnitude) and ``w_prev <- w_global``, queued on the current stream ahead of the trainers.  Returns the mask words, or None
+        when the mask is empty (the first round a run executes, or k = 0)."""
+        nv = self.layout.n_vote
+        self.fused.acquire()                                             # the pass reads w_global
+        if not self._have_prev:
+            self.w_prev.copy_(self.w_global[:nv])
+            self.masked_coords.zero_()
+            self._have_prev = True
+            return None
+        ops.neurotoxin_mask(self.w_global, self.w_prev, nv, self.neurotoxin_k, self.attack_mask, self.masked_coords)
+        return self.attack_mask if self.neurotoxin_k > 0 else None
+
+    def _boost(self, agent, slot):
+        """Model replacement: a corrupt agent's update in its slot scaled by ``--attack_boost``, on the agent's stream."""
+        if self.attack_boost != 1.0 and agent.is_corrupt:
+            ops.boost_update(slot, self.w_global, self.attack_boost, self.layout.n_vote)
+
     def round_result(self):
         """Device->host read of the round's result: (summed local training loss on this rank, number of REAL coordinates whose
         learning rate was flipped this round).  On the fused multi-GPU back-end every rank counts only its own coordinate slice, so
@@ -285,7 +329,12 @@ class FLEngine:
         flipped = self.fused.flipped.double()
         if self.fused.flipped_is_partial:
             flipped = self.ctx.all_reduce_sum(flipped.clone())
-        vals = torch.cat([self.round_loss.double(), flipped]).cpu()
+        parts = [self.round_loss.double(), flipped]
+        if self.neurotoxin_k is not None:
+            parts.append(self.masked_coords.double())                   # |M| of the round, read with the same copy
+        vals = torch.cat(parts).cpu()
+        if self.neurotoxin_k is not None:
+            self.last_masked_coords = int(vals[2])
         n_flip = int(vals[1])
         if self.args.robustLR_threshold > 0:
             n_flip = max(0, n_flip - (self.layout.n_vote - self.layout.n_params))
@@ -343,6 +392,9 @@ class FLEngine:
             loss, flipped = self.round_result()
             rec["train_loss"] = loss / max(1, info["steps"])
             rec["frac_flipped"] = flipped / max(1, self.layout.n_params)
+            if self.last_masked_coords is not None:
+                rec["attack_masked_coords"] = self.last_masked_coords
+                self.logger.add_scalar("Attack/Masked_Coords", self.last_masked_coords, rnd)
             if self.aggregator.last_select is not None:
                 rec["select_corrupt_participants"] = self.aggregator.last_select["Select/Corrupt_Participants"]
                 rec["select_corrupt_admitted"] = self.aggregator.last_select["Select/Corrupt_Admitted"]
@@ -367,8 +419,10 @@ class FLEngine:
                 state = self.fused.server_opt_state()      # every rank takes part: each holds one slice on the fused multi-GPU path
                 if self.ctx.is_main:
                     so = None if state is None else {**self.fused.opt.hparams, "m": state[0], "v": state[1]}
-                    save_checkpoint(args.checkpoint, self.global_params(), rnd, args, self.layout,
-                                    {"cum_poison_acc_mean": self.cum_poison_acc_mean}, so)
+                    extra = {"cum_poison_acc_mean": self.cum_poison_acc_mean}
+                    if self.neurotoxin_k is not None:
+                        extra["neurotoxin_w_prev"] = self.w_prev.cpu()
+                    save_checkpoint(args.checkpoint, self.global_params(), rnd, args, self.layout, extra, so)
         if self.verbose:
             print("Training has finished!")
         return history

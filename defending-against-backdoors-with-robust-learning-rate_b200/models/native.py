@@ -607,6 +607,9 @@ class NativeTrainer:
         self._graphs = {}
         self._eval_nets = {}
         self.bcast = None             # round hand-off source (parallel.FusedAggregator) once attach_broadcast() was called
+        # Neurotoxin: the round's gradient mask (int32 bit words, engine-owned and rewritten in place), applied to corrupt agents only
+        self.attack_mask = None
+        self._grad_mask = None
 
     # ---- round hand-off fused with the first local step ---------------------------------------------------------------------
     def attach_broadcast(self, fused):
@@ -654,13 +657,14 @@ class NativeTrainer:
         logits = self.net.forward_raw(xin, True)                              # bf16 [B,classes], in the head's activation buffer
         _, dl = ops.softmax_xent(logits, self.y[:B], True, self.loss_sum, dlogits=self.net.dlogits_buffer(B))
         self.net.backward(dl)
-        self.opt.step(self.w, self.g, self.m, w0=w0, w_bf16=self.wb, w_in=self.bcast.w_global if first else None)
+        self.opt.step(self.w, self.g, self.m, w0=w0, w_bf16=self.wb, w_in=self.bcast.w_global if first else None,
+                      grad_mask=self._grad_mask)
         ops.ext().advance_cursor(self.cursor, B, self.net.step_counter)       # next batch; next Philox step for the dropout masks
         if first:
             self._bind_normal()
 
     def _get_graph(self, dataset, B, w0, first=False):
-        key = (B, dataset.data.data_ptr(), w0.data_ptr(), bool(first))
+        key = (B, dataset.data.data_ptr(), w0.data_ptr(), bool(first), 0 if self._grad_mask is None else self._grad_mask.data_ptr())
         if key in self._graphs:
             return self._graphs[key]
         keep = (self.w.clone(), self.wb.clone(), self.m.clone(), self.cursor.clone(), self.loss_sum.clone(),
@@ -688,6 +692,7 @@ class NativeTrainer:
         args, bs = self.args, self.bs
         dataset, n = agent.dataset, agent.n_data
         self.loss_sum.zero_()
+        self._grad_mask = self.attack_mask if getattr(agent, "is_corrupt", False) else None
         graphs = self.use_graphs and n <= self.max_shard
         fused = self.bcast is not None and w_global.data_ptr() == self.bcast.w_global.data_ptr()
         if graphs:

@@ -833,6 +833,71 @@ def flame_admit(G, ids, lam):
 
 
 # =====================================================================================================================
+# model-poisoning attackers (DESIGN.md section 3)
+# =====================================================================================================================
+def mask_words(n: int) -> int:
+    """Number of 32-bit words of a coordinate mask over ``n`` coordinates."""
+    return (int(n) + 31) // 32
+
+
+def mask_bits(words, n: int):
+    """Bool tensor ``[n]`` of a coordinate mask stored as int32 bit words (bit ``c % 32`` of word ``c // 32`` = coordinate ``c``)."""
+    shifts = torch.arange(32, dtype=torch.int32, device=words.device)
+    return ((words.view(torch.int32)[:, None] >> shifts) & 1).flatten()[:int(n)].bool()
+
+
+def neurotoxin_statement(w_g, w_prev, n_vote: int, k: int):
+    """Neurotoxin's mask, stated in numpy: ``a[c] = bits(|fp32(w_g[c] - w_prev[c])|)`` for ``c < n_vote`` (the fp32 pattern with the
+    sign bit cleared, so NaN sorts above +inf), ``tau`` = the k-th largest ``a`` counted with multiplicity, and
+    ``M = {c : a[c] >= tau, a[c] > 0}`` (empty for ``k = 0``).  Returns ``(words, |M|)``: ``words`` is a uint32 array of
+    ``mask_words(n_vote)`` words, bit ``c % 32`` of word ``c // 32`` set for ``c`` in M."""
+    n_vote, k = int(n_vote), int(k)
+    if not 0 <= k <= n_vote:
+        raise ValueError(f"k = {k} must lie in [0, n_vote = {n_vote}]")
+    g = w_g[:n_vote].detach().cpu().numpy().astype(np.float32, copy=False)
+    p = w_prev[:n_vote].detach().cpu().numpy().astype(np.float32, copy=False)
+    with np.errstate(invalid="ignore", over="ignore"):
+        a = (g - p).view(np.uint32) & np.uint32(0x7FFFFFFF)
+    m = np.zeros(mask_words(n_vote) * 32, dtype=bool)
+    if k > 0:
+        tau = np.partition(a, n_vote - k)[n_vote - k]
+        m[:n_vote] = a >= max(int(tau), 1)
+    return np.packbits(m, bitorder="little").view("<u4").astype(np.uint32), int(m.sum())
+
+
+def neurotoxin_mask(w_g, w_prev, n_vote: int, k: int, mask, count):
+    """Neurotoxin's mask of the last global update ``w_g - w_prev`` over ``[0, n_vote)`` (``neurotoxin_statement``): writes the
+    ``mask_words(n_vote)`` int32 words of ``mask`` and ``|M|`` into the int64 ``count``, then refreshes ``w_prev[:n_vote] <- w_g``.
+    On the GPU a radix select finds the threshold on the device: no host sync, bitwise reproducible."""
+    if w_g.is_cuda:
+        ext().neurotoxin_mask(w_g, w_prev, int(n_vote), int(k), mask, count)
+        return
+    words, c = neurotoxin_statement(w_g, w_prev, n_vote, k)
+    mask[:words.size].copy_(torch.from_numpy(words.view(np.int32)))
+    count.fill_(c)
+    w_prev[:n_vote].copy_(w_g[:n_vote])
+
+
+def boost_statement(slot, w_g, gamma: float, n_vote: int):
+    """The boosted update in numpy: ``fp32((double)w_g[c] + (double)gamma * (double)fp32(slot[c] - w_g[c]))`` for ``c < n_vote``,
+    each fp64 operation rounded on its own.  Returns a float32 array ``[n_vote]``."""
+    s = slot[:n_vote].detach().cpu().numpy().astype(np.float32, copy=False)
+    g = w_g[:n_vote].detach().cpu().numpy().astype(np.float32, copy=False)
+    with np.errstate(invalid="ignore", over="ignore"):
+        d = (s - g).astype(np.float64)
+        return (g.astype(np.float64) + np.float64(gamma) * d).astype(np.float32)
+
+
+def boost_update(slot, w_g, gamma: float, n_vote: int):
+    """Model replacement: scale the update in ``slot`` by ``gamma`` in place over ``[0, n_vote)`` (``boost_statement``); the
+    BatchNorm running statistics behind ``n_vote`` are left alone."""
+    if slot.is_cuda:
+        ext().boost_update(slot, w_g, float(gamma), int(n_vote))
+        return
+    slot[:n_vote].copy_(torch.from_numpy(boost_statement(slot, w_g, gamma, n_vote)))
+
+
+# =====================================================================================================================
 # optimiser over flat buffers
 # =====================================================================================================================
 def round_init(w_global, w_local=None, w_bf16=None, mom=None):
@@ -863,21 +928,36 @@ class FlatSGD:
         self.n_pgd = int(n if n_pgd is None else n_pgd)
         self.norms = torch.zeros(2, dtype=torch.float64, device=device)  # [||g||^2, ||w-w0||^2]
 
-    def step(self, w, g, m, w0=None, w_bf16=None, w_in=None):
+    def step(self, w, g, m, w0=None, w_bf16=None, w_in=None, grad_mask=None):
         """``w_in``: first local step of a round fused with the hand-off -- parameters are read from ``w_in`` (the round's global
         parameters, i.e. the broadcast buffer) instead of ``w`` and the momentum counts as zero, so no separate
         ``w <- w_global, m <- 0`` pass is needed; coordinates ``>= n_pgd`` (BatchNorm running statistics already updated in ``w``
-        by this step's forward pass) keep their value."""
+        by this step's forward pass) keep their value.
+
+        ``grad_mask``: int32 bit words over ``[0, n_pgd)`` (Neurotoxin): ``g[c]`` counts as zero for every set bit, before the
+        gradient norm is taken, and the PGD projection leaves those coordinates alone.  Same launches as without it."""
         if w.is_cuda:
             e = ext()
             e.memset_zero(self.norms)
-            e.sqnorm(g, self.norms[0:1])
             pgd = self.pgd_clip > 0
+            if grad_mask is None:
+                e.sqnorm(g, self.norms[0:1])
+                e.sgd_step(w, g, m, w0 if pgd else None, w_bf16, self.lr, self.momentum, self.max_grad_norm,
+                           self.norms[0:1], self.norms[1:2] if pgd else None, self.n_pgd, w_in)
+                if pgd:
+                    e.pgd_project(w, w0, w_bf16, self.pgd_clip, self.norms[1:2], self.n_pgd)
+                return
+            e.sqnorm(g, self.norms[0:1], grad_mask, self.n_pgd)
             e.sgd_step(w, g, m, w0 if pgd else None, w_bf16, self.lr, self.momentum, self.max_grad_norm,
-                       self.norms[0:1], self.norms[1:2] if pgd else None, self.n_pgd, w_in)
+                       self.norms[0:1], self.norms[1:2] if pgd else None, self.n_pgd, w_in, grad_mask)
             if pgd:
-                e.pgd_project(w, w0, w_bf16, self.pgd_clip, self.norms[1:2], self.n_pgd)
+                e.pgd_project(w, w0, w_bf16, self.pgd_clip, self.norms[1:2], self.n_pgd, grad_mask)
             return
+        masked = None
+        if grad_mask is not None:
+            masked = mask_bits(grad_mask, self.n_pgd)
+            g = g.clone()
+            g[:self.n_pgd].masked_fill_(masked, 0.0)
         gn = g.double().norm()
         coef = min(1.0, self.max_grad_norm / (float(gn) + 1e-6)) if self.max_grad_norm > 0 else 1.0
         if w_in is not None:
@@ -893,7 +973,8 @@ class FlatSGD:
             d = w[:k] - w0[:k]
             denom = max(1.0, float(d.double().norm()) / self.pgd_clip)
             if denom > 1.0:
-                w[:k].copy_(w0[:k] + d / denom)
+                proj = w0[:k] + d / denom
+                w[:k].copy_(proj if masked is None else torch.where(masked, w[:k], proj))
         if w_bf16 is not None:
             w_bf16.copy_(w.to(torch.bfloat16))
 

@@ -1,0 +1,177 @@
+// Model-poisoning attackers (DESIGN.md section 3): Neurotoxin's top-k mask of the last global update and the boosted update.
+//
+// Neurotoxin (Zhang et al. 2022): a[c] = bits(|fp32(w_g[c] - w_prev[c])|) for c < n_vote (the fp32 pattern with the sign bit cleared:
+// 31-bit unsigned keys that order like the magnitudes, NaN above +inf).  tau is the k-th largest key, counted with multiplicity, found
+// by a radix select over the 31 key bits in three histogram passes (11 + 11 + 9 bits), each restricted to the prefix the previous one
+// fixed.  The bin that crosses k is found on the device by one small CTA between the passes, so tau never leaves the GPU and the whole
+// pass queues on the round's stream without a host sync.  Histogram counts are integer atomics (exact, order-free).  The last pass
+// writes M = {c : a[c] >= tau, a[c] > 0} as ceil(n_vote/32) bit words, its popcount, and w_prev <- w_g.
+//
+// Every pass recomputes a[c] from w_g and w_prev (8 B per coordinate) instead of staging the keys in a 4 B scratch copy: 36 B per
+// coordinate in all (3 x 8 read, 8 read + 4 written by the mask pass) against 32 B with a 45 MB scratch at the ResNet-18 size.
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "common.cuh"
+#include "kernels.h"
+
+namespace rlr {
+
+namespace {
+
+constexpr int kBins = 2048;          // 11-bit digits; the last pass uses 512 of them (9 bits)
+constexpr int kHistThreads = 512;
+
+// pass p: digit bits and the shift of the prefix fixed by the earlier passes
+__device__ __forceinline__ int digit_shift(int pass) { return pass == 0 ? 20 : (pass == 1 ? 9 : 0); }
+__device__ __forceinline__ uint32_t digit_mask(int pass) { return pass == 2 ? 0x1FFu : 0x7FFu; }
+__device__ __forceinline__ int prefix_shift(int pass) { return pass == 1 ? 20 : 9; }
+
+__device__ __forceinline__ uint32_t key_of(float g, float p) { return __float_as_uint(g - p) & 0x7FFFFFFFu; }
+
+struct SelectState {
+    uint32_t prefix;                 // key bits fixed so far (right-aligned)
+    uint32_t krem;                   // rank still to find inside the selected prefix, 1-based from the top
+};
+
+__global__ void __launch_bounds__(kHistThreads) topk_hist_kernel(const float* __restrict__ wg, const float* __restrict__ wp,
+                                                                  long long n4, int pass, const SelectState* __restrict__ st,
+                                                                  uint32_t* __restrict__ hist /*[kBins]*/) {
+    __shared__ uint32_t h[kBins];
+    for (int i = threadIdx.x; i < kBins; i += blockDim.x) h[i] = 0;
+    __syncthreads();
+    const int sh = digit_shift(pass);
+    const uint32_t dm = digit_mask(pass);
+    const int psh = prefix_shift(pass);
+    const uint32_t want = pass == 0 ? 0u : st->prefix;
+    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n4; q += (long long)gridDim.x * blockDim.x) {
+        const float4 g = ld_f4(wg + 4 * q), p = ld_f4(wp + 4 * q);
+        const uint32_t a[4] = {key_of(g.x, p.x), key_of(g.y, p.y), key_of(g.z, p.z), key_of(g.w, p.w)};
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            if (pass == 0 || (a[j] >> psh) == want) atomicAdd(&h[(a[j] >> sh) & dm], 1u);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < kBins; i += blockDim.x)
+        if (h[i]) atomicAdd(&hist[i], h[i]);
+}
+
+// One CTA of kBins/2 threads: the bin where the count from the top reaches krem.  Thread t holds the bins 2047-2t and 2046-2t; an
+// inclusive scan of the pair sums gives every thread the count above its pair, so exactly one thread sees the crossing.
+__global__ void __launch_bounds__(kBins / 2) topk_find_kernel(const uint32_t* __restrict__ hist, int pass, SelectState* st,
+                                                              long long k) {
+    __shared__ uint32_t warp_tot[kBins / 2 / 32];
+    const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
+    const uint32_t krem = pass == 0 ? (uint32_t)k : st->krem;
+    const uint32_t prefix = pass == 0 ? 0u : st->prefix;
+    const uint32_t hi = hist[kBins - 1 - 2 * t], lo = hist[kBins - 2 - 2 * t];
+    uint32_t s = hi + lo;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, s, o);
+        if (lane >= o) s += v;
+    }
+    if (lane == 31) warp_tot[wid] = s;
+    __syncthreads();
+    uint32_t base = 0;
+    for (int w = 0; w < wid; ++w) base += warp_tot[w];
+    const uint32_t incl = base + s, above = incl - (hi + lo);
+    __syncthreads();                 // every thread has read krem / prefix before the winner rewrites them
+    const int bits = pass == 2 ? 9 : 11;
+    if (above < krem && above + hi >= krem) {
+        st->prefix = (prefix << bits) | (uint32_t)(kBins - 1 - 2 * t);
+        st->krem = krem - above;
+    } else if (above + hi < krem && incl >= krem) {
+        st->prefix = (prefix << bits) | (uint32_t)(kBins - 2 - 2 * t);
+        st->krem = krem - above - hi;
+    }
+}
+
+// M = {c < n_vote : a[c] >= max(tau, 1)} as bit words (bit c % 32 of word c / 32), |M| into *count, and w_prev <- w_g.  Each thread
+// takes one float4 (4 mask bits); the 8 lanes that share a word OR their nibbles together.
+__global__ void __launch_bounds__(256) neurotoxin_mask_kernel(const float* __restrict__ wg, float* __restrict__ wp, long long n4,
+                                                              const SelectState* __restrict__ st, uint32_t* __restrict__ mask,
+                                                              unsigned long long* __restrict__ count) {
+    __shared__ unsigned long long scratch[32];
+    const uint32_t tau = max(st->prefix, 1u);
+    unsigned long long pop = 0;
+    // the loop bound keeps whole warps together, so the shuffles below always see all 32 lanes
+    const long long step = (long long)gridDim.x * blockDim.x;
+    const long long n4w = (n4 + 31) / 32 * 32;
+    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n4w; q += step) {
+        uint32_t nib = 0;
+        if (q < n4) {
+            const float4 g = ld_f4(wg + 4 * q), p = ld_f4(wp + 4 * q);
+            nib = (key_of(g.x, p.x) >= tau ? 1u : 0u) | (key_of(g.y, p.y) >= tau ? 2u : 0u) | (key_of(g.z, p.z) >= tau ? 4u : 0u) |
+                  (key_of(g.w, p.w) >= tau ? 8u : 0u);
+            st_f4(wp + 4 * q, g);
+        }
+        uint32_t word = nib << ((q & 7) * 4);
+        word |= __shfl_xor_sync(0xFFFFFFFFu, word, 1);
+        word |= __shfl_xor_sync(0xFFFFFFFFu, word, 2);
+        word |= __shfl_xor_sync(0xFFFFFFFFu, word, 4);
+        if ((q & 7) == 0 && q < n4) mask[q >> 3] = word;
+        pop += __popc(nib);
+    }
+    const unsigned long long tot = block_sum<unsigned long long>(pop, scratch);
+    if (threadIdx.x == 0 && tot) atomicAdd(count, tot);
+}
+
+// slot[c] = fp32(w_g[c] + gamma * fp32(slot[c] - w_g[c])) in fp64, rounded once per operation (no contraction into an FMA), so the
+// numpy statement matches bit for bit
+__global__ void __launch_bounds__(256) boost_update_kernel(float* __restrict__ slot, const float* __restrict__ wg, long long n4,
+                                                           double gamma) {
+    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n4; q += (long long)gridDim.x * blockDim.x) {
+        const float4 s = ld_f4(slot + 4 * q), g = ld_f4(wg + 4 * q);
+        float4 o;
+        o.x = __double2float_rn(__dadd_rn((double)g.x, __dmul_rn(gamma, (double)(s.x - g.x))));
+        o.y = __double2float_rn(__dadd_rn((double)g.y, __dmul_rn(gamma, (double)(s.y - g.y))));
+        o.z = __double2float_rn(__dadd_rn((double)g.z, __dmul_rn(gamma, (double)(s.z - g.z))));
+        o.w = __double2float_rn(__dadd_rn((double)g.w, __dmul_rn(gamma, (double)(s.w - g.w))));
+        st_f4(slot + 4 * q, o);
+    }
+}
+
+inline int sweep_grid(long long n4, int threads, int num_sms, int per_sm) {
+    const long long want = (n4 + threads - 1) / threads, cap = (long long)num_sms * per_sm;
+    return (int)(want < 1 ? 1 : (want > cap ? cap : want));
+}
+
+}  // namespace
+
+cudaError_t launch_neurotoxin_mask(const float* w_g, float* w_prev, long long n_vote, long long k, uint32_t* mask, long long* count,
+                                   int num_sms, cudaStream_t st) {
+    if ((n_vote & 3) || k < 0 || k > n_vote || n_vote >= (1LL << 32)) return cudaErrorInvalidValue;
+    const long long n4 = n_vote / 4, words = (n_vote + 31) / 32;
+    RLR_CUDA_CHECK(cudaMemsetAsync(count, 0, sizeof(long long), st));
+    if (n_vote == 0) return cudaSuccess;
+    if (k == 0) {                    // empty mask: clear it and refresh w_prev
+        RLR_CUDA_CHECK(cudaMemsetAsync(mask, 0, (size_t)words * sizeof(uint32_t), st));
+        return cudaMemcpyAsync(w_prev, w_g, (size_t)n_vote * sizeof(float), cudaMemcpyDeviceToDevice, st);
+    }
+    // three histograms and the select state, zeroed together
+    const size_t bytes = 3 * kBins * sizeof(uint32_t) + sizeof(SelectState);
+    Scratch scr(bytes, st);
+    uint32_t* hist = scr.as<uint32_t>();
+    SelectState* sel = reinterpret_cast<SelectState*>(hist + 3 * kBins);
+    RLR_CUDA_CHECK(cudaMemsetAsync(hist, 0, bytes, st));
+    const int grid = sweep_grid(n4, kHistThreads, num_sms, 4);
+    for (int pass = 0; pass < 3; ++pass) {
+        topk_hist_kernel<<<grid, kHistThreads, 0, st>>>(w_g, w_prev, n4, pass, sel, hist + pass * kBins);
+        RLR_CUDA_CHECK(cudaGetLastError());
+        topk_find_kernel<<<1, kBins / 2, 0, st>>>(hist + pass * kBins, pass, sel, k);
+        RLR_CUDA_CHECK(cudaGetLastError());
+    }
+    neurotoxin_mask_kernel<<<sweep_grid(n4, 256, num_sms, 8), 256, 0, st>>>(w_g, w_prev, n4, sel, mask,
+                                                                              reinterpret_cast<unsigned long long*>(count));
+    return cudaGetLastError();
+}
+
+cudaError_t launch_boost_update(float* slot, const float* w_g, long long n_vote, double gamma, int num_sms, cudaStream_t st) {
+    if (n_vote & 3) return cudaErrorInvalidValue;
+    if (n_vote == 0) return cudaSuccess;
+    boost_update_kernel<<<sweep_grid(n_vote / 4, 256, num_sms, 8), 256, 0, st>>>(slot, w_g, n_vote / 4, gamma);
+    return cudaGetLastError();
+}
+
+}  // namespace rlr

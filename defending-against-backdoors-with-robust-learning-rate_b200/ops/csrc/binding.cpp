@@ -291,16 +291,25 @@ void round_init(at::Tensor w_global, c10::optional<at::Tensor> w_local, c10::opt
                                  ptr_or_null<float>(mom), w_global.numel(), cur_stream()), "round_init");
 }
 
-void sqnorm(at::Tensor x, at::Tensor out) {
+// a gradient mask: int32 bit words covering at least n coordinates
+inline const uint32_t* mask_ptr(const c10::optional<at::Tensor>& mask, int64_t n) {
+    if (!(mask.has_value() && mask->defined())) return nullptr;
+    CHECK_CUDA(*mask);
+    TORCH_CHECK(mask->scalar_type() == at::kInt && mask->numel() * 32 >= n, "mask: int32 bit words covering ", n, " coordinates");
+    return reinterpret_cast<const uint32_t*>(mask->data_ptr());
+}
+
+void sqnorm(at::Tensor x, at::Tensor out, c10::optional<at::Tensor> mask, int64_t n_mask) {
     CHECK_CUDA(x); CHECK_CUDA(out);
     TORCH_CHECK(x.scalar_type() == at::kFloat && out.scalar_type() == at::kDouble);
     c10::cuda::CUDAGuard guard(x.device());
-    check(rlr::launch_sqnorm(x.data_ptr<float>(), x.numel(), out.data_ptr<double>(), num_sms(), cur_stream()), "sqnorm");
+    check(rlr::launch_sqnorm(x.data_ptr<float>(), x.numel(), out.data_ptr<double>(), num_sms(), cur_stream(), mask_ptr(mask, n_mask),
+                             n_mask), "sqnorm");
 }
 
 void sgd_step(at::Tensor w, at::Tensor g, at::Tensor m, c10::optional<at::Tensor> w0, c10::optional<at::Tensor> w_bf16,
               double lr, double momentum, double max_grad_norm, c10::optional<at::Tensor> g_sqnorm,
-              c10::optional<at::Tensor> d_sqnorm, int64_t n_pgd, c10::optional<at::Tensor> w_in) {
+              c10::optional<at::Tensor> d_sqnorm, int64_t n_pgd, c10::optional<at::Tensor> w_in, c10::optional<at::Tensor> mask) {
     CHECK_CUDA(w); CHECK_CUDA(g); CHECK_CUDA(m);
     TORCH_CHECK(w.numel() == g.numel() && w.numel() == m.numel());
     TORCH_CHECK(!(d_sqnorm.has_value() && d_sqnorm->defined()) || (w0.has_value() && w0->defined()), "PGD needs w0");
@@ -308,14 +317,37 @@ void sgd_step(at::Tensor w, at::Tensor g, at::Tensor m, c10::optional<at::Tensor
     check(rlr::launch_sgd_step(w.data_ptr<float>(), g.data_ptr<float>(), m.data_ptr<float>(), ptr_or_null<const float>(w0),
                                ptr_or_null<__nv_bfloat16>(w_bf16), w.numel(), (float)lr, (float)momentum,
                                (float)max_grad_norm, ptr_or_null<const double>(g_sqnorm), ptr_or_null<double>(d_sqnorm),
-                               num_sms(), cur_stream(), n_pgd, ptr_or_null<const float>(w_in)), "sgd_step");
+                               num_sms(), cur_stream(), n_pgd, ptr_or_null<const float>(w_in),
+                               mask_ptr(mask, n_pgd > 0 && n_pgd <= w.numel() ? n_pgd : w.numel())), "sgd_step");
 }
 
-void pgd_project(at::Tensor w, at::Tensor w0, c10::optional<at::Tensor> w_bf16, double clip, at::Tensor d_sqnorm, int64_t n_pgd) {
+void pgd_project(at::Tensor w, at::Tensor w0, c10::optional<at::Tensor> w_bf16, double clip, at::Tensor d_sqnorm, int64_t n_pgd,
+                 c10::optional<at::Tensor> mask) {
     CHECK_CUDA(w); CHECK_CUDA(w0); CHECK_CUDA(d_sqnorm);
     c10::cuda::CUDAGuard guard(w.device());
     check(rlr::launch_pgd_project(w.data_ptr<float>(), w0.data_ptr<float>(), ptr_or_null<__nv_bfloat16>(w_bf16), w.numel(),
-                                  (float)clip, d_sqnorm.data_ptr<double>(), num_sms(), cur_stream(), n_pgd), "pgd_project");
+                                  (float)clip, d_sqnorm.data_ptr<double>(), num_sms(), cur_stream(), n_pgd,
+                                  mask_ptr(mask, n_pgd > 0 && n_pgd <= w.numel() ? n_pgd : w.numel())), "pgd_project");
+}
+
+void neurotoxin_mask(at::Tensor w_g, at::Tensor w_prev, int64_t n_vote, int64_t k, at::Tensor mask, at::Tensor count) {
+    CHECK_CUDA(w_g); CHECK_CUDA(w_prev); CHECK_CUDA(mask); CHECK_CUDA(count);
+    TORCH_CHECK(w_g.scalar_type() == at::kFloat && w_prev.scalar_type() == at::kFloat && count.scalar_type() == at::kLong &&
+                count.numel() >= 1);
+    TORCH_CHECK(w_g.numel() >= n_vote && w_prev.numel() >= n_vote, "neurotoxin_mask: w_g / w_prev shorter than n_vote");
+    mask_ptr(mask, n_vote);
+    c10::cuda::CUDAGuard guard(w_g.device());
+    check(rlr::launch_neurotoxin_mask(w_g.data_ptr<float>(), w_prev.data_ptr<float>(), n_vote, k,
+                                      reinterpret_cast<uint32_t*>(mask.data_ptr()), reinterpret_cast<long long*>(count.data_ptr()), num_sms(), cur_stream()),
+          "neurotoxin_mask");
+}
+
+void boost_update(at::Tensor slot, at::Tensor w_g, double gamma, int64_t n_vote) {
+    CHECK_CUDA(slot); CHECK_CUDA(w_g);
+    TORCH_CHECK(slot.scalar_type() == at::kFloat && w_g.scalar_type() == at::kFloat);
+    TORCH_CHECK(slot.numel() >= n_vote && w_g.numel() >= n_vote, "boost_update: slot / w_g shorter than n_vote");
+    c10::cuda::CUDAGuard guard(slot.device());
+    check(rlr::launch_boost_update(slot.data_ptr<float>(), w_g.data_ptr<float>(), n_vote, gamma, num_sms(), cur_stream()), "boost_update");
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -398,11 +430,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("pad_rows", &pad_rows);
     m.def("unpad_add", &unpad_add);
     m.def("round_init", &round_init);
-    m.def("sqnorm", &sqnorm);
+    m.def("sqnorm", &sqnorm, py::arg("x"), py::arg("out"), py::arg("mask") = py::none(), py::arg("n_mask") = 0);
     m.def("sgd_step", &sgd_step, py::arg("w"), py::arg("g"), py::arg("m"), py::arg("w0"), py::arg("w_bf16"), py::arg("lr"),
-          py::arg("momentum"), py::arg("max_grad_norm"), py::arg("g_sqnorm"), py::arg("d_sqnorm"), py::arg("n_pgd") = 0, py::arg("w_in") = py::none());
+          py::arg("momentum"), py::arg("max_grad_norm"), py::arg("g_sqnorm"), py::arg("d_sqnorm"), py::arg("n_pgd") = 0, py::arg("w_in") = py::none(),
+          py::arg("mask") = py::none());
+    m.def("neurotoxin_mask", &neurotoxin_mask);
+    m.def("boost_update", &boost_update);
     m.def("pgd_project", &pgd_project, py::arg("w"), py::arg("w0"), py::arg("w_bf16"), py::arg("clip"), py::arg("d_sqnorm"),
-          py::arg("n_pgd") = 0);
+          py::arg("n_pgd") = 0, py::arg("mask") = py::none());
     m.def("softmax_xent", &softmax_xent);
     m.def("eval_metrics", &eval_metrics);
     m.def("ipc_alloc", &ipc_alloc);

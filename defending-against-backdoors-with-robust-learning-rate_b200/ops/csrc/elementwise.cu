@@ -353,32 +353,55 @@ cudaError_t launch_round_init(const float* w_global, float* w_local, __nv_bfloat
 // ------------------------------------------------------------------------------------------------------------
 // fused clip_grad_norm_(.,max) + SGD(momentum) [+ ||w-w0||^2 for PGD] over flat buffers   (src/agent.py:50-60)
 // ------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) sqnorm_kernel(const float* __restrict__ x, long long n4, double* part /*[gridDim.x]*/) {
+// MASK: a gradient mask of bit words over [0, 4 * n4_mask) (bit c % 32 of word c / 32 set = coordinate c reads as zero); the thread of
+// float4 q takes the nibble (q % 8) of word q / 8.  The <false> instantiations compile to the same instructions as the unmasked kernels.
+__device__ __forceinline__ float4 apply_mask(float4 v, const uint32_t* __restrict__ mask, long long q, long long n4_mask) {
+    if (q < n4_mask) {
+        const uint32_t nib = (__ldg(mask + (q >> 3)) >> ((q & 7) * 4)) & 0xFu;
+        if (nib) {
+            if (nib & 1u) v.x = 0.f;
+            if (nib & 2u) v.y = 0.f;
+            if (nib & 4u) v.z = 0.f;
+            if (nib & 8u) v.w = 0.f;
+        }
+    }
+    return v;
+}
+
+template <bool MASK>
+__global__ void __launch_bounds__(256) sqnorm_kernel(const float* __restrict__ x, long long n4, double* part /*[gridDim.x]*/,
+                                                     const uint32_t* __restrict__ mask, long long n4_mask) {
     __shared__ double scratch[32];
     double acc = 0.0;
     for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n4; q += (long long)gridDim.x * blockDim.x) {
-        const float4 v = ld_f4(x + 4 * q);
+        float4 v = ld_f4(x + 4 * q);
+        if (MASK) v = apply_mask(v, mask, q, n4_mask);
         acc += (double)(v.x * v.x + v.y * v.y) + (double)(v.z * v.z + v.w * v.w);
     }
     const double tot = block_sum<double>(acc, scratch);
     if (threadIdx.x == 0) part[blockIdx.x] = tot;
 }
-cudaError_t launch_sqnorm(const float* x, long long n, double* out, int num_sms, cudaStream_t st) {
-    if (n & 3) return cudaErrorInvalidValue;
+cudaError_t launch_sqnorm(const float* x, long long n, double* out, int num_sms, cudaStream_t st, const uint32_t* mask,
+                          long long n_mask) {
+    if ((n & 3) || (mask && ((n_mask & 3) || n_mask < 0 || n_mask > n))) return cudaErrorInvalidValue;
     const int grid = grid_for(n / 4, 256, num_sms, 4);
     Scratch part((size_t)grid * sizeof(double), st);
-    sqnorm_kernel<<<grid, 256, 0, st>>>(x, n / 4, part.as<double>());
+    if (mask) sqnorm_kernel<true><<<grid, 256, 0, st>>>(x, n / 4, part.as<double>(), mask, n_mask / 4);
+    else sqnorm_kernel<false><<<grid, 256, 0, st>>>(x, n / 4, part.as<double>(), nullptr, 0);
     RLR_CUDA_CHECK(cudaGetLastError());
     RLR_CUDA_CHECK(launch_ordered_sum(out, part.as<double>(), grid, 1LL, st));
     return cudaGetLastError();
 }
 
+template <bool MASK>
 __global__ void __launch_bounds__(256) sgd_step_kernel(float* __restrict__ w, const float* __restrict__ g,
                                                          float* __restrict__ m, const float* __restrict__ w0,
                                                          __nv_bfloat16* __restrict__ wb, long long n4, float lr,
                                                          float momentum, float max_grad_norm,
                                                          const double* __restrict__ g_sqnorm, double* d_part /*[gridDim.x]*/,
-                                                         long long n4_pgd, const float* __restrict__ w_in, int first) {
+                                                         long long n4_pgd, const float* __restrict__ w_in, int first,
+                                                         const uint32_t* __restrict__ mask) {
+    // MASK: the gradient mask covers [0, n4_pgd) (the model parameters)
     // first = 1: first local step of a round, fused with the round hand-off -- parameters are read from the broadcast buffer w_in
     // (= the round's global parameters) and the momentum is taken as zero (fresh optimizer every round, src/agent.py:37-38), so no
     // separate "w <- w_global, m <- 0" pass exists.  Coordinates >= n4_pgd (BatchNorm running statistics, already updated in w by
@@ -392,8 +415,9 @@ __global__ void __launch_bounds__(256) sgd_step_kernel(float* __restrict__ w, co
     double dacc = 0.0;
     for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n4; q += (long long)gridDim.x * blockDim.x) {
         if (first && q >= n4_pgd) { st_f4(m + 4 * q, make_float4(0.f, 0.f, 0.f, 0.f)); continue; }
-        const float4 gv = ld_f4(g + 4 * q), mv = first ? make_float4(0.f, 0.f, 0.f, 0.f) : ld_f4(m + 4 * q),
-                     wv = ld_f4((first ? w_in : w) + 4 * q);
+        float4 gv = ld_f4(g + 4 * q);
+        if (MASK) gv = apply_mask(gv, mask, q, n4_pgd);
+        const float4 mv = first ? make_float4(0.f, 0.f, 0.f, 0.f) : ld_f4(m + 4 * q), wv = ld_f4((first ? w_in : w) + 4 * q);
         float4 mn, wn;
         mn.x = momentum * mv.x + coef * gv.x; mn.y = momentum * mv.y + coef * gv.y;
         mn.z = momentum * mv.z + coef * gv.z; mn.w = momentum * mv.w + coef * gv.w;
@@ -419,13 +443,17 @@ __global__ void __launch_bounds__(256) sgd_step_kernel(float* __restrict__ w, co
 }
 cudaError_t launch_sgd_step(float* w, const float* g, float* m, const float* w0, __nv_bfloat16* w_bf16, long long n,
                             float lr, float momentum, float max_grad_norm, const double* g_sqnorm, double* d_sqnorm,
-                            int num_sms, cudaStream_t st, long long n_pgd, const float* w_in) {
+                            int num_sms, cudaStream_t st, long long n_pgd, const float* w_in, const uint32_t* mask) {
     if ((n & 3) || (n_pgd & 3)) return cudaErrorInvalidValue;
     if (n_pgd <= 0 || n_pgd > n) n_pgd = n;
     const int grid = grid_for(n / 4, 256, num_sms, 4);
     auto step = [&](double* dp) {
-        sgd_step_kernel<<<grid, 256, 0, st>>>(w, g, m, w0, w_bf16, n / 4, lr, momentum, max_grad_norm, g_sqnorm, dp, n_pgd / 4,
-                                              w_in, w_in ? 1 : 0);
+        if (mask)
+            sgd_step_kernel<true><<<grid, 256, 0, st>>>(w, g, m, w0, w_bf16, n / 4, lr, momentum, max_grad_norm, g_sqnorm, dp,
+                                                        n_pgd / 4, w_in, w_in ? 1 : 0, mask);
+        else
+            sgd_step_kernel<false><<<grid, 256, 0, st>>>(w, g, m, w0, w_bf16, n / 4, lr, momentum, max_grad_norm, g_sqnorm, dp,
+                                                         n_pgd / 4, w_in, w_in ? 1 : 0, nullptr);
         return cudaGetLastError();
     };
     if (!d_sqnorm) return step(nullptr);
@@ -438,27 +466,42 @@ cudaError_t launch_sgd_step(float* w, const float* g, float* m, const float* w0,
 }
 
 // PGD: w <- w0 + (w - w0) / max(1, ||w - w0|| / clip)   (src/agent.py:54-60), no host sync for the norm
+// MASK: masked coordinates (never moved from w0 by a masked step) keep their bits, -0 included
+template <bool MASK>
 __global__ void __launch_bounds__(256) pgd_project_kernel(float* __restrict__ w, const float* __restrict__ w0,
                                                             __nv_bfloat16* __restrict__ wb, long long n4, float clip,
-                                                            const double* __restrict__ d_sqnorm, long long n4_pgd) {
+                                                            const double* __restrict__ d_sqnorm, long long n4_pgd,
+                                                            const uint32_t* __restrict__ mask) {
     const float denom = fmaxf(1.0f, (float)sqrt(*d_sqnorm) / clip);
     const float inv = 1.0f / denom;
     for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n4; q += (long long)gridDim.x * blockDim.x) {
         float4 wv = ld_f4(w + 4 * q);
         if (denom > 1.0f && q < n4_pgd) {
             const float4 o = ld_f4(w0 + 4 * q);
-            wv.x = o.x + (wv.x - o.x) * inv; wv.y = o.y + (wv.y - o.y) * inv;
-            wv.z = o.z + (wv.z - o.z) * inv; wv.w = o.w + (wv.w - o.w) * inv;
+            float4 pv;
+            pv.x = o.x + (wv.x - o.x) * inv; pv.y = o.y + (wv.y - o.y) * inv;
+            pv.z = o.z + (wv.z - o.z) * inv; pv.w = o.w + (wv.w - o.w) * inv;
+            if (MASK) {
+                const uint32_t nib = (__ldg(mask + (q >> 3)) >> ((q & 7) * 4)) & 0xFu;
+                if (!(nib & 1u)) wv.x = pv.x;
+                if (!(nib & 2u)) wv.y = pv.y;
+                if (!(nib & 4u)) wv.z = pv.z;
+                if (!(nib & 8u)) wv.w = pv.w;
+            } else {
+                wv = pv;
+            }
             st_f4(w + 4 * q, wv);
         }
         if (wb) *reinterpret_cast<uint2*>(wb + 4 * q) = make_uint2(pack_bf16x2(wv.x, wv.y), pack_bf16x2(wv.z, wv.w));
     }
 }
 cudaError_t launch_pgd_project(float* w, const float* w0, __nv_bfloat16* w_bf16, long long n, float clip,
-                               const double* d_sqnorm, int num_sms, cudaStream_t st, long long n_pgd) {
+                               const double* d_sqnorm, int num_sms, cudaStream_t st, long long n_pgd, const uint32_t* mask) {
     if ((n & 3) || (n_pgd & 3)) return cudaErrorInvalidValue;
     if (n_pgd <= 0 || n_pgd > n) n_pgd = n;
-    pgd_project_kernel<<<grid_for(n / 4, 256, num_sms, 4), 256, 0, st>>>(w, w0, w_bf16, n / 4, clip, d_sqnorm, n_pgd / 4);
+    const int grid = grid_for(n / 4, 256, num_sms, 4);
+    if (mask) pgd_project_kernel<true><<<grid, 256, 0, st>>>(w, w0, w_bf16, n / 4, clip, d_sqnorm, n_pgd / 4, mask);
+    else pgd_project_kernel<false><<<grid, 256, 0, st>>>(w, w0, w_bf16, n / 4, clip, d_sqnorm, n_pgd / 4, nullptr);
     return cudaGetLastError();
 }
 

@@ -117,13 +117,27 @@ cudaError_t launch_unpad_add(const float* src, float* dst, long long R, int K, i
 // ---- optimiser over flat buffers -------------------------------------------------------------------------
 cudaError_t launch_round_init(const float* w_global, float* w_local, __nv_bfloat16* w_bf16, float* mom, long long n,
                               cudaStream_t st);
-cudaError_t launch_sqnorm(const float* x, long long n, double* out /*accumulates*/, int num_sms, cudaStream_t st);
+// mask (optional): gradient mask bit words (bit c % 32 of word c / 32 set = g[c] reads as zero) over [0, n_mask) for sqnorm and over
+// [0, n_pgd) for sgd_step; pgd_project leaves masked coordinates untouched
+cudaError_t launch_sqnorm(const float* x, long long n, double* out /*accumulates*/, int num_sms, cudaStream_t st,
+                          const uint32_t* mask = nullptr, long long n_mask = 0);
 cudaError_t launch_sgd_step(float* w, const float* g, float* m, const float* w0, __nv_bfloat16* w_bf16, long long n,
                             float lr, float momentum, float max_grad_norm, const double* g_sqnorm, double* d_sqnorm,
                             int num_sms, cudaStream_t st, long long n_pgd = 0 /*PGD norm over [0, n_pgd); 0 = n*/,
-                            const float* w_in = nullptr /*first step of a round: read params from w_in, momentum = 0, keep w[n_pgd:]*/);
+                            const float* w_in = nullptr /*first step of a round: read params from w_in, momentum = 0, keep w[n_pgd:]*/,
+                            const uint32_t* mask = nullptr);
 cudaError_t launch_pgd_project(float* w, const float* w0, __nv_bfloat16* w_bf16, long long n, float clip,
-                               const double* d_sqnorm, int num_sms, cudaStream_t st, long long n_pgd = 0);
+                               const double* d_sqnorm, int num_sms, cudaStream_t st, long long n_pgd = 0, const uint32_t* mask = nullptr);
+
+// ---- model-poisoning attackers (attack.cu) ----------------------------------------------------------------------------------------
+// Neurotoxin: a[c] = bits(|fp32(w_g[c] - w_prev[c])|) over [0, n_vote); tau = the k-th largest a (with multiplicity) by an on-device
+// radix select; mask = {c : a[c] >= tau, a[c] > 0} as ceil(n_vote/32) bit words; *count = |mask|; then w_prev <- w_g[:n_vote].
+// k = 0: empty mask.  No host sync, no float atomics: bitwise reproducible.  n_vote % 4 == 0, 0 <= k <= n_vote < 2^32.
+cudaError_t launch_neurotoxin_mask(const float* w_g, float* w_prev, long long n_vote, long long k, uint32_t* mask, long long* count,
+                                   int num_sms, cudaStream_t st);
+// boosted update: slot[c] = fp32((double)w_g[c] + gamma * (double)fp32(slot[c] - w_g[c])) over [0, n_vote), each fp64 operation
+// rounded on its own
+cudaError_t launch_boost_update(float* slot, const float* w_g, long long n_vote, double gamma, int num_sms, cudaStream_t st);
 
 // ---- loss / evaluation -----------------------------------------------------------------------------------
 // logits [B,C] (kind 0 fp32 / 1 bf16); writes dlogits (same kind, scaled by 1/B) and accumulates loss_sum / correct.

@@ -127,6 +127,13 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--flame_lambda", type=float, default=None,
                    help=f"--aggr flame: noise factor lambda >= 0; the round's Gaussian noise has std lambda * S, S the median update norm "
                         f"the admitted updates are clipped to (default {FLAME_LAMBDA})")
+    p.add_argument("--attack_boost", type=float, default=1.0,
+                   help="model replacement (Bhagoji et al. 2019, Bagdasaryan et al. 2020): every corrupt agent scales its update by this "
+                        "factor gamma > 0 before submitting it, after its --clip projection (1 = off; needs --num_corrupt > 0)")
+    p.add_argument("--attack_neurotoxin", type=float, default=0.0,
+                   help="Neurotoxin (Zhang et al. 2022): corrupt agents never update the top p fraction of coordinates by magnitude of "
+                        "the last global update; their gradient is zeroed there at every local step.  0 <= p < 1 (0 = off; needs "
+                        "--num_corrupt > 0)")
     return p
 
 
@@ -158,7 +165,22 @@ def finalize_args(args: argparse.Namespace) -> argparse.Namespace:
     _finalize_fltrust(args)
     _finalize_rfa(args)
     _finalize_flame(args)
+    _finalize_attack(args)
     return args
+
+
+def _finalize_attack(args) -> None:
+    """Validate the model-poisoning attack flags in place: ``attack_boost`` finite and > 0, ``attack_neurotoxin`` finite in [0, 1), and
+    either attack, when active, only with corrupt agents to run it."""
+    gamma = float(getattr(args, "attack_boost", 1.0))
+    p = float(getattr(args, "attack_neurotoxin", 0.0))
+    if not (math.isfinite(gamma) and gamma > 0):
+        raise ValueError(f"--attack_boost {gamma} must be a finite number > 0")
+    if not (math.isfinite(p) and 0.0 <= p < 1.0):
+        raise ValueError(f"--attack_neurotoxin {p} must be a finite number in [0, 1)")
+    if (gamma != 1.0 or p > 0) and args.num_corrupt <= 0:
+        raise ValueError("--attack_boost / --attack_neurotoxin need corrupt agents (--num_corrupt > 0)")
+    args.attack_boost, args.attack_neurotoxin = gamma, p
 
 
 def _finalize_flame(args) -> None:
@@ -291,4 +313,6 @@ def print_exp_details(args) -> None:
         print(f"    RFA passes / nu: {args.rfa_iters} / {args.rfa_nu}")
     if args.aggr == "flame":
         print(f"    FLAME lambda: {args.flame_lambda}")
+    if getattr(args, "attack_boost", 1.0) != 1.0 or getattr(args, "attack_neurotoxin", 0.0) > 0:
+        print(f"    Attack (boost / neurotoxin): {args.attack_boost} / {args.attack_neurotoxin}")
     print("======================================")

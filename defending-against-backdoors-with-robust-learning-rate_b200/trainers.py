@@ -42,6 +42,9 @@ class TorchTrainer:
         self.max_shard = max_shard
         self._graphs = {}
         self._w0 = None
+        # Neurotoxin: the round's gradient mask (int32 bit words, engine-owned and rewritten in place), applied to corrupt agents only
+        self.attack_mask = None
+        self._grad_mask = None
         # training augmentation (--crop_pad / --hflip): the Philox stream word of the current epoch, set before the graphs replay
         self.aug_stream = torch.zeros(1, dtype=torch.int64, device=device)
         self.aug = ops.training_augment(args, self.aug_stream)
@@ -58,7 +61,7 @@ class TorchTrainer:
         logits = self.net(x)
         loss = F.cross_entropy(logits, y)
         loss.backward()
-        self.opt.step(self.w, self.g, self.m, w0=w0)
+        self.opt.step(self.w, self.g, self.m, w0=w0, grad_mask=self._grad_mask)
         self.loss_sum += loss.detach()
 
     def _graph_body(self, dataset, B, w0):
@@ -69,7 +72,7 @@ class TorchTrainer:
         self._step(self.x[:B], self.y[:B], w0)
 
     def _get_graph(self, dataset, B, w0):
-        key = (B, dataset.data.data_ptr(), w0.data_ptr())
+        key = (B, dataset.data.data_ptr(), w0.data_ptr(), 0 if self._grad_mask is None else self._grad_mask.data_ptr())
         if key in self._graphs:
             return self._graphs[key]
         meta = dataset.meta
@@ -100,6 +103,7 @@ class TorchTrainer:
         self.net.train()
         self.loss_sum.zero_()
         steps = 0
+        self._grad_mask = self.attack_mask if getattr(agent, "is_corrupt", False) else None
         graphs = self.use_graphs and n <= self.max_shard
         if graphs:  # capture (first call only) BEFORE the round state is set up: capture warm-up scribbles on w/m
             full = self._get_graph(dataset, bs, w_global) if n >= bs else None

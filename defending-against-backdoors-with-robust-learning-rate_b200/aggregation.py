@@ -8,7 +8,9 @@ With ``--select krum | multikrum`` a selection stage runs first: the participant
 ``--aggr fltrust`` and ``--aggr rfa`` are the same weighted-mean launch with weights from a per-participant pass: FLTrust's trust
 scores (``ops.trust_stats``) or RFA's smoothed Weiszfeld weights (``ops.rfa`` over ``ops.rfa_sqdist`` passes).  ``--aggr flame`` is
 that launch too: the Gram matrix of the updates (``ops.pairwise_gram``) gives FLAME's cosine clustering, median-norm clip scales and
-noise (``ops.flame_admit``), and the admitted participants' clipped updates are averaged with equal weights.
+noise (``ops.flame_admit``), and the admitted participants' clipped updates are averaged with equal weights.  ``--aggr foolsgold`` keeps
+every agent's summed updates across rounds (``ops.history_accumulate``) and weights the mean by FoolsGold's ``ops.foolsgold_weights`` on
+the Gram matrix of those histories (``ops.history_gram``), so agents that keep pushing the model the same way lose their weight.
 The reference's dead / disabled pieces are available behind flags: ``clip_updates`` (``--server_clip``) and the
 diagnostics ``plot_norms`` / ``comp_diag_fisher`` / ``plot_sign_agreement`` (``--diagnostics``), the latter with the
 reference's latent bugs fixed (model built on the right device; Fisher uses log-probabilities -- SURVEY.md quirk 7).
@@ -46,6 +48,8 @@ class Aggregation:
         self.last_trust = None        # the Trust/* scalars of the last round (--aggr fltrust)
         self.last_rfa = None          # the RFA/* scalars of the last round (--aggr rfa)
         self.last_flame = None        # the FLAME/* scalars of the last round (--aggr flame)
+        self.last_foolsgold = None    # the FoolsGold/* scalars of the last round (--aggr foolsgold)
+        self.history = None           # [num_agents][n_vote] FoolsGold histories of the in-process form (allocated on first use)
         self.opt = None               # full-length server optimizer state of the in-process form (allocated on first use)
 
     # ---- the server step ------------------------------------------------------------------------------------
@@ -67,6 +71,7 @@ class Aggregation:
         gram = lambda members: ops.pairwise_gram([ws[j] for j in members], w_global, nv)
         keep, weights, scales, total, noise_std = self._admission(ids, clip, distances,
                                                                   lambda: ops.trust_stats(ws, root_params, w_global, nv), rfa_pass, gram,
+                                                                  lambda members: self._history_pass(w_global, ws, ids, members, nv),
                                                                   cur_round)
         if keep is not None and len(keep) < len(ids):
             ids, ws, weights = [ids[j] for j in keep], [ws[j] for j in keep], [weights[j] for j in keep]
@@ -93,14 +98,15 @@ class Aggregation:
         norms = self.fused.update_norms(K) if self._server_clip or diag else None
         clip = self._clip_scales(norms) if self._server_clip else None
         copies, gathered = None, None
-        if (self._select or self._fltrust or self._flame or (self._rfa and self.args.rfa_iters > 0)) and self.fused.gathers(K):
+        if (self._select or self._fltrust or self._flame or self._foolsgold or (self._rfa and self.args.rfa_iters > 0)) and self.fused.gathers(K):
             # on the gather transport every pass reads the same all-gathered copies (one all_gather per round; the root job included)
             gathered = self.fused.gather_participants(K + 1 if self._fltrust else K)
             copies = gathered[:K]
         keep, weights, scales, total, noise_std = self._admission(
             participants, clip, lambda: self.fused.pairwise_sqdist(K, clip, copies), lambda: self.fused.trust_stats(K, K, gathered),
             lambda b, members: self.fused.rfa_sqdist(K, b, clip, members, copies),
-            lambda members: self.fused.pairwise_gram(K, members, copies), cur_round)
+            lambda members: self.fused.pairwise_gram(K, members, copies),
+            lambda members: self.fused.foolsgold_gram(K, participants, members, copies), cur_round)
         if diag:   # the sign-agreement analysis needs the pre-step global parameters and every admitted participant's parameters
             prev = self.fused.w_global.clone()
             ws = [w.clone() for w in self.fused.gather_participants(K)]
@@ -122,10 +128,11 @@ class Aggregation:
     def _select(self):
         return getattr(self.args, "select", "none") != "none"
 
-    def _admission(self, ids, clip, distances, trust_stats, rfa_pass, gram, cur_round):
+    def _admission(self, ids, clip, distances, trust_stats, rfa_pass, gram, history, cur_round):
         """Admission of the participants ``ids`` shared by both forms of the step: Krum / Multi-Krum on ``distances()`` (``--select``),
-        then FLTrust on ``trust_stats()`` (``--aggr fltrust``), RFA's weights from ``rfa_pass(b, members)`` (``--aggr rfa``) or FLAME on
-        the Gram matrix ``gram(members)`` (``--aggr flame``).  ``clip``: the server-clipping scales or None.  Returns
+        then FLTrust on ``trust_stats()`` (``--aggr fltrust``), RFA's weights from ``rfa_pass(b, members)`` (``--aggr rfa``), FLAME on
+        the Gram matrix ``gram(members)`` (``--aggr flame``) or FoolsGold on ``history(members)``, the Gram matrix of the members' update
+        histories after this round's updates are folded in (``--aggr foolsgold``).  ``clip``: the server-clipping scales or None.  Returns
         ``(members, weights, scales, total_weight, noise_std)`` for the step: members None admits everyone; weights are per position in
         ``ids``."""
         keep = self._admit(distances(), ids, cur_round) if self._select else None
@@ -135,6 +142,9 @@ class Aggregation:
         if self._flame:
             return self._flame_step(ids, keep, gram, cur_round)
         weights = [float(self.agent_data_sizes[i]) for i in ids]
+        if self._foolsgold:
+            members, weights, total = self._foolsgold_step(ids, keep, weights, history, cur_round)
+            return members, weights, clip, total, noise_std
         if self._rfa:
             return (*self._rfa_weights(ids, keep, weights, clip, rfa_pass, cur_round), noise_std)
         return keep, weights, clip, None, noise_std
@@ -165,10 +175,54 @@ class Aggregation:
         return self.args.aggr == "flame"
 
     @property
+    def _foolsgold(self):
+        return self.args.aggr == "foolsgold"
+
+    @property
     def _mode(self):
         """The aggregate kernel's rule: FLTrust is its weighted mean with trust weights and per-participant scales, RFA with its
-        Weiszfeld weights, FLAME with equal weights and its clip scales."""
-        return "avg" if self._fltrust or self._rfa or self._flame else self.args.aggr
+        Weiszfeld weights, FLAME with equal weights and its clip scales, FoolsGold with its weights times the data sizes."""
+        return "avg" if self._fltrust or self._rfa or self._flame or self._foolsgold else self.args.aggr
+
+    def _history_pass(self, w_global, ws, ids, members, nv):
+        """In-process form of the FoolsGold history pass: fold the updates of the participants at positions ``members`` into the rows of
+        their agents in ``self.history`` (a full-length ``[num_agents][n_vote]`` table on ``w_global``'s device, zero at the start) and
+        return the Gram matrix of those rows."""
+        nv = w_global.numel() if nv is None else int(nv)
+        if self.history is None:
+            self.history = torch.zeros((self.args.num_agents, nv), dtype=torch.float32, device=w_global.device)
+        rows = [self.history[ids[j]] for j in members]
+        ops.history_accumulate(rows, [ws[j] for j in members], w_global, 0, nv)
+        return ops.history_gram(rows, nv)
+
+    def _foolsgold_step(self, ids, keep, weights, history, cur_round):
+        """FoolsGold over the positions ``keep`` that selection admitted (all when None): ``ops.foolsgold_weights`` on ``history(candidates)``.
+        Returns ``(members, weights, total_weight)`` for the step: the candidates with alpha > 0, weights alpha times the data sizes
+        ``weights`` and total weight their sum -- or, when every alpha is 0, every candidate with weight 0 and total weight 1, so the
+        aggregate is 0 plus noise.  A round in which every alpha is 1 is the avg step bit for bit.  Records ``last_admitted`` and logs the
+        mean alpha of honest (ids >= num_corrupt) and corrupt candidates and the admitted count."""
+        K = len(ids)
+        cand = list(range(K)) if keep is None else [int(j) for j in keep]
+        alpha = ops.foolsgold_weights(history(cand))
+        members = [j for j, a in zip(cand, alpha) if a > 0]
+        w = [0.0] * K
+        for j, a in zip(cand, alpha):
+            w[j] = float(a) * weights[j]
+        total = sum(w[j] for j in members)
+        self.last_admitted = [ids[j] for j in members]
+        if not members:
+            members, w, total = cand, [0.0] * K, 1.0
+        nc = self.args.num_corrupt
+        honest = [float(a) for j, a in zip(cand, alpha) if ids[j] >= nc]
+        corrupt = [float(a) for j, a in zip(cand, alpha) if ids[j] < nc]
+        self.last_foolsgold = {"FoolsGold/Avg_Honest_Weight": sum(honest) / len(honest) if honest else None,
+                               "FoolsGold/Avg_Corrupt_Weight": sum(corrupt) / len(corrupt) if corrupt else None,
+                               "FoolsGold/Admitted": len(self.last_admitted)}
+        if self.writer is not None:
+            for k, v in self.last_foolsgold.items():
+                if v is not None:
+                    self.writer.add_scalar(k, v, cur_round)
+        return members, w, total
 
     def _flame_step(self, ids, keep, gram, cur_round):
         """FLAME over the positions ``keep`` that selection admitted (all when None): ``ops.flame_admit`` on ``gram(candidates)``.

@@ -110,7 +110,7 @@ class FLEngine:
             backend = "gloo"
         self.fused = FusedAggregator(ctx, self.layout.n_total, self.layout.n_vote, max_slots, backend,
                                      transport=getattr(args, "agg_transport", "auto"), server_opt=server_opt_spec(args),
-                                     n_part=self.n_part)
+                                     n_part=self.n_part, history_agents=args.num_agents if args.aggr == "foolsgold" else 0)
         init = torch.zeros(self.layout.n_total, dtype=torch.float32)
         self.layout.init_(init, args.seed)
         self.fused.w_global.copy_(init.to(dev))
@@ -177,6 +177,11 @@ class FLEngine:
                     raise ValueError("checkpoint has no Neurotoxin state (w_prev), but this run uses --attack_neurotoxin")
                 self.w_prev.copy_(w_prev.to(dev))
                 self._have_prev = True
+            if self.fused.history is not None:
+                hist = ck["extra"].get("foolsgold_history")
+                if hist is None:
+                    raise ValueError("checkpoint has no FoolsGold history, but this run uses --aggr foolsgold")
+                self.fused.load_foolsgold_history(hist)
         ctx.barrier()
 
     def _jobs(self):
@@ -410,6 +415,10 @@ class FLEngine:
                 rec["flame_corrupt_admitted"] = self.aggregator.last_flame["FLAME/Corrupt_Admitted"]
                 rec["flame_clip_bound"] = self.aggregator.last_flame["FLAME/Clip_Bound"]
                 rec["flame_noise_std"] = self.aggregator.last_flame["FLAME/Noise_Std"]
+            if self.aggregator.last_foolsgold is not None:
+                rec["foolsgold_avg_honest"] = self.aggregator.last_foolsgold["FoolsGold/Avg_Honest_Weight"]
+                rec["foolsgold_avg_corrupt"] = self.aggregator.last_foolsgold["FoolsGold/Avg_Corrupt_Weight"]
+                rec["foolsgold_admitted"] = self.aggregator.last_foolsgold["FoolsGold/Admitted"]
             rec.update({f"ms_{k}": v for k, v in self.timer.elapsed().items()})
             if args.profile_phases and self.verbose:
                 print({k: round(v, 3) for k, v in rec.items() if k.startswith("ms_")})
@@ -417,11 +426,14 @@ class FLEngine:
             history.append({"round": rnd, **rec})
             if args.checkpoint and ((args.ckpt_every and rnd % args.ckpt_every == 0) or rnd == rounds):
                 state = self.fused.server_opt_state()      # every rank takes part: each holds one slice on the fused multi-GPU path
+                hist = self.fused.foolsgold_history() if self.fused.history is not None else None      # collective, likewise
                 if self.ctx.is_main:
                     so = None if state is None else {**self.fused.opt.hparams, "m": state[0], "v": state[1]}
                     extra = {"cum_poison_acc_mean": self.cum_poison_acc_mean}
                     if self.neurotoxin_k is not None:
                         extra["neurotoxin_w_prev"] = self.w_prev.cpu()
+                    if hist is not None:
+                        extra["foolsgold_history"] = hist
                     save_checkpoint(args.checkpoint, self.global_params(), rnd, args, self.layout, extra, so)
         if self.verbose:
             print("Training has finished!")

@@ -833,6 +833,99 @@ def flame_admit(G, ids, lam):
 
 
 # =====================================================================================================================
+# FoolsGold (Fung, Yoon, Beschastnikh, RAID 2020): per-agent update histories kept across rounds
+# =====================================================================================================================
+def history_statement(rows, w_agents, w_global, lo, hi):
+    """fp32 statement of the history update over coordinates ``[lo, hi)``: ``rows[k][c] + fp32(w_k[c] - w_global[c])``, each operation one
+    fp32 rounding.  ``rows[k]`` is candidate k's history row, indexed by absolute coordinate.  Returns the new ``[lo, hi)`` slices."""
+    g = w_global[lo:hi].float()
+    return [h[lo:hi].float() + (w[lo:hi].float() - g) for h, w in zip(rows, w_agents)]
+
+
+def history_accumulate(rows, w_agents, w_global, lo=0, hi=None):
+    """Fold each candidate's update ``w_k - w_global`` into its history row ``rows[k]`` in place over ``[lo, hi)`` (default
+    ``[0, len(rows[0]))``), bit for bit ``history_statement``.  On CUDA this launches ``history_accumulate_kernel``
+    (ops/csrc/foolsgold.cu) for any number of candidates; on CPU it evaluates the statement."""
+    hi = rows[0].numel() if hi is None else int(hi)
+    lo = int(lo)
+    if not rows[0].is_cuda:
+        for h, new in zip(rows, history_statement(rows, w_agents, w_global, lo, hi)):
+            h[lo:hi].copy_(new)
+        return
+    assert lo % 4 == 0 and hi % 4 == 0, "flat buffers are padded to multiples of 4"
+    for t in (*rows, *w_agents, w_global):
+        assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.numel() >= hi
+    dev = w_global.device
+    agents = PtrTable([w.data_ptr() for w in w_agents], dev, w_agents)
+    tab = PtrTable([h.data_ptr() for h in rows], dev, rows)
+    ext().history_accumulate(agents.tensor, tab.tensor, w_global.data_ptr(), lo, hi, None, None, 0, 1, 0)
+
+
+def history_gram_statement(rows, lo, hi):
+    """fp64 statement of the FoolsGold Gram pass over coordinates ``[lo, hi)``: ``G[i][j] = sum_c rows[i][c] rows[j][c]``."""
+    K = len(rows)
+    G = torch.zeros(K, K, dtype=torch.float64, device=rows[0].device)
+    step = max(4, (1 << 24) // max(1, K))                 # coordinates per pass: K * step fp64 values
+    for c in range(lo, hi, step):
+        e = min(hi, c + step)
+        x = torch.stack([h[c:e] for h in rows]).double()
+        G += x @ x.T
+    return G
+
+
+def history_gram(rows, n_vote=None):
+    """K x K float64 Gram matrix of the history rows over ``[0, n_vote)`` (``history_gram_statement``'s values).  On CUDA this launches
+    ``pairwise_sqdist_kernel<true, true>`` (ops/csrc/select.cu); on CPU, and for more rows than the kernel's tables hold (recorded as a
+    library fall-through), it evaluates ``history_gram_statement``."""
+    nv = rows[0].numel() if n_vote is None else int(n_vote)
+    K = len(rows)
+    return _participant_pass("history_gram", rows, (), nv, (K, K), lambda: history_gram_statement(rows, 0, nv),
+                             lambda tab, out: ext().history_gram(tab, 0, nv, out))
+
+
+def foolsgold_weights(G):
+    """FoolsGold's weights on the host, in fp64, shared by every form of the server step: the authors' released ``foolsgold()`` on the
+    cosines of the candidates' histories, with its divisions by zero defined.  ``G``: the Gram matrix of the history rows
+    (``history_gram_statement``'s layout).
+
+    ``cs_ij = G_ij / sqrt(G_ii G_jj)`` clamped to [-1, 1] for ``i != j`` (0 when a norm is 0 or the cosine is NaN; a candidate whose
+    ``G_kk`` is not finite has cosine 0 with everyone); ``v_i = max(0, max_{j != i} cs_ij)`` (0 for one candidate: the released code
+    subtracts the identity from the cosines, so its row maxima include a diagonal 0); pardoning ``cs_ij *= v_i / v_j`` where
+    ``v_i < v_j`` (so ``v_j > 0`` and the factor lies in [0, 1): a candidate anti-correlated with everyone has ``v_i = 0`` and its
+    cosines are not turned positive); ``wv_i = clip(1 - max_{j != i} cs_ij, 0, 1)``.  When ``max wv = 0``
+    every weight is 0; else ``wv /= max wv``, 1 becomes 0.99 and ``alpha_i = clip(ln(wv_i / (1 - wv_i)) + 0.5, 0, 1)`` (0 where
+    ``wv_i = 0``).  A candidate with a non-finite ``G_kk`` gets 0.  Returns float64 numpy ``[K]``."""
+    g = np.asarray(torch.as_tensor(G).detach().double().cpu().numpy(), dtype=np.float64)
+    K = g.shape[0]
+    if g.shape != (K, K):
+        raise ValueError(f"foolsgold_weights: a {g.shape} Gram matrix")
+    q = np.diag(g).copy()
+    ok = np.isfinite(q)
+    with np.errstate(all="ignore"):
+        nrm = np.sqrt(np.outer(q, q))
+        cs = np.where(nrm > 0, g / np.where(nrm > 0, nrm, 1.0), 0.0)
+    cs = np.clip(np.nan_to_num(cs, nan=0.0), -1.0, 1.0)              # NaN -> 0; clip sends +-inf to +-1
+    cs[~ok, :] = 0.0
+    cs[:, ~ok] = 0.0
+    off = ~np.eye(K, dtype=bool)
+    v = np.maximum(np.where(off, cs, -np.inf).max(axis=1), 0.0) if K > 1 else np.zeros(1)
+    vi, vj = v[:, None], v[None, :]
+    pardon = off & (vi < vj)                                           # v_i >= 0, so v_j > 0 here
+    cs = np.where(pardon, cs * vi / np.where(pardon, vj, 1.0), cs)
+    top = np.where(off, cs, -np.inf).max(axis=1) if K > 1 else np.zeros(1)
+    wv = np.clip(1.0 - top, 0.0, 1.0)
+    alpha = np.zeros(K, dtype=np.float64)
+    m = wv.max()
+    if m > 0:
+        wv = wv / m
+        wv[wv == 1.0] = 0.99
+        pos = wv > 0
+        alpha[pos] = np.clip(np.log(wv[pos] / (1.0 - wv[pos])) + 0.5, 0.0, 1.0)
+    alpha[~ok] = 0.0
+    return alpha
+
+
+# =====================================================================================================================
 # model-poisoning attackers (DESIGN.md section 3)
 # =====================================================================================================================
 def mask_words(n: int) -> int:

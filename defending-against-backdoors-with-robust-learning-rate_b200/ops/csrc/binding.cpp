@@ -134,6 +134,41 @@ void pairwise_gram(at::Tensor w_agent_ptrs, int64_t w_global_ptr, int64_t begin,
     check(rlr::launch_pairwise_gram(p, out.data_ptr<double>(), num_sms(), cur_stream()), "pairwise_gram");
 }
 
+// FoolsGold: fold each candidate's update w_k - w_global into its history row over coordinates [begin, end).  row_ptrs holds the
+// rows' addresses, offset so that absolute coordinates index them.  world > 1: the fused multi-GPU form, which first runs the
+// aggregation's barrier-in at `epoch`.
+void history_accumulate(at::Tensor w_agent_ptrs, at::Tensor row_ptrs, int64_t w_global_ptr, int64_t begin, int64_t end,
+                        c10::optional<at::Tensor> flag_ptrs, c10::optional<at::Tensor> local_sync, int64_t rank, int64_t world, int64_t epoch) {
+    CHECK_CUDA(w_agent_ptrs); CHECK_CUDA(row_ptrs);
+    TORCH_CHECK(w_agent_ptrs.scalar_type() == at::kLong && row_ptrs.scalar_type() == at::kLong, "pointer tables must be int64");
+    TORCH_CHECK(row_ptrs.numel() == w_agent_ptrs.numel(), "one history row per participant");
+    TORCH_CHECK(w_global_ptr, "history_accumulate needs w_global");
+    c10::cuda::CUDAGuard guard(w_agent_ptrs.device());
+    rlr::HistParams p{};
+    p.w_agents = reinterpret_cast<const float* const*>(w_agent_ptrs.data_ptr());
+    p.rows = reinterpret_cast<float* const*>(row_ptrs.data_ptr());
+    p.w_global = reinterpret_cast<const float*>(w_global_ptr);
+    p.begin = begin; p.end = end;
+    p.K = (int)w_agent_ptrs.numel();
+    p.gate = gate_of(flag_ptrs, local_sync, rank, world, epoch);
+    check(rlr::launch_history_accumulate(p, num_sms(), cur_stream()), "history_accumulate");
+}
+
+// FoolsGold: K x K fp64 Gram matrix of the history rows (row_ptrs, offset so that absolute coordinates index them) over [begin, end).
+void history_gram(at::Tensor row_ptrs, int64_t begin, int64_t end, at::Tensor out) {
+    CHECK_CUDA(row_ptrs); CHECK_CUDA(out);
+    TORCH_CHECK(row_ptrs.scalar_type() == at::kLong, "pointer table must be int64");
+    const int64_t K = row_ptrs.numel();
+    TORCH_CHECK(out.scalar_type() == at::kDouble && out.numel() == K * K, "out must be a float64 [K, K] tensor");
+    c10::cuda::CUDAGuard guard(out.device());
+    rlr::DistParams p{};
+    p.w_agents = reinterpret_cast<const float* const*>(row_ptrs.data_ptr());
+    p.begin = begin; p.end = end;
+    p.K = (int)K;
+    p.gate = rlr::Gate{nullptr, nullptr, 0, 1, 0};
+    check(rlr::launch_history_gram(p, out.data_ptr<double>(), num_sms(), cur_stream()), "history_gram");
+}
+
 // FLTrust statistics over coordinates [begin, end): fp64 [2K + 1] = (Δk.Δ0 for every k, |Δk|^2 for every k, |Δ0|^2), Δk = w_k - w_global,
 // Δ0 = w_ref - w_global.  world > 1: the fused multi-GPU form, which first runs the aggregation's barrier-in at `epoch`.
 void trust_stats(at::Tensor w_agent_ptrs, int64_t w_ref_ptr, int64_t w_global_ptr, int64_t begin, int64_t end, at::Tensor out,
@@ -420,6 +455,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("acquire_slices", &acquire_slices);
     m.def("pairwise_sqdist", &pairwise_sqdist);
     m.def("pairwise_gram", &pairwise_gram);
+    m.def("history_accumulate", &history_accumulate);
+    m.def("history_gram", &history_gram);
     m.def("trust_stats", &trust_stats);
     m.def("rfa_sqdist", &rfa_sqdist);
     m.def("gather_normalize", &gather_normalize);

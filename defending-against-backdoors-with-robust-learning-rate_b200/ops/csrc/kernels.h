@@ -65,6 +65,22 @@ cudaError_t launch_pairwise_sqdist(const DistParams& p, double* out, int num_sms
 // FLAME's Gram matrix of the updates: out[i][j] = sum_{begin <= c < end} Δi[c] Δj[c] in fp64 ([K][K], symmetric, diagonal = squared
 // update norms), Δk = w_k - w_global formed in fp32.  Same kernel, tiles and fixed-order sums as the distances; needs w_global, no scales.
 cudaError_t launch_pairwise_gram(const DistParams& p, double* out, int num_sms, cudaStream_t st);
+// FoolsGold's Gram matrix of history rows taken as they are: out[i][j] = sum_{begin <= c < end} w_agents[i][c] w_agents[j][c] in fp64
+// (the w_agents are the candidates' history rows, offset so that absolute coordinates index them).  Same kernel, tiles and fixed-order
+// sums as the distances; reads neither w_global nor scales.
+cudaError_t launch_history_gram(const DistParams& p, double* out, int num_sms, cudaStream_t st);
+
+// ---- FoolsGold: each candidate's update folded into its agent's history row ------------------------------------------------------
+// rows[k][c] <- fp32(rows[k][c] + fp32(w_agents[k][c] - w_global[c])) for begin <= c < end.  Exact fp32: bitwise reproducible.
+struct HistParams {
+    const float* const* w_agents;   // [K] device pointers (local or peer-mapped)
+    float* const* rows;             // [K] history rows, offset so that absolute coordinates index them
+    const float* w_global;          // this rank's global parameters
+    long long begin, end;           // coordinate range (multiples of 4), already clipped to [0, n_vote)
+    int K;
+    Gate gate;                      // world > 1: the aggregation's barrier-in
+};
+cudaError_t launch_history_accumulate(const HistParams& p, int num_sms, cudaStream_t st);
 
 // ---- FLTrust: each participant's update against the server's root update Δ0 = w_ref - w_global -----------------------------------------
 // out[k] = sum_c Δk[c] Δ0[c], out[K + k] = sum_c Δk[c]^2, out[2K] = sum_c Δ0[c]^2 over [begin, end), fp64 [2K + 1], Δk = w_k - w_global.

@@ -18,6 +18,7 @@
 // The same kernel with GRAM = true is FLAME's Gram pass: G[i][j] = sum_c Δi[c] Δj[c] with Δk = w_k - w_global formed per coordinate in
 // fp32 while staging, one FMA per pair and coordinate, and the diagonal (the squared update norms) kept.  Cosines are taken from G
 // directly: deriving them from D through (|a|^2 + |b|^2 - D) / 2 cancels near cos = 0, where honest high-dimensional updates sit.
+// With ROWS = true as well it is FoolsGold's Gram pass over the candidates' history rows, staged as they are (no w_global).
 #include "common.cuh"
 #include "kernels.h"
 
@@ -39,7 +40,7 @@ struct DistKernelParams {
     double* ws;                                         // [splits][K][K]
 };
 
-template <bool GRAM>
+template <bool GRAM, bool ROWS = false>
 __global__ void __launch_bounds__(kDistThreads, 2) pairwise_sqdist_kernel(DistKernelParams kp) {
     extern __shared__ float4 stage4[];
     float* const stage = reinterpret_cast<float*>(stage4);
@@ -108,7 +109,7 @@ __global__ void __launch_bounds__(kDistThreads, 2) pairwise_sqdist_kernel(DistKe
                 if (idx < P * G && g < ng && wp[q]) {
                     const long long i = cc + 4 * g;
                     v[u] = ld_f4(wp[q] + i);
-                    if (GRAM) {
+                    if (GRAM && !ROWS) {
                         const float4 gg = ld_f4(p.w_global + i);
                         v[u] = make_float4(v[u].x - gg.x, v[u].y - gg.y, v[u].z - gg.z, v[u].w - gg.w);
                     } else if (p.scales) {
@@ -192,15 +193,15 @@ __global__ void __launch_bounds__(kDistThreads, 2) pairwise_sqdist_kernel(DistKe
     }
 }
 
-template <bool GRAM>
+template <bool GRAM, bool ROWS = false>
 static cudaError_t launch_pairwise(const DistParams& p, double* out, int num_sms, cudaStream_t st) {
     if (p.K < 1 || p.K > kDistMaxAgents) return cudaErrorInvalidValue;
     if ((p.begin & 3) || (p.end & 3) || p.end < p.begin) return cudaErrorInvalidValue;
-    if (((GRAM || p.scales) && !p.w_global) || (GRAM && p.scales) || !gate_ok(p.gate)) return cudaErrorInvalidValue;
+    if ((((GRAM && !ROWS) || p.scales) && !p.w_global) || (GRAM && p.scales) || !gate_ok(p.gate)) return cudaErrorInvalidValue;
     static int occ = 0;
     if (!occ) {
-        RLR_CUDA_CHECK(cudaFuncSetAttribute(pairwise_sqdist_kernel<GRAM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDistSmem));
-        RLR_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pairwise_sqdist_kernel<GRAM>, kDistThreads, kDistSmem));
+        RLR_CUDA_CHECK(cudaFuncSetAttribute(pairwise_sqdist_kernel<GRAM, ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDistSmem));
+        RLR_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pairwise_sqdist_kernel<GRAM, ROWS>, kDistThreads, kDistSmem));
         occ = occ < 1 ? 1 : occ;
     }
     DistKernelParams kp{};
@@ -214,7 +215,7 @@ static cudaError_t launch_pairwise(const DistParams& p, double* out, int num_sms
     Scratch ws((size_t)(splits * kk) * sizeof(double), st);
     kp.ws = ws.as<double>();
     RLR_CUDA_CHECK(cudaMemsetAsync(out, 0, (size_t)kk * sizeof(double), st));
-    pairwise_sqdist_kernel<GRAM><<<dim3((unsigned)tiles, (unsigned)splits), kDistThreads, kDistSmem, st>>>(kp);
+    pairwise_sqdist_kernel<GRAM, ROWS><<<dim3((unsigned)tiles, (unsigned)splits), kDistThreads, kDistSmem, st>>>(kp);
     RLR_CUDA_CHECK(cudaGetLastError());
     return launch_ordered_sum(out, kp.ws, (int)splits, kk, st);
 }
@@ -225,6 +226,10 @@ cudaError_t launch_pairwise_sqdist(const DistParams& p, double* out, int num_sms
 
 cudaError_t launch_pairwise_gram(const DistParams& p, double* out, int num_sms, cudaStream_t st) {
     return launch_pairwise<true>(p, out, num_sms, st);
+}
+
+cudaError_t launch_history_gram(const DistParams& p, double* out, int num_sms, cudaStream_t st) {
+    return launch_pairwise<true, true>(p, out, num_sms, st);
 }
 
 }  // namespace rlr

@@ -14,7 +14,7 @@ import math
 import torch
 
 DATASETS = ("fmnist", "fedemnist", "cifar10")
-AGGREGATORS = ("avg", "comed", "sign", "fltrust", "rfa", "flame")
+AGGREGATORS = ("avg", "comed", "sign", "fltrust", "rfa", "flame", "foolsgold")
 ROOT_SIZE = 100                  # FLTrust root set: the paper's 100 clean samples
 RFA_ITERS = 3                    # RFA: a few smoothed Weiszfeld passes per round
 RFA_NU = 1e-6                    # RFA smoothing: distances below nu count as nu
@@ -41,7 +41,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--aggr", type=str, default="avg",
                    help="aggregation rule: avg | comed | sign | fltrust (trust-weighted mean against a server-trained root update) | "
                         "rfa (smoothed geometric median by Weiszfeld passes, Pillutla et al. 2022) | flame (cosine clustering, "
-                        "median-norm clipping and adaptive noise, Nguyen et al. 2022)")
+                        "median-norm clipping and adaptive noise, Nguyen et al. 2022) | foolsgold (a weighted mean that "
+                        "down-weights agents whose summed update histories are too similar to another's, Fung et al. 2020)")
     p.add_argument("--local_ep", type=int, default=2, help="number of local epochs: E")
     p.add_argument("--bs", type=int, default=256, help="local batch size: B")
     p.add_argument("--client_lr", type=float, default=0.1, help="clients' learning rate")

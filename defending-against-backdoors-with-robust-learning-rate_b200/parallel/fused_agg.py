@@ -31,7 +31,9 @@ gathered copies locally; on CPU it runs the fp64 oracle.
 
 Server optimizer state (``--server_opt`` other than sgd; ``ops.ServerOptState``) lives in ordinary device memory, allocated once:
 on the fused multi-GPU path rank r keeps only the state of its slice [begin, end) -- it is the only rank that ever steps those
-coordinates -- and with every other transport each rank keeps the full vector (identical on all ranks).
+coordinates -- and with every other transport each rank keeps the full vector (identical on all ranks).  FoolsGold's per-agent update
+histories (``--aggr foolsgold``) are laid out the same way: ``[num_agents][slice ∩ [0, n_vote)]`` on the fused multi-GPU path, the full
+``[num_agents][n_vote]`` table on every rank otherwise.
 """
 from __future__ import annotations
 
@@ -47,9 +49,10 @@ FLAG_BYTES = 4096
 
 class FusedAggregator:
     def __init__(self, ctx, n_total: int, n_vote: int, max_slots: int, backend: str = "auto", with_bf16: bool = True,
-                 transport: str = "auto", server_opt=None, n_part: int | None = None):
+                 transport: str = "auto", server_opt=None, n_part: int | None = None, history_agents: int = 0):
         """``server_opt``: optional ``dict(kind=..., beta1=..., beta2=..., tau=...)``; ``n_part``: participants per round (default
-        every slot), which fixes whether the fused multi-GPU kernel or the gather fallback runs, and so the state layout."""
+        every slot), which fixes whether the fused multi-GPU kernel or the gather fallback runs, and so the state layout;
+        ``history_agents``: agents whose FoolsGold update history this aggregator keeps (``--aggr foolsgold``: ``--num_agents``; 0 = none)."""
         self.ctx = ctx
         # nccl / gloo back-ends: "gather" all-gathers every participant's parameters and runs the kernel on the copies (any
         # aggregator); "reduce" all-reduces per-coordinate partial sums (vote, weighted update sum) -- O(N) instead of O(K N)
@@ -116,6 +119,23 @@ class FusedAggregator:
             self.opt = ops.ServerOptState(kind, self.end - self.begin, device=dev, base=self.begin, **so)
         else:
             self.opt = ops.ServerOptState(kind, n, device=dev, **so)
+        # FoolsGold's update histories (history_agents > 0): [history_agents][hist_hi - hist_lo] fp32, zero at the start.  On the fused
+        # multi-GPU path rank r keeps the columns of its slice that lie below n_vote (the only rank that ever reads or writes them);
+        # with every other transport each rank keeps the full [0, n_vote) table, identical on all ranks.
+        self.history = None
+        if history_agents:
+            self._alloc_history(int(history_agents))
+
+    def _alloc_history(self, agents: int):
+        """Allocate the zero FoolsGold history of ``agents`` rows over ``[hist_lo, hist_hi)``: this rank's slice below n_vote on the
+        fused multi-GPU path (empty when the slice lies past n_vote), all of ``[0, n_vote)`` otherwise.  Refuses a table that does not
+        fit in the free device memory."""
+        self.hist_lo, self.hist_hi = (self.begin, max(self.begin, min(self.end, self.n_vote))) if self.sharded else (0, self.n_vote)
+        width = self.hist_hi - self.hist_lo
+        dev = self.ctx.device
+        if dev.type == "cuda":
+            check_history_memory(agents, width, torch.cuda.mem_get_info(dev)[0])
+        self.history = torch.zeros((agents, width), dtype=torch.float32, device=dev)
 
     # ---- hand-off fused with the next round's first GEMM -------------------------------------------------------------------
     def enable_handoff(self):
@@ -272,6 +292,77 @@ class FusedAggregator:
         agents = self._participants(n_part, participants)
         return ops.pairwise_gram([agents[j] for j in idx], self.w_global, self.n_vote)
 
+    def foolsgold_gram(self, n_part: int, agent_ids, members=None, participants=None):
+        """FoolsGold history pass: fold the updates ``w_j - w_global`` of the participants at positions ``members`` (ascending; every one of
+        the round's ``n_part`` when None) into the history rows of their agents ``agent_ids[j]`` over ``[0, n_vote)``, then return the
+        float64 Gram matrix of those rows (``ops.history_gram_statement``), identical on every rank.  Call it after the slots are final
+        and before ``aggregate`` of the same round.
+
+        Fused multi-GPU path: one ``_fused_pass``.  Each rank runs ``history_accumulate_kernel`` over its coordinate slice of the
+        peer-mapped slots behind the aggregation kernel's barrier-in (an epoch of its own) into its own columns of the history, then the
+        Gram kernel over those columns; the ranks all_gather their partial matrices and add them in rank order.  The pass reads
+        ``w_global``, so it first acquires the broadcast slices of a fused hand-off.  Gather transport and single process: the same
+        kernels over ``participants`` (``gather_participants``' copies; gathered here when not given) and the full table every rank
+        keeps.  The reduce transport never holds every participant on one rank, so the pass takes the gather transport, as FLAME's does."""
+        if self.history is None:
+            raise ValueError("this aggregator keeps no FoolsGold history (history_agents = 0)")
+        if self._p2p(n_part) != self.sharded:
+            raise ValueError(f"{n_part} participants: the FoolsGold history was laid out for the "
+                             f"{'fused multi-GPU' if self.sharded else 'gather'} path")
+        idx = list(range(n_part)) if members is None else [int(j) for j in members]
+        if self._p2p(n_part):
+            self.acquire()
+            dev = self.ctx.device
+            table = self._agent_table(n_part) if idx == list(range(n_part)) else self._member_table(idx)
+            width = self.hist_hi - self.hist_lo
+            # row pointers offset by hist_lo so that absolute coordinates index them (only [hist_lo, hist_hi) is ever touched)
+            base = self.history.data_ptr() - 4 * self.hist_lo
+            tab = ops.PtrTable([base + 4 * width * int(agent_ids[j]) for j in idx], dev)
+
+            def launch(begin, end, out, flag_ptrs, local_sync, rank, world, epoch):
+                ops.ext().history_accumulate(table.tensor, tab.tensor, self.w_global.data_ptr(), begin, end, flag_ptrs, local_sync, rank,
+                                             world, epoch)
+                ops.ext().history_gram(tab.tensor, begin, end, out)
+            return self._fused_pass((len(idx), len(idx)), launch)
+        agents = self._participants(n_part, participants)
+        rows = [self.history[int(agent_ids[j])] for j in idx]
+        ops.history_accumulate(rows, [agents[j] for j in idx], self.w_global, 0, self.n_vote)
+        return ops.history_gram(rows, self.n_vote)
+
+    def foolsgold_history(self, chunk_bytes: int = 256 << 20):
+        """The full ``[history_agents, n_vote]`` fp32 FoolsGold history on the host of the main rank (what a checkpoint saves); None on the
+        other ranks.  Collective on the fused multi-GPU path, where each rank contributes its columns: the rows are all-gathered in chunks
+        of about ``chunk_bytes`` of gathered data, so no rank holds more than one chunk of extra device memory, and only the main rank
+        copies them to the host."""
+        main = self.ctx.is_main
+        if not self.sharded:
+            if not main:
+                return None
+            return self.history.cpu() if self.history.is_cuda else self.history.clone()
+        A = self.history.shape[0]
+        world, per = self.ctx.world, self.per
+        full = torch.empty((A, self.n_vote), dtype=torch.float32) if main else None
+        rows = max(1, int(chunk_bytes) // (4 * per * world))
+        width = self.hist_hi - self.hist_lo
+        for a0 in range(0, A, rows):
+            a1 = min(A, a0 + rows)
+            part = torch.zeros((a1 - a0, per), dtype=torch.float32, device=self.history.device)
+            part[:, :width] = self.history[a0:a1]
+            allp = self.ctx.all_gather(part)                                 # [world, rows, per]: rank r holds columns [r per, r per + per)
+            if main:
+                full[a0:a1] = allp.permute(1, 0, 2).reshape(a1 - a0, world * per)[:, : self.n_vote].cpu()
+            del part, allp
+        return full
+
+    def load_foolsgold_history(self, full):
+        """Set the history from a full ``[history_agents, n_vote]`` table (this rank's columns of it on the fused multi-GPU path)."""
+        if self.history is None:
+            raise ValueError("this aggregator keeps no FoolsGold history (history_agents = 0)")
+        if tuple(full.shape) != (self.history.shape[0], self.n_vote):
+            raise ValueError(f"FoolsGold history of shape {tuple(full.shape)}; this run keeps {self.history.shape[0]} agents x "
+                             f"{self.n_vote} voted coordinates")
+        self.history.copy_(full[:, self.hist_lo:self.hist_hi])
+
     def aggregate(self, weights, mode, theta, server_lr, noise_std=0.0, seed=0, rnd=0, scales=None, members=None, participants=None,
                   total_weight=None):
         """Aggregate the round's ``len(weights)`` participants (participant j lives in ``slot_owner(j)``; ``weights`` and ``scales`` are
@@ -400,6 +491,16 @@ class FusedAggregator:
 
     def close(self):
         self.buf.close()
+
+
+def check_history_memory(num_agents: int, width: int, free_bytes: int):
+    """Refuse a FoolsGold history of ``num_agents`` rows of ``width`` fp32 values that does not fit in ``free_bytes`` of device memory."""
+    nbytes = 4 * int(num_agents) * int(width)
+    if nbytes > int(free_bytes):
+        raise ValueError(f"--aggr foolsgold keeps one fp32 update history per agent: {nbytes} bytes on this GPU for --num_agents "
+                         f"{num_agents} x {width} voted coordinates, but only {int(free_bytes)} bytes are free.  Use fewer agents or "
+                         "more GPUs (the fused multi-GPU path shards the history over the ranks)")
+    return nbytes
 
 
 class _Solo:

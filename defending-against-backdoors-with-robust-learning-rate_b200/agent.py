@@ -14,6 +14,7 @@ import torch
 
 from .data import DatasetSplit, poison_dataset
 from .data.datasets import h5_to_device_dataset, load_fedemnist_client
+from .options import attack_schedule_set
 
 
 class Agent:
@@ -22,6 +23,8 @@ class Agent:
         self.args = args
         self.is_corrupt = id < args.num_corrupt
         self.poisoned_idxs = []
+        # attack schedules: (indices, rows, labels) of the poisoned samples before poisoning, which the engine swaps in for quiet rounds
+        self.clean_copy = [] if attack_schedule_set(args) else None
         rng = random.Random(1_000_003 * (seed + 1) + id)
         if train_dataset is None:
             # Fed-EMNIST: one pre-partitioned file per client (src/agent.py:16-20)
@@ -29,13 +32,13 @@ class Agent:
             self.dataset = shard
             self.idxs = torch.arange(len(shard), device=shard.device)
             if self.is_corrupt:
-                self.poisoned_idxs = poison_dataset(shard, args, None, agent_idx=id, rng=rng)
+                self.poisoned_idxs = poison_dataset(shard, args, None, agent_idx=id, rng=rng, clean_copy=self.clean_copy)
         else:
             self.dataset = train_dataset
             self.idxs = torch.as_tensor(list(data_idxs), dtype=torch.int64, device=train_dataset.device)
             if self.is_corrupt:
                 # poisons the SHARED dataset in place at this agent's indices (src/agent.py:24-25)
-                self.poisoned_idxs = poison_dataset(train_dataset, args, self.idxs, agent_idx=id, rng=rng)
+                self.poisoned_idxs = poison_dataset(train_dataset, args, self.idxs, agent_idx=id, rng=rng, clean_copy=self.clean_copy)
         self.n_data = int(self.idxs.shape[0])
         self._gen = None
 

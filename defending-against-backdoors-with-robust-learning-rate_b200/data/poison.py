@@ -90,15 +90,19 @@ def select_poison_idxs(dataset, base_class: int, poison_frac: float, data_idxs=N
     return rng.sample(all_idxs, floor(poison_frac * len(all_idxs)))
 
 
-def poison_dataset(dataset, args, data_idxs=None, poison_all=False, agent_idx=-1, rng: random.Random | None = None):
+def poison_dataset(dataset, args, data_idxs=None, poison_all=False, agent_idx=-1, rng: random.Random | None = None,
+                   clean_copy: list | None = None):
     """Poison ``dataset`` in place (reference ``poison_dataset``, src/utils.py:160-178): stamp the pattern on
-    the chosen base-class images and relabel them ``target_class``.  Returns the poisoned indices."""
+    the chosen base-class images and relabel them ``target_class``.  Returns the poisoned indices.  With a ``clean_copy`` list (attack
+    schedules), ``(indices, rows, labels)`` of the poisoned samples as they were before stamping are appended to it first."""
     frac = 1 if poison_all else args.poison_frac
     idxs = select_poison_idxs(dataset, args.base_class, frac, data_idxs, rng)
     if not idxs:
         return idxs
     rows, cols, vals, mode = pattern_pixels(args.data, args.pattern_type, agent_idx)
     sel = torch.as_tensor(idxs, dtype=torch.int64, device=dataset.device)
+    if clean_copy is not None:
+        clean_copy.append((sel, dataset.data[sel], dataset.targets[sel]))
     if rows:
         ops.stamp_pixels(dataset.data, sel, rows, cols, vals, mode)
     dataset.targets[sel] = args.target_class  # label flips even when no pixel changed (src/utils.py:177)

@@ -29,10 +29,11 @@ from .aggregation import Aggregation, server_opt_spec
 from .data import distribute_data, get_datasets, make_poisoned_val
 from .data.datasets import DeviceDataset, h5_to_device_dataset, load_fedemnist_client
 from .models import get_layout
-from .options import print_exp_details
+from .options import attack_schedule_set, is_attack_round, last_attack_round, print_exp_details
 from .parallel import FusedAggregator, init_distributed
 from .trainers import make_trainer
-from .utils import MetricLogger, PhaseTimer, get_loss_n_accuracy, load_checkpoint, restore_server_opt, save_checkpoint
+from .utils import (MetricLogger, PhaseTimer, backdoor_lifespan, get_loss_n_accuracy, load_checkpoint, restore_server_opt,
+                    save_checkpoint)
 
 
 _ROOT_SET_TAG = 0x464C5472           # "FLTr": keeps the root-set draw apart from every other stream seeded by --seed
@@ -48,6 +49,20 @@ def draw_root_set(n_train: int, excluded, size: int, seed: int):
     if not 1 <= size <= pool.size:
         raise ValueError(f"--root_size {size}: only {pool.size} of {n_train} training samples are unpoisoned")
     return np.sort(np.random.default_rng([int(seed), _ROOT_SET_TAG]).choice(pool, int(size), replace=False)).astype(np.int64)
+
+
+def force_participants(drawn, num_corrupt: int):
+    """Forced participation in an attack round: the corrupt ids (``< num_corrupt``) missing from ``drawn``, in ascending order, take
+    the places of the honest ids from the last position of the draw toward the first, until no corrupt id is missing or no honest id
+    is left.  A draw that already holds every corrupt id comes back unchanged."""
+    out = list(drawn)
+    missing = [a for a in range(num_corrupt) if a not in set(out)]
+    for pos in range(len(out) - 1, -1, -1):
+        if not missing:
+            break
+        if out[pos] >= num_corrupt:
+            out[pos] = missing.pop(0)
+    return out
 
 
 class FLEngine:
@@ -91,6 +106,13 @@ class FLEngine:
                 self.agents.append(Agent(_id, args, self.train_dataset, groups[_id], seed=args.seed))
         for a in self.agents:
             self.agent_data_sizes[a.id] = a.n_data
+        # ---- attack schedule (DESIGN.md section 3): one side copy per poisoned dataset, swapped in for quiet rounds --------------------
+        self.schedule = attack_schedule_set(args)
+        self._swaps = self._build_swaps() if self.schedule else []
+        self._data_poisoned = True                                      # the datasets as the agents left them
+        self.last_attack_active = None
+        self.last_attack = last_attack_round(args.attack_start, args.attack_stop, args.attack_every)
+        self.backdoor_lifespan = None
         # ---- FLTrust: the server's root job, an agent (id num_agents, never corrupt) on a clean sample of the training set -----------
         self.root_agent = None
         if args.aggr == "fltrust":
@@ -177,12 +199,43 @@ class FLEngine:
                     raise ValueError("checkpoint has no Neurotoxin state (w_prev), but this run uses --attack_neurotoxin")
                 self.w_prev.copy_(w_prev.to(dev))
                 self._have_prev = True
+            if self.last_attack is not None:
+                if "backdoor_lifespan" not in ck["extra"]:
+                    raise ValueError("checkpoint has no backdoor lifespan, but this run uses --attack_stop")
+                self.backdoor_lifespan = ck["extra"]["backdoor_lifespan"]
             if self.fused.history is not None:
                 hist = ck["extra"].get("foolsgold_history")
                 if hist is None:
                     raise ValueError("checkpoint has no FoolsGold history, but this run uses --aggr foolsgold")
                 self.fused.load_foolsgold_history(hist)
         ctx.barrier()
+
+    def _build_swaps(self):
+        """The corrupt agents' side copies, concatenated per poisoned dataset: ``[(dataset, idx, rows, labels)]``.  The indices of one
+        dataset are checked distinct here, once, so a swap needs no host sync."""
+        by_ds = {}
+        for a in self.agents:
+            for sel, x, y in a.clean_copy or ():
+                by_ds.setdefault(id(a.dataset), (a.dataset, []))[1].append((sel, x, y))
+        swaps = []
+        for ds, parts in by_ds.values():
+            idx = torch.cat([p[0] for p in parts])
+            if torch.unique(idx).numel() != idx.numel():
+                raise ValueError("attack schedule: two corrupt agents poisoned the same training sample")
+            swaps.append((ds, idx, torch.cat([p[1] for p in parts]), torch.cat([p[2] for p in parts])))
+        return swaps
+
+    def attack_active(self, rnd: int) -> bool:
+        """Whether round ``rnd`` is an attack round of ``--attack_start / --attack_stop / --attack_every``."""
+        a = self.args
+        return is_attack_round(rnd, a.attack_start, a.attack_stop, a.attack_every)
+
+    def _set_poisoned(self, poisoned: bool):
+        """Bring every poisoned dataset to the wanted state: one swap launch per dataset on the current stream when it differs."""
+        if poisoned != self._data_poisoned:
+            for ds, idx, x, y in self._swaps:
+                ops.swap_samples(ds.data, ds.targets, idx, x, y)
+            self._data_poisoned = poisoned
 
     def _jobs(self):
         """Every agent this engine may train: the clients, then the FLTrust root job."""
@@ -221,6 +274,8 @@ class FLEngine:
         keeps the device addresses (and therefore the captured CUDA graphs) identical no matter which agent a rank hosts in a
         round.  Returns the total bytes of all shards."""
         from .data import DeviceDataset
+        if self.schedule:
+            raise ValueError("input streaming keeps one fixed copy of every shard and cannot follow an attack schedule")
         self._stream_src = {}
         dev = self.ctx.device
         pin = (lambda t: t.cpu().pin_memory()) if dev.type == "cuda" else (lambda t: t.cpu().clone())
@@ -250,13 +305,19 @@ class FLEngine:
 
     # ---- one federated round (src/federated.py:66-74) --------------------------------------------------------
     def run_round(self, rnd: int, stream_inputs: bool = False):
-        chosen = self.place_participants(self.sample_agents(rnd))
+        attack = self.attack_active(rnd)
+        drawn = self.sample_agents(rnd)
+        if attack and self.args.attack_force:
+            drawn = force_participants(drawn, self.args.num_corrupt)
+        chosen = self.place_participants(drawn)
         ctx, fused = self.ctx, self.fused
+        self.last_attack_active = attack
         self.round_loss.zero_()
         steps = 0
         h2d = 0
         self.timer.start("local_train")
-        mask = self._neurotoxin_mask() if self.neurotoxin_k is not None else None
+        self._set_poisoned(attack)                                       # queued ahead of every trainer stream
+        mask = self._neurotoxin_mask(attack) if self.neurotoxin_k is not None else None
         for t in self.trainers:
             t.attack_mask = mask
         concurrent = len(self.trainers) > 1
@@ -282,14 +343,14 @@ class FLEngine:
                     if stream_inputs:
                         h2d += self._upload_shard(agent, self._stream_bufs[i])     # on stream i: ordered after trainer i's previous agent
                     st = agent.local_train(self.trainers[i], self.w_global, fused.slots[s], rnd)
-                    self._boost(agent, fused.slots[s])
+                    self._boost(agent, fused.slots[s], attack)
                     if client:
                         self._loss_parts[i] += st["loss_sum"]
             else:
                 if stream_inputs:
                     h2d += self._upload_shard(agent)
                 st = agent.local_train(self.trainer, self.w_global, fused.slots[s], rnd)
-                self._boost(agent, fused.slots[s])
+                self._boost(agent, fused.slots[s], attack)
                 if client:
                     self.round_loss += st["loss_sum"]
             if client:
@@ -307,13 +368,13 @@ class FLEngine:
         self.timer.stop("aggregate")
         return {"chosen": chosen, "steps": steps, "h2d_bytes": h2d}
 
-    def _neurotoxin_mask(self):
+    def _neurotoxin_mask(self, attack: bool = True):
         """Start of a round with Neurotoxin on: the mask of the last global update ``w_global - w_prev`` (the top-k coordinates by
         magnitude) and ``w_prev <- w_global``, queued on the current stream ahead of the trainers.  Returns the mask words, or None
-        when the mask is empty (the first round a run executes, or k = 0)."""
+        when the mask is empty (the first round a run executes, or k = 0) and in a quiet round, which only refreshes ``w_prev``."""
         nv = self.layout.n_vote
         self.fused.acquire()                                             # the pass reads w_global
-        if not self._have_prev:
+        if not self._have_prev or not attack:
             self.w_prev.copy_(self.w_global[:nv])
             self.masked_coords.zero_()
             self._have_prev = True
@@ -321,9 +382,10 @@ class FLEngine:
         ops.neurotoxin_mask(self.w_global, self.w_prev, nv, self.neurotoxin_k, self.attack_mask, self.masked_coords)
         return self.attack_mask if self.neurotoxin_k > 0 else None
 
-    def _boost(self, agent, slot):
-        """Model replacement: a corrupt agent's update in its slot scaled by ``--attack_boost``, on the agent's stream."""
-        if self.attack_boost != 1.0 and agent.is_corrupt:
+    def _boost(self, agent, slot, attack: bool = True):
+        """Model replacement: a corrupt agent's update in its slot scaled by ``--attack_boost`` in an attack round, on the agent's
+        stream."""
+        if self.attack_boost != 1.0 and agent.is_corrupt and attack:
             ops.boost_update(slot, self.w_global, self.attack_boost, self.layout.n_vote)
 
     def round_result(self):
@@ -374,6 +436,13 @@ class FLEngine:
             print(f"| Val_Loss/Val_Acc: {val_loss:.3f} / {val_acc:.3f} |")
             print(f"| Val_Per_Class_Acc: {per_class} ")
             print(f"| Poison Loss/Poison Acc: {poison_loss:.3f} / {poison_acc:.3f} |")
+        if self.last_attack is not None and self.backdoor_lifespan is None:
+            span = backdoor_lifespan([(rnd, poison_acc)], self.last_attack, args.lifespan_threshold)
+            if span is not None:                                         # logged once, in the round the backdoor is gone
+                self.backdoor_lifespan = out["backdoor_lifespan"] = span
+                lg.add_scalar("Poison/Lifespan", span, rnd)
+                if self.verbose:
+                    print(f"| Backdoor lifespan: {span} rounds |")
         return out
 
     # ---- the training loop --------------------------------------------------------------------------------
@@ -400,6 +469,11 @@ class FLEngine:
             if self.last_masked_coords is not None:
                 rec["attack_masked_coords"] = self.last_masked_coords
                 self.logger.add_scalar("Attack/Masked_Coords", self.last_masked_coords, rnd)
+            if self.schedule:
+                rec["attack_active"] = self.last_attack_active
+                self.logger.add_scalar("Attack/Active", int(self.last_attack_active), rnd)
+            if rnd == rounds and self.last_attack is not None and self.backdoor_lifespan is None and rnd >= self.last_attack:
+                rec["backdoor_lifespan_at_least"] = rnd - self.last_attack
             if self.aggregator.last_select is not None:
                 rec["select_corrupt_participants"] = self.aggregator.last_select["Select/Corrupt_Participants"]
                 rec["select_corrupt_admitted"] = self.aggregator.last_select["Select/Corrupt_Admitted"]
@@ -434,8 +508,12 @@ class FLEngine:
                         extra["neurotoxin_w_prev"] = self.w_prev.cpu()
                     if hist is not None:
                         extra["foolsgold_history"] = hist
+                    if self.last_attack is not None:
+                        extra["backdoor_lifespan"] = self.backdoor_lifespan
                     save_checkpoint(args.checkpoint, self.global_params(), rnd, args, self.layout, extra, so)
         if self.verbose:
+            if history and "backdoor_lifespan_at_least" in history[-1]:
+                print(f"| Backdoor lifespan: > {history[-1]['backdoor_lifespan_at_least']} rounds |")
             print("Training has finished!")
         return history
 

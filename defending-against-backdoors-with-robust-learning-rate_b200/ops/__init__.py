@@ -990,6 +990,20 @@ def boost_update(slot, w_g, gamma: float, n_vote: int):
     slot[:n_vote].copy_(torch.from_numpy(boost_statement(slot, w_g, gamma, n_vote)))
 
 
+def swap_samples(data, targets, idx, side_data, side_targets):
+    """Attack schedules: exchange the dataset rows and labels at ``idx`` with the side copy in place, ``data[idx[i]] <-> side_data[i]``
+    and ``targets[idx[i]] <-> side_targets[i]``.  The ``idx`` must be distinct (checked once, where the side copy is built), so the
+    swap is its own inverse and every tensor keeps its address.  One launch on the GPU, none for an empty ``idx``."""
+    if data.is_cuda:
+        ext().swap_samples(data, targets, idx, side_data, side_targets)
+        return
+    x, y = data[idx], targets[idx]
+    data[idx] = side_data
+    targets[idx] = side_targets
+    side_data.copy_(x)
+    side_targets.copy_(y)
+
+
 # =====================================================================================================================
 # optimiser over flat buffers
 # =====================================================================================================================

@@ -132,12 +132,60 @@ __global__ void __launch_bounds__(256) boost_update_kernel(float* __restrict__ s
     }
 }
 
+// Attack schedules: data[idx[i]] <-> side[i] (row_bytes each) and targets[idx[i]] <-> side_targets[i] for i < n.  One warp per row in
+// a grid-stride loop over the rows, the lanes striding over the row's W-sized words; lane 0 swaps the label.  The idx are distinct, so
+// no two threads touch the same byte: no atomics, and the swap is its own inverse.
+template <typename W>
+__global__ void __launch_bounds__(256) swap_samples_kernel(unsigned char* __restrict__ data, long long* __restrict__ targets,
+                                                           const long long* __restrict__ idx, unsigned char* __restrict__ side,
+                                                           long long* __restrict__ side_targets, long long n, int row_words) {
+    pdl_wait();
+    pdl_trigger();
+    const int lane = threadIdx.x & 31;
+    const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long i = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); i < n; i += warps) {
+        const long long j = idx[i];
+        W* a = reinterpret_cast<W*>(data) + j * row_words;
+        W* b = reinterpret_cast<W*>(side) + i * row_words;
+#pragma unroll 2                     // the default 4-way unroll of the 16-byte words spills
+        for (int w = lane; w < row_words; w += 32) {
+            const W x = a[w], y = b[w];
+            a[w] = y;
+            b[w] = x;
+        }
+        if (lane == 0) {
+            const long long x = targets[j];
+            targets[j] = side_targets[i];
+            side_targets[i] = x;
+        }
+    }
+}
+
 inline int sweep_grid(long long n4, int threads, int num_sms, int per_sm) {
     const long long want = (n4 + threads - 1) / threads, cap = (long long)num_sms * per_sm;
     return (int)(want < 1 ? 1 : (want > cap ? cap : want));
 }
 
 }  // namespace
+
+cudaError_t launch_swap_samples(void* data, long long* targets, const long long* idx, void* side, long long* side_targets, long long n,
+                                long long row_bytes, int num_sms, cudaStream_t st) {
+    if (n < 0 || row_bytes <= 0) return cudaErrorInvalidValue;
+    if (n == 0) return cudaSuccess;
+    const dim3 grid(sweep_grid(n * 32, 256, num_sms, 8)), block(256);
+    auto* d = static_cast<unsigned char*>(data);
+    auto* s = static_cast<unsigned char*>(side);
+    // the widest word that divides the row and both base addresses
+    const uintptr_t align = reinterpret_cast<uintptr_t>(data) | reinterpret_cast<uintptr_t>(side) | (uintptr_t)row_bytes;
+    if (align % 16 == 0)
+        return launch_kernel(swap_samples_kernel<uint4>, grid, block, (size_t)0, st, d, targets, idx, s, side_targets, n,
+                             (int)(row_bytes / 16));
+    if (align % 4 == 0)
+        return launch_kernel(swap_samples_kernel<uint32_t>, grid, block, (size_t)0, st, d, targets, idx, s, side_targets, n,
+                             (int)(row_bytes / 4));
+    return launch_kernel(swap_samples_kernel<unsigned char>, grid, block, (size_t)0, st, d, targets, idx, s, side_targets, n,
+                         (int)row_bytes);
+}
 
 cudaError_t launch_neurotoxin_mask(const float* w_g, float* w_prev, long long n_vote, long long k, uint32_t* mask, long long* count,
                                    int num_sms, cudaStream_t st) {

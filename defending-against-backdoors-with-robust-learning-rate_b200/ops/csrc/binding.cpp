@@ -385,6 +385,26 @@ void boost_update(at::Tensor slot, at::Tensor w_g, double gamma, int64_t n_vote)
     check(rlr::launch_boost_update(slot.data_ptr<float>(), w_g.data_ptr<float>(), n_vote, gamma, num_sms(), cur_stream()), "boost_update");
 }
 
+void swap_samples(at::Tensor data, at::Tensor targets, at::Tensor idx, at::Tensor side_data, at::Tensor side_targets) {
+    CHECK_CUDA(data); CHECK_CUDA(targets); CHECK_CUDA(idx); CHECK_CUDA(side_data); CHECK_CUDA(side_targets);
+    TORCH_CHECK(targets.scalar_type() == at::kLong && idx.scalar_type() == at::kLong && side_targets.scalar_type() == at::kLong,
+                "swap_samples: targets, idx and side_targets must be int64");
+    TORCH_CHECK(data.scalar_type() == side_data.scalar_type() && data.dim() >= 1 && side_data.dim() >= 1,
+                "swap_samples: data and side_data must share a dtype");
+    const int64_t n = idx.numel();
+    TORCH_CHECK(side_data.size(0) == n && side_targets.numel() == n && targets.numel() == data.size(0),
+                "swap_samples: one side row and label per index, one label per data row");
+    TORCH_CHECK(data.size(0) > 0 || n == 0, "swap_samples: empty dataset");
+    const int64_t row_bytes = data.size(0) > 0 ? data.numel() / data.size(0) * data.element_size() : 0;
+    TORCH_CHECK(n == 0 || side_data.numel() / n * side_data.element_size() == row_bytes, "swap_samples: side rows differ in size");
+    if (n == 0) return;
+    c10::cuda::CUDAGuard guard(data.device());
+    check(rlr::launch_swap_samples(data.data_ptr(), reinterpret_cast<long long*>(targets.data_ptr()),
+                                   reinterpret_cast<const long long*>(idx.data_ptr()), side_data.data_ptr(),
+                                   reinterpret_cast<long long*>(side_targets.data_ptr()), n, row_bytes, num_sms(), cur_stream()),
+          "swap_samples");
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 void softmax_xent(at::Tensor logits, at::Tensor labels, c10::optional<at::Tensor> dlogits, c10::optional<at::Tensor> loss_sum,
                   c10::optional<at::Tensor> correct, double grad_scale) {
@@ -473,6 +493,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("mask") = py::none());
     m.def("neurotoxin_mask", &neurotoxin_mask);
     m.def("boost_update", &boost_update);
+    m.def("swap_samples", &swap_samples);
     m.def("pgd_project", &pgd_project, py::arg("w"), py::arg("w0"), py::arg("w_bf16"), py::arg("clip"), py::arg("d_sqnorm"),
           py::arg("n_pgd") = 0, py::arg("mask") = py::none());
     m.def("softmax_xent", &softmax_xent);

@@ -154,6 +154,10 @@ cudaError_t launch_neurotoxin_mask(const float* w_g, float* w_prev, long long n_
 // boosted update: slot[c] = fp32((double)w_g[c] + gamma * (double)fp32(slot[c] - w_g[c])) over [0, n_vote), each fp64 operation
 // rounded on its own
 cudaError_t launch_boost_update(float* slot, const float* w_g, long long n_vote, double gamma, int num_sms, cudaStream_t st);
+// attack schedules: data[idx[i]] <-> side[i] (row_bytes bytes each) and targets[idx[i]] <-> side_targets[i] for i < n, in one launch.
+// The idx must be distinct and in range (checked by the caller once, when the side copy is built).  n = 0 launches nothing.
+cudaError_t launch_swap_samples(void* data, long long* targets, const long long* idx, void* side, long long* side_targets, long long n,
+                                long long row_bytes, int num_sms, cudaStream_t st);
 
 // ---- loss / evaluation -----------------------------------------------------------------------------------
 // logits [B,C] (kind 0 fp32 / 1 bf16); writes dlogits (same kind, scaled by 1/B) and accumulates loss_sum / correct.

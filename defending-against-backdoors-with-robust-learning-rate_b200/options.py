@@ -19,6 +19,7 @@ ROOT_SIZE = 100                  # FLTrust root set: the paper's 100 clean sampl
 RFA_ITERS = 3                    # RFA: a few smoothed Weiszfeld passes per round
 RFA_NU = 1e-6                    # RFA smoothing: distances below nu count as nu
 FLAME_LAMBDA = 1e-3              # FLAME noise factor: the paper's value for image classification
+LIFESPAN_THRESHOLD = 0.5         # poison accuracy below which the backdoor counts as gone
 SERVER_OPTS = ("sgd", "momentum", "adagrad", "adam", "yogi")
 SELECTIONS = ("none", "krum", "multikrum")
 PATTERNS = ("plus", "square", "copyright", "apple")
@@ -135,7 +136,34 @@ def build_parser() -> argparse.ArgumentParser:
                    help="Neurotoxin (Zhang et al. 2022): corrupt agents never update the top p fraction of coordinates by magnitude of "
                         "the last global update; their gradient is zeroed there at every local step.  0 <= p < 1 (0 = off; needs "
                         "--num_corrupt > 0)")
+    p.add_argument("--attack_start", type=int, default=1, help="attack schedule: the first round the corrupt agents attack (>= 1)")
+    p.add_argument("--attack_stop", type=int, default=0,
+                   help="attack schedule: the last round that may be an attack round (0 = no end).  In the other rounds a corrupt agent "
+                        "trains on its clean samples, unmasked and unboosted, like an honest client")
+    p.add_argument("--attack_every", type=int, default=1, help="attack schedule: attack every F-th round from --attack_start (>= 1)")
+    p.add_argument("--attack_force", action="store_true",
+                   help="attack schedule: every corrupt agent takes part in every attack round; the round's draw keeps its size and "
+                        "honest participants give way from the end of the draw")
+    p.add_argument("--lifespan_threshold", type=float, default=LIFESPAN_THRESHOLD,
+                   help="poison accuracy below which the backdoor counts as gone; the rounds from the last attack round until then are "
+                        "logged as the backdoor's lifespan.  In (0, 1]; needs --attack_stop > 0")
     return p
+
+
+def attack_schedule_set(args) -> bool:
+    """True when any attack-schedule flag differs from its default (every round an attack round, no forced participation)."""
+    return (getattr(args, "attack_start", 1) != 1 or getattr(args, "attack_stop", 0) != 0 or getattr(args, "attack_every", 1) != 1
+            or bool(getattr(args, "attack_force", False)))
+
+
+def is_attack_round(rnd: int, start: int = 1, stop: int = 0, every: int = 1) -> bool:
+    """Round ``rnd`` is an attack round iff ``rnd >= start``, ``stop == 0 or rnd <= stop`` and ``(rnd - start) % every == 0``."""
+    return rnd >= start and (stop == 0 or rnd <= stop) and (rnd - start) % every == 0
+
+
+def last_attack_round(start: int, stop: int, every: int):
+    """The last attack round ``L = start + every * floor((stop - start) / every)`` of a schedule with a stop round, else None."""
+    return start + every * ((stop - start) // every) if stop > 0 else None
 
 
 def finalize_args(args: argparse.Namespace) -> argparse.Namespace:
@@ -182,6 +210,28 @@ def _finalize_attack(args) -> None:
     if (gamma != 1.0 or p > 0) and args.num_corrupt <= 0:
         raise ValueError("--attack_boost / --attack_neurotoxin need corrupt agents (--num_corrupt > 0)")
     args.attack_boost, args.attack_neurotoxin = gamma, p
+    _finalize_schedule(args)
+
+
+def _finalize_schedule(args) -> None:
+    """Validate the attack-schedule flags: start >= 1, stop 0 or >= start, every >= 1, the lifespan threshold finite in (0, 1] and only
+    with a stop round, and any schedule only with corrupt agents to follow it."""
+    start, stop, every = (int(getattr(args, k, d)) for k, d in (("attack_start", 1), ("attack_stop", 0), ("attack_every", 1)))
+    theta = float(getattr(args, "lifespan_threshold", LIFESPAN_THRESHOLD))
+    if start < 1:
+        raise ValueError(f"--attack_start {start} must be >= 1")
+    if stop != 0 and stop < start:
+        raise ValueError(f"--attack_stop {stop} must be 0 (no end) or >= --attack_start {start}")
+    if every < 1:
+        raise ValueError(f"--attack_every {every} must be >= 1")
+    if not (math.isfinite(theta) and 0.0 < theta <= 1.0):
+        raise ValueError(f"--lifespan_threshold {theta} must be a finite number in (0, 1]")
+    if theta != LIFESPAN_THRESHOLD and stop == 0:
+        raise ValueError("--lifespan_threshold needs --attack_stop > 0")
+    args.attack_start, args.attack_stop, args.attack_every, args.lifespan_threshold = start, stop, every, theta
+    args.attack_force = bool(getattr(args, "attack_force", False))
+    if attack_schedule_set(args) and args.num_corrupt <= 0:
+        raise ValueError("--attack_start / --attack_stop / --attack_every / --attack_force need corrupt agents (--num_corrupt > 0)")
 
 
 def _finalize_flame(args) -> None:
@@ -316,4 +366,7 @@ def print_exp_details(args) -> None:
         print(f"    FLAME lambda: {args.flame_lambda}")
     if getattr(args, "attack_boost", 1.0) != 1.0 or getattr(args, "attack_neurotoxin", 0.0) > 0:
         print(f"    Attack (boost / neurotoxin): {args.attack_boost} / {args.attack_neurotoxin}")
+    if attack_schedule_set(args):
+        print(f"    Attack schedule (start / stop / every / force): {args.attack_start} / {args.attack_stop} / {args.attack_every} / "
+              f"{args.attack_force}")
     print("======================================")

@@ -1,5 +1,5 @@
 """Evaluation, logging, timing, checkpointing (SURVEY.md section 5 auxiliary subsystems)."""
-from .evaluate import get_loss_n_accuracy
+from .evaluate import backdoor_lifespan, get_loss_n_accuracy
 from .logging import MetricLogger
 from .timers import PhaseTimer
 from .checkpoint import save_checkpoint, load_checkpoint, restore_server_opt
@@ -19,4 +19,4 @@ def __getattr__(name):
     raise AttributeError(name)
 
 
-__all__ = ["get_loss_n_accuracy", "MetricLogger", "PhaseTimer", "save_checkpoint", "load_checkpoint", "restore_server_opt"]
+__all__ = ["backdoor_lifespan", "get_loss_n_accuracy", "MetricLogger", "PhaseTimer", "save_checkpoint", "load_checkpoint", "restore_server_opt"]

@@ -39,3 +39,13 @@ def get_loss_n_accuracy(forward, dataset, bs: int = 256, num_classes: int = 10, 
     accuracy = float(conf.diag().sum()) / total
     per_class = conf.diag() / conf.sum(1)  # NaN for absent classes, like the reference's 0/0
     return avg_loss, (accuracy, per_class.float())
+
+
+def backdoor_lifespan(evals, last_attack: int, threshold: float):
+    """Rounds the backdoor outlived the attack: ``r* - last_attack`` for the first evaluated round ``r* >= last_attack`` whose poison
+    accuracy is below ``threshold``, or None if there is none.  ``evals``: ``(round, poison_acc)`` pairs in round order; the resolution
+    is the evaluation interval (``--snap``)."""
+    for rnd, acc in evals:
+        if rnd >= last_attack and acc < threshold:
+            return rnd - last_attack
+    return None

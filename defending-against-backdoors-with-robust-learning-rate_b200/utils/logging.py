@@ -39,7 +39,7 @@ class MetricLogger:
             self.tb.add_scalar(tag, float(value), step)
 
     def record(self, rnd: int, **fields):
-        rec = {"round": rnd, **{k: (float(v) if hasattr(v, "__float__") else v) for k, v in fields.items()}}
+        rec = {"round": rnd, **{k: (float(v) if hasattr(v, "__float__") and not isinstance(v, bool) else v) for k, v in fields.items()}}
         self.history.append(rec)
         if self.jsonl is not None:
             self.jsonl.write(json.dumps(rec) + "\n")

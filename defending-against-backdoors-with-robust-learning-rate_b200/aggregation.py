@@ -11,6 +11,10 @@ that launch too: the Gram matrix of the updates (``ops.pairwise_gram``) gives FL
 noise (``ops.flame_admit``), and the admitted participants' clipped updates are averaged with equal weights.  ``--aggr foolsgold`` keeps
 every agent's summed updates across rounds (``ops.history_accumulate``) and weights the mean by FoolsGold's ``ops.foolsgold_weights`` on
 the Gram matrix of those histories (``ops.history_gram``), so agents that keep pushing the model the same way lose their weight.
+``--detect fldetector`` is a stage ahead of the rule: every round it predicts each agent's update from its last one and an L-BFGS
+Hessian-vector product of the recent global updates (``ops.fld_hvp_coefficients`` on the Gram matrix of the update ring,
+``ops.fld_hvp``), scores the distance to the prediction (``ops.fld_predict``) and, once the gap statistic finds a minority cluster of high
+scores (``ops.fld_detect``), removes those agents from every later round's admission.
 The reference's dead / disabled pieces are available behind flags: ``clip_updates`` (``--server_clip``) and the
 diagnostics ``plot_norms`` / ``comp_diag_fisher`` / ``plot_sign_agreement`` (``--diagnostics``), the latter with the
 reference's latent bugs fixed (model built on the right device; Fisher uses log-probabilities -- SURVEY.md quirk 7).
@@ -29,6 +33,12 @@ def server_opt_spec(args):
     """``ops.ServerOptState`` keyword arguments of the ``--server_opt*`` flags."""
     return dict(kind=getattr(args, "server_opt", "sgd"), beta1=getattr(args, "server_beta1", 0.9),
                 beta2=getattr(args, "server_beta2", 0.99), tau=getattr(args, "server_tau", 1e-3))
+
+
+# TensorBoard tags of FLDetector's record fields (a list of flagged ids is logged as its length)
+_FLD_TAGS = {"fld_avg_honest_score": "FLDetector/Avg_Honest_Score", "fld_avg_corrupt_score": "FLDetector/Avg_Corrupt_Score",
+             "fld_clusters": "FLDetector/Clusters", "fld_fallback": "FLDetector/Fallback", "fld_flagged": "FLDetector/Flagged",
+             "fld_corrupt_flagged": "FLDetector/Corrupt_Flagged", "fld_excluded": "FLDetector/Excluded"}
 
 
 class Aggregation:
@@ -51,6 +61,14 @@ class Aggregation:
         self.last_foolsgold = None    # the FoolsGold/* scalars of the last round (--aggr foolsgold)
         self.history = None           # [num_agents][n_vote] FoolsGold histories of the in-process form (allocated on first use)
         self.opt = None               # full-length server optimizer state of the in-process form (allocated on first use)
+        # FLDetector (--detect fldetector): host state identical on every rank, and the in-process form's tables (allocated on first use)
+        self.last_fld = None          # the fld_* record fields of the last round
+        self.fld_count = 0            # valid ring rows (at most N + 1)
+        self.fld_pos = 0              # the ring row the next global update goes to (the oldest one once the ring is full)
+        self.fld_window = []          # the last N round scores, oldest first: float64 [num_agents] each
+        self.fld_flagged = []         # agent ids flagged at detection (ascending)
+        self.fld_detect_round = None  # the round of the detection, None until then
+        self.fld_tables = None        # (table [num_agents][n_vote], ring [N + 1][n_vote], w_prev [n_vote]) of the in-process form
 
     # ---- the server step ------------------------------------------------------------------------------------
     def aggregate_updates(self, w_global, agent_params, cur_round, n_vote=None, root_params=None):
@@ -69,7 +87,8 @@ class Aggregation:
             [ws[j] for j in members], b, nv, w_global if clip is not None else None,
             clip[torch.as_tensor(members, device=clip.device)] if clip is not None else None)
         gram = lambda members: ops.pairwise_gram([ws[j] for j in members], w_global, nv)
-        keep, weights, scales, total, noise_std = self._admission(ids, clip, distances,
+        detection = lambda: self._fld_stage(ids, cur_round, *self._fld_local(w_global, ws, ids, nv))
+        keep, weights, scales, total, noise_std = self._admission(ids, clip, detection, distances,
                                                                   lambda: ops.trust_stats(ws, root_params, w_global, nv), rfa_pass, gram,
                                                                   lambda members: self._history_pass(w_global, ws, ids, members, nv),
                                                                   cur_round)
@@ -98,12 +117,16 @@ class Aggregation:
         norms = self.fused.update_norms(K) if self._server_clip or diag else None
         clip = self._clip_scales(norms) if self._server_clip else None
         copies, gathered = None, None
-        if (self._select or self._fltrust or self._flame or self._foolsgold or (self._rfa and self.args.rfa_iters > 0)) and self.fused.gathers(K):
+        if (self._select or self._fltrust or self._flame or self._foolsgold or self._detecting or (self._rfa and self.args.rfa_iters > 0)) \
+                and self.fused.gathers(K):
             # on the gather transport every pass reads the same all-gathered copies (one all_gather per round; the root job included)
             gathered = self.fused.gather_participants(K + 1 if self._fltrust else K)
             copies = gathered[:K]
+        fused = self.fused
+        detection = lambda: self._fld_stage(participants, cur_round, fused.fld_ring_update, fused.fld_gram,
+                                            lambda order, coef: fused.fld_predict(K, participants, order, coef, copies))
         keep, weights, scales, total, noise_std = self._admission(
-            participants, clip, lambda: self.fused.pairwise_sqdist(K, clip, copies), lambda: self.fused.trust_stats(K, K, gathered),
+            participants, clip, detection, lambda: self.fused.pairwise_sqdist(K, clip, copies), lambda: self.fused.trust_stats(K, K, gathered),
             lambda b, members: self.fused.rfa_sqdist(K, b, clip, members, copies),
             lambda members: self.fused.pairwise_gram(K, members, copies),
             lambda members: self.fused.foolsgold_gram(K, participants, members, copies), cur_round)
@@ -128,14 +151,15 @@ class Aggregation:
     def _select(self):
         return getattr(self.args, "select", "none") != "none"
 
-    def _admission(self, ids, clip, distances, trust_stats, rfa_pass, gram, history, cur_round):
-        """Admission of the participants ``ids`` shared by both forms of the step: Krum / Multi-Krum on ``distances()`` (``--select``),
+    def _admission(self, ids, clip, detection, distances, trust_stats, rfa_pass, gram, history, cur_round):
+        """Admission of the participants ``ids`` shared by both forms of the step: FLDetector's ``detection()`` (``--detect``), which returns
+        the positions of the agents it has not flagged (None while it has flagged nobody), or Krum / Multi-Krum on ``distances()`` (``--select``),
         then FLTrust on ``trust_stats()`` (``--aggr fltrust``), RFA's weights from ``rfa_pass(b, members)`` (``--aggr rfa``), FLAME on
         the Gram matrix ``gram(members)`` (``--aggr flame``) or FoolsGold on ``history(members)``, the Gram matrix of the members' update
         histories after this round's updates are folded in (``--aggr foolsgold``).  ``clip``: the server-clipping scales or None.  Returns
         ``(members, weights, scales, total_weight, noise_std)`` for the step: members None admits everyone; weights are per position in
         ``ids``."""
-        keep = self._admit(distances(), ids, cur_round) if self._select else None
+        keep = self._admit(distances(), ids, cur_round) if self._select else (detection() if self._detect else None)
         noise_std = self.args.noise * self.args.clip
         if self._fltrust:
             return (*self._trust(trust_stats(), ids, keep, cur_round), noise_std)
@@ -148,6 +172,100 @@ class Aggregation:
         if self._rfa:
             return (*self._rfa_weights(ids, keep, weights, clip, rfa_pass, cur_round), noise_std)
         return keep, weights, clip, None, noise_std
+
+    @property
+    def _detect(self):
+        return getattr(self.args, "detect", "none") == "fldetector"
+
+    @property
+    def _detecting(self):
+        """True while the FLDetector pass runs: from the first round until the detection."""
+        return self._detect and self.fld_detect_round is None
+
+    def _fld_local(self, w_global, ws, ids, nv):
+        """The ring, Gram and prediction passes of the in-process form, on full tables kept here (zero at the start)."""
+        nv = w_global.numel() if nv is None else int(nv)
+        if self.fld_tables is None:
+            z = lambda *shape: torch.zeros(shape, dtype=torch.float32, device=w_global.device)
+            self.fld_tables = (z(self.args.num_agents, nv), z(self.args.fld_window + 1, nv), z(nv))
+        table, ring, w_prev = self.fld_tables
+
+        def predict(order, coef):
+            hv = ops.fld_hvp([ring[i] for i in order], coef, 0, nv) if coef is not None else None
+            return ops.fld_predict([table[i] for i in ids], ws, w_global, hv, 0, nv)
+        return (lambda row: ops.fld_ring(w_global, w_prev, None if row is None else ring[row], 0, nv),
+                lambda order: ops.history_gram([ring[i] for i in order], nv), predict)
+
+    def _fld_stage(self, ids, cur_round, ring, gram, predict):
+        """FLDetector ahead of the rule (DESIGN.md section 3), over the participants ``ids`` (every agent: all take part in every round).
+        Until the detection: ``ring(row)`` writes the round's global update into ring row ``row`` (None in round 1: only w_prev), from round
+        N + 2 on ``gram(order)`` gives the ring's Gram matrix, ``ops.fld_hvp_coefficients`` the Hessian-vector product and ``predict(order,
+        coef)`` the squared distances to the predictions (``predict(None, None)`` before: record only); the round scores enter the window
+        and from round max(R, 2N + 1) on ``ops.fld_detect`` decides.  Returns the positions of the agents not flagged, or None while nobody
+        is flagged.  Records ``last_fld`` and logs it."""
+        a = self.args
+        N, nc = a.fld_window, a.num_corrupt
+        rec = {}
+        if self.fld_detect_round is None:
+            if cur_round >= 2:
+                ring(self.fld_pos)
+                self.fld_pos = (self.fld_pos + 1) % (N + 1)
+                self.fld_count = min(N + 1, self.fld_count + 1)
+            else:
+                ring(None)
+            if cur_round >= N + 2:
+                if self.fld_count != N + 1:
+                    raise ValueError(f"FLDetector: round {cur_round} with {self.fld_count} of {N + 1} ring rows")
+                order = [(self.fld_pos + i) % (N + 1) for i in range(N + 1)]       # oldest first: pos is the next row to overwrite
+                coef = ops.fld_hvp_coefficients(gram(order))
+                d = np.sqrt(np.maximum(predict(order, coef).double().cpu().numpy(), 0.0))
+                tot = float(d.sum())
+                score = np.zeros(a.num_agents, dtype=np.float64)
+                score[np.asarray(ids, dtype=np.int64)] = d / tot if tot > 0 else 0.0
+                self.fld_window = (self.fld_window + [score])[-N:]
+                rec["fld_fallback"] = int(not np.any(coef))
+            else:
+                predict(None, None)
+            if len(self.fld_window) == N:
+                sus = self.fld_window[0].copy()
+                for w in self.fld_window[1:]:
+                    sus = sus + w
+                sus = sus / N
+                cand = sorted(int(i) for i in ids)
+                honest, corrupt = [sus[i] for i in cand if i >= nc], [sus[i] for i in cand if i < nc]
+                rec["fld_avg_honest_score"] = float(np.mean(honest)) if honest else None
+                rec["fld_avg_corrupt_score"] = float(np.mean(corrupt)) if corrupt else None
+                if cur_round >= max(a.fld_start, 2 * N + 1):
+                    flagged, khat = ops.fld_detect(sus[cand], a.seed, cur_round)
+                    rec["fld_clusters"] = khat
+                    if flagged:
+                        self.fld_flagged = [cand[j] for j in flagged]
+                        self.fld_detect_round = cur_round
+                        rec["fld_flagged"] = list(self.fld_flagged)
+                        rec["fld_corrupt_flagged"] = sum(1 for i in self.fld_flagged if i < nc)
+                        rec["fld_detect_round"] = cur_round
+        keep = None
+        if self.fld_flagged:
+            out = set(self.fld_flagged)
+            keep = [j for j, i in enumerate(ids) if int(i) not in out]
+            rec["fld_excluded"] = len(ids) - len(keep)
+        self.last_fld = rec
+        if self.writer is not None:
+            for k, v in rec.items():
+                if k in _FLD_TAGS and v is not None:
+                    self.writer.add_scalar(_FLD_TAGS[k], len(v) if isinstance(v, list) else v, cur_round)
+        return keep
+
+    def fld_state(self):
+        """FLDetector's host state, as a checkpoint carries it."""
+        return {"count": self.fld_count, "pos": self.fld_pos, "window": [torch.from_numpy(w.copy()) for w in self.fld_window],
+                "flagged": list(self.fld_flagged), "detect_round": self.fld_detect_round}
+
+    def load_fld_state(self, st):
+        self.fld_count, self.fld_pos = int(st["count"]), int(st["pos"])
+        self.fld_window = [w.double().numpy().copy() for w in st["window"]]
+        self.fld_flagged = [int(i) for i in st["flagged"]]
+        self.fld_detect_round = st["detect_round"]
 
     def _admit(self, D, ids, cur_round):
         """Krum / Multi-Krum admission from the pairwise distances ``D`` of the participants ``ids``: the admitted positions

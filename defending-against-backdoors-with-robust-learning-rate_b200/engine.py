@@ -120,6 +120,7 @@ class FLEngine:
             root = draw_root_set(len(self.train_dataset), poisoned, args.root_size, args.seed)
             self.root_agent = Agent(args.num_agents, args, self.train_dataset, root.tolist(), seed=args.seed)
         self.n_part = max(1, math.floor(args.num_agents * args.agent_frac))
+        self.detect = getattr(args, "detect", "none") == "fldetector"
         n_jobs = self.n_part + (1 if self.root_agent is not None else 0)   # the root job is position n_part of every round
         max_slots = (n_jobs + ctx.world - 1) // ctx.world
         max_shard = max(a.n_data for a in self._jobs())
@@ -132,7 +133,8 @@ class FLEngine:
             backend = "gloo"
         self.fused = FusedAggregator(ctx, self.layout.n_total, self.layout.n_vote, max_slots, backend,
                                      transport=getattr(args, "agg_transport", "auto"), server_opt=server_opt_spec(args),
-                                     n_part=self.n_part, history_agents=args.num_agents if args.aggr == "foolsgold" else 0)
+                                     n_part=self.n_part, history_agents=args.num_agents if args.aggr == "foolsgold" else 0,
+                                     fld_agents=args.num_agents if self.detect else 0, fld_window=args.fld_window if self.detect else 0)
         init = torch.zeros(self.layout.n_total, dtype=torch.float32)
         self.layout.init_(init, args.seed)
         self.fused.w_global.copy_(init.to(dev))
@@ -208,6 +210,12 @@ class FLEngine:
                 if hist is None:
                     raise ValueError("checkpoint has no FoolsGold history, but this run uses --aggr foolsgold")
                 self.fused.load_foolsgold_history(hist)
+            if self.detect:
+                fld = ck["extra"].get("fldetector")
+                if fld is None:
+                    raise ValueError("checkpoint has no FLDetector state, but this run uses --detect fldetector")
+                self.fused.load_fld_tables(fld["table"], fld["ring"], fld["w_prev"])
+                self.aggregator.load_fld_state(fld)
         ctx.barrier()
 
     def _build_swaps(self):
@@ -493,6 +501,10 @@ class FLEngine:
                 rec["foolsgold_avg_honest"] = self.aggregator.last_foolsgold["FoolsGold/Avg_Honest_Weight"]
                 rec["foolsgold_avg_corrupt"] = self.aggregator.last_foolsgold["FoolsGold/Avg_Corrupt_Weight"]
                 rec["foolsgold_admitted"] = self.aggregator.last_foolsgold["FoolsGold/Admitted"]
+            if self.detect and self.aggregator.last_fld is not None:
+                rec.update(self.aggregator.last_fld)
+                if "fld_flagged" in rec and self.verbose:
+                    print(f"| FLDetector: flagged {rec['fld_flagged']} in round {rnd} ({rec['fld_corrupt_flagged']} corrupt) |")
             rec.update({f"ms_{k}": v for k, v in self.timer.elapsed().items()})
             if args.profile_phases and self.verbose:
                 print({k: round(v, 3) for k, v in rec.items() if k.startswith("ms_")})
@@ -501,6 +513,7 @@ class FLEngine:
             if args.checkpoint and ((args.ckpt_every and rnd % args.ckpt_every == 0) or rnd == rounds):
                 state = self.fused.server_opt_state()      # every rank takes part: each holds one slice on the fused multi-GPU path
                 hist = self.fused.foolsgold_history() if self.fused.history is not None else None      # collective, likewise
+                fld = self.fused.fld_tables() if self.detect else None                                    # collective, likewise
                 if self.ctx.is_main:
                     so = None if state is None else {**self.fused.opt.hparams, "m": state[0], "v": state[1]}
                     extra = {"cum_poison_acc_mean": self.cum_poison_acc_mean}
@@ -508,6 +521,8 @@ class FLEngine:
                         extra["neurotoxin_w_prev"] = self.w_prev.cpu()
                     if hist is not None:
                         extra["foolsgold_history"] = hist
+                    if fld is not None:
+                        extra["fldetector"] = {"table": fld[0], "ring": fld[1], "w_prev": fld[2], **self.aggregator.fld_state()}
                     if self.last_attack is not None:
                         extra["backdoor_lifespan"] = self.backdoor_lifespan
                     save_checkpoint(args.checkpoint, self.global_params(), rnd, args, self.layout, extra, so)

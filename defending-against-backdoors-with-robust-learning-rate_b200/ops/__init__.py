@@ -926,6 +926,213 @@ def foolsgold_weights(G):
 
 
 # =====================================================================================================================
+# FLDetector (Zhang, Cao, Jia, Gong, KDD 2022): predicted updates and the detection of agents far from their predictions
+# =====================================================================================================================
+FLD_REF_SETS = 10                        # B: uniform reference sets of the gap statistic
+FLD_MAX_CLUSTERS = 10                    # the gap statistic tries k = 1 .. min(10, n - 1)
+_FLD_GAP_TAG = 0x464C4447                # "FLDG": keeps the reference-set draws apart from every other stream seeded by --seed
+
+
+def fld_ring_statement(w_g, w_prev, lo, hi):
+    """fp32 statement of the ring pass over ``[lo, hi)``: the global update ``fp32(w_g[c] - w_prev[c])``."""
+    return w_g[lo:hi].float() - w_prev[lo:hi].float()
+
+
+def fld_ring(w_g, w_prev, s=None, lo=0, hi=None):
+    """``s[lo:hi] <- fp32(w_g - w_prev)`` (skipped when ``s`` is None), then ``w_prev[lo:hi] <- w_g[lo:hi]``, in place.  ``w_prev`` and ``s``
+    are indexed by absolute coordinate.  On CUDA this launches ``fld_ring_kernel`` (ops/csrc/fldetector.cu); on CPU it evaluates the
+    statement."""
+    hi = w_prev.numel() if hi is None else int(hi)
+    lo = int(lo)
+    if not w_g.is_cuda:
+        if s is not None:
+            s[lo:hi].copy_(fld_ring_statement(w_g, w_prev, lo, hi))
+        w_prev[lo:hi].copy_(w_g[lo:hi])
+        return
+    for t in (w_g, w_prev) + ((s,) if s is not None else ()):
+        assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.numel() >= hi
+    ext().fld_ring(w_g.data_ptr(), w_prev.data_ptr(), s.data_ptr() if s is not None else 0, lo, hi)
+
+
+def fld_hvp_statement(ring, coef, lo, hi):
+    """Statement of the Hessian-vector product over ``[lo, hi)``: ``fp32(sum_i coef[i] * ring[i][c])`` with the sum in fp64 over the ring
+    rows in the order given (chronological), every product and addition rounded on its own, and one rounding to fp32 at the end.  These
+    bits are specified exactly.  Returns float32 ``[hi - lo]``."""
+    acc = torch.zeros(hi - lo, dtype=torch.float64, device=ring[0].device)
+    for c, s in zip(np.asarray(coef, dtype=np.float64).tolist(), ring):
+        acc = acc + c * s[lo:hi].double()
+    return acc.float()
+
+
+def fld_hvp(ring, coef, lo=0, hi=None):
+    """The Hessian-vector product ``Hv`` over ``[lo, hi)`` of the ring rows ``ring`` (chronological, indexed by absolute coordinate) with
+    the coefficients ``coef`` of ``fld_hvp_coefficients``: float32 ``[hi - lo]``, bit for bit ``fld_hvp_statement``.  On CUDA this
+    launches ``fld_hvp_kernel``; on CPU it evaluates the statement."""
+    hi = ring[0].numel() if hi is None else int(hi)
+    lo = int(lo)
+    if not ring[0].is_cuda:
+        return fld_hvp_statement(ring, coef, lo, hi)
+    dev = ring[0].device
+    for t in ring:
+        assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.numel() >= hi
+    hv = torch.empty(hi - lo, dtype=torch.float32, device=dev)
+    tab = PtrTable([t.data_ptr() for t in ring], dev, ring)
+    ext().fld_hvp(tab.tensor, torch.as_tensor(np.asarray(coef, dtype=np.float64)).to(dev), hv.data_ptr() - 4 * lo, lo, hi)
+    return hv
+
+
+def fld_predict_statement(rows, w_agents, w_global, hv, lo, hi):
+    """Statement of the prediction pass over ``[lo, hi)``: for candidate k the update ``u_k = fp32(w_k - w_global)``, and with ``hv``
+    (``[hi - lo]``) the squared distance ``d_k^2 = sum_c fp32(fp32(rows[k][c] + hv[c]) - u_k[c])^2`` in fp64.  ``rows[k]`` is the
+    candidate's last-update row, indexed by absolute coordinate.  Returns ``(new row slices u_k, float64 d^2 [K] or None)``."""
+    g = w_global[lo:hi].float()
+    us = [w[lo:hi].float() - g for w in w_agents]
+    if hv is None:
+        return us, None
+    d2 = torch.stack([(((h[lo:hi].float() + hv) - u).double() ** 2).sum() for h, u in zip(rows, us)])
+    return us, d2
+
+
+def fld_predict(rows, w_agents, w_global, hv=None, lo=0, hi=None):
+    """The prediction pass: with ``hv`` (``fld_hvp``'s ``[hi - lo]`` vector) return each candidate's fp64 squared distance to its
+    prediction ``rows[k] + hv`` over ``[lo, hi)``; with or without it, then record ``rows[k][lo:hi] <- fp32(w_k - w_global)`` in place.
+    Without ``hv`` it returns None.  On CUDA this launches ``fld_predict_kernel`` (``<true>`` with ``hv``, ``<false>`` without); on CPU,
+    and for more candidates than the kernels' tables hold (recorded as a library fall-through), it evaluates ``fld_predict_statement``."""
+    hi = rows[0].numel() if hi is None else int(hi)
+    lo = int(lo)
+    K = len(rows)
+
+    def statement():
+        us, d2 = fld_predict_statement(rows, w_agents, w_global, hv, lo, hi)
+        for h, u in zip(rows, us):
+            h[lo:hi].copy_(u)
+        return d2 if d2 is not None else torch.zeros(K, dtype=torch.float64, device=rows[0].device)
+
+    def launch(tab, out):
+        dev = w_global.device
+        rt = PtrTable([h.data_ptr() for h in rows], dev, rows)
+        ext().fld_predict(tab, rt.tensor, w_global.data_ptr(), hv.data_ptr() - 4 * lo if hv is not None else 0, lo, hi,
+                          out if hv is not None else None, None, None, 0, 1, 0)
+        if hv is None:
+            out.zero_()
+
+    d2 = _participant_pass("fld_predict", list(w_agents), (w_global, *rows), hi, (K,), statement, launch)
+    return d2 if hv is not None else None
+
+
+def fld_hvp_coefficients(G):
+    """L-BFGS Hessian-vector product of FLDetector on the host, in fp64: ``G`` is the ``(N + 1) x (N + 1)`` Gram matrix of the ring
+    ``s_{r-N} .. s_r`` (chronological).  With ``S = [s_{r-N} .. s_{r-1}]``, ``Y = [y_i = s_{i+1} - s_i]``, ``v = s_r``,
+    ``sigma = y_{r-1}.s_{r-1} / s_{r-1}.s_{r-1}``, ``L`` the strictly lower triangle of ``S^T Y`` and ``D = diag(S^T Y)``, it solves
+    ``[[sigma S^T S, L], [L^T, -D]] q = [sigma S^T v; Y^T v]`` and writes ``Bv = sigma v - sigma S q1 - Y q2`` as ``sum_i c_i s_i``.
+    Returns ``c`` (float64 numpy ``[N + 1]``).  Fallback -- ``s_{r-1}.s_{r-1} = 0``, a singular system or anything non-finite -- gives
+    ``c = 0`` (the prediction is the last update); an all-zero ``c`` marks it."""
+    g = np.asarray(torch.as_tensor(G).detach().double().cpu().numpy(), dtype=np.float64)
+    n1 = g.shape[0]
+    if g.ndim != 2 or g.shape != (n1, n1) or n1 < 2:
+        raise ValueError(f"fld_hvp_coefficients: a {g.shape} Gram matrix (need (N + 1) x (N + 1), N >= 1)")
+    N = n1 - 1
+    zero = np.zeros(n1, dtype=np.float64)
+    A_S = np.eye(n1, N)                                       # S = R A_S over the ring basis R
+    A_Y = np.eye(n1, N, -1) - np.eye(n1, N)                   # y_i = s_{i+1} - s_i
+    e_v = np.eye(n1)[:, N]
+    with np.errstate(all="ignore"):
+        StS, StY = A_S.T @ g @ A_S, A_S.T @ g @ A_Y
+        Stv, Ytv = A_S.T @ g @ e_v, A_Y.T @ g @ e_v
+        ss = StS[N - 1, N - 1]
+        if not np.all(np.isfinite(g)) or not ss != 0:
+            return zero
+        sigma = StY[N - 1, N - 1] / ss
+        L, D = np.tril(StY, -1), np.diag(np.diag(StY))
+        M = np.block([[sigma * StS, L], [L.T, -D]])
+        try:
+            q = np.linalg.solve(M, np.concatenate([sigma * Stv, Ytv]))
+        except np.linalg.LinAlgError:
+            return zero
+        c = sigma * e_v - sigma * (A_S @ q[:N]) - A_Y @ q[N:]
+    return c if np.all(np.isfinite(c)) and np.isfinite(sigma) else zero
+
+
+def fld_kmeans_sse(x, kmax):
+    """Exact 1-D k-means: the least within-cluster sum of squares ``W_k`` of the sorted values ``x`` in ``k = 1 .. kmax`` contiguous
+    groups, by dynamic programming over split points (deterministic; no k-means++).  A group whose values are all equal costs exactly 0.
+    Returns float64 ``[kmax]`` (``W_1 .. W_kmax``)."""
+    x = np.asarray(x, dtype=np.float64)
+    n = x.size
+    p1 = np.concatenate([[0.0], np.cumsum(x)])
+    p2 = np.concatenate([[0.0], np.cumsum(x * x)])
+
+    def cost(a, b):                          # SSE of x[a:b] for arrays of a (b fixed), b > a
+        m = b - a
+        c = (p2[b] - p2[a]) - (p1[b] - p1[a]) ** 2 / m
+        return np.where(x[a] == x[b - 1], 0.0, np.maximum(c, 0.0))
+
+    W = np.empty(kmax, dtype=np.float64)
+    prev = np.array([cost(np.array([0]), b)[0] for b in range(1, n + 1)])     # prev[b - 1] = W_1 of x[:b]
+    W[0] = prev[n - 1]
+    for k in range(2, kmax + 1):
+        cur = np.full(n, np.inf)
+        for b in range(k, n + 1):
+            a = np.arange(k - 1, b)          # the last group is x[a:b], the first a values form k - 1 groups
+            cur[b - 1] = np.min(prev[a - 1] + cost(a, b))
+        prev = cur
+        W[k - 1] = prev[n - 1]
+    return W
+
+
+def fld_two_means(x):
+    """The optimal split of the sorted values ``x`` (n >= 2) into two contiguous groups by exact 2-means: the index ``i`` in ``[1, n)``
+    that minimises ``SSE(x[:i]) + SSE(x[i:])``, the lowest one on a tie."""
+    x = np.asarray(x, dtype=np.float64)
+    n = x.size
+    sse = [float(np.sum((x[:i] - x[:i].mean()) ** 2) + np.sum((x[i:] - x[i:].mean()) ** 2)) for i in range(1, n)]
+    return 1 + int(np.argmin(sse))
+
+
+def fld_gap_clusters(z, seed, rnd):
+    """FLDetector's gap statistic on the values ``z`` in [0, 1]: ``W_k`` the exact 1-D k-means SSE, ``k = 1 .. K_max = min(10, n - 1)``,
+    B = 10 uniform reference sets of n points in [0, 1] from a numpy Generator seeded by (seed, round) alone, ``Gap(k) = mean_b log W_kb -
+    log W_k`` and ``sd_k = std_b(log W_kb) sqrt(1 + 1/B)`` (a zero W counts as the smallest positive double).  Returns the smallest
+    ``k < K_max`` with ``Gap(k) >= Gap(k + 1) - sd_{k + 1}``, else ``K_max``."""
+    z = np.sort(np.asarray(z, dtype=np.float64))
+    n = z.size
+    kmax = min(FLD_MAX_CLUSTERS, n - 1)
+    if kmax < 1:
+        return 1
+    tiny = np.nextafter(0.0, 1.0)
+    logw = np.log(np.maximum(fld_kmeans_sse(z, kmax), tiny))
+    ref = np.random.default_rng([int(seed), int(rnd), _FLD_GAP_TAG]).random((FLD_REF_SETS, n))
+    logr = np.stack([np.log(np.maximum(fld_kmeans_sse(np.sort(r), kmax), tiny)) for r in ref])
+    gap = logr.mean(axis=0) - logw
+    sd = logr.std(axis=0) * math.sqrt(1.0 + 1.0 / FLD_REF_SETS)
+    for k in range(1, kmax):
+        if gap[k - 1] >= gap[k] - sd[k]:
+            return k
+    return kmax
+
+
+def fld_detect(scores, seed, rnd):
+    """FLDetector's decision on the host, shared by every form of the server step: ``scores`` are the candidates' suspicious scores.
+    They are min-max normalised to z (all equal: no attack); when the gap statistic (``fld_gap_clusters``) finds more than one cluster,
+    sorted z is split by exact 2-means (``fld_two_means``) and the upper group is flagged if it holds fewer than half of the candidates.
+    Returns ``(flagged positions in scores, ascending; k_hat)``."""
+    s = np.asarray(scores, dtype=np.float64)
+    n = s.size
+    if n == 0 or not np.all(np.isfinite(s)) or s.max() == s.min():
+        return [], 1
+    z = (s - s.min()) / (s.max() - s.min())
+    khat = fld_gap_clusters(z, seed, rnd)
+    if khat <= 1:
+        return [], khat
+    order = np.argsort(z, kind="stable")
+    i = fld_two_means(z[order])
+    upper = order[i:]
+    if 2 * upper.size >= n:
+        return [], khat
+    return sorted(int(j) for j in upper), khat
+
+
+# =====================================================================================================================
 # model-poisoning attackers (DESIGN.md section 3)
 # =====================================================================================================================
 def mask_words(n: int) -> int:

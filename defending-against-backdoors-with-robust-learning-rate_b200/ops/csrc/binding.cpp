@@ -169,6 +169,53 @@ void history_gram(at::Tensor row_ptrs, int64_t begin, int64_t end, at::Tensor ou
     check(rlr::launch_history_gram(p, out.data_ptr<double>(), num_sms(), cur_stream()), "history_gram");
 }
 
+// FLDetector ring pass over [begin, end): s_ptr (0 = none) <- w_g - w_prev, then w_prev <- w_g.  Pointers offset so that absolute
+// coordinates index them.
+void fld_ring(int64_t w_g_ptr, int64_t w_prev_ptr, int64_t s_ptr, int64_t begin, int64_t end) {
+    TORCH_CHECK(w_g_ptr && w_prev_ptr, "fld_ring needs w_g and w_prev");
+    check(rlr::launch_fld_ring(reinterpret_cast<const float*>(w_g_ptr), reinterpret_cast<float*>(w_prev_ptr), reinterpret_cast<float*>(s_ptr),
+                               begin, end, num_sms(), cur_stream()), "fld_ring");
+}
+
+// FLDetector Hessian-vector product over [begin, end): hv_ptr <- fp32(sum_r coef[r] ring_ptrs[r]) (offset pointers).
+void fld_hvp(at::Tensor ring_ptrs, at::Tensor coef, int64_t hv_ptr, int64_t begin, int64_t end) {
+    CHECK_CUDA(ring_ptrs); CHECK_CUDA(coef);
+    TORCH_CHECK(ring_ptrs.scalar_type() == at::kLong, "pointer table must be int64");
+    TORCH_CHECK(coef.scalar_type() == at::kDouble && coef.numel() == ring_ptrs.numel(), "coef must be float64, one per ring row");
+    TORCH_CHECK(hv_ptr, "fld_hvp needs an output");
+    c10::cuda::CUDAGuard guard(coef.device());
+    check(rlr::launch_fld_hvp(reinterpret_cast<const float* const*>(ring_ptrs.data_ptr()), coef.data_ptr<double>(), (int)coef.numel(),
+                              reinterpret_cast<float*>(hv_ptr), begin, end, num_sms(), cur_stream()), "fld_hvp");
+}
+
+// FLDetector prediction pass over [begin, end): hv_ptr != 0 predicts (out: float64 [K] squared distances) and records, hv_ptr = 0 only
+// records u_k into the rows (out ignored).  world > 1: the fused multi-GPU form, which first runs the aggregation's barrier-in at `epoch`.
+void fld_predict(at::Tensor w_agent_ptrs, at::Tensor row_ptrs, int64_t w_global_ptr, int64_t hv_ptr, int64_t begin, int64_t end,
+                 c10::optional<at::Tensor> out, c10::optional<at::Tensor> flag_ptrs, c10::optional<at::Tensor> local_sync, int64_t rank,
+                 int64_t world, int64_t epoch) {
+    CHECK_CUDA(w_agent_ptrs); CHECK_CUDA(row_ptrs);
+    TORCH_CHECK(w_agent_ptrs.scalar_type() == at::kLong && row_ptrs.scalar_type() == at::kLong, "pointer tables must be int64");
+    TORCH_CHECK(row_ptrs.numel() == w_agent_ptrs.numel(), "one last-update row per candidate");
+    TORCH_CHECK(w_global_ptr, "fld_predict needs w_global");
+    double* o = nullptr;
+    if (hv_ptr) {
+        TORCH_CHECK(out.has_value() && out->defined(), "a prediction pass needs out");
+        CHECK_CUDA(*out);
+        TORCH_CHECK(out->scalar_type() == at::kDouble && out->numel() == w_agent_ptrs.numel(), "out must be a float64 [K] tensor");
+        o = out->data_ptr<double>();
+    }
+    c10::cuda::CUDAGuard guard(w_agent_ptrs.device());
+    rlr::FldParams p{};
+    p.w_agents = reinterpret_cast<const float* const*>(w_agent_ptrs.data_ptr());
+    p.rows = reinterpret_cast<float* const*>(row_ptrs.data_ptr());
+    p.w_global = reinterpret_cast<const float*>(w_global_ptr);
+    p.hv = reinterpret_cast<const float*>(hv_ptr);
+    p.begin = begin; p.end = end;
+    p.K = (int)w_agent_ptrs.numel();
+    p.gate = gate_of(flag_ptrs, local_sync, rank, world, epoch);
+    check(rlr::launch_fld_predict(p, o, num_sms(), cur_stream()), "fld_predict");
+}
+
 // FLTrust statistics over coordinates [begin, end): fp64 [2K + 1] = (Δk.Δ0 for every k, |Δk|^2 for every k, |Δ0|^2), Δk = w_k - w_global,
 // Δ0 = w_ref - w_global.  world > 1: the fused multi-GPU form, which first runs the aggregation's barrier-in at `epoch`.
 void trust_stats(at::Tensor w_agent_ptrs, int64_t w_ref_ptr, int64_t w_global_ptr, int64_t begin, int64_t end, at::Tensor out,
@@ -477,6 +524,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("pairwise_gram", &pairwise_gram);
     m.def("history_accumulate", &history_accumulate);
     m.def("history_gram", &history_gram);
+    m.def("fld_ring", &fld_ring);
+    m.def("fld_hvp", &fld_hvp);
+    m.def("fld_predict", &fld_predict);
     m.def("trust_stats", &trust_stats);
     m.def("rfa_sqdist", &rfa_sqdist);
     m.def("gather_normalize", &gather_normalize);

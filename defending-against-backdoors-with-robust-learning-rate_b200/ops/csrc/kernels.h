@@ -82,6 +82,26 @@ struct HistParams {
 };
 cudaError_t launch_history_accumulate(const HistParams& p, int num_sms, cudaStream_t st);
 
+// ---- FLDetector (fldetector.cu): the global-update ring, the Hessian-vector product and the prediction pass --------------------------
+// ring: s[c] = fp32(w_g[c] - w_prev[c]) (s may be null), then w_prev[c] <- w_g[c], over [begin, end); w_prev and s offset so that absolute
+// coordinates index them.
+cudaError_t launch_fld_ring(const float* w_g, float* w_prev, float* s, long long begin, long long end, int num_sms, cudaStream_t st);
+// Hv[c] = fp32(sum_{r < rows} coef[r] * ring[r][c]), fp64 products and sums each rounded on their own, r ascending.
+cudaError_t launch_fld_hvp(const float* const* ring, const double* coef, int rows, float* hv, long long begin, long long end, int num_sms,
+                           cudaStream_t st);
+// per candidate k over [begin, end): u = fp32(w_agents[k][c] - w_global[c]); with hv: out[k] = sum_c fp32(fp32(rows[k][c] + hv[c]) - u)^2
+// in fp64 (fixed-order sums); then rows[k][c] <- u.  Without hv only the rows are written (out untouched, may be null).
+struct FldParams {
+    const float* const* w_agents;   // [K] device pointers (local or peer-mapped)
+    float* const* rows;             // [K] last-update rows, offset so that absolute coordinates index them
+    const float* w_global;          // this rank's global parameters
+    const float* hv;                // Hv, offset so that absolute coordinates index it, or nullptr (record only)
+    long long begin, end;           // coordinate range (multiples of 4), already clipped to [0, n_vote)
+    int K;
+    Gate gate;                      // world > 1: the aggregation's barrier-in
+};
+cudaError_t launch_fld_predict(const FldParams& p, double* out, int num_sms, cudaStream_t st);
+
 // ---- FLTrust: each participant's update against the server's root update Δ0 = w_ref - w_global -----------------------------------------
 // out[k] = sum_c Δk[c] Δ0[c], out[K + k] = sum_c Δk[c]^2, out[2K] = sum_c Δ0[c]^2 over [begin, end), fp64 [2K + 1], Δk = w_k - w_global.
 // Fixed-order sums, no atomics: bitwise reproducible.

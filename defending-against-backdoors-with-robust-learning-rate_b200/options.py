@@ -22,6 +22,9 @@ FLAME_LAMBDA = 1e-3              # FLAME noise factor: the paper's value for ima
 LIFESPAN_THRESHOLD = 0.5         # poison accuracy below which the backdoor counts as gone
 SERVER_OPTS = ("sgd", "momentum", "adagrad", "adam", "yogi")
 SELECTIONS = ("none", "krum", "multikrum")
+DETECTORS = ("none", "fldetector")
+FLD_WINDOW = 10                  # FLDetector: the L-BFGS memory and the score window N
+FLD_START = 0                    # FLDetector: the first round detection may run (it also waits for round 2N + 1)
 PATTERNS = ("plus", "square", "copyright", "apple")
 MODELS = ("auto", "cnn_mnist", "cnn_cifar", "resnet18", "resnet34", "vgg11", "vgg16", "resnet18_gn", "resnet34_gn", "vgg11_gn", "vgg16_gn")
 
@@ -129,6 +132,15 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--flame_lambda", type=float, default=None,
                    help=f"--aggr flame: noise factor lambda >= 0; the round's Gaussian noise has std lambda * S, S the median update norm "
                         f"the admitted updates are clipped to (default {FLAME_LAMBDA})")
+    p.add_argument("--detect", type=str, default="none", choices=DETECTORS,
+                   help="detection ahead of the --aggr rule: fldetector (Zhang et al. 2022) predicts every agent's update from its last "
+                        "one and an L-BFGS Hessian estimate, scores how far each update lies from its prediction, and once the gap "
+                        "statistic finds a minority cluster of high scores stops listening to those agents for the rest of the run.  "
+                        "Every agent has to take part in every round")
+    p.add_argument("--fld_window", type=int, default=None,
+                   help=f"--detect fldetector: the L-BFGS memory and the score window N >= 1 (default {FLD_WINDOW})")
+    p.add_argument("--fld_start", type=int, default=None,
+                   help=f"--detect fldetector: detection runs only in rounds >= max(R, 2N + 1) (default R = {FLD_START})")
     p.add_argument("--attack_boost", type=float, default=1.0,
                    help="model replacement (Bhagoji et al. 2019, Bagdasaryan et al. 2020): every corrupt agent scales its update by this "
                         "factor gamma > 0 before submitting it, after its --clip projection (1 = off; needs --num_corrupt > 0)")
@@ -195,7 +207,42 @@ def finalize_args(args: argparse.Namespace) -> argparse.Namespace:
     _finalize_rfa(args)
     _finalize_flame(args)
     _finalize_attack(args)
+    _finalize_detect(args)
     return args
+
+
+def _finalize_detect(args) -> None:
+    """Validate the detection flags and resolve ``fld_window`` / ``fld_start`` in place (``FLD_WINDOW`` / ``FLD_START`` under
+    ``--detect fldetector``): every agent in every round, at least 3 agents, no ``--select``, and an RLR threshold no larger than the
+    fewest voters detection leaves (it flags at most ceil(K/2) - 1 of K agents, so floor(K/2) + 1 remain; under FLAME, which admits
+    floor(K'/2) + 1 of its K' candidates, floor(K'/2) + 1 of those)."""
+    detect = getattr(args, "detect", "none")
+    window, start = getattr(args, "fld_window", None), getattr(args, "fld_start", None)
+    if detect not in DETECTORS:
+        raise ValueError(f"unknown --detect {detect!r}; expected one of {DETECTORS}")
+    if detect == "none":
+        if window is not None or start is not None:
+            raise ValueError("--fld_window / --fld_start need --detect fldetector")
+        return
+    window = FLD_WINDOW if window is None else window
+    start = FLD_START if start is None else start
+    if int(window) != window or window < 1:
+        raise ValueError(f"--fld_window {window} must be an integer >= 1")
+    if int(start) != start or start < 0:
+        raise ValueError(f"--fld_start {start} must be an integer >= 0")
+    K = math.floor(args.num_agents * args.agent_frac)
+    if K != args.num_agents or args.num_agents < 3:
+        raise ValueError(f"--detect fldetector needs every agent in every round and at least 3 agents: floor(--num_agents {args.num_agents} "
+                         f"x --agent_frac {args.agent_frac}) = {K}")
+    if getattr(args, "select", "none") != "none":
+        raise ValueError("--detect fldetector does not combine with --select: Krum's K >= 2F + 3 and its M are defined over all participants")
+    fewest = K // 2 + 1
+    if args.aggr == "flame":
+        fewest = fewest // 2 + 1
+    if args.robustLR_threshold > fewest:
+        raise ValueError(f"--robustLR_threshold {args.robustLR_threshold} > {fewest}, the fewest voters --detect fldetector leaves"
+                         f"{' under --aggr flame' if args.aggr == 'flame' else ''} of {K}, could flip every coordinate")
+    args.fld_window, args.fld_start = int(window), int(start)
 
 
 def _finalize_attack(args) -> None:
@@ -366,6 +413,8 @@ def print_exp_details(args) -> None:
         print(f"    FLAME lambda: {args.flame_lambda}")
     if getattr(args, "attack_boost", 1.0) != 1.0 or getattr(args, "attack_neurotoxin", 0.0) > 0:
         print(f"    Attack (boost / neurotoxin): {args.attack_boost} / {args.attack_neurotoxin}")
+    if getattr(args, "detect", "none") != "none":
+        print(f"    Detection (window / start): {args.detect} ({args.fld_window} / {args.fld_start})")
     if attack_schedule_set(args):
         print(f"    Attack schedule (start / stop / every / force): {args.attack_start} / {args.attack_stop} / {args.attack_every} / "
               f"{args.attack_force}")

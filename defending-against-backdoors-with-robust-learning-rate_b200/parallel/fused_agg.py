@@ -33,7 +33,8 @@ Server optimizer state (``--server_opt`` other than sgd; ``ops.ServerOptState``)
 on the fused multi-GPU path rank r keeps only the state of its slice [begin, end) -- it is the only rank that ever steps those
 coordinates -- and with every other transport each rank keeps the full vector (identical on all ranks).  FoolsGold's per-agent update
 histories (``--aggr foolsgold``) are laid out the same way: ``[num_agents][slice ∩ [0, n_vote)]`` on the fused multi-GPU path, the full
-``[num_agents][n_vote]`` table on every rank otherwise.
+``[num_agents][n_vote]`` table on every rank otherwise.  FLDetector's state (``--detect fldetector``: the per-agent last-update table,
+the ring of the last N + 1 global updates and the previous global parameters) uses the same column layout.
 """
 from __future__ import annotations
 
@@ -49,10 +50,12 @@ FLAG_BYTES = 4096
 
 class FusedAggregator:
     def __init__(self, ctx, n_total: int, n_vote: int, max_slots: int, backend: str = "auto", with_bf16: bool = True,
-                 transport: str = "auto", server_opt=None, n_part: int | None = None, history_agents: int = 0):
+                 transport: str = "auto", server_opt=None, n_part: int | None = None, history_agents: int = 0, fld_agents: int = 0,
+                 fld_window: int = 0):
         """``server_opt``: optional ``dict(kind=..., beta1=..., beta2=..., tau=...)``; ``n_part``: participants per round (default
         every slot), which fixes whether the fused multi-GPU kernel or the gather fallback runs, and so the state layout;
-        ``history_agents``: agents whose FoolsGold update history this aggregator keeps (``--aggr foolsgold``: ``--num_agents``; 0 = none)."""
+        ``history_agents``: agents whose FoolsGold update history this aggregator keeps (``--aggr foolsgold``: ``--num_agents``; 0 = none);
+        ``fld_agents`` / ``fld_window``: agents and window N of the FLDetector state (``--detect fldetector``; 0 = none)."""
         self.ctx = ctx
         # nccl / gloo back-ends: "gather" all-gathers every participant's parameters and runs the kernel on the copies (any
         # aggregator); "reduce" all-reduces per-coordinate partial sums (vote, weighted update sum) -- O(N) instead of O(K N)
@@ -122,20 +125,32 @@ class FusedAggregator:
         # FoolsGold's update histories (history_agents > 0): [history_agents][hist_hi - hist_lo] fp32, zero at the start.  On the fused
         # multi-GPU path rank r keeps the columns of its slice that lie below n_vote (the only rank that ever reads or writes them);
         # with every other transport each rank keeps the full [0, n_vote) table, identical on all ranks.
+        # FLDetector (fld_window > 0): the last-update table [fld_agents][width], the ring [fld_window + 1][width] and w_prev [width], in
+        # the same columns as the history.
         self.history = None
-        if history_agents:
-            self._alloc_history(int(history_agents))
+        self.fld_table = self.fld_ring = self.fld_w_prev = None
+        if history_agents or fld_window:
+            self._alloc_history(int(history_agents or fld_agents), int(fld_window), foolsgold=bool(history_agents))
 
-    def _alloc_history(self, agents: int):
-        """Allocate the zero FoolsGold history of ``agents`` rows over ``[hist_lo, hist_hi)``: this rank's slice below n_vote on the
-        fused multi-GPU path (empty when the slice lies past n_vote), all of ``[0, n_vote)`` otherwise.  Refuses a table that does not
-        fit in the free device memory."""
+    def _alloc_history(self, agents: int, fld_window: int = 0, foolsgold: bool = True):
+        """Allocate the zero FoolsGold history (``foolsgold``) and / or the zero FLDetector state (``fld_window`` > 0) of ``agents`` rows over
+        ``[hist_lo, hist_hi)``: this rank's slice below n_vote on the fused multi-GPU path (empty when the slice lies past n_vote), all of
+        ``[0, n_vote)`` otherwise.  Refuses tables that together do not fit in the free device memory."""
         self.hist_lo, self.hist_hi = (self.begin, max(self.begin, min(self.end, self.n_vote))) if self.sharded else (0, self.n_vote)
         width = self.hist_hi - self.hist_lo
         dev = self.ctx.device
         if dev.type == "cuda":
-            check_history_memory(agents, width, torch.cuda.mem_get_info(dev)[0])
-        self.history = torch.zeros((agents, width), dtype=torch.float32, device=dev)
+            check_history_memory(agents, width, torch.cuda.mem_get_info(dev)[0], fld_window, foolsgold)
+        if foolsgold:
+            self.history = torch.zeros((agents, width), dtype=torch.float32, device=dev)
+        if fld_window:
+            self.fld_table = torch.zeros((agents, width), dtype=torch.float32, device=dev)
+            self.fld_ring = torch.zeros((fld_window + 1, width), dtype=torch.float32, device=dev)
+            self.fld_w_prev = torch.zeros(width, dtype=torch.float32, device=dev)
+
+    def _col_ptr(self, t, row: int = 0):
+        """Address of row ``row`` of a column-sliced table, offset by ``hist_lo`` so that absolute coordinates index it."""
+        return t.data_ptr() + 4 * (t.shape[-1] * int(row) - self.hist_lo)
 
     # ---- hand-off fused with the next round's first GEMM -------------------------------------------------------------------
     def enable_handoff(self):
@@ -334,20 +349,27 @@ class FusedAggregator:
         other ranks.  Collective on the fused multi-GPU path, where each rank contributes its columns: the rows are all-gathered in chunks
         of about ``chunk_bytes`` of gathered data, so no rank holds more than one chunk of extra device memory, and only the main rank
         copies them to the host."""
+        return self._gather_columns(self.history, chunk_bytes)
+
+    def _gather_columns(self, table, chunk_bytes: int = 256 << 20):
+        """The full ``[rows, n_vote]`` fp32 form of a column-sliced ``table`` on the host of the main rank; None on the other ranks.
+        Collective on the fused multi-GPU path, where each rank contributes its columns: the rows are all-gathered in chunks of about
+        ``chunk_bytes`` of gathered data, so no rank holds more than one chunk of extra device memory, and only the main rank copies them
+        to the host."""
         main = self.ctx.is_main
         if not self.sharded:
             if not main:
                 return None
-            return self.history.cpu() if self.history.is_cuda else self.history.clone()
-        A = self.history.shape[0]
+            return table.cpu() if table.is_cuda else table.clone()
+        A = table.shape[0]
         world, per = self.ctx.world, self.per
         full = torch.empty((A, self.n_vote), dtype=torch.float32) if main else None
         rows = max(1, int(chunk_bytes) // (4 * per * world))
         width = self.hist_hi - self.hist_lo
         for a0 in range(0, A, rows):
             a1 = min(A, a0 + rows)
-            part = torch.zeros((a1 - a0, per), dtype=torch.float32, device=self.history.device)
-            part[:, :width] = self.history[a0:a1]
+            part = torch.zeros((a1 - a0, per), dtype=torch.float32, device=table.device)
+            part[:, :width] = table[a0:a1]
             allp = self.ctx.all_gather(part)                                 # [world, rows, per]: rank r holds columns [r per, r per + per)
             if main:
                 full[a0:a1] = allp.permute(1, 0, 2).reshape(a1 - a0, world * per)[:, : self.n_vote].cpu()
@@ -362,6 +384,91 @@ class FusedAggregator:
             raise ValueError(f"FoolsGold history of shape {tuple(full.shape)}; this run keeps {self.history.shape[0]} agents x "
                              f"{self.n_vote} voted coordinates")
         self.history.copy_(full[:, self.hist_lo:self.hist_hi])
+
+    # ---- FLDetector ----------------------------------------------------------------------------------------------
+    def _fld_check(self, n_part: int):
+        if self.fld_table is None:
+            raise ValueError("this aggregator keeps no FLDetector state (fld_window = 0)")
+        if self._p2p(n_part) != self.sharded:
+            raise ValueError(f"{n_part} participants: the FLDetector state was laid out for the "
+                             f"{'fused multi-GPU' if self.sharded else 'gather'} path")
+
+    def fld_ring_update(self, row=None):
+        """The ring pass on this rank's columns: ring row ``row`` <- ``fp32(w_global - w_prev)`` (skipped when None), then ``w_prev <-
+        w_global``.  Purely local; it reads ``w_global``, so it first acquires the broadcast slices of a fused hand-off."""
+        if self.fld_table is None:
+            raise ValueError("this aggregator keeps no FLDetector state (fld_window = 0)")
+        self.acquire()
+        if self.sharded:
+            ops.ext().fld_ring(self.w_global.data_ptr(), self._col_ptr(self.fld_w_prev), 0 if row is None else self._col_ptr(self.fld_ring, row),
+                               self.hist_lo, self.hist_hi)
+        else:
+            ops.fld_ring(self.w_global, self.fld_w_prev, None if row is None else self.fld_ring[int(row)], 0, self.n_vote)
+
+    def fld_gram(self, order):
+        """The float64 Gram matrix of the ring rows ``order`` (chronological) over ``[0, n_vote)``, identical on every rank: one
+        ``_fused_pass`` of ``pairwise_sqdist_kernel<true, true>`` over this rank's columns on the fused multi-GPU path, the same kernel over
+        the full ring otherwise."""
+        if self.fld_table is None:
+            raise ValueError("this aggregator keeps no FLDetector state (fld_window = 0)")
+        order = [int(i) for i in order]
+        if self.sharded:
+            tab = ops.PtrTable([self._col_ptr(self.fld_ring, i) for i in order], self.ctx.device)
+            return self._fused_pass((len(order), len(order)), lambda begin, end, out, *gate: ops.ext().history_gram(tab.tensor, begin, end, out))
+        return ops.history_gram([self.fld_ring[i] for i in order], self.n_vote)
+
+    def fld_predict(self, n_part: int, agent_ids, order=None, coef=None, participants=None):
+        """FLDetector's prediction pass over the round's ``n_part`` participants, whose agents are ``agent_ids``: with ``coef``
+        (``ops.fld_hvp_coefficients`` of the ring rows ``order``) the float64 squared distances ``d^2 [n_part]`` of every update to its
+        prediction, identical on every rank; then every participant's update is recorded in its agent's row of the last-update table.
+        Without ``coef`` it only records and returns None.  Call it after the slots are final and before ``aggregate`` of the same round.
+
+        Fused multi-GPU path: one ``_fused_pass``.  Each rank forms ``Hv`` over its columns of the ring (``fld_hvp_kernel``) and runs
+        ``fld_predict_kernel`` over its coordinate slice of the peer-mapped slots behind the aggregation kernel's barrier-in (an epoch of its
+        own); the ranks all_gather their partials and add them in rank order.  Gather transport and single process: the same kernels over
+        ``participants`` (``gather_participants``' copies; gathered here when not given) and the full tables every rank keeps."""
+        self._fld_check(n_part)
+        ids = [int(a) for a in agent_ids]
+        if self._p2p(n_part):
+            self.acquire()
+            dev = self.ctx.device
+            table = self._agent_table(n_part)
+            rows = ops.PtrTable([self._col_ptr(self.fld_table, a) for a in ids], dev)
+            if coef is not None:
+                ring = ops.PtrTable([self._col_ptr(self.fld_ring, i) for i in order], dev)
+                ct = torch.as_tensor(coef, dtype=torch.float64).to(dev)
+                hv = torch.empty(max(4, self.hist_hi - self.hist_lo), dtype=torch.float32, device=dev)
+
+            def launch(begin, end, out, flag_ptrs, local_sync, rank, world, epoch):
+                hv_ptr = 0
+                if coef is not None:
+                    hv_ptr = hv.data_ptr() - 4 * begin
+                    ops.ext().fld_hvp(ring.tensor, ct, hv_ptr, begin, end)
+                else:
+                    out.zero_()
+                ops.ext().fld_predict(table.tensor, rows.tensor, self.w_global.data_ptr(), hv_ptr, begin, end, out, flag_ptrs, local_sync,
+                                      rank, world, epoch)
+            d2 = self._fused_pass((n_part,), launch)
+            return d2 if coef is not None else None
+        agents = self._participants(n_part, participants)
+        hv = ops.fld_hvp([self.fld_ring[int(i)] for i in order], coef, 0, self.n_vote) if coef is not None else None
+        return ops.fld_predict([self.fld_table[a] for a in ids], agents, self.w_global, hv, 0, self.n_vote)
+
+    def fld_tables(self):
+        """``(table, ring, w_prev)``: the full fp32 ``[agents, n_vote]``, ``[N + 1, n_vote]`` and ``[n_vote]`` FLDetector state on the host of
+        the main rank (what a checkpoint saves); None on the other ranks.  Collective on the fused multi-GPU path."""
+        table, ring = self._gather_columns(self.fld_table), self._gather_columns(self.fld_ring)
+        w_prev = self._gather_columns(self.fld_w_prev[None])
+        return None if table is None else (table, ring, w_prev[0])
+
+    def load_fld_tables(self, table, ring, w_prev):
+        """Set the FLDetector state from its full tables (this rank's columns of them on the fused multi-GPU path)."""
+        if self.fld_table is None:
+            raise ValueError("this aggregator keeps no FLDetector state (fld_window = 0)")
+        for name, dst, src in (("table", self.fld_table, table), ("ring", self.fld_ring, ring), ("w_prev", self.fld_w_prev[None], w_prev[None])):
+            if tuple(src.shape) != (dst.shape[0], self.n_vote):
+                raise ValueError(f"FLDetector {name} of shape {tuple(src.shape)}; this run keeps {dst.shape[0]} x {self.n_vote}")
+            dst.copy_(src[:, self.hist_lo:self.hist_hi])
 
     def aggregate(self, weights, mode, theta, server_lr, noise_std=0.0, seed=0, rnd=0, scales=None, members=None, participants=None,
                   total_weight=None):
@@ -493,13 +600,17 @@ class FusedAggregator:
         self.buf.close()
 
 
-def check_history_memory(num_agents: int, width: int, free_bytes: int):
-    """Refuse a FoolsGold history of ``num_agents`` rows of ``width`` fp32 values that does not fit in ``free_bytes`` of device memory."""
-    nbytes = 4 * int(num_agents) * int(width)
+def check_history_memory(num_agents: int, width: int, free_bytes: int, fld_window: int = 0, foolsgold: bool = True):
+    """Refuse per-agent state of ``width`` fp32 columns that does not fit in ``free_bytes`` of device memory: FoolsGold's history
+    (``foolsgold``: ``4 num_agents width`` bytes) plus FLDetector's state (``fld_window`` = N > 0: the last-update table, the ring of N + 1
+    global updates and w_prev, ``4 num_agents width + 4 (N + 2) width`` bytes).  Returns the bytes."""
+    A, W, N = int(num_agents), int(width), int(fld_window)
+    nbytes = (4 * A * W if foolsgold else 0) + ((4 * A * W + 4 * (N + 2) * W) if N else 0)
     if nbytes > int(free_bytes):
-        raise ValueError(f"--aggr foolsgold keeps one fp32 update history per agent: {nbytes} bytes on this GPU for --num_agents "
-                         f"{num_agents} x {width} voted coordinates, but only {int(free_bytes)} bytes are free.  Use fewer agents or "
-                         "more GPUs (the fused multi-GPU path shards the history over the ranks)")
+        what = " and ".join(x for x in (("--aggr foolsgold" if foolsgold else ""), (f"--detect fldetector (--fld_window {N})" if N else "")) if x)
+        raise ValueError(f"{what} keep fp32 per-agent state: {nbytes} bytes on this GPU for --num_agents {num_agents} x {width} voted "
+                         f"coordinates, but only {int(free_bytes)} bytes are free.  Use fewer agents, a smaller --fld_window or more GPUs "
+                         "(the fused multi-GPU path shards this state over the ranks)")
     return nbytes
 
 

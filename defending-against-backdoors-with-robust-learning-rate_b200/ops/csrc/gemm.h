@@ -95,6 +95,10 @@ cudaError_t launch_conv_wgrad_bf16(const void* dy, const void* x, float* dW, int
                                    cudaStream_t st, int in_stride = 1);
 cudaError_t launch_conv_wgrad_halo_bf16(const void* dy, const void* x, float* dW, int NB, int H, int W, int Cin_valid, int Cout,
                                         int num_sms, cudaStream_t st);
+// test hook: off = the whole-row 3x3 stride-1 weight gradients run umma_wgrad_kernel<64, 3> instead of the filter-row kernel
+void set_wgrad_rows(int on);
+// launches so far of umma_wgrad_kernel, umma_wgrad_halo_kernel and umma_wgrad_rows_kernel (out[3])
+void wgrad_launch_counts(long long* out);
 cudaError_t launch_linear_wgrad_bf16(const void* dy, const void* x, float* dW, int B, int N, int K, int num_sms, cudaStream_t st);
 
 // ---- norm.cu: NHWC bf16 layer kernels -----------------------------------------------------------------------------

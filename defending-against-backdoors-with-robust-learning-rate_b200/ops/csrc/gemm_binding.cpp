@@ -384,6 +384,12 @@ void register_gemm_bindings(py::module_& m) {
     m.def("set_pdl", [](bool on) { rlr::set_pdl(on ? 1 : 0); });
     m.def("set_conv_occ3", [](int64_t level) { rlr::set_conv_occ3((int)level); });
     m.def("set_conv_one_wave", [](bool on) { rlr::set_conv_one_wave(on ? 1 : 0); });
+    m.def("set_wgrad_rows", [](bool on) { rlr::set_wgrad_rows(on ? 1 : 0); });
+    m.def("wgrad_launch_counts", [] {
+        long long c[3];
+        rlr::wgrad_launch_counts(c);
+        return std::vector<int64_t>{c[0], c[1], c[2]};
+    });
     m.def("set_conv_tma_store", [](bool on) { rlr::set_conv_tma_store(on ? 1 : 0); });
     m.def("set_conv_split_producer", [](bool on) { rlr::set_conv_split_producer(on ? 1 : 0); });
     m.def("set_conv_trace", [](c10::optional<at::Tensor> buf) {   // int64 [CTAs * 8] timeline buffer for the next generic conv / GEMM launches

@@ -57,6 +57,11 @@ struct __align__(8) WgShared {
     uint64_t empty[WG_STAGES];
 };
 
+// Host-side count of the weight-gradient launches of each kernel: [0] umma_wgrad_kernel, [1] umma_wgrad_halo_kernel,
+// [2] umma_wgrad_rows_kernel.  Tests read it (wgrad_launch_counts) to check which kernel a shape is dispatched to.
+static long long g_wgrad_launches[3] = {0, 0, 0};
+void wgrad_launch_counts(long long* out) { for (int i = 0; i < 3; ++i) out[i] = g_wgrad_launches[i]; }
+
 // acc column c of warpgroup row `co` (fragment layout) -> dW[co][tap0 + c / BNW][ci0 + c % BNW], pairs of adjacent columns per thread;
 // with `part` the values are stored into this split's slot of the partial buffer instead of being added into dW
 template <int NACC, int BNW>
@@ -103,7 +108,7 @@ umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
     if (warp == 8 && lane == 0) {
         prefetch_tmap(&tmA); prefetch_tmap(&tmB);
-        for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&sh->full[s], 1); mbar_init(&sh->empty[s], 8); }
+        for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&sh->full[s], 1); mbar_init(&sh->empty[s], 4 * p.a_groups); }
         fence_barrier_init();
     }
     __syncthreads();
@@ -139,11 +144,11 @@ umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (nkb > 0) {
-        // warpgroup wgi: output channels co_tile * 128 + 64 wgi + [0, 64) = A group wgi; it idles (but still releases stages) when that
-        // group does not exist (a_groups == 1)
+    } else if (nkb > 0 && (threadIdx.x >> 7) < p.a_groups) {
+        // warpgroup wgi: output channels co_tile * 128 + 64 wgi + [0, 64) = A group wgi.  When that group does not exist (a_groups == 1)
+        // the warpgroup has no work and leaves at once: the stage-release barriers count only the warps of the active warpgroups, and
+        // no MMA sits under a per-warpgroup branch (which makes ptxas serialize every wgmma of the kernel)
         const int wgi = threadIdx.x >> 7, t = threadIdx.x & 127;
-        const bool active = wgi < p.a_groups;
         float acc[NACC / 2];
 #pragma unroll
         for (int i = 0; i < NACC / 2; ++i) acc[i] = 0.f;
@@ -151,29 +156,42 @@ umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         uint32_t phase = 0;
         for (int i = 0; i < nkb; ++i) {
             mbar_wait(&sh->full[stage], phase);
-            if (active) {
-                const uint32_t sa = smem_u32(smem + stage * WG_STAGE_BYTES) + wgi * 8192;
-                const uint32_t sb = smem_u32(smem + stage * WG_STAGE_BYTES) + WG_A_BYTES;
-                wgmma_fence();
+            const uint32_t sa = smem_u32(smem + stage * WG_STAGE_BYTES) + wgi * 8192;
+            const uint32_t sb = smem_u32(smem + stage * WG_STAGE_BYTES) + WG_A_BYTES;
+            wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < WG_BK / 16; ++k) {   // 16 pixel rows (2 swizzle atoms) per MMA
-                    // B: the tap tiles (and 64-wide ci groups inside them) are N groups 8 KB apart -> one MMA covers all kTaps taps
-                    wgmma_bf16<NACC, 1, 1>(acc, smem_desc_sw128(sa + k * 2048, 8192, 1024), smem_desc_sw128(sb + k * 2048, 8192, 1024),
-                                           (i > 0 || k > 0) ? 1u : 0u);
-                }
-                wgmma_commit();
-                wgmma_wait<1>();
+            for (int k = 0; k < WG_BK / 16; ++k) {   // 16 pixel rows (2 swizzle atoms) per MMA
+                // B: the tap tiles (and 64-wide ci groups inside them) are N groups 8 KB apart -> one MMA covers all kTaps taps
+                wgmma_bf16<NACC, 1, 1>(acc, smem_desc_sw128(sa + k * 2048, 8192, 1024), smem_desc_sw128(sb + k * 2048, 8192, 1024),
+                                       (i > 0 || k > 0) ? 1u : 0u);
             }
+            wgmma_commit();
+            wgmma_wait<1>();
             if (prev >= 0 && lane == 0) mbar_arrive(&sh->empty[prev]);
             prev = stage;
             if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
         }
-        if (active) {
-            wgmma_wait<0>();
-            fence_acc(acc);
-            wgrad_flush<NACC, BNW>(acc, p.dW, p.part, co_tile * WG_BM + wgi * 64 + frag_row(t, 0), p.Cout, p.T, tap0, ci_tile * WG_BN, p.Cin_valid, t);
-        }
+        wgmma_wait<0>();
+        fence_acc(acc);
+        wgrad_flush<NACC, BNW>(acc, p.dW, p.part, co_tile * WG_BM + wgi * 64 + frag_row(t, 0), p.Cout, p.T, tap0, ci_tile * WG_BN, p.Cin_valid, t);
     }
+}
+
+// split-K so that the grid of `base` CTAs per split is (at most) a whole number of waves of one CTA per SM: no ragged tail wave.
+// Below one wave, `low_waves` (0 = 1) waves.  Returns the split count and the k-blocks per split; the split count fixes the
+// order of every dW element's sum, so the filter-row kernel computes it from the CTA count of the kernel it replaces.
+static int wg_splits(int base, int num_kb, int num_sms, int low_waves, int* kb_per_cta) {
+    const int waves = base >= num_sms ? (base + num_sms - 1) / num_sms : (low_waves > 0 ? low_waves : 1);
+    int splits = (waves * num_sms) / base;
+    if (splits > num_kb) splits = num_kb;
+    if (splits < 1) splits = 1;
+    *kb_per_cta = (num_kb + splits - 1) / splits;
+    return (num_kb + *kb_per_cta - 1) / *kb_per_cta;
+}
+// one wave measured faster (fewer split-K atomics), RLR_WG_WAVES overrides
+static int wg_tune_waves() {
+    static const int w = [] { const char* e = getenv("RLR_WG_WAVES"); return e ? atoi(e) : 0; }();
+    return w;
 }
 
 template <int BNW, int kTaps>
@@ -184,16 +202,9 @@ static cudaError_t launch_wg(const CUtensorMap& tmA, const CUtensorMap& tmB, Wgr
         RLR_CUDA_CHECK(cudaFuncSetAttribute(umma_wgrad_kernel<BNW, kTaps>, cudaFuncAttributeMaxDynamicSharedMemorySize, WgCfg<BNW>::kSmem));
         configured = true;
     }
-    // split-K so that the grid is (at most) a whole number of waves of one CTA per SM: no ragged tail wave
-    const int base = co_tiles * p.ci_tiles * tap_groups;
-    static const int tune_waves = [] { const char* e = getenv("RLR_WG_WAVES"); return e ? atoi(e) : 0; }();
-    int waves = base >= num_sms ? (base + num_sms - 1) / num_sms : (tune_waves > 0 ? tune_waves : 1);   // one wave measured faster (fewer split-K atomics), RLR_WG_WAVES overrides
-    int splits = (waves * num_sms) / base;
-    if (splits > p.num_kb) splits = p.num_kb;
-    if (splits < 1) splits = 1;
-    p.kb_per_cta = (p.num_kb + splits - 1) / splits;
-    splits = (p.num_kb + p.kb_per_cta - 1) / p.kb_per_cta;
-    dim3 grid(co_tiles * p.ci_tiles, tap_groups, splits);
+    const int splits = wg_splits(co_tiles * p.ci_tiles * tap_groups, p.num_kb, num_sms, wg_tune_waves(), &p.kb_per_cta);
+    const dim3 grid(co_tiles * p.ci_tiles, tap_groups, splits);
+    ++g_wgrad_launches[0];
     if (splits == 1) return launch_kernel(umma_wgrad_kernel<BNW, kTaps>, grid, dim3(WG_THREADS), (size_t)WgCfg<BNW>::kSmem, st, tmA, tmB, p);
     const long long plane = (long long)p.Cout * p.T * p.Cin_valid;
     Scratch part((size_t)splits * plane * sizeof(float), st);
@@ -243,7 +254,7 @@ umma_wgrad_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 
     if (warp == 8 && lane == 0) {
         prefetch_tmap(&tmA); prefetch_tmap(&tmB);
-        for (int s = 0; s < WH_STAGES; ++s) { mbar_init(&sh->full[s], 1); mbar_init(&sh->empty[s], 8); }
+        for (int s = 0; s < WH_STAGES; ++s) { mbar_init(&sh->full[s], 1); mbar_init(&sh->empty[s], 4 * p.a_groups); }
         fence_barrier_init();
     }
     __syncthreads();
@@ -268,9 +279,8 @@ umma_wgrad_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
                 if (++stage == WH_STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (nkb > 0) {
+    } else if (nkb > 0 && (threadIdx.x >> 7) < p.a_groups) {   // as in umma_wgrad_kernel: a warpgroup without an A group leaves
         const int wgi = threadIdx.x >> 7, t = threadIdx.x & 127;
-        const bool active = wgi < p.a_groups;
         float acc[96];
 #pragma unroll
         for (int i = 0; i < 96; ++i) acc[i] = 0.f;
@@ -278,35 +288,186 @@ umma_wgrad_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
         uint32_t phase = 0;
         for (int i = 0; i < nkb; ++i) {
             mbar_wait(&sh->full[stage], phase);
-            if (active) {
-                const uint32_t sa = smem_u32(smem + stage * WH_STAGE_BYTES) + wgi * 16384;
-                const uint32_t halo = smem_u32(smem + stage * WH_STAGE_BYTES) + WH_A_BYTES;
-                wgmma_fence();
+            const uint32_t sa = smem_u32(smem + stage * WH_STAGE_BYTES) + wgi * 16384;
+            const uint32_t halo = smem_u32(smem + stage * WH_STAGE_BYTES) + WH_A_BYTES;
+            wgmma_fence();
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {                     // 16 pixels = output rows 2j, 2j+1 of the tile
-                    // N groups 0,1,2 = taps dx = 0,1,2: same halo view shifted by one pixel -> LBO = 128 B; SBO = one image row
-                    wgmma_bf16<192, 1, 1>(acc, smem_desc_sw128(sa + j * 2048, 16384, 1024),
-                                          smem_desc_sw128(halo + ((2 * j + dy) * 16) * 128, 128, 2048), (i > 0 || j > 0) ? 1u : 0u);
-                }
-                wgmma_commit();
-                wgmma_wait<1>();
+            for (int j = 0; j < 8; ++j) {                     // 16 pixels = output rows 2j, 2j+1 of the tile
+                // N groups 0,1,2 = taps dx = 0,1,2: same halo view shifted by one pixel -> LBO = 128 B; SBO = one image row
+                wgmma_bf16<192, 1, 1>(acc, smem_desc_sw128(sa + j * 2048, 16384, 1024),
+                                      smem_desc_sw128(halo + ((2 * j + dy) * 16) * 128, 128, 2048), (i > 0 || j > 0) ? 1u : 0u);
             }
+            wgmma_commit();
+            wgmma_wait<1>();
             if (prev >= 0 && lane == 0) mbar_arrive(&sh->empty[prev]);
             prev = stage;
             if (++stage == WH_STAGES) { stage = 0; phase ^= 1; }
         }
-        if (active) {
-            wgmma_wait<0>();
-            fence_acc(acc);
-            wgrad_flush<192, 64>(acc, p.dW, p.part, co_tile * WG_BM + wgi * 64 + frag_row(t, 0), p.Cout, 9, tap0, 0, p.Cin_valid, t);
-        }
+        wgmma_wait<0>();
+        fence_acc(acc);
+        wgrad_flush<192, 64>(acc, p.dW, p.part, co_tile * WG_BM + wgi * 64 + frag_row(t, 0), p.Cout, 9, tap0, 0, p.Cin_valid, t);
     }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Filter-row variant for 3x3 / stride-1 / pad-1 filters: ONE CTA computes all nine taps of a 64-co x 64-ci filter tile for one
+// split-K range.  A k-block loads one dY box (64 co) and one input halo, shared by three consumer warpgroups, one per filter
+// row dy; warpgroup dy reads the three dx taps as the halo's MN-major view shifted by one pixel (LBO = 128 B, as in
+// umma_wgrad_halo_kernel), starting at halo row dy.  Zero padding is the TMA zero fill of the halo.
+// The output tile of a k-block is TH x TW = 64 pixels, whole rows of one image (umma_wgrad_kernel's box when TN == 1 and TW == Wo,
+// TW % 8 == 0); its halo is (TH + 2) x (TW + 2) pixels at (h0 - 1, w0 - 1).  Output pixel 16j = (row r, column c) starts
+// k-step j; r * TW + c = 16j, so the view of filter row dy starts at halo pixel (r + dy) (TW + 2) + c = 16j + 2r + dy (TW + 2), and the second 8-pixel core group of the k-step
+// is 8 pixels further (TW >= 16, SBO = 1024 B) or one halo row further (TW = 8, SBO = (TW + 2) * 128 B).
+// That is the pixel order of umma_wgrad_kernel<64, 3>, so every dW element gets the same products through the same k16 steps in
+// the same k-block order, and the caller keeps that kernel's split count: the result is bit-identical.
+// Bytes per k-block: 8 KB of dY + 13.5 KB of halo (16 x 4 tile) instead of 3 x (16 + 3 x 8) KB over the three filter-row CTAs.
+// The same scheme on umma_wgrad_halo_kernel's 16 x 8 tiles (Cin = 64) ran layer 1 of ResNet-18 on 44 CTAs at 84 us, slower than the
+// halo kernel on 132, and did not shorten the training step (docs/PROFILE_H100.md), so those shapes keep the halo kernel.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int WR_STAGES = 4;
+constexpr int WR_KSTEPS = 4;                                 // 64 pixels per k-block
+constexpr int WR_THREADS = 3 * 128 + 32;                     // one consumer warpgroup per filter row + the TMA producer warp
+
+struct __align__(8) WgRowsShared {
+    uint64_t full[WR_STAGES];
+    uint64_t empty[WR_STAGES];
+};
+
+struct WgRowsParams {
+    int num_kb, kb_per_cta;
+    int TW, TH, log2_tw;      // output tile of one k-block (TW, TH powers of two, TW * TH = 64)
+    int tiles_w, tiles_h;     // k-block kb = (n * tiles_h + th) * tiles_w + tw
+    int stage_bytes;          // dY box + halo, rounded up to 1024 B
+    uint32_t halo_bytes;      // (TH + 2) (TW + 2) 128 B
+    uint32_t sbo;             // byte offset of the second 8-pixel core group of a k-step
+    int ci_tiles;
+    int Cout, Cin_valid;
+    float* dW;                // [Cout][9][Cin_valid]
+    float* part;              // split-K > 1: [splits][Cout][9][Cin_valid] partial gradients (one slot per blockIdx.z)
+};
+
+__global__ void __launch_bounds__(WR_THREADS, 1)
+umma_wgrad_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const WgRowsParams p) {
+    constexpr int kSteps = WR_KSTEPS;
+    constexpr uint32_t kABytes = kSteps * 2048;               // 64 pixel rows x 128 B
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    WgRowsShared* sh = reinterpret_cast<WgRowsShared*>(smem + WR_STAGES * p.stage_bytes);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int co_tile = blockIdx.x / p.ci_tiles, ci_tile = blockIdx.x - co_tile * p.ci_tiles;
+    const int kb_begin = blockIdx.z * p.kb_per_cta;
+    const int kb_end = min(p.num_kb, kb_begin + p.kb_per_cta);
+    const int nkb = kb_end - kb_begin;
+
+    if (warp == 12 && lane == 0) {
+        prefetch_tmap(&tmA); prefetch_tmap(&tmB);
+        for (int s = 0; s < WR_STAGES; ++s) { mbar_init(&sh->full[s], 1); mbar_init(&sh->empty[s], 12); }
+        fence_barrier_init();
+    }
+    __syncthreads();
+    pdl_wait();        // prologue above: parameters and shared memory only
+    pdl_trigger();
+
+    if (warp == 12) {
+        if (lane == 0) {
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int i = 0; i < nkb; ++i) {
+                const int kb = kb_begin + i;
+                const int tw = kb % p.tiles_w, th = (kb / p.tiles_w) % p.tiles_h, n = kb / (p.tiles_w * p.tiles_h);
+                const int w0 = tw * p.TW, h0 = th * p.TH;
+                mbar_wait(&sh->empty[stage], phase ^ 1);
+                uint8_t* sa = smem + stage * p.stage_bytes;
+                mbar_expect_tx(&sh->full[stage], kABytes + p.halo_bytes);
+                tma_load_4d(&tmA, &sh->full[stage], sa, co_tile * 64, w0, h0, n);
+                tma_load_4d(&tmB, &sh->full[stage], sa + kABytes, ci_tile * 64, w0 - 1, h0 - 1, n);
+                if (++stage == WR_STAGES) { stage = 0; phase ^= 1; }
+            }
+        }
+    } else if (nkb > 0) {
+        const int dy = threadIdx.x >> 7, t = threadIdx.x & 127;
+        const uint32_t row0 = dy * (p.TW + 2);                // first halo pixel of filter row dy
+        float acc[96];
+#pragma unroll
+        for (int i = 0; i < 96; ++i) acc[i] = 0.f;
+        int stage = 0, prev = -1;
+        uint32_t phase = 0;
+        for (int i = 0; i < nkb; ++i) {
+            mbar_wait(&sh->full[stage], phase);
+            const uint32_t sa = smem_u32(smem + stage * p.stage_bytes);
+            const uint32_t halo = sa + kABytes + row0 * 128;
+            wgmma_fence();
+#pragma unroll
+            for (int j = 0; j < kSteps; ++j) {                   // 16 output pixels 16j .. 16j + 15
+                const uint32_t px = 16 * j + 2 * ((16 * j) >> p.log2_tw);
+                wgmma_bf16<192, 1, 1>(acc, smem_desc_sw128(sa + j * 2048, kABytes, 1024), smem_desc_sw128(halo + px * 128, 128, p.sbo),
+                                      (i > 0 || j > 0) ? 1u : 0u);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (prev >= 0 && lane == 0) mbar_arrive(&sh->empty[prev]);
+            prev = stage;
+            if (++stage == WR_STAGES) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        fence_acc(acc);
+        wgrad_flush<192, 64>(acc, p.dW, p.part, co_tile * 64 + frag_row(t, 0), p.Cout, 9, 3 * dy, ci_tile * 64, p.Cin_valid, t);
+    }
+}
+
+static int g_wgrad_rows = 1;
+void set_wgrad_rows(int on) { g_wgrad_rows = on ? 1 : 0; }
+
+// dW[Cout][9][Cin_valid] += wgrad3x3(dy[NB][H][W][Cout], x[NB][H][W][Cin]), stride 1, pad 1, over TH x TW output tiles (TW == W,
+// TH | H or the last tile row zero-filled, TW >= 8, TW * TH = 64), with the split count of `splits_base` CTAs per split.
+static cudaError_t launch_wgrad_rows(const void* dy, const void* x, float* dW, int NB, int H, int W, int Cin, int Cin_valid, int Cout,
+                                     int TW, int TH, int splits_base, int low_waves, int num_sms, cudaStream_t st) {
+    constexpr int kSteps = WR_KSTEPS;
+    constexpr int kSmemMax = WR_STAGES * (kSteps * 2048 + 25600) + 2048;   // 25600: the largest halo, 66 x 3 pixels (TW = 64)
+    static bool configured = false;
+    if (!configured) {
+        RLR_CUDA_CHECK(cudaFuncSetAttribute(umma_wgrad_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
+        configured = true;
+    }
+    WgRowsParams p{};
+    p.TW = TW; p.TH = TH;
+    while ((1 << p.log2_tw) < TW) ++p.log2_tw;
+    p.tiles_w = (W + TW - 1) / TW; p.tiles_h = (H + TH - 1) / TH; p.num_kb = p.tiles_w * p.tiles_h * NB;
+    p.halo_bytes = (uint32_t)((TW + 2) * (TH + 2) * 128);
+    p.stage_bytes = (int)((kSteps * 2048 + p.halo_bytes + 1023) / 1024 * 1024);
+    p.sbo = TW >= 16 ? 1024u : (uint32_t)((TW + 2) * 128);
+    p.ci_tiles = Cin / 64; p.Cout = Cout; p.Cin_valid = Cin_valid; p.dW = dW;
+    const size_t smem = (size_t)WR_STAGES * p.stage_bytes + 2048;
+    if (TW * TH != 16 * kSteps || TW < 8 || (TW & (TW - 1)) || smem > (size_t)kSmemMax) return cudaErrorInvalidValue;
+    const int splits = wg_splits(splits_base, p.num_kb, num_sms, low_waves, &p.kb_per_cta);
+    CUtensorMap tmA, tmB;
+    {
+        const uint64_t d[4] = {(uint64_t)Cout, (uint64_t)W, (uint64_t)H, (uint64_t)NB};
+        const uint64_t s[3] = {(uint64_t)Cout * 2, (uint64_t)W * Cout * 2, (uint64_t)H * W * Cout * 2};
+        const uint32_t b[4] = {64, (uint32_t)TW, (uint32_t)TH, 1};
+        RLR_CUDA_CHECK(make_tmap_bf16(&tmA, dy, 4, d, s, b));
+    }
+    {
+        const uint64_t d[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)NB};
+        const uint64_t s[3] = {(uint64_t)Cin * 2, (uint64_t)W * Cin * 2, (uint64_t)H * W * Cin * 2};
+        const uint32_t b[4] = {64, (uint32_t)TW + 2, (uint32_t)TH + 2, 1};
+        RLR_CUDA_CHECK(make_tmap_bf16(&tmB, x, 4, d, s, b));
+    }
+    const dim3 grid((Cout + 63) / 64 * p.ci_tiles, 1, splits);
+    ++g_wgrad_launches[2];
+    if (splits == 1) return launch_kernel(umma_wgrad_rows_kernel, grid, dim3(WR_THREADS), smem, st, tmA, tmB, p);
+    const long long plane = (long long)Cout * 9 * Cin_valid;
+    Scratch part((size_t)splits * plane * sizeof(float), st);
+    p.part = part.as<float>();
+    RLR_CUDA_CHECK(launch_kernel(umma_wgrad_rows_kernel, grid, dim3(WR_THREADS), smem, st, tmA, tmB, p));
+    return launch_ordered_sum(dW, p.part, splits, plane, st);
 }
 
 // dW[Cout][9][Cin_valid] += wgrad3x3(dy[NB][H][W][Cout], x[NB][H][W][64]); stride 1, pad 1, H % 16 == 0, W % 8 == 0
 cudaError_t launch_conv_wgrad_halo_bf16(const void* dy, const void* x, float* dW, int NB, int H, int W, int Cin_valid, int Cout,
                                         int num_sms, cudaStream_t st) {
     if (H % 16 || W % 8 || Cout % 8 || !((Cout <= 64) || Cout % 128 == 0)) return cudaErrorInvalidValue;
+    const int co_tiles = (Cout + WG_BM - 1) / WG_BM;
     static bool configured = false;
     if (!configured) {
         RLR_CUDA_CHECK(cudaFuncSetAttribute(umma_wgrad_halo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WH_SMEM));
@@ -315,14 +476,7 @@ cudaError_t launch_conv_wgrad_halo_bf16(const void* dy, const void* x, float* dW
     WgHaloParams p{};
     p.NB = NB; p.H = H; p.W = W; p.tiles_h = H / 16; p.tiles_w = W / 8; p.num_kb = NB * p.tiles_h * p.tiles_w;
     p.a_groups = (Cout % 128 == 0) ? 2 : 1; p.Cout = Cout; p.Cin_valid = Cin_valid; p.dW = dW;
-    const int co_tiles = (Cout + WG_BM - 1) / WG_BM;
-    const int base = co_tiles * 3;
-    int waves = base >= num_sms ? (base + num_sms - 1) / num_sms : 1;
-    int splits = (waves * num_sms) / base;
-    if (splits > p.num_kb) splits = p.num_kb;
-    if (splits < 1) splits = 1;
-    p.kb_per_cta = (p.num_kb + splits - 1) / splits;
-    splits = (p.num_kb + p.kb_per_cta - 1) / p.kb_per_cta;
+    const int splits = wg_splits(co_tiles * 3, p.num_kb, num_sms, 1, &p.kb_per_cta);
     CUtensorMap tmA, tmB;
     {
         const uint64_t d[4] = {(uint64_t)Cout, (uint64_t)W, (uint64_t)H, (uint64_t)NB};
@@ -336,6 +490,7 @@ cudaError_t launch_conv_wgrad_halo_bf16(const void* dy, const void* x, float* dW
         const uint32_t b[4] = {64, 16, 18, 1};
         RLR_CUDA_CHECK(make_tmap_bf16(&tmB, x, 4, d, s, b));
     }
+    ++g_wgrad_launches[1];
     if (splits == 1) return launch_kernel(umma_wgrad_halo_kernel, dim3(co_tiles, 3, splits), dim3(WG_THREADS), (size_t)WH_SMEM, st, tmA, tmB, p);
     const long long plane = (long long)Cout * 9 * Cin_valid;
     Scratch part((size_t)splits * plane * sizeof(float), st);
@@ -345,6 +500,13 @@ cudaError_t launch_conv_wgrad_halo_bf16(const void* dy, const void* x, float* dW
 }
 
 static int pow2_ceil_(int x) { int q = 1; while (q < x) q <<= 1; return q; }
+
+// tap t = (dy, dx) reads input pixel (h + dy - 1, w + dx - 1) of the same plane
+static bool standard_3x3_taps(const int* dh, const int* dw, const int* dplane) {
+    for (int t = 0; t < 9; ++t)
+        if (dh[t] != t / 3 - 1 || dw[t] != t % 3 - 1 || dplane[t] != 0) return false;
+    return true;
+}
 
 // dW[Cout][T][Cin_valid] += wgrad(dy[NB][Ho][Wo][Cout], x[planes*NB][Hin][Win][Cin])   (Cin multiple of 64)
 cudaError_t launch_conv_wgrad_bf16(const void* dy, const void* x, float* dW, int NB, int planes, int Hin, int Win, int Cin, int Cin_valid,
@@ -357,6 +519,12 @@ cudaError_t launch_conv_wgrad_bf16(const void* dy, const void* x, float* dW, int
     int TW = pow2_ceil_(Wo); if (TW > 64) TW = 64;
     int TH = pow2_ceil_(Ho); if (TW * TH > 64) TH = 64 / TW;
     const int TN = 64 / (TW * TH);
+    // the filter-row kernel takes 3x3 / stride-1 / pad-1 filters whose tile is whole rows of one image, at least one 8-pixel core
+    // group wide, on unpadded channels; same split count as umma_wgrad_kernel<64, 3> (128-co tiles, three filter-row CTAs)
+    if (g_wgrad_rows && ntaps == 9 && in_stride == 1 && planes == 1 && Hin == Ho && Win == Wo && TN == 1 && TW == Wo && TW % 8 == 0 &&
+        Cin_valid == Cin && standard_3x3_taps(dh, dw, dplane))
+        return launch_wgrad_rows(dy, x, dW, NB, Ho, Wo, Cin, Cin_valid, Cout, TW, TH, (Cout + WG_BM - 1) / WG_BM * (Cin / 64) * 3,
+                                    wg_tune_waves(), num_sms, st);
     p.mode = 1; p.TW = TW; p.TH = TH; p.TN = TN;
     p.tiles_w = (Wo + TW - 1) / TW; p.tiles_h = (Ho + TH - 1) / TH;
     p.num_kb = p.tiles_w * p.tiles_h * ((NB + TN - 1) / TN);

@@ -1,10 +1,11 @@
 """Per-kernel profile of one training step of the bench.py workload (ResNet-18, CIFAR shape, batch 256, one GPU).
 
-    python scripts/profile_step.py [--out DIR] [--replays N] [--bs 256] [--model resnet18] [--previous_tiles]
+    python scripts/profile_step.py [--out DIR] [--replays N] [--bs 256] [--model resnet18] [--previous_tiles] [--previous_wgrad]
 
 ``--model`` profiles another zoo model in the same configuration (e.g. ``resnet18_gn``).  ``--bn_reps`` sets the launches per call
 of the BatchNorm isolation and copy-reference measurements.  ``--previous_tiles`` profiles the step without the one-wave conv tiles
 (``set_conv_one_wave(False)``), for an A/B in one session.
+``--previous_wgrad`` profiles it with the weight-gradient kernels the filter-row kernel replaces (``set_wgrad_rows(False)``).
 
 Builds the engine exactly as ``bench.py`` does, runs one warm-up round (which captures the training-step CUDA graph), then
 replays the captured full-batch step ``--replays`` times under ``torch.profiler`` with CUDA activities.  The kernels inside the
@@ -121,6 +122,120 @@ def install_recorder(ext, sms, log):
                  ("stem_gemm_bf16", stem_gemm_bf16), ("advance_cursor", advance_cursor)):
         setattr(ext, n, f)
     return orig
+
+
+ROWS = True            # False: the weight-gradient kernels of set_wgrad_rows(False)
+WG_KERNELS = ("umma_wgrad_kernel", "umma_wgrad_halo_kernel", "umma_wgrad_rows_kernel")
+
+
+def wg_splits(base, num_kb, sms, low_waves=1):
+    """Split-K count of the weight-gradient launchers (wg_splits in wgrad.cu)."""
+    waves = -(-base // sms) if base >= sms else low_waves
+    splits = min(max((waves * sms) // base, 1), num_kb)
+    per = -(-num_kb // splits)
+    return -(-num_kb // per)
+
+
+def wgrad_launch(NB, Hin, Win, Cin, Ho, Wo, Cout, k, stride, pad, sms, cin_valid=None, rows=None):
+    """Kernel, grid, FLOP and L2 operand bytes of one conv weight-gradient launch (launch_conv_wgrad_bf16 / _halo_bf16 in wgrad.cu):
+    L2 operand bytes = every CTA's TMA boxes per k-block (dY tiles and input boxes or halos) over its split-K range."""
+    rows = ROWS if rows is None else rows
+    cin_valid = Cin if cin_valid is None else cin_valid
+    flop = 2.0 * NB * Ho * Wo * Cout * k * k * cin_valid
+    co128 = -(-Cout // 128)
+    std3 = k == 3 and stride == 1 and pad == 1
+    if std3 and Cin == 64 and Hin % 16 == 0 and Win % 8 == 0:                 # 16 x 8 tiles of 128 pixels
+        num_kb = NB * (Hin // 16) * (Win // 8)
+        splits = wg_splits(co128 * 3, num_kb, sms)
+        a_groups = 2 if Cout % 128 == 0 else 1
+        return {"kernel": "umma_wgrad_halo_kernel", "grid": (co128, 3, splits), "ctas": co128 * 3 * splits, "splits": splits,
+                "flop": flop, "l2_bytes": co128 * 3 * num_kb * (a_groups * 16384 + 18 * 16 * 128)}
+    TW = min(_pow2_ceil(Wo), 64)
+    TH = _pow2_ceil(Ho)
+    if TW * TH > 64:
+        TH = 64 // TW
+    TN = 64 // (TW * TH)
+    num_kb = -(-Wo // TW) * -(-Ho // TH) * -(-NB // TN)
+    ci_tiles = Cin // 64
+    if rows and std3 and TN == 1 and TW == Wo and TW % 8 == 0 and cin_valid == Cin:
+        splits = wg_splits(co128 * ci_tiles * 3, num_kb, sms)
+        tiles = -(-Cout // 64) * ci_tiles
+        return {"kernel": "umma_wgrad_rows_kernel", "grid": (tiles, 1, splits), "ctas": tiles * splits, "splits": splits,
+                "flop": flop, "l2_bytes": tiles * num_kb * (8192 + (TW + 2) * (TH + 2) * 128)}
+    wide = Cin % 128 == 0 and cin_valid == Cin and k == 1
+    taps = 3 if k == 3 else 1
+    groups = 2 if wide else 1
+    ci_tiles = Cin // (64 * groups)
+    a_groups = 2 if Cout > 64 else 1
+    splits = wg_splits(co128 * ci_tiles * (k * k // taps), num_kb, sms)
+    grid = (co128 * ci_tiles, k * k // taps, splits)
+    return {"kernel": f"umma_wgrad_kernel<{64 * groups}, {taps}>", "grid": grid, "ctas": grid[0] * grid[1] * splits, "splits": splits,
+            "flop": flop, "l2_bytes": grid[0] * grid[1] * num_kb * (a_groups * 8192 + taps * groups * 8192)}
+
+
+def install_wgrad_recorder(ext, sms, log):
+    """Wrap the extension's conv weight-gradient entry points so every call appends its ``wgrad_launch`` record to ``log``, with a
+    step delimiter at every ``advance_cursor``."""
+    orig = {n: getattr(ext, n) for n in ("conv_wgrad_bf16", "conv_wgrad_halo_bf16", "conv_wgrad_bf16_strided", "advance_cursor")}
+
+    def rec(dy, x, dW, stride, cin_valid, planes=1):
+        NB, Ho, Wo, Cout = dy.shape
+        k = dW.shape[1] if dW.dim() == 4 else 3
+        Hin, Win, Cin = x.shape[1], x.shape[2], x.shape[3]
+        if planes == 4:                                      # parity-split copy: each plane is one stride-2 phase
+            Hin, Win = 2 * Hin, 2 * Win
+        pad = (k - 1) // 2
+        r = wgrad_launch(NB, Hin, Win, Cin, Ho, Wo, Cout, k, stride, pad, sms, cin_valid)
+        r["shape"] = f"{k}x{k}/s{stride} {Hin}x{Win} {Cin}->{Cout}"
+        log.append(r)
+
+    def conv_wgrad_bf16(dy, x, dW, NB, planes, cin_valid, dh, dw, pl):
+        rec(dy, x, dW, 2 if planes == 4 else 1, cin_valid, planes)
+        return orig["conv_wgrad_bf16"](dy, x, dW, NB, planes, cin_valid, dh, dw, pl)
+
+    def conv_wgrad_halo_bf16(dy, x, dW, cin_valid):
+        rec(dy, x, dW, 1, cin_valid)
+        return orig["conv_wgrad_halo_bf16"](dy, x, dW, cin_valid)
+
+    def conv_wgrad_bf16_strided(dy, x, dW, cin_valid, dh, dw, in_stride):
+        rec(dy, x, dW, in_stride, cin_valid)
+        return orig["conv_wgrad_bf16_strided"](dy, x, dW, cin_valid, dh, dw, in_stride)
+
+    def advance_cursor(*a, **k):
+        log.append(None)
+        return orig["advance_cursor"](*a, **k)
+
+    for n, f in (("conv_wgrad_bf16", conv_wgrad_bf16), ("conv_wgrad_halo_bf16", conv_wgrad_halo_bf16),
+                 ("conv_wgrad_bf16_strided", conv_wgrad_bf16_strided), ("advance_cursor", advance_cursor)):
+        setattr(ext, n, f)
+    return orig
+
+
+def wgrad_table(wg_launches, kernels, replays):
+    """Rows of the weight-gradient table: traced weight-gradient kernels keyed by (kernel, grid), matched to the step's launch
+    records; the ordered split-K sums that follow them are in the kernel table (``ordered_sum``)."""
+    per = collections.defaultdict(lambda: [0, 0.0])
+    for e in kernels:
+        nm = short_name(e["name"])
+        if nm.startswith(WG_KERNELS):
+            g = tuple(e.get("args", {}).get("grid", [0, 0, 0])[:3])
+            per[(nm, g)][0] += 1
+            per[(nm, g)][1] += float(e["dur"])
+    by_key = collections.defaultdict(list)
+    for r in wg_launches:
+        by_key[(r["kernel"].replace(" ", ""), tuple(r["grid"]))].append(r)
+    out = []
+    for (nm, g), (cnt, us) in sorted(per.items(), key=lambda kv: -kv[1][1]):
+        calls = cnt / replays
+        us_step = us / replays
+        recs = by_key.get((nm.replace(" ", ""), g), [])
+        ok = bool(recs) and len(recs) == round(calls) and us_step > 0
+        flop = sum(r["flop"] for r in recs)
+        l2 = sum(r["l2_bytes"] for r in recs)
+        out.append({"kernel": nm, "grid": list(g), "calls_per_step": calls, "us_per_step": us_step,
+                    "launches": sorted({r["shape"] for r in recs}), "gflop": flop / 1e9, "l2_mb": l2 / 1e6,
+                    "tflops": flop / (us_step * 1e-6) / 1e12 if ok else None, "l2_tb_s": l2 / (us_step * 1e-6) / 1e12 if ok else None})
+    return out
 
 
 BN_KERNELS = ("channel_reduce_kernel", "bn_apply_kernel", "bn_bwd_apply_kernel", "ordered_sum")
@@ -319,6 +434,18 @@ def one_step_launches(log):
     return next(s for s in steps if s[0]["M"] == top)
 
 
+def one_step_launches_any(log):
+    """Launch records of the longest step in a log with ``None`` step delimiters (the full-batch eager warm-up step)."""
+    steps, cur = [], []
+    for r in log:
+        if r is None:
+            steps.append(cur)
+            cur = []
+        else:
+            cur.append(r)
+    return max(steps, key=len) if steps else []
+
+
 def gpu_info():
     q = "name,power.limit,clocks.max.sm"
     try:
@@ -344,6 +471,8 @@ def main():
     ap.add_argument("--crop_pad", type=int, default=0, help="training augmentation of the profiled step (engine flag --crop_pad)")
     ap.add_argument("--hflip", action="store_true", help="training augmentation of the profiled step (engine flag --hflip)")
     ap.add_argument("--previous_tiles", action="store_true", help="profile without the one-wave conv tiles (set_conv_one_wave(False))")
+    ap.add_argument("--previous_wgrad", action="store_true",
+                    help="profile with the weight-gradient kernels the filter-row kernel replaces (set_wgrad_rows(False))")
     ap.add_argument("--bn_reps", type=int, default=20, help="launches per BatchNorm call in the isolation and copy measurements")
     a = ap.parse_args()
 
@@ -361,8 +490,14 @@ def main():
         global ONE_WAVE
         ONE_WAVE = False
         ops.ext().set_conv_one_wave(False)
+    if a.previous_wgrad:
+        global ROWS
+        ROWS = False
+        ops.ext().set_wgrad_rows(False)
     log = []
     install_recorder(ops.ext(), sms, log)
+    wg_log = []
+    install_wgrad_recorder(ops.ext(), sms, wg_log)
     bn_log = []
     install_bn_recorder(ops.ext(), bn_log)
     ctx = init_distributed(None, None)
@@ -400,6 +535,7 @@ def main():
     kernels = _trace_kernels(prof)
     gpu = gpu_info()
     bn_launches = [r for r in one_step_launches(bn_log)] if any(bn_log) else []
+    wg_rows = wgrad_table(one_step_launches_any(wg_log), kernels, a.replays)
     bn_rows = bn_tables(bn_launches, kernels, a.replays, ops.ext(), torch.device("cuda", 0), a.bn_reps) if bn_launches else []
     eng.close()
 
@@ -442,7 +578,7 @@ def main():
            "kernel_us_per_step": total_us, "gemm_kernel_us_per_step": gemm_us, "gemm_kernel_share": gemm_us / total_us,
            "gemm_gflop_per_step": gemm_flop / 1e9, "gemm_tflops": gemm_flop / (gemm_us * 1e-6) / 1e12 if gemm_us else None,
            "conv_cluster": os.environ.get("RLR_CONV_CLUSTER", "default"), "one_wave_tiles": ONE_WAVE, "kernels": rows, "gemm_shapes": shape_rows,
-           "bn_shapes": bn_rows}
+           "bn_shapes": bn_rows, "wgrad_rows_kernel": ROWS, "wgrad_shapes": wg_rows}
     os.makedirs(a.out, exist_ok=True)
     with open(os.path.join(a.out, "profile_step.json"), "w") as f:
         json.dump(res, f, indent=1)
@@ -461,6 +597,16 @@ def main():
         bw = f'{r["l2_tb_s"]:.1f}' if r["l2_tb_s"] else "-"
         md.append(f'| `{r["kernel"].replace(KERNEL, "")}` | {r["grid"][0]}x{r["grid"][1]} | {r["calls_per_step"]:.0f} | '
                   f'{r["us_per_step"]:.1f} | {"; ".join(r["launches"]) or "-"} | {r["gflop"]:.1f} | {r["l2_mb"]:.0f} | {tf} | {bw} |')
+    if wg_rows:
+        md += ["", f"Weight gradients by launch grid ({'filter-row kernel' if ROWS else 'set_wgrad_rows(False)'}); GFLOP and L2 operand MB "
+               "from the launch shapes (every CTA's TMA boxes per k-block):", "",
+               "| kernel | grid | calls/step | us/step | launches | GFLOP | L2 operand MB | TFLOP/s | L2 TB/s |",
+               "|---|---|---:|---:|---|---:|---:|---:|---:|"]
+        for r in wg_rows:
+            tf = f'{r["tflops"]:.0f}' if r["tflops"] else "-"
+            bw = f'{r["l2_tb_s"]:.1f}' if r["l2_tb_s"] else "-"
+            md.append(f'| `{r["kernel"]}` | {"x".join(map(str, r["grid"]))} | {r["calls_per_step"]:.0f} | {r["us_per_step"]:.1f} | '
+                      f'{"; ".join(r["launches"]) or "-"} | {r["gflop"]:.1f} | {r["l2_mb"]:.0f} | {tf} | {bw} |')
     if bn_rows:
         fam = sum(r["us_per_step"] for r in bn_rows)
         md += ["", f"BatchNorm family by launch shape (kernel, grid): {fam:.1f} us/step in the step. MB = HBM bytes the pass must move "

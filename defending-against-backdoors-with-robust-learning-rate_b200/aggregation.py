@@ -5,6 +5,8 @@ step, executed by ONE fused kernel over the flat parameter vector (``ops.fused_a
 ``parallel.FusedAggregator`` across GPUs) instead of the reference's ~30 elementwise fp64 passes (SURVEY.md 2.4b).
 With ``--select krum | multikrum`` a selection stage runs first: the participants' pairwise update distances
 (``ops.pairwise_sqdist``), Krum scores on the host (``ops.krum_select``), and only the admitted participants enter the step.
+``--select dnc`` is that stage on DnC's spectral scores: the Gram matrices of the updates centred at random coordinate subsamples
+(``ops.dnc_grams``), and on the host the top eigenvector's outlier scores and the intersection of the kept sets (``ops.dnc_select``).
 ``--aggr fltrust`` and ``--aggr rfa`` are the same weighted-mean launch with weights from a per-participant pass: FLTrust's trust
 scores (``ops.trust_stats``) or RFA's smoothed Weiszfeld weights (``ops.rfa`` over ``ops.rfa_sqdist`` passes).  ``--aggr flame`` is
 that launch too: the Gram matrix of the updates (``ops.pairwise_gram``) gives FLAME's cosine clustering, median-norm clip scales and
@@ -20,6 +22,8 @@ diagnostics ``plot_norms`` / ``comp_diag_fisher`` / ``plot_sign_agreement`` (``-
 reference's latent bugs fixed (model built on the right device; Fisher uses log-probabilities -- SURVEY.md quirk 7).
 """
 from __future__ import annotations
+
+import math
 
 import numpy as np
 import torch
@@ -81,14 +85,15 @@ class Aggregation:
             raise ValueError("--aggr fltrust needs the server's root parameters (root_params)")
         clip = self._clip_scales(ops.update_norms(w_global, ws, nv)) if self._server_clip else None
         all_ids, all_ws = ids, ws
-        distances = lambda: ops.pairwise_sqdist(ws, nv if nv is not None else w_global.numel(), w_global if clip is not None else None,
-                                                clip)
+        n_voted = nv if nv is not None else w_global.numel()
+        distances = lambda: ops.pairwise_sqdist(ws, n_voted, w_global if clip is not None else None, clip)
+        dnc = lambda: ops.dnc_grams(ws, w_global, self._dnc_samples(cur_round, n_voted), n_voted, clip)
         rfa_pass = lambda b, members: ops.rfa_sqdist(
             [ws[j] for j in members], b, nv, w_global if clip is not None else None,
             clip[torch.as_tensor(members, device=clip.device)] if clip is not None else None)
         gram = lambda members: ops.pairwise_gram([ws[j] for j in members], w_global, nv)
         detection = lambda: self._fld_stage(ids, cur_round, *self._fld_local(w_global, ws, ids, nv))
-        keep, weights, scales, total, noise_std = self._admission(ids, clip, detection, distances,
+        keep, weights, scales, total, noise_std = self._admission(ids, clip, detection, distances, dnc,
                                                                   lambda: ops.trust_stats(ws, root_params, w_global, nv), rfa_pass, gram,
                                                                   lambda members: self._history_pass(w_global, ws, ids, members, nv),
                                                                   cur_round)
@@ -117,7 +122,7 @@ class Aggregation:
         norms = self.fused.update_norms(K) if self._server_clip or diag else None
         clip = self._clip_scales(norms) if self._server_clip else None
         copies, gathered = None, None
-        if (self._select or self._fltrust or self._flame or self._foolsgold or self._detecting or (self._rfa and self.args.rfa_iters > 0)) \
+        if (self._selecting or self._fltrust or self._flame or self._foolsgold or self._detecting or (self._rfa and self.args.rfa_iters > 0)) \
                 and self.fused.gathers(K):
             # on the gather transport every pass reads the same all-gathered copies (one all_gather per round; the root job included)
             gathered = self.fused.gather_participants(K + 1 if self._fltrust else K)
@@ -126,7 +131,9 @@ class Aggregation:
         detection = lambda: self._fld_stage(participants, cur_round, fused.fld_ring_update, fused.fld_gram,
                                             lambda order, coef: fused.fld_predict(K, participants, order, coef, copies))
         keep, weights, scales, total, noise_std = self._admission(
-            participants, clip, detection, lambda: self.fused.pairwise_sqdist(K, clip, copies), lambda: self.fused.trust_stats(K, K, gathered),
+            participants, clip, detection, lambda: self.fused.pairwise_sqdist(K, clip, copies),
+            lambda: self.fused.dnc_grams(K, self._dnc_samples(cur_round, self.fused.n_vote), clip, None, copies),
+            lambda: self.fused.trust_stats(K, K, gathered),
             lambda b, members: self.fused.rfa_sqdist(K, b, clip, members, copies),
             lambda members: self.fused.pairwise_gram(K, members, copies),
             lambda members: self.fused.foolsgold_gram(K, participants, members, copies), cur_round)
@@ -151,15 +158,16 @@ class Aggregation:
     def _select(self):
         return getattr(self.args, "select", "none") != "none"
 
-    def _admission(self, ids, clip, detection, distances, trust_stats, rfa_pass, gram, history, cur_round):
+    def _admission(self, ids, clip, detection, distances, dnc_grams, trust_stats, rfa_pass, gram, history, cur_round):
         """Admission of the participants ``ids`` shared by both forms of the step: FLDetector's ``detection()`` (``--detect``), which returns
-        the positions of the agents it has not flagged (None while it has flagged nobody), or Krum / Multi-Krum on ``distances()`` (``--select``),
+        the positions of the agents it has not flagged (None while it has flagged nobody), or Krum / Multi-Krum on ``distances()`` or DnC
+        on its Gram matrices ``dnc_grams()`` (``--select``),
         then FLTrust on ``trust_stats()`` (``--aggr fltrust``), RFA's weights from ``rfa_pass(b, members)`` (``--aggr rfa``), FLAME on
         the Gram matrix ``gram(members)`` (``--aggr flame``) or FoolsGold on ``history(members)``, the Gram matrix of the members' update
         histories after this round's updates are folded in (``--aggr foolsgold``).  ``clip``: the server-clipping scales or None.  Returns
         ``(members, weights, scales, total_weight, noise_std)`` for the step: members None admits everyone; weights are per position in
         ``ids``."""
-        keep = self._admit(distances(), ids, cur_round) if self._select else (detection() if self._detect else None)
+        keep = self._admit(ids, cur_round, distances, dnc_grams) if self._select else (detection() if self._detect else None)
         noise_std = self.args.noise * self.args.clip
         if self._fltrust:
             return (*self._trust(trust_stats(), ids, keep, cur_round), noise_std)
@@ -267,10 +275,18 @@ class Aggregation:
         self.fld_flagged = [int(i) for i in st["flagged"]]
         self.fld_detect_round = st["detect_round"]
 
-    def _admit(self, D, ids, cur_round):
-        """Krum / Multi-Krum admission from the pairwise distances ``D`` of the participants ``ids``: the admitted positions
-        (ascending).  Records ``last_admitted`` and logs how many corrupt participants (ids < num_corrupt) came and got through."""
-        keep = ops.krum_select(D, ids, self.args.select_f, self.args.select_m)
+    def _admit(self, ids, cur_round, distances, dnc_grams):
+        """``--select`` admission of the participants ``ids``: Krum / Multi-Krum from the pairwise distances ``distances()``, or DnC from
+        the Gram matrices ``dnc_grams()`` of this round's subsamples (everyone, with nothing launched, when it removes ``floor(c F) = 0``).
+        Returns the admitted positions (ascending).  Records ``last_admitted`` and logs how many corrupt participants (ids < num_corrupt)
+        came and got through."""
+        a = self.args
+        if a.select != "dnc":
+            keep = ops.krum_select(distances(), ids, a.select_f, a.select_m)
+        elif self._selecting:
+            keep = ops.dnc_select(dnc_grams(), ids, a.select_f, a.dnc_frac)
+        else:
+            keep = list(range(len(ids)))
         self.last_admitted = [ids[j] for j in keep]
         nc = self.args.num_corrupt
         self.last_select = {"Select/Corrupt_Participants": sum(1 for i in ids if i < nc),
@@ -279,6 +295,18 @@ class Aggregation:
             for k, v in self.last_select.items():
                 self.writer.add_scalar(k, v, cur_round)
         return keep
+
+    @property
+    def _selecting(self):
+        """True when ``--select`` runs a device pass this round: always for krum / multikrum, for dnc unless it removes nobody."""
+        if getattr(self.args, "select", "none") == "dnc":
+            return math.floor(self.args.dnc_frac * self.args.select_f) > 0
+        return self._select
+
+    def _dnc_samples(self, cur_round, n_vote):
+        """This round's DnC subsamples: ``ops.dnc_sample`` of every iteration, int64 numpy ``[T][min(b, n_vote)]``."""
+        a = self.args
+        return np.stack([ops.dnc_sample(a.seed, cur_round, t, a.dnc_dim, n_vote) for t in range(a.dnc_iters)])
 
     @property
     def _fltrust(self):

@@ -598,6 +598,137 @@ def krum_select(D, ids, f, m):
 
 
 # =====================================================================================================================
+# participant selection (DnC, Shejwalkar and Houmansadr, NDSS 2021): spectral scores on coordinate subsamples
+# =====================================================================================================================
+_DNC_TAG = 0x446E4321                    # "DnC!": keeps the subsample draws apart from every other stream seeded by --seed
+
+
+def dnc_sample(seed, rnd, t, b, n_vote):
+    """DnC's coordinate subsample of iteration ``t`` in round ``rnd``: ``min(b, n_vote)`` distinct coordinates of ``[0, n_vote)`` drawn
+    without replacement by a numpy Generator seeded by (seed, round, t) alone, sorted ascending (``b >= n_vote``: every coordinate).
+    Every rank, and a resumed run, draws the same sample.  Returns int64 numpy."""
+    n_vote, b = int(n_vote), int(b)
+    if n_vote >= 1 << 31:
+        raise ValueError(f"DnC samples int32 coordinates: n_vote {n_vote} >= 2^31")
+    if b >= n_vote:
+        return np.arange(n_vote, dtype=np.int64)
+    rng = np.random.default_rng([int(seed), int(rnd), int(t), _DNC_TAG])
+    return np.sort(rng.choice(n_vote, size=b, replace=False)).astype(np.int64)
+
+
+def dnc_gather_statement(w_agents, w_global, sample, scales=None):
+    """fp64 statement of DnC's gather over the coordinates ``sample``: ``x_k = (w_k - w_global)`` (``* scales[k]``) in fp64,
+    ``mu = (sum of the finite x_k, k ascending) / their count`` and ``Y[k] = fp32(x_k - mu)``, every operation rounded on its own -- the
+    bits ``dnc_gather_kernel`` writes.  With every update finite ``mu`` is the plain mean over the K participants; a non-finite ``x_k``
+    stays out of it and leaves its own entry non-finite.  Returns float32 ``[K][len(sample)]``."""
+    dev = w_global.device
+    idx = torch.as_tensor(np.asarray(sample, dtype=np.int64), device=dev)
+    g = w_global[idx].double()
+    x = [w[idx].double() - g for w in w_agents]
+    if scales is not None:
+        sc = torch.as_tensor(scales, dtype=torch.float32).to(dev).double()
+        x = [xk * sc[k] for k, xk in enumerate(x)]
+    mu = torch.zeros_like(g)
+    n = torch.zeros_like(g)
+    for xk in x:
+        fin = torch.isfinite(xk)
+        mu = torch.where(fin, mu + xk, mu)
+        n = n + fin.double()
+    mu = torch.where(n > 0, mu / n.clamp_min(1.0), torch.zeros_like(mu))
+    return torch.stack([(xk - mu).float() for xk in x])
+
+
+def dnc_gram_statement(w_agents, w_global, samples, scales=None):
+    """fp64 statement of DnC's device pass: for each iteration's sample (row ``t`` of ``samples``), the Gram matrix ``C_t = Y Y^T`` in fp64
+    of ``Y = dnc_gather_statement(...)``.  Returns float64 ``[T][K][K]``."""
+    out = [(lambda y: y @ y.T)(dnc_gather_statement(w_agents, w_global, s, scales).double()) for s in samples]
+    return torch.stack(out)
+
+
+def _dnc_ranges(samples, lo, hi):
+    """Per iteration, the positions ``[a, b)`` of the sorted sample rows that hold coordinates in ``[lo, hi)``, and the padded row
+    length: the largest ``b - a`` rounded up to a multiple of 4 (at least 4)."""
+    r = [(int(np.searchsorted(s, lo, "left")), int(np.searchsorted(s, hi, "left"))) for s in samples]
+    longest = max(b - a for a, b in r)
+    return r, max(4, (longest + 3) // 4 * 4)
+
+
+def dnc_launch(table, K, w_global_ptr, samples, scales, out, dev, lo=0, hi=None, gate=(None, None, 0, 1, 0)):
+    """DnC's device pass over the coordinates of ``samples`` (int64 numpy ``[T][S]``, rows sorted) that lie in ``[lo, hi)``: one
+    ``dnc_gather_kernel`` launch behind ``gate`` (flag_ptrs, local_sync, rank, world, epoch) into ``Y [T][K][len_pad]``, then one
+    ``history_gram`` launch per iteration into ``out[t]`` (float64 ``[T][K][K]``)."""
+    samples = np.asarray(samples, dtype=np.int64)
+    T = samples.shape[0]
+    hi = int(samples.max(initial=-1)) + 1 if hi is None else int(hi)
+    ranges, len_pad = _dnc_ranges(samples, lo, hi)
+    samp = torch.from_numpy(samples.astype(np.int32)).to(dev)
+    rng = torch.tensor(ranges, dtype=torch.int32).to(dev)
+    y = torch.empty((T, K, len_pad), dtype=torch.float32, device=dev)
+    rows = PtrTable([y[t, k].data_ptr() for t in range(T) for k in range(K)], dev, (y,))
+    sc = torch.as_tensor(scales, dtype=torch.float32).to(dev) if scales is not None else None
+    ext().dnc_gather(table, w_global_ptr, sc, samp, rng, y, *gate)
+    for t in range(T):
+        ext().history_gram(rows.tensor[t * K:(t + 1) * K], 0, len_pad, out[t])
+    return out
+
+
+def dnc_grams(w_agents, w_global, samples, n_vote=None, scales=None):
+    """DnC's Gram matrices, float64 ``[T][K][K]`` (``dnc_gram_statement``'s values), of the participants' centred updates at the sorted
+    coordinate samples ``samples`` (``[T][S]``, every coordinate ``< n_vote``).  ``scales``: the server-clipping scales or None.  On CUDA
+    this launches ``dnc_gather_kernel`` and one ``pairwise_sqdist_kernel<true, true>`` per iteration (ops/csrc/select.cu); on CPU, and for
+    more participants than the kernels' tables hold (recorded as a library fall-through), it evaluates ``dnc_gram_statement``."""
+    nv = w_global.numel() if n_vote is None else int(n_vote)
+    samples = np.asarray(samples, dtype=np.int64).reshape(len(samples), -1)
+    if samples.size and (samples.min() < 0 or samples.max() >= nv):
+        raise ValueError(f"DnC sample coordinates must lie in [0, n_vote={nv})")
+    if nv >= 1 << 31:
+        raise ValueError(f"DnC samples int32 coordinates: n_vote {nv} >= 2^31")
+    for w in (*w_agents, w_global):
+        if w.numel() < nv:
+            raise ValueError(f"a flat buffer of {w.numel()} values for n_vote {nv}")
+    K, T = len(w_agents), samples.shape[0]
+    # the gather reads only the sampled coordinates, so n_vote need not be a multiple of 4 (the lengths were checked above)
+    return _participant_pass("dnc_grams", w_agents, (w_global,), 0, (T, K, K),
+                             lambda: dnc_gram_statement(w_agents, w_global, samples, scales),
+                             lambda tab, out: dnc_launch(tab, K, w_global.data_ptr(), samples, scales, out, out.device, 0, nv))
+
+
+def dnc_scores(C):
+    """DnC's outlier scores of one iteration from its Gram matrix ``C = Y Y^T`` (float64 ``[K][K]``), on the host in fp64: with ``(lam, u)``
+    the top eigenpair of ``C`` (``numpy.linalg.eigh``), ``s_k = lam * u_k^2`` -- the squared projection ``<Y_k, v>^2`` of the centred update
+    onto the top right singular vector ``v`` of ``Y``.  A participant whose ``C_kk`` is not finite scores +inf and the others are scored on
+    their own block of ``C``; a NaN score counts as +inf.  Returns float64 numpy ``[K]``."""
+    c = np.asarray(torch.as_tensor(C).detach().double().cpu().numpy(), dtype=np.float64)
+    K = c.shape[0]
+    s = np.full(K, np.inf)
+    ok = np.flatnonzero(np.isfinite(np.diag(c)))
+    sub = c[np.ix_(ok, ok)]
+    if ok.size and np.all(np.isfinite(sub)):
+        lam, u = np.linalg.eigh(sub)
+        s[ok] = lam[-1] * u[:, -1] ** 2
+    s[np.isnan(s)] = np.inf
+    return s
+
+
+def dnc_select(grams, ids, f, c):
+    """DnC admission on the host, shared by every path: for each iteration's Gram matrix (``grams[t]``) the ``K - floor(c f)`` positions
+    with the lowest ``dnc_scores`` are kept, ties to the lower id in ``ids``; the admitted set is the intersection over the iterations.
+    Returns the admitted positions (indices into ``ids``) in ascending order."""
+    g = torch.as_tensor(grams).detach().double().cpu()
+    K = len(ids)
+    if g.dim() != 3 or tuple(g.shape[1:]) != (K, K):
+        raise ValueError(f"dnc_select: Gram matrices of shape {tuple(g.shape)} for {K} participants")
+    n_keep = K - math.floor(float(c) * int(f))
+    if n_keep < 1:
+        raise ValueError(f"DnC keeps K - floor(c F) >= 1 participants per iteration (K={K}, c={c}, F={f})")
+    keep = set(range(K))
+    for t in range(g.shape[0]):
+        s = dnc_scores(g[t]).tolist()
+        keep &= set(sorted(range(K), key=lambda k: (s[k], ids[k]))[:n_keep])
+    return sorted(keep)
+
+
+# =====================================================================================================================
 # FLTrust (Cao, Fang, Liu, Gong, NDSS 2021): trust scores against the server's root update
 # =====================================================================================================================
 def trust_statement(w_agents, w_ref, w_global, lo, hi):

@@ -169,6 +169,36 @@ void history_gram(at::Tensor row_ptrs, int64_t begin, int64_t end, at::Tensor ou
     check(rlr::launch_history_gram(p, out.data_ptr<double>(), num_sms(), cur_stream()), "history_gram");
 }
 
+// DnC: y [T][K][len_pad] fp32 <- the participants' centred updates at sample[t][ranges[t][0] .. ranges[t][1]), zero-padded.  world > 1:
+// the fused multi-GPU form, which first runs the aggregation's barrier-in at `epoch`.
+void dnc_gather(at::Tensor w_agent_ptrs, int64_t w_global_ptr, c10::optional<at::Tensor> scales, at::Tensor sample, at::Tensor ranges,
+                at::Tensor y, c10::optional<at::Tensor> flag_ptrs, c10::optional<at::Tensor> local_sync, int64_t rank, int64_t world,
+                int64_t epoch) {
+    CHECK_CUDA(w_agent_ptrs); CHECK_CUDA(sample); CHECK_CUDA(ranges); CHECK_CUDA(y);
+    TORCH_CHECK(w_agent_ptrs.scalar_type() == at::kLong, "pointer table must be int64");
+    TORCH_CHECK(sample.scalar_type() == at::kInt && sample.dim() == 2, "sample must be int32 [T, S]");
+    const int64_t T = sample.size(0), K = w_agent_ptrs.numel();
+    TORCH_CHECK(ranges.scalar_type() == at::kInt && ranges.numel() == 2 * T, "ranges must be int32 [T, 2]");
+    TORCH_CHECK(y.scalar_type() == at::kFloat && y.dim() == 3 && y.size(0) == T && y.size(1) == K, "y must be float32 [T, K, len_pad]");
+    TORCH_CHECK(w_global_ptr, "dnc_gather needs w_global");
+    const float* sc = ptr_or_null<const float>(scales);
+    if (sc) {
+        CHECK_CUDA(*scales);
+        TORCH_CHECK(scales->scalar_type() == at::kFloat && scales->numel() == K, "scales: float32 [K]");
+    }
+    c10::cuda::CUDAGuard guard(y.device());
+    rlr::DncParams p{};
+    p.w_agents = reinterpret_cast<const float* const*>(w_agent_ptrs.data_ptr());
+    p.w_global = reinterpret_cast<const float*>(w_global_ptr);
+    p.scales = sc;
+    p.sample = sample.data_ptr<int>();
+    p.ranges = ranges.data_ptr<int>();
+    p.y = y.data_ptr<float>();
+    p.T = (int)T; p.K = (int)K; p.stride = (int)sample.size(1); p.len_pad = (int)y.size(2);
+    p.gate = gate_of(flag_ptrs, local_sync, rank, world, epoch);
+    check(rlr::launch_dnc_gather(p, num_sms(), cur_stream()), "dnc_gather");
+}
+
 // FLDetector ring pass over [begin, end): s_ptr (0 = none) <- w_g - w_prev, then w_prev <- w_g.  Pointers offset so that absolute
 // coordinates index them.
 void fld_ring(int64_t w_g_ptr, int64_t w_prev_ptr, int64_t s_ptr, int64_t begin, int64_t end) {
@@ -524,6 +554,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("pairwise_gram", &pairwise_gram);
     m.def("history_accumulate", &history_accumulate);
     m.def("history_gram", &history_gram);
+    m.def("dnc_gather", &dnc_gather);
     m.def("fld_ring", &fld_ring);
     m.def("fld_hvp", &fld_hvp);
     m.def("fld_predict", &fld_predict);

@@ -69,6 +69,21 @@ cudaError_t launch_pairwise_gram(const DistParams& p, double* out, int num_sms, 
 // (the w_agents are the candidates' history rows, offset so that absolute coordinates index them).  Same kernel, tiles and fixed-order
 // sums as the distances; reads neither w_global nor scales.
 cudaError_t launch_history_gram(const DistParams& p, double* out, int num_sms, cudaStream_t st);
+// DnC: the participants' updates at T sampled coordinate sets, centred per coordinate.  For iteration t the coordinates are
+// sample[t][ranges[2t] .. ranges[2t + 1]) (sorted, < 2^31); y[t][k][q] = fp32(x_k - mu) at the q-th of them, x_k = (w_k - w_global)
+// (* scales[k]) in fp64 and mu the fp64 mean of the finite x_k in ascending k; rows zero-padded to len_pad (a multiple of 4), so
+// launch_history_gram takes them as its table.  No reductions across threads: bitwise reproducible.
+struct DncParams {
+    const float* const* w_agents;   // [K] device pointers (local or peer-mapped)
+    const float* w_global;          // this rank's global parameters
+    const float* scales;            // [K] server clipping scales or nullptr
+    const int* sample;              // [T][stride] sorted coordinates
+    const int* ranges;              // [T][2] position range [lo, hi) of row t that this launch gathers (hi - lo <= len_pad)
+    float* y;                       // [T][K][len_pad]
+    int T, K, stride, len_pad;
+    Gate gate;                      // world > 1: the aggregation's barrier-in
+};
+cudaError_t launch_dnc_gather(const DncParams& p, int num_sms, cudaStream_t st);
 
 // ---- FoolsGold: each candidate's update folded into its agent's history row ------------------------------------------------------
 // rows[k][c] <- fp32(rows[k][c] + fp32(w_agents[k][c] - w_global[c])) for begin <= c < end.  Exact fp32: bitwise reproducible.

@@ -232,4 +232,57 @@ cudaError_t launch_history_gram(const DistParams& p, double* out, int num_sms, c
     return launch_pairwise<true, true>(p, out, num_sms, st);
 }
 
+// DnC's sampled, centred updates (Shejwalkar and Houmansadr, NDSS 2021).  One thread per (iteration t, row position q): with c the
+// sample's coordinate at position lo_t + q, x_k = (w_k[c] - w_global[c]) (* s_k) in fp64, mu = (sum of the finite x_k, k ascending) /
+// (their count), and Y[t][k][q] = fp32(x_k - mu), every fp64 operation rounded on its own (the bits ops.dnc_gather_statement gives).
+// A non-finite x_k stays out of the mean and leaves its own entry non-finite, so it spoils only its own row of the Gram matrix.
+// Positions q >= hi_t - lo_t are written as zeros, the rows' padding to a multiple of 4.  Grid-stride loop over T * len_pad positions
+// on at most one wave of CTAs (every CTA has to be resident while the leader waits in barrier_in); nothing is reduced across threads.
+constexpr int kDncThreads = 256;
+
+__global__ void __launch_bounds__(kDncThreads) dnc_gather_kernel(DncParams p) {
+    barrier_in(p.gate, blockIdx.x == 0);
+    const long long total = (long long)p.T * p.len_pad;
+    for (long long e = (long long)blockIdx.x * kDncThreads + threadIdx.x; e < total; e += (long long)gridDim.x * kDncThreads) {
+        const int t = (int)(e / p.len_pad), q = (int)(e - (long long)t * p.len_pad);
+        float* const y = p.y + (size_t)t * p.K * p.len_pad + q;
+        const int lo = p.ranges[2 * t], hi = p.ranges[2 * t + 1];
+        if (q >= hi - lo) {
+            for (int k = 0; k < p.K; ++k) y[(size_t)k * p.len_pad] = 0.f;
+            continue;
+        }
+        const long long c = p.sample[(size_t)t * p.stride + lo + q];
+        const double g = (double)ld_f1(p.w_global + c);
+        auto x = [&](int k) {
+            const double d = __dsub_rn((double)ld_f1(p.w_agents[k] + c), g);
+            return p.scales ? __dmul_rn(d, (double)p.scales[k]) : d;
+        };
+        double mu = 0.0;
+        int n = 0;
+        for (int k = 0; k < p.K; ++k) {
+            const double v = x(k);
+            if (isfinite(v)) { mu = __dadd_rn(mu, v); ++n; }
+        }
+        mu = n ? __ddiv_rn(mu, (double)n) : 0.0;
+        for (int k = 0; k < p.K; ++k) y[(size_t)k * p.len_pad] = __double2float_rn(__dsub_rn(x(k), mu));
+    }
+}
+
+cudaError_t launch_dnc_gather(const DncParams& p, int num_sms, cudaStream_t st) {
+    if (p.K < 1 || p.T < 1 || p.len_pad < 4 || (p.len_pad & 3) || p.stride < 0 || !p.w_agents || !p.w_global || !p.sample || !p.ranges || !p.y)
+        return cudaErrorInvalidValue;
+    if (!gate_ok(p.gate)) return cudaErrorInvalidValue;
+    static int occ = 0;
+    if (!occ) {
+        RLR_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, dnc_gather_kernel, kDncThreads, 0));
+        occ = occ < 1 ? 1 : occ;
+    }
+    // every rank launches at least one CTA, whatever its share of the sample: the barrier-in waits for all of them
+    const long long need = ((long long)p.T * p.len_pad + kDncThreads - 1) / kDncThreads;
+    const long long cap = (long long)occ * num_sms;
+    const int grid = (int)(need < 1 ? 1 : (need < cap ? need : cap));
+    dnc_gather_kernel<<<grid, kDncThreads, 0, st>>>(p);
+    return cudaGetLastError();
+}
+
 }  // namespace rlr

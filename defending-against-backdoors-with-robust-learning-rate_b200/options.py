@@ -21,7 +21,10 @@ RFA_NU = 1e-6                    # RFA smoothing: distances below nu count as nu
 FLAME_LAMBDA = 1e-3              # FLAME noise factor: the paper's value for image classification
 LIFESPAN_THRESHOLD = 0.5         # poison accuracy below which the backdoor counts as gone
 SERVER_OPTS = ("sgd", "momentum", "adagrad", "adam", "yogi")
-SELECTIONS = ("none", "krum", "multikrum")
+SELECTIONS = ("none", "krum", "multikrum", "dnc")
+DNC_DIM = 10000                  # DnC: coordinates per subsample b
+DNC_ITERS = 1                    # DnC: subsample iterations T
+DNC_FRAC = 1.0                   # DnC: filtering fraction c; each iteration removes floor(c F) participants
 DETECTORS = ("none", "fldetector")
 FLD_WINDOW = 10                  # FLDetector: the L-BFGS memory and the score window N
 FLD_START = 0                    # FLDetector: the first round detection may run (it also waits for round 2N + 1)
@@ -114,12 +117,22 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--server_beta2", type=float, default=0.99, help="adam / yogi second-moment decay, in [0, 1)")
     p.add_argument("--server_tau", type=float, default=1e-3, help="adagrad / adam / yogi adaptivity tau > 0 (v starts at tau^2)")
     p.add_argument("--select", type=str, default="none", choices=SELECTIONS,
-                   help="participant selection before the --aggr rule (Blanchard et al. 2017): krum admits the participant whose update "
-                        "is closest to its K-F-2 nearest neighbours; multikrum the M best such scores.  Rejected participants take no "
-                        "part in the round (vote, rule, BatchNorm mean, noise, server optimizer)")
+                   help="participant selection before the --aggr rule: krum (Blanchard et al. 2017) admits the participant whose update "
+                        "is closest to its K-F-2 nearest neighbours; multikrum the M best such scores; dnc (Shejwalkar and Houmansadr "
+                        "2021) removes, on each of --dnc_iters random coordinate subsamples, the floor(c F) participants whose centred "
+                        "updates lie furthest along their top principal direction.  Rejected participants take no part in the round "
+                        "(vote, rule, BatchNorm mean, noise, server optimizer)")
     p.add_argument("--select_f", type=int, default=-1,
                    help="Byzantine participants the selection assumes (-1 = ceil(num_corrupt * K / num_agents), K participants per round)")
     p.add_argument("--select_m", type=int, default=0, help="participants multikrum admits (0 = K - F; krum admits 1)")
+    p.add_argument("--dnc_dim", type=int, default=None,
+                   help=f"--select dnc: coordinates b >= 1 of each subsample of the voted coordinates (default {DNC_DIM}; b >= n_vote "
+                        "takes every coordinate)")
+    p.add_argument("--dnc_iters", type=int, default=None,
+                   help=f"--select dnc: subsamples T >= 1 per round; the admitted set is the intersection of their kept sets "
+                        f"(default {DNC_ITERS})")
+    p.add_argument("--dnc_frac", type=float, default=None,
+                   help=f"--select dnc: filtering fraction c >= 0; each subsample removes floor(c F) participants (default {DNC_FRAC})")
     p.add_argument("--root_size", type=int, default=None,
                    help=f"--aggr fltrust: clean training samples the server trains its root update on each round (default {ROOT_SIZE}); "
                         "drawn once from --seed, never a poisoned sample")
@@ -297,7 +310,8 @@ def _finalize_flame(args) -> None:
         raise ValueError("--noise does not combine with --aggr flame, which adds noise of std --flame_lambda times the clip bound")
     # FLAME admits at least floor(K'/2) + 1 of the K' candidates whenever their norms are finite: the fewest voters it guarantees
     K = max(1, math.floor(args.num_agents * args.agent_frac))
-    cand = args.select_m if getattr(args, "select", "none") != "none" else K
+    select = getattr(args, "select", "none")
+    cand = dnc_fewest(args) if select == "dnc" else (args.select_m if select != "none" else K)
     if args.robustLR_threshold > cand // 2 + 1:
         raise ValueError(f"--robustLR_threshold {args.robustLR_threshold} > {cand // 2 + 1}, the fewest participants --aggr flame admits "
                          f"of {cand}, could flip every coordinate")
@@ -336,14 +350,41 @@ def _finalize_fltrust(args) -> None:
     args.root_size = int(root_size)
 
 
+def dnc_fewest(args) -> int:
+    """The fewest participants ``--select dnc`` can admit: ``K - T floor(c F)``, every iteration removing others."""
+    K = max(1, math.floor(args.num_agents * args.agent_frac))
+    return K - args.dnc_iters * math.floor(args.dnc_frac * args.select_f)
+
+
+def _finalize_dnc(args) -> None:
+    """Validate the DnC flags and resolve their defaults in place (``DNC_DIM`` / ``DNC_ITERS`` / ``DNC_FRAC`` under ``--select dnc``)."""
+    dim, iters, frac = (getattr(args, k, None) for k in ("dnc_dim", "dnc_iters", "dnc_frac"))
+    if getattr(args, "select", "none") != "dnc":
+        if dim is not None or iters is not None or frac is not None:
+            raise ValueError("--dnc_dim / --dnc_iters / --dnc_frac need --select dnc")
+        return
+    dim = DNC_DIM if dim is None else dim
+    iters = DNC_ITERS if iters is None else iters
+    frac = DNC_FRAC if frac is None else frac
+    if int(dim) != dim or dim < 1:
+        raise ValueError(f"--dnc_dim {dim} must be an integer >= 1")
+    if int(iters) != iters or iters < 1:
+        raise ValueError(f"--dnc_iters {iters} must be an integer >= 1")
+    if not (math.isfinite(frac) and frac >= 0):
+        raise ValueError(f"--dnc_frac {frac} must be a finite number >= 0")
+    args.dnc_dim, args.dnc_iters, args.dnc_frac = int(dim), int(iters), float(frac)
+
+
 def _finalize_select(args) -> None:
-    """Validate ``--select`` and resolve its defaults in place: ``select_f`` = F, ``select_m`` = M (1 for krum)."""
+    """Validate ``--select`` and resolve its defaults in place: ``select_f`` = F, ``select_m`` = M (1 for krum; unused by dnc) and,
+    under dnc, its flags (``_finalize_dnc``)."""
     select = getattr(args, "select", "none")
     if select not in SELECTIONS:
         raise ValueError(f"unknown --select {select!r}; expected one of {SELECTIONS}")
+    _finalize_dnc(args)
     if select == "none":
         if getattr(args, "select_f", -1) != -1 or getattr(args, "select_m", 0) != 0:
-            raise ValueError("--select_f / --select_m need --select krum or multikrum")
+            raise ValueError("--select_f / --select_m need --select krum or multikrum (--select_f also dnc)")
         return
     K = max(1, math.floor(args.num_agents * args.agent_frac))
     f = args.select_f
@@ -351,6 +392,18 @@ def _finalize_select(args) -> None:
         raise ValueError(f"--select_f {f} must be >= 0 (or -1 for the default)")
     if f == -1:
         f = math.ceil(args.num_corrupt * K / args.num_agents)
+    if select == "dnc":
+        if getattr(args, "select_m", 0) != 0:
+            raise ValueError(f"--select_m {args.select_m} needs --select multikrum; dnc admits what its iterations keep")
+        args.select_f = f
+        fewest = dnc_fewest(args)
+        if fewest < 1:
+            raise ValueError(f"--select dnc could admit nobody: K - T floor(c F) = {K} - {args.dnc_iters} x floor({args.dnc_frac} x {f}) "
+                             f"= {fewest} < 1")
+        if args.robustLR_threshold > fewest:
+            raise ValueError(f"--robustLR_threshold {args.robustLR_threshold} > {fewest}, the fewest participants --select dnc admits, "
+                             "could flip every coordinate")
+        return
     if K < 2 * f + 3:
         raise ValueError(f"--select {select} needs K >= 2F + 3 participants per round (K={K}, F={f})")
     m = args.select_m
@@ -403,8 +456,10 @@ def print_exp_details(args) -> None:
     print(f"    Crop pad / hflip: {args.crop_pad} / {args.hflip}")
     if getattr(args, "server_opt", "sgd") != "sgd":
         print(f"    Server optimizer (beta1 / beta2 / tau): {args.server_opt} ({args.server_beta1} / {args.server_beta2} / {args.server_tau})")
-    if getattr(args, "select", "none") != "none":
+    if getattr(args, "select", "none") in ("krum", "multikrum"):
         print(f"    Selection (F / M): {args.select} ({args.select_f} / {args.select_m})")
+    if getattr(args, "select", "none") == "dnc":
+        print(f"    Selection DnC (F / c / b / T): {args.select_f} / {args.dnc_frac} / {args.dnc_dim} / {args.dnc_iters}")
     if args.aggr == "fltrust":
         print(f"    Root set: {args.root_size}")
     if args.aggr == "rfa":

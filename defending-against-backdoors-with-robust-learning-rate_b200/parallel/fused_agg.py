@@ -40,6 +40,7 @@ from __future__ import annotations
 
 from functools import partial
 
+import numpy as np
 import torch
 
 from .. import ops
@@ -236,6 +237,35 @@ class FusedAggregator:
                                                               self.w_global.data_ptr() if sc is not None else 0, sc))
         agents = self._participants(n_part, participants)
         return ops.pairwise_sqdist(agents, self.n_vote, self.w_global if scales is not None else None, scales)
+
+    def dnc_grams(self, n_part: int, samples, scales=None, members=None, participants=None):
+        """DnC pass (``ops.dnc_gram_statement``): the float64 ``[T][K][K]`` Gram matrices of the centred updates of the participants at
+        positions ``members`` (ascending; every one of the round's ``n_part`` when None) at the sorted coordinate samples ``samples``
+        (``[T][S]``, ``ops.dnc_sample``'s rows), identical on every rank.  ``scales`` (server clipping) is per participant.  Call it after
+        the slots are final and before ``aggregate`` of the same round.
+
+        Fused multi-GPU path: one ``_fused_pass``.  Each rank takes the sample positions whose coordinates lie in its slice of
+        ``[0, n_vote)`` (``searchsorted`` on the sorted rows; centring works one coordinate at a time, so the split is exact), runs
+        ``dnc_gather_kernel`` over the peer-mapped slots behind the aggregation kernel's barrier-in (an epoch of its own) and the Gram
+        kernel over its rows; the ranks all_gather their partial matrices and add them in rank order.  The gather reads ``w_global``,
+        so it first acquires the broadcast slices of a fused hand-off.  Gather transport and single process: the same kernels over
+        ``participants`` (``gather_participants``' copies; gathered here when not given).  The reduce transport never holds every
+        participant on one rank, so the pass takes the gather transport, as Krum's does."""
+        idx = list(range(n_part)) if members is None else [int(j) for j in members]
+        if scales is not None:
+            scales = scales[torch.as_tensor(idx, device=scales.device)] if torch.is_tensor(scales) else [scales[j] for j in idx]
+        samples = np.asarray(samples, dtype=np.int64).reshape(len(samples), -1)
+        if self._p2p(n_part):
+            if self.n_vote >= 1 << 31:
+                raise ValueError(f"DnC samples int32 coordinates: n_vote {self.n_vote} >= 2^31")
+            self.acquire()
+            dev = self.ctx.device
+            table = self._agent_table(n_part) if idx == list(range(n_part)) else self._member_table(idx)
+            K = len(idx)
+            return self._fused_pass((samples.shape[0], K, K), lambda begin, end, out, *gate: ops.dnc_launch(
+                table.tensor, K, self.w_global.data_ptr(), samples, scales, out, dev, begin, end, gate))
+        agents = self._participants(n_part, participants)
+        return ops.dnc_grams([agents[j] for j in idx], self.w_global, samples, self.n_vote, scales)
 
     def trust_stats(self, n_part: int, ref: int, participants=None):
         """FLTrust statistics (``ops.trust_statement``'s float64 ``[2 n_part + 1]`` layout) of the round's ``n_part`` participants against

@@ -184,6 +184,9 @@ class FLEngine:
         p = float(getattr(args, "attack_neurotoxin", 0.0))
         self.neurotoxin_k = math.floor(p * self.layout.n_params) if p > 0 else None
         self.last_masked_coords = None
+        # colluding attackers (DESIGN.md section 3): stateless, so nothing is allocated and checkpoints are unchanged
+        self.collude = getattr(args, "attack_collude", "none")
+        self.last_collude = None
         if self.neurotoxin_k is not None:
             nv = self.layout.n_vote
             self.w_prev = torch.zeros(nv, dtype=torch.float32, device=dev)
@@ -372,6 +375,7 @@ class FLEngine:
                 self.round_loss += part
         self.timer.stop("local_train")
         self.timer.start("aggregate")
+        self.last_collude = self._collude(chosen, rnd) if (attack and self.collude != "none") else None
         self.aggregator.aggregate_slots(chosen, rnd)
         self.timer.stop("aggregate")
         return {"chosen": chosen, "steps": steps, "h2d_bytes": h2d}
@@ -395,6 +399,26 @@ class FLEngine:
         stream."""
         if self.attack_boost != 1.0 and agent.is_corrupt and attack:
             ops.boost_update(slot, self.w_global, self.attack_boost, self.layout.n_vote)
+
+    def _collude(self, chosen, rnd: int):
+        """Colluding attackers in an attack round: every corrupt participant's slot gets the update crafted from the honest participants'
+        ones (``FusedAggregator.collude``).  Returns the round's log fields, or None when no corrupt agent takes part (nothing is launched).
+        With no honest participant there is nothing to craft from: the corrupt updates stay as trained, and the round logs H = 0."""
+        corrupt = [j for j, a in enumerate(chosen) if self.agents[a].is_corrupt]
+        if not corrupt:
+            return None
+        honest = [j for j, a in enumerate(chosen) if not self.agents[a].is_corrupt]
+        if not honest:
+            if self.verbose:
+                print(f"| Collude: no honest participant in round {rnd}; the corrupt updates are left as trained |")
+            return {"collude_honest": 0}
+        alie = self.collude == "alie"
+        z = (self.args.alie_z if self.args.alie_z is not None else ops.collude_z(len(honest), len(corrupt))) if alie else None
+        info = self.fused.collude(len(chosen), honest, corrupt, self.collude, self.args.collude_dir, z)
+        rec = {"collude_honest": len(honest), "collude_deviation": info["deviation"]}
+        if alie:
+            rec["collude_z"] = z
+        return rec
 
     def round_result(self):
         """Device->host read of the round's result: (summed local training loss on this rank, number of REAL coordinates whose
@@ -477,6 +501,11 @@ class FLEngine:
             if self.last_masked_coords is not None:
                 rec["attack_masked_coords"] = self.last_masked_coords
                 self.logger.add_scalar("Attack/Masked_Coords", self.last_masked_coords, rnd)
+            if self.last_collude is not None:
+                rec.update(self.last_collude)
+                for key, tag in (("collude_honest", "Honest"), ("collude_deviation", "Deviation"), ("collude_z", "Z")):
+                    if key in self.last_collude:
+                        self.logger.add_scalar(f"Attack/Collude_{tag}", self.last_collude[key], rnd)
             if self.schedule:
                 rec["attack_active"] = self.last_attack_active
                 self.logger.add_scalar("Attack/Active", int(self.last_attack_active), rnd)

@@ -1328,6 +1328,156 @@ def boost_update(slot, w_g, gamma: float, n_vote: int):
     slot[:n_vote].copy_(torch.from_numpy(boost_statement(slot, w_g, gamma, n_vote)))
 
 
+# ---- colluding attackers: ALIE (Baruch et al. 2019), Min-Max / Min-Sum (Shejwalkar and Houmansadr 2021) --------------------------------
+COLLUDE_DIR_IDS = {"backdoor": 0, "std": 1, "sign": 2, "unit": 3}     # ColludeParams::dir of ops/csrc/collude.cu
+
+
+def collude_z(H: int, C: int) -> float:
+    """ALIE's default z for ``H`` honest and ``C`` corrupt participants: ``Phi^-1((K - s) / K)`` with ``K = H + C`` and
+    ``s = max(1, floor(K / 2) + 1 - C)``, floored at 0."""
+    from statistics import NormalDist
+    K = int(H) + int(C)
+    s = max(1, K // 2 + 1 - int(C))
+    p = (K - s) / K if K > 0 else 0.0
+    return max(0.0, NormalDist().inv_cdf(p)) if 0.0 < p < 1.0 else 0.0
+
+
+def collude_gamma(mode: str, a, e, q, D) -> float:
+    """The largest ``gamma >= 0`` for which ``m = mu - gamma u`` meets the Min-Max (``max_k ||m - x_k||^2 <= max_ij D_ij``) or Min-Sum
+    (``sum_k ||m - x_k||^2 <= max_i sum_j D_ij``) constraint, in closed form in fp64 on the host.  ``a_k = ||mu - x_k||^2``,
+    ``e_k = <mu - x_k, u>`` and ``q = ||u||^2`` over the H honest participants, ``D`` their squared-distance matrix.  Since
+    ``||m - x_k||^2 = a_k - 2 gamma e_k + gamma^2 q``: Min-Max takes ``min_k (e_k + sqrt(e_k^2 + q (Dmax - a_k))) / q`` and Min-Sum
+    ``(E + sqrt(E^2 + H q (S - A))) / (H q)`` with ``E = sum e_k``, ``A = sum a_k``.  A discriminant below 0 (rounding) counts as 0;
+    ``q = 0``, a non-finite input or result, or a result below 0 gives 0."""
+    if mode not in ("minmax", "minsum"):
+        raise ValueError(f"collude_gamma: unknown mode {mode!r}")
+    a = np.asarray(torch.as_tensor(a).double().cpu(), dtype=np.float64).reshape(-1)
+    e = np.asarray(torch.as_tensor(e).double().cpu(), dtype=np.float64).reshape(-1)
+    D = np.asarray(torch.as_tensor(D).double().cpu(), dtype=np.float64).reshape(a.size, a.size)
+    q = float(q)
+    if not (math.isfinite(q) and q > 0 and np.isfinite(a).all() and np.isfinite(e).all() and np.isfinite(D).all()):
+        return 0.0
+    with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+        if mode == "minmax":
+            disc = np.maximum(e * e + q * (D.max() - a), 0.0)
+            g = float(((e + np.sqrt(disc)) / q).min())
+        else:
+            E, A, Hq = float(e.sum()), float(a.sum()), a.size * q
+            disc = E * E + Hq * (float(D.sum(1).max()) - A)
+            g = (E + math.sqrt(max(disc, 0.0))) / Hq if math.isfinite(disc) else math.nan
+    return g if (math.isfinite(g) and g > 0) else 0.0
+
+
+def _collude_coords(honest, corrupt, w_g, lo, hi, direction, need_sig):
+    """fp64 ``(g, x, fin, mu, sig, xc, u)`` over coordinates ``[lo, hi)``, every operation a separate torch op rounded on its own."""
+    H = len(honest)
+    g = w_g[lo:hi].double()
+    x = torch.stack([w[lo:hi] for w in (*honest, *corrupt)]).double() - g
+    fin = torch.isfinite(x)
+    z = torch.zeros_like(g)
+    s, n = z.clone(), fin[:H].sum(0)
+    for j in range(H):
+        s = torch.where(fin[j], s + x[j], s)
+    mu = torch.where(n > 0, s / n.clamp(min=1).double(), z)
+    sig = z
+    if need_sig:
+        v = z.clone()
+        for j in range(H):
+            d = x[j] - mu
+            v = torch.where(fin[j], v + d * d, v)
+        sig = torch.where(n >= 2, torch.sqrt(v / (n - 1).clamp(min=1).double()), z)
+    xc = mu
+    if direction == "backdoor":
+        sc, nc = z.clone(), fin[H:].sum(0)
+        for j in range(H, x.shape[0]):
+            sc = torch.where(fin[j], sc + x[j], sc)
+        xc = torch.where(nc > 0, sc / nc.clamp(min=1).double(), mu)
+    u = {"std": lambda: sig, "sign": lambda: (mu > 0).double() - (mu < 0).double(), "unit": lambda: mu,
+         "backdoor": lambda: mu - xc}[direction]()
+    return g, x, fin, mu, sig, xc, u
+
+
+def collude_statement(honest, corrupt, w_g, n_vote, mode, direction, z=None, gamma=None, D=None, lo=0, hi=None):
+    """The colluding attackers' crafted update over coordinates ``[lo, hi)`` (default ``[lo, n_vote)``) in fp64, every operation rounded
+    on its own (ops/csrc/collude.cu states the rule).  ``honest`` / ``corrupt``: the flat parameter vectors of the round's honest and
+    corrupt participants, each in position order.  ``z`` (alie) defaults to ``collude_z``; ``gamma`` (minmax / minsum) defaults to
+    ``collude_gamma`` on this statement's ``a``, ``e``, ``q`` and ``D`` (the honest squared distances, ``sqdist_statement``'s by default).
+    Returns a dict: ``slot`` (fp32 ``[hi - lo]``, what every corrupt participant submits there), ``a`` / ``e`` (float64 ``[H]``), ``q``,
+    ``dev2 = sum (m - mu)^2``, ``gamma`` and ``z``."""
+    H, C = len(honest), len(corrupt)
+    hi = int(n_vote) if hi is None else int(hi)
+    dev = w_g.device
+    alie = mode == "alie"
+    if alie and z is None:
+        z = collude_z(H, C)
+    need_sig = alie or direction == "std"
+    step = max(4, (1 << 24) // max(1, H + C))
+    a = torch.zeros(H, dtype=torch.float64, device=dev)
+    e = torch.zeros(H, dtype=torch.float64, device=dev)
+    q = torch.zeros((), dtype=torch.float64, device=dev)
+    if not alie:
+        for c in range(lo, hi, step):
+            _, x, fin, mu, _, _, u = _collude_coords(honest, corrupt, w_g, c, min(hi, c + step), direction, need_sig)
+            d = torch.where(fin[:H], mu - x[:H], torch.zeros_like(x[:H]))
+            a += (d * d).sum(1)
+            e += (d * u).sum(1)
+            q += (u * u).sum()
+        if gamma is None:
+            D = sqdist_statement(list(honest), lo, hi) if D is None else D
+            gamma = collude_gamma(mode, a, e, q, D)
+    slot = torch.empty(hi - lo, dtype=torch.float32, device=dev)
+    dev2 = torch.zeros((), dtype=torch.float64, device=dev)
+    for c in range(lo, hi, step):
+        g, _, _, mu, sig, xc, u = _collude_coords(honest, corrupt, w_g, c, min(hi, c + step), direction, need_sig)
+        if alie:
+            t = float(z) * sig
+            m = mu - t if direction == "std" else torch.minimum(torch.maximum(xc, mu - t), mu + t)
+        else:
+            m = mu - float(gamma) * u
+        slot[c - lo:min(hi, c + step) - lo] = (g + m).float()
+        dev2 += ((m - mu) ** 2).sum()
+    return {"slot": slot, "a": a, "e": e, "q": float(q), "dev2": float(dev2), "gamma": None if alie else float(gamma),
+            "z": float(z) if alie else None}
+
+
+def collude_stats(honest, corrupt, w_g, n_vote, direction):
+    """Min-Max / Min-Sum statistics pass: float64 ``[2H + 1]`` = ``(a_k, e_k, q)`` over ``[0, n_vote)`` (``collude_statement``'s values).
+    On CUDA this launches ``collude_kernel<STATS>`` (ops/csrc/collude.cu); on CPU, and for more participants than the kernel's tables hold
+    (recorded as a library fall-through), it evaluates the statement."""
+    H = len(honest)
+    nv = int(n_vote)
+
+    def statement():
+        st = collude_statement(honest, corrupt, w_g, nv, "minmax", direction, gamma=0.0)
+        return torch.cat([st["a"], st["e"], torch.tensor([st["q"]], dtype=torch.float64, device=st["a"].device)])
+
+    def launch(tab, out):
+        ext().collude_stats(tab, H, w_g.data_ptr(), COLLUDE_DIR_IDS[direction], 0, nv, out, None, None, 0, 1, 0)
+    return _participant_pass("collude_stats", [*honest, *corrupt], (w_g,), nv, (2 * H + 1,), statement, launch)
+
+
+def collude_write(honest, corrupt, outs, w_g, n_vote, mode, direction, z=0.0, gamma=0.0):
+    """Write pass: every buffer of ``outs`` (the corrupt participants' slots; they may be the ``corrupt`` inputs themselves) gets the
+    crafted update over ``[0, n_vote)`` (``collude_statement``'s ``slot``, with ``z`` for alie and ``gamma`` for minmax / minsum); the
+    BatchNorm statistics behind ``n_vote`` are left alone.  Returns float64 ``[1]`` = ``sum (m - mu)^2``.  On CUDA this launches
+    ``collude_kernel<WRITE>`` (ops/csrc/collude.cu); on CPU, and for more participants than the kernel's tables hold (recorded as a
+    library fall-through), it evaluates the statement."""
+    H = len(honest)
+    nv = int(n_vote)
+
+    def statement():
+        st = collude_statement(honest, corrupt, w_g, nv, mode, direction, z=z, gamma=gamma)
+        for o in outs:
+            o[:nv].copy_(st["slot"])
+        return torch.tensor([st["dev2"]], dtype=torch.float64, device=w_g.device)
+
+    def launch(tab, out):
+        ot = PtrTable([o.data_ptr() for o in outs], out.device, list(outs)) if outs else None
+        ext().collude_write(tab, H, ot.tensor if ot is not None else None, w_g.data_ptr(), 0 if mode == "alie" else 1,
+                            COLLUDE_DIR_IDS[direction], float(z or 0.0), float(gamma or 0.0), 0, nv, out, None, None, 0, 1, 0)
+    return _participant_pass("collude_write", [*honest, *corrupt], (w_g, *outs), nv, (1,), statement, launch)
+
+
 def swap_samples(data, targets, idx, side_data, side_targets):
     """Attack schedules: exchange the dataset rows and labels at ``idx`` with the side copy in place, ``data[idx[i]] <-> side_data[i]``
     and ``targets[idx[i]] <-> side_targets[i]``.  The ``idx`` must be distinct (checked once, where the side copy is built), so the

@@ -293,6 +293,49 @@ void rfa_sqdist(at::Tensor w_agent_ptrs, at::Tensor b, int64_t w_global_ptr, c10
     check(rlr::launch_rfa_sqdist(p, out.data_ptr<double>(), num_sms(), cur_stream()), "rfa_sqdist");
 }
 
+// Colluding attackers: the statistics pass (out = float64 [2H + 1]: a_k, e_k, q) or, with out_ptrs, the write pass (out = float64 [1]:
+// sum (m - mu)^2) over coordinates [begin, end) of the H honest then C corrupt participants in w_agent_ptrs.  world > 1: the fused
+// multi-GPU form, which first runs the aggregation's barrier-in at `epoch`.
+rlr::ColludeParams collude_params(const at::Tensor& w_agent_ptrs, int64_t H, int64_t w_global_ptr, int64_t mode, int64_t dir, int64_t begin,
+                                  int64_t end, const at::Tensor& out, int64_t nout) {
+    CHECK_CUDA(w_agent_ptrs); CHECK_CUDA(out);
+    TORCH_CHECK(w_agent_ptrs.scalar_type() == at::kLong, "pointer table must be int64");
+    TORCH_CHECK(H >= 1 && H <= w_agent_ptrs.numel(), "collude: 1 <= H <= participants");
+    TORCH_CHECK(out.scalar_type() == at::kDouble && out.numel() == nout, "collude: out must be a float64 tensor of ", nout, " values");
+    TORCH_CHECK(w_global_ptr, "collude: w_global is required");
+    rlr::ColludeParams p{};
+    p.w_agents = reinterpret_cast<const float* const*>(w_agent_ptrs.data_ptr());
+    p.w_global = reinterpret_cast<const float*>(w_global_ptr);
+    p.begin = begin; p.end = end;
+    p.H = (int)H; p.C = (int)(w_agent_ptrs.numel() - H);
+    p.mode = (int)mode; p.dir = (int)dir;
+    return p;
+}
+
+void collude_stats(at::Tensor w_agent_ptrs, int64_t H, int64_t w_global_ptr, int64_t dir, int64_t begin, int64_t end, at::Tensor out,
+                   c10::optional<at::Tensor> flag_ptrs, c10::optional<at::Tensor> local_sync, int64_t rank, int64_t world, int64_t epoch) {
+    rlr::ColludeParams p = collude_params(w_agent_ptrs, H, w_global_ptr, 1, dir, begin, end, out, 2 * H + 1);
+    c10::cuda::CUDAGuard guard(out.device());
+    p.gate = gate_of(flag_ptrs, local_sync, rank, world, epoch);
+    check(rlr::launch_collude_stats(p, out.data_ptr<double>(), num_sms(), cur_stream()), "collude_stats");
+}
+
+void collude_write(at::Tensor w_agent_ptrs, int64_t H, c10::optional<at::Tensor> out_ptrs, int64_t w_global_ptr, int64_t mode, int64_t dir,
+                   double z, double gamma, int64_t begin, int64_t end, at::Tensor out, c10::optional<at::Tensor> flag_ptrs,
+                   c10::optional<at::Tensor> local_sync, int64_t rank, int64_t world, int64_t epoch) {
+    rlr::ColludeParams p = collude_params(w_agent_ptrs, H, w_global_ptr, mode, dir, begin, end, out, 1);
+    if (out_ptrs.has_value() && out_ptrs->defined()) {
+        CHECK_CUDA(*out_ptrs);
+        TORCH_CHECK(out_ptrs->scalar_type() == at::kLong, "output pointer table must be int64");
+        p.w_out = reinterpret_cast<float* const*>(out_ptrs->data_ptr());
+        p.n_out = (int)out_ptrs->numel();
+    }
+    p.z = z; p.gamma = gamma;
+    c10::cuda::CUDAGuard guard(out.device());
+    p.gate = gate_of(flag_ptrs, local_sync, rank, world, epoch);
+    check(rlr::launch_collude_write(p, out.data_ptr<double>(), num_sms(), cur_stream()), "collude_write");
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // training augmentation of the gathers: crop pad, flip, Philox key and the device int64 stream word (needed when either is on)
 inline const long long* aug_stream_ptr(const c10::optional<at::Tensor>& stream, int64_t crop_pad, bool flip) {
@@ -560,6 +603,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("fld_predict", &fld_predict);
     m.def("trust_stats", &trust_stats);
     m.def("rfa_sqdist", &rfa_sqdist);
+    m.def("collude_stats", &collude_stats);
+    m.def("collude_write", &collude_write);
     m.def("gather_normalize", &gather_normalize);
     m.def("gather_im2col", &gather_im2col);
     m.def("stamp_pixels", &stamp_pixels);

@@ -144,6 +144,24 @@ struct RfaParams {
 };
 cudaError_t launch_rfa_sqdist(const RfaParams& p, double* out, int num_sms, cudaStream_t st);
 
+// ---- colluding attackers (collude.cu): ALIE and Min-Max / Min-Sum craft one update from the round's honest ones ---------------------
+// Per coordinate of [begin, end): mu, sig (ddof 1) and the corrupt mean xc of x_k = w_k - w_global in fp64, the direction u and the
+// crafted m (the statement is in collude.cu).  stats: out[2H + 1] = (a_k, e_k for the H honest participants, q).  write: every w_out slot
+// gets fp32(w_global + m) and out[1] = sum (m - mu)^2.  Fixed-order sums, no atomics: bitwise reproducible.
+struct ColludeParams {
+    const float* const* w_agents;   // [H + C] device pointers (local or peer-mapped): the honest participants, then the corrupt ones
+    float* const* w_out;            // [n_out] slots the write pass fills with the crafted update (may be the corrupt inputs)
+    const float* w_global;
+    long long begin, end;           // coordinate range (multiples of 4), already clipped to [0, n_vote)
+    int H, C, n_out;
+    int mode;                       // 0 alie, 1 minmax / minsum (m = mu - gamma u)
+    int dir;                        // u: 0 backdoor (mu - xc), 1 std (sig), 2 sign (sign mu), 3 unit (mu)
+    double z, gamma;                // alie's z; the host's gamma* of minmax / minsum
+    Gate gate;                      // world > 1: the aggregation's barrier-in
+};
+cudaError_t launch_collude_stats(const ColludeParams& p, double* out, int num_sms, cudaStream_t st);
+cudaError_t launch_collude_write(const ColludeParams& p, double* out, int num_sms, cudaStream_t st);
+
 // ---- data path ---------------------------------------------------------------------------------------
 // out_kind: 0 fp32, 1 bf16.  nchw: output layout NCHW (Cpad ignored) else NHWC with channels padded to c_pad.
 // Both gathers: crop_pad > 0 or flip turns on the training augmentation (AugSpec, common.cuh): sample b of the batch is drawn

@@ -28,6 +28,8 @@ DNC_FRAC = 1.0                   # DnC: filtering fraction c; each iteration rem
 DETECTORS = ("none", "fldetector")
 FLD_WINDOW = 10                  # FLDetector: the L-BFGS memory and the score window N
 FLD_START = 0                    # FLDetector: the first round detection may run (it also waits for round 2N + 1)
+COLLUDE_MODES = ("none", "alie", "minmax", "minsum")
+COLLUDE_DIRS = ("backdoor", "std", "sign", "unit")
 PATTERNS = ("plus", "square", "copyright", "apple")
 MODELS = ("auto", "cnn_mnist", "cnn_cifar", "resnet18", "resnet34", "vgg11", "vgg16", "resnet18_gn", "resnet34_gn", "vgg11_gn", "vgg16_gn")
 
@@ -161,6 +163,16 @@ def build_parser() -> argparse.ArgumentParser:
                    help="Neurotoxin (Zhang et al. 2022): corrupt agents never update the top p fraction of coordinates by magnitude of "
                         "the last global update; their gradient is zeroed there at every local step.  0 <= p < 1 (0 = off; needs "
                         "--num_corrupt > 0)")
+    p.add_argument("--attack_collude", default="none", choices=COLLUDE_MODES,
+                   help="colluding attackers with full knowledge: in attack rounds every corrupt participant submits one update crafted "
+                        "from the round's honest updates: alie (A Little Is Enough, Baruch et al. 2019) or the Min-Max / Min-Sum attacks "
+                        "(Shejwalkar and Houmansadr 2021).  Needs --num_corrupt > 0 and --attack_boost 1")
+    p.add_argument("--collude_dir", default=None, choices=COLLUDE_DIRS,
+                   help="--attack_collude: the direction u the crafted update leaves the honest mean along: backdoor (towards the "
+                        "corrupt agents' own mean update), std, sign or unit (default backdoor; alie takes backdoor or std)")
+    p.add_argument("--alie_z", type=float, default=None,
+                   help="--attack_collude alie: the number z >= 0 of honest standard deviations the update may lie from the mean "
+                        "(default per round: the inverse normal CDF at (K - s) / K, s = max(1, floor(K/2) + 1 - C), floored at 0)")
     p.add_argument("--attack_start", type=int, default=1, help="attack schedule: the first round the corrupt agents attack (>= 1)")
     p.add_argument("--attack_stop", type=int, default=0,
                    help="attack schedule: the last round that may be an attack round (0 = no end).  In the other rounds a corrupt agent "
@@ -220,8 +232,39 @@ def finalize_args(args: argparse.Namespace) -> argparse.Namespace:
     _finalize_rfa(args)
     _finalize_flame(args)
     _finalize_attack(args)
+    _finalize_collude(args)
     _finalize_detect(args)
     return args
+
+
+def _finalize_collude(args) -> None:
+    """Validate the colluding-attacker flags and resolve ``collude_dir`` in place (``backdoor`` under ``--attack_collude``): a mode only
+    with corrupt agents and no boost, the direction and z only with a mode, alie only along backdoor or std, and z finite and >= 0."""
+    mode = getattr(args, "attack_collude", "none")
+    d = getattr(args, "collude_dir", None)
+    z = getattr(args, "alie_z", None)
+    if mode not in COLLUDE_MODES:
+        raise ValueError(f"unknown --attack_collude {mode!r}; expected one of {COLLUDE_MODES}")
+    if mode == "none":
+        if d is not None or z is not None:
+            raise ValueError("--collude_dir / --alie_z need --attack_collude")
+        return
+    if args.num_corrupt <= 0:
+        raise ValueError(f"--attack_collude {mode} needs corrupt agents (--num_corrupt > 0)")
+    if float(getattr(args, "attack_boost", 1.0)) != 1.0:
+        raise ValueError("--attack_collude chooses the crafted update's size itself: it refuses --attack_boost other than 1")
+    d = "backdoor" if d is None else d
+    if d not in COLLUDE_DIRS:
+        raise ValueError(f"unknown --collude_dir {d!r}; expected one of {COLLUDE_DIRS}")
+    if mode == "alie" and d not in ("backdoor", "std"):
+        raise ValueError(f"--attack_collude alie takes --collude_dir backdoor or std, not {d}")
+    if z is not None:
+        if mode != "alie":
+            raise ValueError("--alie_z needs --attack_collude alie")
+        z = float(z)
+        if not (math.isfinite(z) and z >= 0):
+            raise ValueError(f"--alie_z {z} must be a finite number >= 0")
+    args.collude_dir, args.alie_z = d, z
 
 
 def _finalize_detect(args) -> None:
@@ -468,6 +511,9 @@ def print_exp_details(args) -> None:
         print(f"    FLAME lambda: {args.flame_lambda}")
     if getattr(args, "attack_boost", 1.0) != 1.0 or getattr(args, "attack_neurotoxin", 0.0) > 0:
         print(f"    Attack (boost / neurotoxin): {args.attack_boost} / {args.attack_neurotoxin}")
+    if getattr(args, "attack_collude", "none") != "none":
+        z = "per round" if args.alie_z is None else args.alie_z
+        print(f"    Attack (collude / dir / z): {args.attack_collude} / {args.collude_dir} / {z if args.attack_collude == 'alie' else '-'}")
     if getattr(args, "detect", "none") != "none":
         print(f"    Detection (window / start): {args.detect} ({args.fld_window} / {args.fld_start})")
     if attack_schedule_set(args):

@@ -38,6 +38,7 @@ the ring of the last N + 1 global updates and the previous global parameters) us
 """
 from __future__ import annotations
 
+import math
 from functools import partial
 
 import numpy as np
@@ -317,6 +318,50 @@ class FusedAggregator:
                                                          self.w_global.data_ptr() if sc is not None else 0, sc))
         agents = self._participants(n_part, participants)
         return ops.rfa_sqdist([agents[j] for j in idx], b, self.n_vote, self.w_global if scales is not None else None, scales)
+
+    def collude(self, n_part: int, honest, corrupt, mode: str, direction: str, z=None):
+        """Colluding attackers (``ops.collude_statement``): overwrite the voted coordinates of the slots of the round's corrupt participants
+        (positions ``corrupt``) with one update crafted from the honest ones (positions ``honest``, at least one), identically on every rank.
+        ``z``: alie's z (required for alie).  Call it after the slots are final and before any selection, detection or aggregation pass
+        of the same round.  Returns ``{"gamma": gamma* or None, "deviation": ||m - mu||}``.
+
+        Fused multi-GPU path: for minmax / minsum the honest distances (``pairwise_sqdist_kernel`` over the honest members) and the
+        statistics pass each run as a ``_fused_pass`` behind the aggregation kernel's barrier-in, so gamma* is the same on every rank; then
+        each rank writes its coordinate slice of every corrupt slot through the peer pointers (alie needs only this pass).  Every later
+        slice pass reads slice r on rank r, on the stream that wrote it.  The all_gather of the write pass's partials orders every rank's
+        writes before anything a rank queues afterwards, so readers of whole slots (``update_norms``, ``gather_participants``) see the
+        crafted update.  The passes read ``w_global``, so they first acquire the broadcast slices of a fused hand-off.  Gather and reduce
+        transports and single process: the same kernels over ``gather_participants``' copies, identical on every rank, and each rank
+        writes the corrupt slots it owns, whole."""
+        honest, corrupt = [int(j) for j in honest], [int(j) for j in corrupt]
+        H = len(honest)
+        if H < 1:
+            raise ValueError("collude: the craft needs at least one honest participant")
+        dirn, mid = ops.COLLUDE_DIR_IDS[direction], 0 if mode == "alie" else 1
+        gamma = None
+        if self._p2p(n_part):
+            self.acquire()
+            table = self._member_table(honest + corrupt)
+            outs = self._member_table(corrupt)
+            wg = self.w_global.data_ptr()
+            if mode != "alie":
+                D = torch.zeros((1, 1), dtype=torch.float64)
+                if H > 1:
+                    D = self._fused_pass((H, H), partial(ops.ext().pairwise_sqdist, self._member_table(honest).tensor, 0, None))
+                st = self._fused_pass((2 * H + 1,), partial(ops.ext().collude_stats, table.tensor, H, wg, dirn))
+                gamma = ops.collude_gamma(mode, st[:H], st[H:2 * H], st[2 * H], D)
+            dev2 = self._fused_pass((1,), partial(ops.ext().collude_write, table.tensor, H, outs.tensor, wg, mid, dirn, float(z or 0.0),
+                                                  float(gamma or 0.0)))
+        else:
+            copies = self.gather_participants(n_part)
+            hon, cor = [copies[j] for j in honest], [copies[j] for j in corrupt]
+            outs = [self.slots[s] for r, s in map(self.slot_owner, corrupt) if r == self.ctx.rank]
+            if mode != "alie":
+                D = ops.pairwise_sqdist(hon, self.n_vote) if H > 1 else torch.zeros((1, 1), dtype=torch.float64)
+                st = ops.collude_stats(hon, cor, self.w_global, self.n_vote, direction)
+                gamma = ops.collude_gamma(mode, st[:H], st[H:2 * H], st[2 * H], D)
+            dev2 = ops.collude_write(hon, cor, outs, self.w_global, self.n_vote, mode, direction, z, gamma)
+        return {"gamma": gamma, "deviation": math.sqrt(max(0.0, float(dev2.reshape(-1)[0])))}
 
     def pairwise_gram(self, n_part: int, members=None, participants=None):
         """FLAME Gram pass (``ops.gram_statement``): the float64 Gram matrix of the updates ``w_j - w_global`` of the participants at

@@ -331,6 +331,7 @@ class FLEngine:
         mask = self._neurotoxin_mask(attack) if self.neurotoxin_k is not None else None
         for t in self.trainers:
             t.attack_mask = mask
+            t.attack_round = attack                                      # --attack_constrain's objective for corrupt agents
         concurrent = len(self.trainers) > 1
         if concurrent:
             for part in self._loss_parts:

@@ -27,6 +27,7 @@ import torch
 import torch.nn.functional as F
 
 from .. import ops
+from ..options import local_objective
 from .graph import FlatLayout
 
 ACT = torch.bfloat16   # default activation / GEMM-operand dtype on GPU (tests may run the plan in fp32 on CPU)
@@ -610,6 +611,9 @@ class NativeTrainer:
         # Neurotoxin: the round's gradient mask (int32 bit words, engine-owned and rewritten in place), applied to corrupt agents only
         self.attack_mask = None
         self._grad_mask = None
+        # whether the round is an attack round of the schedule (engine-set): corrupt agents then train on --attack_constrain's objective
+        self.attack_round = True
+        self._objective = None
 
     # ---- round hand-off fused with the first local step ---------------------------------------------------------------------
     def attach_broadcast(self, fused):
@@ -658,13 +662,14 @@ class NativeTrainer:
         _, dl = ops.softmax_xent(logits, self.y[:B], True, self.loss_sum, dlogits=self.net.dlogits_buffer(B))
         self.net.backward(dl)
         self.opt.step(self.w, self.g, self.m, w0=w0, w_bf16=self.wb, w_in=self.bcast.w_global if first else None,
-                      grad_mask=self._grad_mask)
+                      grad_mask=self._grad_mask, objective=self._objective)
         ops.ext().advance_cursor(self.cursor, B, self.net.step_counter)       # next batch; next Philox step for the dropout masks
         if first:
             self._bind_normal()
 
     def _get_graph(self, dataset, B, w0, first=False):
-        key = (B, dataset.data.data_ptr(), w0.data_ptr(), bool(first), 0 if self._grad_mask is None else self._grad_mask.data_ptr())
+        key = (B, dataset.data.data_ptr(), w0.data_ptr(), bool(first), 0 if self._grad_mask is None else self._grad_mask.data_ptr(),
+               self._objective)
         if key in self._graphs:
             return self._graphs[key]
         keep = (self.w.clone(), self.wb.clone(), self.m.clone(), self.cursor.clone(), self.loss_sum.clone(),
@@ -693,6 +698,7 @@ class NativeTrainer:
         dataset, n = agent.dataset, agent.n_data
         self.loss_sum.zero_()
         self._grad_mask = self.attack_mask if getattr(agent, "is_corrupt", False) else None
+        self._objective = local_objective(args, getattr(agent, "is_corrupt", False) and self.attack_round)
         graphs = self.use_graphs and n <= self.max_shard
         fused = self.bcast is not None and w_global.data_ptr() == self.bcast.w_global.data_ptr()
         if graphs:

@@ -1508,12 +1508,50 @@ def round_init(w_global, w_local=None, w_bf16=None, mom=None):
         mom.zero_()
 
 
+def objective_gradient(g, w, w0, objective, n_pgd: int, masked=None):
+    """The gradient ``G`` of the local objective ``a CE + b ||d|| + (mu/2) ||d||^2`` that ``FlatSGD`` applies, with ``g`` the
+    cross-entropy gradient (Neurotoxin-masked already), ``objective = (a, b, mu)`` and ``d = w - w0`` over the model parameters
+    ``[0, n_pgd)`` (the BatchNorm tail behind them never counts).  ``w`` is the parameters the step reads (``w_in`` on a first step).
+
+    The statement, in fp64 unless a rounding ``r()`` to the buffers' dtype (fp32 in training) is written:
+
+    * ``a, b, mu`` are taken at the buffers' precision: ``a = r(a)``, ``b = r(b)``, ``mu = r(mu)``;
+    * ``d = r(w - w0)`` over ``[0, n_pgd)``, and ``d[c] = 0`` where the mask zeroes ``g[c]`` (a masked step never moves ``w`` off
+      ``w0`` there, so this changes nothing in a run; it keeps ``G[c] = 0`` on the mask);
+    * ``S_gg = sum g^2`` over every coordinate, ``S_gd = sum g d`` and ``S_dd = sum d^2`` over ``[0, n_pgd)``;
+    * ``beta = b / sqrt(S_dd) + mu``, with ``b / sqrt(S_dd) := 0`` when ``S_dd = 0`` (the subgradient torch's norm backward takes at
+      0; it covers the first step of every round, where ``d = 0``);
+    * ``||G||^2 = max(0, a^2 S_gg + 2 a beta S_gd + beta^2 S_dd)``;
+    * ``G = r(r(a g) + r(r(beta) d))`` over ``[0, n_pgd)`` and ``G = r(a g)`` behind it.
+
+    Returns ``(G, ||G||, (S_gg, S_gd, S_dd))``.  The sm_90a kernels compute the three sums with fp32-squared ``g^2`` pairs and exact
+    fp64 products for ``g d`` and ``d^2``, added in a fixed order, and every other step exactly as written here."""
+    k = int(n_pgd)
+    rnd = lambda x: float(torch.tensor(float(x), dtype=g.dtype))  # noqa: E731
+    a, b, mu = (rnd(x) for x in objective)
+    d = w[:k] - w0[:k]
+    if masked is not None:
+        d = d.masked_fill(masked, 0.0)
+    s_gg = float((g.double() * g.double()).sum())
+    s_gd = float((g[:k].double() * d.double()).sum())
+    s_dd = float((d.double() * d.double()).sum())
+    dn = math.sqrt(s_dd)
+    beta = (b / dn if dn > 0 else 0.0) + mu
+    G = g * a
+    G[:k] += d * rnd(beta)
+    return G, math.sqrt(max(0.0, a * a * s_gg + 2 * a * beta * s_gd + beta * beta * s_dd)), (s_gg, s_gd, s_dd)
+
+
 class FlatSGD:
     """Fused ``clip_grad_norm_(., max_grad_norm)`` + momentum SGD + optional PGD projection over flat buffers.
 
     Reference: src/agent.py:37-38 (SGD, fresh momentum each round), :50 (clip 10), :54-60 (PGD onto the L2 ball of
     radius ``clip`` around the round's global params).  All norms stay on the device (the reference syncs to the host
     for ``max(1, norm/clip)``); the whole step is 2 kernels (+2 with PGD) regardless of the number of tensors.
+
+    A local objective ``(a, b, mu)`` other than plain cross-entropy (FedProx, constrain-and-scale) replaces ``g`` by its gradient
+    ``G`` (``objective_gradient``) ahead of the same chain: mask, ``clip_grad_norm_`` on ``||G||``, momentum SGD, PGD.  It takes
+    the same launches: the norm pass also reads ``w`` and ``w0``, and the step ``w0``.
     """
 
     def __init__(self, n, device, lr, momentum, max_grad_norm=10.0, pgd_clip=0.0, n_pgd=None):
@@ -1521,20 +1559,37 @@ class FlatSGD:
         # the PGD ball is measured and projected over the model parameters [0, n_pgd) only (layout.n_vote): BatchNorm running
         # statistics behind them are not in the reference's parameters_to_vector() (src/agent.py:54-60)
         self.n_pgd = int(n if n_pgd is None else n_pgd)
-        self.norms = torch.zeros(2, dtype=torch.float64, device=device)  # [||g||^2, ||w-w0||^2]
+        # [||g||^2, ||w-w0||^2, S_gg, S_gd, S_dd]: the last three are the objective's norm pass (only a step with an objective writes
+        # them, and its ||g||^2 is S_gg)
+        self.norms = torch.zeros(5, dtype=torch.float64, device=device)
 
-    def step(self, w, g, m, w0=None, w_bf16=None, w_in=None, grad_mask=None):
+    def step(self, w, g, m, w0=None, w_bf16=None, w_in=None, grad_mask=None, objective=None):
         """``w_in``: first local step of a round fused with the hand-off -- parameters are read from ``w_in`` (the round's global
         parameters, i.e. the broadcast buffer) instead of ``w`` and the momentum counts as zero, so no separate
         ``w <- w_global, m <- 0`` pass is needed; coordinates ``>= n_pgd`` (BatchNorm running statistics already updated in ``w``
         by this step's forward pass) keep their value.
 
         ``grad_mask``: int32 bit words over ``[0, n_pgd)`` (Neurotoxin): ``g[c]`` counts as zero for every set bit, before the
-        gradient norm is taken, and the PGD projection leaves those coordinates alone.  Same launches as without it."""
+        gradient norm is taken, and the PGD projection leaves those coordinates alone.  Same launches as without it.
+
+        ``objective``: ``(a, b, mu)`` of the local objective ``a CE + b ||w - w0|| + (mu/2) ||w - w0||^2`` (``objective_gradient``),
+        needs ``w0``; None or ``(1, 0, 0)`` is plain cross-entropy, the step as it is without the argument."""
+        if objective is not None and tuple(float(x) for x in objective) == (1.0, 0.0, 0.0):
+            objective = None
+        if objective is not None and w0 is None:
+            raise ValueError("FlatSGD.step: a local objective pulls toward w0, which is missing")
         if w.is_cuda:
             e = ext()
             e.memset_zero(self.norms)
             pgd = self.pgd_clip > 0
+            if objective is not None:
+                sums = self.norms[2:5]
+                e.sqnorm(g, sums, grad_mask, self.n_pgd, w_in if w_in is not None else w, w0, self.n_pgd)
+                e.sgd_step(w, g, m, w0, w_bf16, self.lr, self.momentum, self.max_grad_norm, sums, self.norms[1:2] if pgd else None,
+                           self.n_pgd, w_in, grad_mask, [float(x) for x in objective])
+                if pgd:
+                    e.pgd_project(w, w0, w_bf16, self.pgd_clip, self.norms[1:2], self.n_pgd, grad_mask)
+                return
             if grad_mask is None:
                 e.sqnorm(g, self.norms[0:1])
                 e.sgd_step(w, g, m, w0 if pgd else None, w_bf16, self.lr, self.momentum, self.max_grad_norm,
@@ -1553,8 +1608,11 @@ class FlatSGD:
             masked = mask_bits(grad_mask, self.n_pgd)
             g = g.clone()
             g[:self.n_pgd].masked_fill_(masked, 0.0)
-        gn = g.double().norm()
-        coef = min(1.0, self.max_grad_norm / (float(gn) + 1e-6)) if self.max_grad_norm > 0 else 1.0
+        if objective is None:
+            gn = float(g.double().norm())
+        else:
+            g, gn, _ = objective_gradient(g, w_in if w_in is not None else w, w0, objective, self.n_pgd, masked)
+        coef = min(1.0, self.max_grad_norm / (gn + 1e-6)) if self.max_grad_norm > 0 else 1.0
         if w_in is not None:
             k = self.n_pgd
             m.zero_()

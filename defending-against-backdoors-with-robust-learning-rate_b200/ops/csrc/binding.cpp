@@ -454,26 +454,44 @@ inline const uint32_t* mask_ptr(const c10::optional<at::Tensor>& mask, int64_t n
     return reinterpret_cast<const uint32_t*>(mask->data_ptr());
 }
 
-void sqnorm(at::Tensor x, at::Tensor out, c10::optional<at::Tensor> mask, int64_t n_mask) {
+// with w0: the local objective's norm pass, out[0:3] += [sum x^2, sum x d, sum d^2], d = fp32(w - w0) over [0, n_pgd)
+void sqnorm(at::Tensor x, at::Tensor out, c10::optional<at::Tensor> mask, int64_t n_mask, c10::optional<at::Tensor> w,
+            c10::optional<at::Tensor> w0, int64_t n_pgd) {
     CHECK_CUDA(x); CHECK_CUDA(out);
     TORCH_CHECK(x.scalar_type() == at::kFloat && out.scalar_type() == at::kDouble);
+    const bool prox = w0.has_value() && w0->defined();
+    if (prox) {
+        TORCH_CHECK(w.has_value() && w->defined(), "sqnorm: the objective's norm pass needs w and w0");
+        CHECK_CUDA(*w); CHECK_CUDA(*w0);
+        TORCH_CHECK(w->scalar_type() == at::kFloat && w0->scalar_type() == at::kFloat && w->numel() == x.numel() &&
+                    w0->numel() >= n_pgd && out.numel() >= 3, "sqnorm: fp32 w [n], w0 [>= n_pgd], fp64 out [3]");
+    }
     c10::cuda::CUDAGuard guard(x.device());
     check(rlr::launch_sqnorm(x.data_ptr<float>(), x.numel(), out.data_ptr<double>(), num_sms(), cur_stream(), mask_ptr(mask, n_mask),
-                             n_mask), "sqnorm");
+                             n_mask, prox ? w->data_ptr<float>() : nullptr, prox ? w0->data_ptr<float>() : nullptr, n_pgd), "sqnorm");
 }
 
 void sgd_step(at::Tensor w, at::Tensor g, at::Tensor m, c10::optional<at::Tensor> w0, c10::optional<at::Tensor> w_bf16,
               double lr, double momentum, double max_grad_norm, c10::optional<at::Tensor> g_sqnorm,
-              c10::optional<at::Tensor> d_sqnorm, int64_t n_pgd, c10::optional<at::Tensor> w_in, c10::optional<at::Tensor> mask) {
+              c10::optional<at::Tensor> d_sqnorm, int64_t n_pgd, c10::optional<at::Tensor> w_in, c10::optional<at::Tensor> mask,
+              c10::optional<std::vector<double>> objective) {
     CHECK_CUDA(w); CHECK_CUDA(g); CHECK_CUDA(m);
     TORCH_CHECK(w.numel() == g.numel() && w.numel() == m.numel());
     TORCH_CHECK(!(d_sqnorm.has_value() && d_sqnorm->defined()) || (w0.has_value() && w0->defined()), "PGD needs w0");
+    float obj[3] = {1.f, 0.f, 0.f};
+    if (objective.has_value()) {
+        TORCH_CHECK(objective->size() == 3, "sgd_step: objective = (a, b, mu)");
+        TORCH_CHECK(w0.has_value() && w0->defined() && g_sqnorm.has_value() && g_sqnorm->defined() && g_sqnorm->numel() >= 3,
+                    "sgd_step: the objective needs w0 and the norm pass's three sums");
+        for (int i = 0; i < 3; ++i) obj[i] = (float)(*objective)[i];
+    }
     c10::cuda::CUDAGuard guard(w.device());
     check(rlr::launch_sgd_step(w.data_ptr<float>(), g.data_ptr<float>(), m.data_ptr<float>(), ptr_or_null<const float>(w0),
                                ptr_or_null<__nv_bfloat16>(w_bf16), w.numel(), (float)lr, (float)momentum,
                                (float)max_grad_norm, ptr_or_null<const double>(g_sqnorm), ptr_or_null<double>(d_sqnorm),
                                num_sms(), cur_stream(), n_pgd, ptr_or_null<const float>(w_in),
-                               mask_ptr(mask, n_pgd > 0 && n_pgd <= w.numel() ? n_pgd : w.numel())), "sgd_step");
+                               mask_ptr(mask, n_pgd > 0 && n_pgd <= w.numel() ? n_pgd : w.numel()), objective.has_value() ? obj : nullptr),
+          "sgd_step");
 }
 
 void pgd_project(at::Tensor w, at::Tensor w0, c10::optional<at::Tensor> w_bf16, double clip, at::Tensor d_sqnorm, int64_t n_pgd,
@@ -613,10 +631,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("pad_rows", &pad_rows);
     m.def("unpad_add", &unpad_add);
     m.def("round_init", &round_init);
-    m.def("sqnorm", &sqnorm, py::arg("x"), py::arg("out"), py::arg("mask") = py::none(), py::arg("n_mask") = 0);
+    m.def("sqnorm", &sqnorm, py::arg("x"), py::arg("out"), py::arg("mask") = py::none(), py::arg("n_mask") = 0, py::arg("w") = py::none(),
+          py::arg("w0") = py::none(), py::arg("n_pgd") = 0);
     m.def("sgd_step", &sgd_step, py::arg("w"), py::arg("g"), py::arg("m"), py::arg("w0"), py::arg("w_bf16"), py::arg("lr"),
           py::arg("momentum"), py::arg("max_grad_norm"), py::arg("g_sqnorm"), py::arg("d_sqnorm"), py::arg("n_pgd") = 0, py::arg("w_in") = py::none(),
-          py::arg("mask") = py::none());
+          py::arg("mask") = py::none(), py::arg("objective") = py::none());
     m.def("neurotoxin_mask", &neurotoxin_mask);
     m.def("boost_update", &boost_update);
     m.def("swap_samples", &swap_samples);

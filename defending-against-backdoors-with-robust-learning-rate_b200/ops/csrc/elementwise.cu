@@ -3,6 +3,7 @@
 // loss / evaluation reductions.  Reference call sites: src/agent.py:41-60 (step), src/utils.py:52-54 (per-sample
 // host transforms), :160-178 (poisoning), :128-157 (evaluation).
 #include "common.cuh"
+#include "flat_sgd.cuh"
 #include "kernels.h"
 
 #include <cstdlib>
@@ -353,107 +354,40 @@ cudaError_t launch_round_init(const float* w_global, float* w_local, __nv_bfloat
 // ------------------------------------------------------------------------------------------------------------
 // fused clip_grad_norm_(.,max) + SGD(momentum) [+ ||w-w0||^2 for PGD] over flat buffers   (src/agent.py:50-60)
 // ------------------------------------------------------------------------------------------------------------
-// MASK: a gradient mask of bit words over [0, 4 * n4_mask) (bit c % 32 of word c / 32 set = coordinate c reads as zero); the thread of
-// float4 q takes the nibble (q % 8) of word q / 8.  The <false> instantiations compile to the same instructions as the unmasked kernels.
-__device__ __forceinline__ float4 apply_mask(float4 v, const uint32_t* __restrict__ mask, long long q, long long n4_mask) {
-    if (q < n4_mask) {
-        const uint32_t nib = (__ldg(mask + (q >> 3)) >> ((q & 7) * 4)) & 0xFu;
-        if (nib) {
-            if (nib & 1u) v.x = 0.f;
-            if (nib & 2u) v.y = 0.f;
-            if (nib & 4u) v.z = 0.f;
-            if (nib & 8u) v.w = 0.f;
-        }
-    }
-    return v;
-}
-
-template <bool MASK>
-__global__ void __launch_bounds__(256) sqnorm_kernel(const float* __restrict__ x, long long n4, double* part /*[gridDim.x]*/,
-                                                     const uint32_t* __restrict__ mask, long long n4_mask) {
-    __shared__ double scratch[32];
-    double acc = 0.0;
-    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n4; q += (long long)gridDim.x * blockDim.x) {
-        float4 v = ld_f4(x + 4 * q);
-        if (MASK) v = apply_mask(v, mask, q, n4_mask);
-        acc += (double)(v.x * v.x + v.y * v.y) + (double)(v.z * v.z + v.w * v.w);
-    }
-    const double tot = block_sum<double>(acc, scratch);
-    if (threadIdx.x == 0) part[blockIdx.x] = tot;
-}
+// the norm pass and the step are templates in flat_sgd.cuh; a local objective's launches go to objective.cu
 cudaError_t launch_sqnorm(const float* x, long long n, double* out, int num_sms, cudaStream_t st, const uint32_t* mask,
-                          long long n_mask) {
+                          long long n_mask, const float* w, const float* w0, long long n_pgd) {
     if ((n & 3) || (mask && ((n_mask & 3) || n_mask < 0 || n_mask > n))) return cudaErrorInvalidValue;
+    if (w0 && (!w || (n_pgd & 3) || n_pgd <= 0 || n_pgd > n)) return cudaErrorInvalidValue;
     const int grid = grid_for(n / 4, 256, num_sms, 4);
-    Scratch part((size_t)grid * sizeof(double), st);
-    if (mask) sqnorm_kernel<true><<<grid, 256, 0, st>>>(x, n / 4, part.as<double>(), mask, n_mask / 4);
-    else sqnorm_kernel<false><<<grid, 256, 0, st>>>(x, n / 4, part.as<double>(), nullptr, 0);
+    const long long nout = w0 ? 3 : 1;
+    Scratch part((size_t)grid * nout * sizeof(double), st);
+    if (w0) launch_sqnorm_objective(grid, st, x, n / 4, part.as<double>(), mask, n_mask / 4, w, w0, n_pgd / 4);
+    else if (mask) sqnorm_kernel<true, false><<<grid, 256, 0, st>>>(x, n / 4, part.as<double>(), mask, n_mask / 4, nullptr, nullptr, 0);
+    else sqnorm_kernel<false, false><<<grid, 256, 0, st>>>(x, n / 4, part.as<double>(), nullptr, 0, nullptr, nullptr, 0);
     RLR_CUDA_CHECK(cudaGetLastError());
-    RLR_CUDA_CHECK(launch_ordered_sum(out, part.as<double>(), grid, 1LL, st));
+    RLR_CUDA_CHECK(launch_ordered_sum(out, part.as<double>(), grid, nout, st));
     return cudaGetLastError();
 }
 
-template <bool MASK>
-__global__ void __launch_bounds__(256) sgd_step_kernel(float* __restrict__ w, const float* __restrict__ g,
-                                                         float* __restrict__ m, const float* __restrict__ w0,
-                                                         __nv_bfloat16* __restrict__ wb, long long n4, float lr,
-                                                         float momentum, float max_grad_norm,
-                                                         const double* __restrict__ g_sqnorm, double* d_part /*[gridDim.x]*/,
-                                                         long long n4_pgd, const float* __restrict__ w_in, int first,
-                                                         const uint32_t* __restrict__ mask) {
-    // MASK: the gradient mask covers [0, n4_pgd) (the model parameters)
-    // first = 1: first local step of a round, fused with the round hand-off -- parameters are read from the broadcast buffer w_in
-    // (= the round's global parameters) and the momentum is taken as zero (fresh optimizer every round, src/agent.py:37-38), so no
-    // separate "w <- w_global, m <- 0" pass exists.  Coordinates >= n4_pgd (BatchNorm running statistics, already updated in w by
-    // this step's forward pass) keep their value.
-    __shared__ double scratch[32];
-    float coef = 1.0f;
-    if (max_grad_norm > 0.f && g_sqnorm) {
-        // torch.nn.utils.clip_grad_norm_: coef = max_norm / (total_norm + 1e-6), clamped to 1
-        coef = fminf(1.0f, max_grad_norm / ((float)sqrt(*g_sqnorm) + 1e-6f));
-    }
-    double dacc = 0.0;
-    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n4; q += (long long)gridDim.x * blockDim.x) {
-        if (first && q >= n4_pgd) { st_f4(m + 4 * q, make_float4(0.f, 0.f, 0.f, 0.f)); continue; }
-        float4 gv = ld_f4(g + 4 * q);
-        if (MASK) gv = apply_mask(gv, mask, q, n4_pgd);
-        const float4 mv = first ? make_float4(0.f, 0.f, 0.f, 0.f) : ld_f4(m + 4 * q), wv = ld_f4((first ? w_in : w) + 4 * q);
-        float4 mn, wn;
-        mn.x = momentum * mv.x + coef * gv.x; mn.y = momentum * mv.y + coef * gv.y;
-        mn.z = momentum * mv.z + coef * gv.z; mn.w = momentum * mv.w + coef * gv.w;
-        wn.x = wv.x - lr * mn.x; wn.y = wv.y - lr * mn.y; wn.z = wv.z - lr * mn.z; wn.w = wv.w - lr * mn.w;
-        st_f4(m + 4 * q, mn);
-        st_f4(w + 4 * q, wn);
-        if (d_part) {
-            // PGD radius is measured over the model parameters only ([0, n_pgd): the reference projects parameters_to_vector(),
-            // src/agent.py:54-60); BatchNorm running statistics stored behind them never count and are never rescaled
-            if (q < n4_pgd) {
-                const float4 o = ld_f4(w0 + 4 * q);
-                const float d0 = wn.x - o.x, d1 = wn.y - o.y, d2 = wn.z - o.z, d3 = wn.w - o.w;
-                dacc += (double)(d0 * d0 + d1 * d1) + (double)(d2 * d2 + d3 * d3);
-            }
-        } else if (wb) {
-            *reinterpret_cast<uint2*>(wb + 4 * q) = make_uint2(pack_bf16x2(wn.x, wn.y), pack_bf16x2(wn.z, wn.w));
-        }
-    }
-    if (d_part) {
-        const double tot = block_sum<double>(dacc, scratch);
-        if (threadIdx.x == 0) d_part[blockIdx.x] = tot;
-    }
-}
 cudaError_t launch_sgd_step(float* w, const float* g, float* m, const float* w0, __nv_bfloat16* w_bf16, long long n,
                             float lr, float momentum, float max_grad_norm, const double* g_sqnorm, double* d_sqnorm,
-                            int num_sms, cudaStream_t st, long long n_pgd, const float* w_in, const uint32_t* mask) {
+                            int num_sms, cudaStream_t st, long long n_pgd, const float* w_in, const uint32_t* mask,
+                            const float* objective) {
     if ((n & 3) || (n_pgd & 3)) return cudaErrorInvalidValue;
+    if (objective && (!w0 || !g_sqnorm)) return cudaErrorInvalidValue;
     if (n_pgd <= 0 || n_pgd > n) n_pgd = n;
     const int grid = grid_for(n / 4, 256, num_sms, 4);
     auto step = [&](double* dp) {
-        if (mask)
-            sgd_step_kernel<true><<<grid, 256, 0, st>>>(w, g, m, w0, w_bf16, n / 4, lr, momentum, max_grad_norm, g_sqnorm, dp,
-                                                        n_pgd / 4, w_in, w_in ? 1 : 0, mask);
+        if (objective)
+            launch_sgd_step_objective(grid, st, w, g, m, w0, w_bf16, n / 4, lr, momentum, max_grad_norm, g_sqnorm, dp, n_pgd / 4, w_in,
+                                      mask, objective[0], objective[1], objective[2]);
+        else if (mask)
+            sgd_step_kernel<true, false><<<grid, 256, 0, st>>>(w, g, m, w0, w_bf16, n / 4, lr, momentum, max_grad_norm, g_sqnorm, dp,
+                                                               n_pgd / 4, w_in, w_in ? 1 : 0, mask, 1.f, 0.f, 0.f);
         else
-            sgd_step_kernel<false><<<grid, 256, 0, st>>>(w, g, m, w0, w_bf16, n / 4, lr, momentum, max_grad_norm, g_sqnorm, dp,
-                                                         n_pgd / 4, w_in, w_in ? 1 : 0, nullptr);
+            sgd_step_kernel<false, false><<<grid, 256, 0, st>>>(w, g, m, w0, w_bf16, n / 4, lr, momentum, max_grad_norm, g_sqnorm, dp,
+                                                                n_pgd / 4, w_in, w_in ? 1 : 0, nullptr, 1.f, 0.f, 0.f);
         return cudaGetLastError();
     };
     if (!d_sqnorm) return step(nullptr);

@@ -188,13 +188,17 @@ cudaError_t launch_round_init(const float* w_global, float* w_local, __nv_bfloat
                               cudaStream_t st);
 // mask (optional): gradient mask bit words (bit c % 32 of word c / 32 set = g[c] reads as zero) over [0, n_mask) for sqnorm and over
 // [0, n_pgd) for sgd_step; pgd_project leaves masked coordinates untouched
+// Local objective a CE + b ||d|| + (mu/2) ||d||^2, d = fp32(w - w0) over [0, n_pgd) (FlatSGD, ops/__init__.py): with w0, sqnorm
+// accumulates out[0:3] += [sum g^2, sum g d, sum d^2] (g and d masked alike; w = the parameters the step will read, w_in on a first
+// step), and sgd_step with objective = host {a, b, mu} reads those three sums through g_sqnorm and applies G = a g + beta d
 cudaError_t launch_sqnorm(const float* x, long long n, double* out /*accumulates*/, int num_sms, cudaStream_t st,
-                          const uint32_t* mask = nullptr, long long n_mask = 0);
+                          const uint32_t* mask = nullptr, long long n_mask = 0, const float* w = nullptr, const float* w0 = nullptr,
+                          long long n_pgd = 0);
 cudaError_t launch_sgd_step(float* w, const float* g, float* m, const float* w0, __nv_bfloat16* w_bf16, long long n,
                             float lr, float momentum, float max_grad_norm, const double* g_sqnorm, double* d_sqnorm,
                             int num_sms, cudaStream_t st, long long n_pgd = 0 /*PGD norm over [0, n_pgd); 0 = n*/,
                             const float* w_in = nullptr /*first step of a round: read params from w_in, momentum = 0, keep w[n_pgd:]*/,
-                            const uint32_t* mask = nullptr);
+                            const uint32_t* mask = nullptr, const float* objective = nullptr /*host [3]: a, b, mu*/);
 cudaError_t launch_pgd_project(float* w, const float* w0, __nv_bfloat16* w_bf16, long long n, float clip,
                                const double* d_sqnorm, int num_sms, cudaStream_t st, long long n_pgd = 0, const uint32_t* mask = nullptr);
 

@@ -163,6 +163,13 @@ def build_parser() -> argparse.ArgumentParser:
                    help="Neurotoxin (Zhang et al. 2022): corrupt agents never update the top p fraction of coordinates by magnitude of "
                         "the last global update; their gradient is zeroed there at every local step.  0 <= p < 1 (0 = off; needs "
                         "--num_corrupt > 0)")
+    p.add_argument("--attack_constrain", type=float, default=1.0,
+                   help="constrain-and-scale (Bagdasaryan et al. 2020): in attack rounds corrupt agents train on alpha CE + (1 - alpha) "
+                        "||w - w_g||, which keeps the poisoned model close to the global one; combine with --attack_boost to scale it.  "
+                        "0 < alpha <= 1 (1 = off; needs --num_corrupt > 0)")
+    p.add_argument("--prox_mu", type=float, default=0.0,
+                   help="FedProx (Li et al. 2020): every client, and the FLTrust root job, trains on CE + (mu/2) ||w - w_g||^2, a pull "
+                        "toward the round's global parameters w_g.  mu >= 0 (0 = off)")
     p.add_argument("--attack_collude", default="none", choices=COLLUDE_MODES,
                    help="colluding attackers with full knowledge: in attack rounds every corrupt participant submits one update crafted "
                         "from the round's honest updates: alie (A Little Is Enough, Baruch et al. 2019) or the Min-Max / Min-Sum attacks "
@@ -313,7 +320,31 @@ def _finalize_attack(args) -> None:
     if (gamma != 1.0 or p > 0) and args.num_corrupt <= 0:
         raise ValueError("--attack_boost / --attack_neurotoxin need corrupt agents (--num_corrupt > 0)")
     args.attack_boost, args.attack_neurotoxin = gamma, p
+    _finalize_objective(args)
     _finalize_schedule(args)
+
+
+def _finalize_objective(args) -> None:
+    """Validate the local-objective flags in place: ``prox_mu`` finite and >= 0, ``attack_constrain`` finite in (0, 1] and, when not 1,
+    only with corrupt agents to train on it."""
+    mu = float(getattr(args, "prox_mu", 0.0))
+    alpha = float(getattr(args, "attack_constrain", 1.0))
+    if not (math.isfinite(mu) and mu >= 0.0):
+        raise ValueError(f"--prox_mu {mu} must be a finite number >= 0")
+    if not (math.isfinite(alpha) and 0.0 < alpha <= 1.0):
+        raise ValueError(f"--attack_constrain {alpha} must be a finite number in (0, 1]")
+    if alpha != 1.0 and args.num_corrupt <= 0:
+        raise ValueError("--attack_constrain needs corrupt agents (--num_corrupt > 0)")
+    args.prox_mu, args.attack_constrain = mu, alpha
+
+
+def local_objective(args, attacking: bool):
+    """``(a, b, mu)`` of an agent's local objective ``a CE + b ||w - w_g|| + (mu/2) ||w - w_g||^2`` (``ops.FlatSGD``), or None for plain
+    cross-entropy.  ``attacking``: a corrupt agent in an attack round, which trains with ``(a, b) = (alpha, 1 - alpha)``; every other
+    agent, the FLTrust root job and a corrupt agent in a quiet round train with ``(1, 0)``.  ``mu = --prox_mu`` for all."""
+    mu = float(getattr(args, "prox_mu", 0.0))
+    alpha = float(getattr(args, "attack_constrain", 1.0)) if attacking else 1.0
+    return None if (alpha == 1.0 and mu == 0.0) else (alpha, 1.0 - alpha, mu)
 
 
 def _finalize_schedule(args) -> None:
@@ -511,6 +542,8 @@ def print_exp_details(args) -> None:
         print(f"    FLAME lambda: {args.flame_lambda}")
     if getattr(args, "attack_boost", 1.0) != 1.0 or getattr(args, "attack_neurotoxin", 0.0) > 0:
         print(f"    Attack (boost / neurotoxin): {args.attack_boost} / {args.attack_neurotoxin}")
+    if getattr(args, "prox_mu", 0.0) != 0.0 or getattr(args, "attack_constrain", 1.0) != 1.0:
+        print(f"    Local objective (prox mu / constrain alpha): {args.prox_mu} / {args.attack_constrain}")
     if getattr(args, "attack_collude", "none") != "none":
         z = "per round" if args.alie_z is None else args.alie_z
         print(f"    Attack (collude / dir / z): {args.attack_collude} / {args.collude_dir} / {z if args.attack_collude == 'alie' else '-'}")

@@ -16,6 +16,7 @@ import torch.nn.functional as F
 
 from . import ops
 from .models.graph import GraphNet
+from .options import local_objective
 
 
 def _agent_round_seed(seed: int, agent_id: int, rnd: int) -> int:
@@ -45,6 +46,9 @@ class TorchTrainer:
         # Neurotoxin: the round's gradient mask (int32 bit words, engine-owned and rewritten in place), applied to corrupt agents only
         self.attack_mask = None
         self._grad_mask = None
+        # whether the round is an attack round of the schedule (engine-set): corrupt agents then train on --attack_constrain's objective
+        self.attack_round = True
+        self._objective = None
         # training augmentation (--crop_pad / --hflip): the Philox stream word of the current epoch, set before the graphs replay
         self.aug_stream = torch.zeros(1, dtype=torch.int64, device=device)
         self.aug = ops.training_augment(args, self.aug_stream)
@@ -61,7 +65,7 @@ class TorchTrainer:
         logits = self.net(x)
         loss = F.cross_entropy(logits, y)
         loss.backward()
-        self.opt.step(self.w, self.g, self.m, w0=w0, grad_mask=self._grad_mask)
+        self.opt.step(self.w, self.g, self.m, w0=w0, grad_mask=self._grad_mask, objective=self._objective)
         self.loss_sum += loss.detach()
 
     def _graph_body(self, dataset, B, w0):
@@ -72,7 +76,7 @@ class TorchTrainer:
         self._step(self.x[:B], self.y[:B], w0)
 
     def _get_graph(self, dataset, B, w0):
-        key = (B, dataset.data.data_ptr(), w0.data_ptr(), 0 if self._grad_mask is None else self._grad_mask.data_ptr())
+        key = (B, dataset.data.data_ptr(), w0.data_ptr(), 0 if self._grad_mask is None else self._grad_mask.data_ptr(), self._objective)
         if key in self._graphs:
             return self._graphs[key]
         meta = dataset.meta
@@ -104,6 +108,7 @@ class TorchTrainer:
         self.loss_sum.zero_()
         steps = 0
         self._grad_mask = self.attack_mask if getattr(agent, "is_corrupt", False) else None
+        self._objective = local_objective(args, getattr(agent, "is_corrupt", False) and self.attack_round)
         graphs = self.use_graphs and n <= self.max_shard
         if graphs:  # capture (first call only) BEFORE the round state is set up: capture warm-up scribbles on w/m
             full = self._get_graph(dataset, bs, w_global) if n >= bs else None

@@ -73,6 +73,9 @@ class Aggregation:
         self.fld_flagged = []         # agent ids flagged at detection (ascending)
         self.fld_detect_round = None  # the round of the detection, None until then
         self.fld_tables = None        # (table [num_agents][n_vote], ring [N + 1][n_vote], w_prev [n_vote]) of the in-process form
+        # SparseFed (--server_topk) of the in-process form: the error vector [n_vote] (allocated on first use) and the last round's fields
+        self.sparse_e = None
+        self.last_sparse = None
 
     # ---- the server step ------------------------------------------------------------------------------------
     def aggregate_updates(self, w_global, agent_params, cur_round, n_vote=None, root_params=None):
@@ -104,10 +107,20 @@ class Aggregation:
         flipped = torch.zeros(1, dtype=torch.int64, device=w_global.device)
         if self.opt is None:
             self.opt = ops.ServerOptState(n=w_global.numel(), device=w_global.device, **server_opt_spec(self.args))
+        p = float(getattr(self.args, "server_topk", 0.0))
+        out = torch.empty_like(w_global) if p > 0 else w_global      # SparseFed: the plain step's result w' goes to a scratch vector
         ops.fused_aggregate(w_global, ws, weights, self._mode, self.args.robustLR_threshold, self.server_lr, noise_std, self.args.seed,
                             cur_round,
                             n_vote if n_vote is not None else (self.layout.n_vote if self.layout else None),
-                            scales, out=w_global, flipped=flipped, opt=self.opt, total_weight=total)
+                            scales, out=out, flipped=flipped, opt=self.opt, total_weight=total)
+        if p > 0:
+            k = ops.sparsefed_k(p, self.n_params)
+            if self.sparse_e is None:
+                self.sparse_e = torch.zeros(n_voted, dtype=torch.float32, device=w_global.device)
+            stats = torch.zeros(3, dtype=torch.float64, device=w_global.device)
+            ops.sparsefed_step(w_global, out, self.sparse_e, n_voted, k, stats)
+            s = stats.tolist()
+            self.last_sparse = {"sparse_applied": int(s[0]), "sparse_threshold": s[1], "sparse_error_norm": s[2]}
         self.last_flipped = flipped
         if self.args.diagnostics:
             self.plot_norms(dict(zip(all_ids, ops.update_norms(prev, all_ws, nv).tolist())), cur_round)

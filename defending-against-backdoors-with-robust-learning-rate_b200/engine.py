@@ -75,7 +75,7 @@ class FLEngine:
         self.verbose = verbose and ctx.is_main
         torch.manual_seed(args.seed); np.random.seed(args.seed); random.seed(args.seed)
         if self.verbose:
-            print_exp_details(args)
+            print_exp_details(args, get_layout(args.model).n_params)
 
         # ---- data (device resident), partition, poisoned validation set (src/federated.py:34-45) ------------
         if datasets is None:
@@ -131,10 +131,15 @@ class FLEngine:
             backend = "local"
         if backend == "auto" and ctx.is_dist and ctx.backend == "gloo":
             backend = "gloo"
+        # SparseFed (--server_topk; DESIGN.md section 3): k of the top-k server step, its error vector and scratch live in the aggregator
+        p = float(getattr(args, "server_topk", 0.0))
+        self.topk_k = ops.sparsefed_k(p, self.layout.n_params) if p > 0 else 0
+        self.last_sparse = None
         self.fused = FusedAggregator(ctx, self.layout.n_total, self.layout.n_vote, max_slots, backend,
                                      transport=getattr(args, "agg_transport", "auto"), server_opt=server_opt_spec(args),
                                      n_part=self.n_part, history_agents=args.num_agents if args.aggr == "foolsgold" else 0,
-                                     fld_agents=args.num_agents if self.detect else 0, fld_window=args.fld_window if self.detect else 0)
+                                     fld_agents=args.num_agents if self.detect else 0, fld_window=args.fld_window if self.detect else 0,
+                                     topk_k=self.topk_k)
         init = torch.zeros(self.layout.n_total, dtype=torch.float32)
         self.layout.init_(init, args.seed)
         self.fused.w_global.copy_(init.to(dev))
@@ -195,6 +200,8 @@ class FLEngine:
             self._have_prev = False
         if args.resume:
             ck = load_checkpoint(args.resume, self.w_global, self.layout)
+            if self.fused.w_bf16 is not None:
+                self.fused.w_bf16.copy_(self.w_global.to(torch.bfloat16))   # the hand-off's first step reads the shadow
             restore_server_opt(ck, self.fused)
             self.start_round = ck["round"] + 1
             self.cum_poison_acc_mean = ck["extra"].get("cum_poison_acc_mean", 0.0)
@@ -219,6 +226,11 @@ class FLEngine:
                     raise ValueError("checkpoint has no FLDetector state, but this run uses --detect fldetector")
                 self.fused.load_fld_tables(fld["table"], fld["ring"], fld["w_prev"])
                 self.aggregator.load_fld_state(fld)
+            if self.topk_k:
+                e = ck["extra"].get("sparsefed_error")
+                if e is None:
+                    raise ValueError("checkpoint has no SparseFed state (error vector), but this run uses --server_topk")
+                self.fused.load_sparsefed_error(e)
         ctx.barrier()
 
     def _build_swaps(self):
@@ -432,9 +444,14 @@ class FLEngine:
         parts = [self.round_loss.double(), flipped]
         if self.neurotoxin_k is not None:
             parts.append(self.masked_coords.double())                   # |M| of the round, read with the same copy
+        if self.topk_k:
+            parts.append(self.fused.sparse_stats)                       # SparseFed's |M|, tau and ||e||, likewise
         vals = torch.cat(parts).cpu()
         if self.neurotoxin_k is not None:
             self.last_masked_coords = int(vals[2])
+        if self.topk_k:
+            s = vals[-3:].tolist()
+            self.last_sparse = {"sparse_applied": int(s[0]), "sparse_threshold": s[1], "sparse_error_norm": s[2]}
         n_flip = int(vals[1])
         if self.args.robustLR_threshold > 0:
             n_flip = max(0, n_flip - (self.layout.n_vote - self.layout.n_params))
@@ -502,6 +519,10 @@ class FLEngine:
             if self.last_masked_coords is not None:
                 rec["attack_masked_coords"] = self.last_masked_coords
                 self.logger.add_scalar("Attack/Masked_Coords", self.last_masked_coords, rnd)
+            if self.last_sparse is not None:
+                rec.update(self.last_sparse)
+                for key, tag in (("sparse_applied", "Applied"), ("sparse_threshold", "Threshold"), ("sparse_error_norm", "Error_Norm")):
+                    self.logger.add_scalar(f"SparseFed/{tag}", self.last_sparse[key], rnd)
             if self.last_collude is not None:
                 rec.update(self.last_collude)
                 for key, tag in (("collude_honest", "Honest"), ("collude_deviation", "Deviation"), ("collude_z", "Z")):
@@ -549,6 +570,8 @@ class FLEngine:
                     extra = {"cum_poison_acc_mean": self.cum_poison_acc_mean}
                     if self.neurotoxin_k is not None:
                         extra["neurotoxin_w_prev"] = self.w_prev.cpu()
+                    if self.topk_k:
+                        extra["sparsefed_error"] = self.fused.sparsefed_error()     # replicated on every rank: no collective
                     if hist is not None:
                         extra["foolsgold_history"] = hist
                     if fld is not None:

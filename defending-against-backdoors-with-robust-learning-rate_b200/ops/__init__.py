@@ -1309,6 +1309,58 @@ def neurotoxin_mask(w_g, w_prev, n_vote: int, k: int, mask, count):
     w_prev[:n_vote].copy_(w_g[:n_vote])
 
 
+def sparsefed_statement(w, w_new, e, n_vote: int, k: int):
+    """SparseFed's server step (Panda et al. 2022), stated in numpy, after the plain server step took ``w`` to ``w_new`` (both fp32
+    ``[n]``; ``e`` is the fp32 error vector ``[n_vote]``):
+
+    * ``u = fp32(w_new - w)`` and ``e' = fp32(e + u)`` over ``[0, n_vote)``;
+    * ``key = bits(|e'|)`` (the fp32 pattern with the sign bit cleared, so NaN sorts above +inf) and ``tau`` = the k-th largest key,
+      counted with multiplicity (``neurotoxin_statement``'s convention);
+    * ``M = {c : key[c] >= max(tau, 1)}``: every tie at tau is taken, and an error of ±0 is never applied;
+    * on M ``w'' = fp32(w + e')`` and ``e'' = 0``, elsewhere ``w'' = w`` and ``e'' = e'``; behind ``n_vote`` ``w'' = w_new``.
+
+    Returns ``(w'' [n] fp32, e'' [n_vote] fp32, |M|, float(tau), ||e''||_2 in fp64)``.  ``1 <= k <= n_vote``."""
+    n_vote, k = int(n_vote), int(k)
+    if not 1 <= k <= n_vote:
+        raise ValueError(f"k = {k} must lie in [1, n_vote = {n_vote}]")
+    f32 = lambda t: (t.detach().cpu().numpy() if torch.is_tensor(t) else np.asarray(t)).astype(np.float32, copy=False)
+    w, wn, e = f32(w), f32(w_new), f32(e)[:n_vote]
+    with np.errstate(invalid="ignore", over="ignore"):
+        e1 = e + (wn[:n_vote] - w[:n_vote])
+        key = e1.view(np.uint32) & np.uint32(0x7FFFFFFF)
+        tau = np.partition(key, n_vote - k)[n_vote - k]
+        m = key >= max(int(tau), 1)
+        out = wn.copy()
+        out[:n_vote] = np.where(m, w[:n_vote] + e1, w[:n_vote])
+    e2 = np.where(m, np.float32(0.0), e1).astype(np.float32)
+    norm = float(np.sqrt(np.sum(e2.astype(np.float64) ** 2)))
+    return out, e2, int(m.sum()), float(np.uint32(tau).view(np.float32)), norm
+
+
+def sparsefed_step(w, w_new, e, n_vote: int, k: int, stats, w_bf16=None):
+    """SparseFed's step in place (``sparsefed_statement``): ``w`` (and its bf16 shadow ``w_bf16``, when given) becomes ``w''`` and ``e``
+    becomes ``e''``; the float64 ``stats[:3]`` = ``(|M|, float(tau), ||e''||_2)``.  On the GPU the accumulate pass, the radix select and
+    the apply pass queue without a host sync and are bitwise reproducible."""
+    if w.is_cuda:
+        ext().sparsefed(w_new, w, w_bf16, e, int(n_vote), int(k), stats)
+        return
+    out, e2, applied, tau, norm = sparsefed_statement(w, w_new, e, n_vote, k)
+    w.copy_(torch.from_numpy(out))
+    e[:int(n_vote)].copy_(torch.from_numpy(e2))
+    if w_bf16 is not None:
+        w_bf16.copy_(w.to(torch.bfloat16))
+    stats[:3].copy_(torch.tensor([applied, tau, norm], dtype=torch.float64))
+
+
+def sparsefed_k(p: float, n_params: int) -> int:
+    """SparseFed's k for ``--server_topk p``: ``floor(p * n_params)``, as Neurotoxin sizes its mask.  Refuses ``p > 0`` with ``k = 0``."""
+    k = math.floor(float(p) * int(n_params))
+    if p > 0 and k < 1:
+        raise ValueError(f"--server_topk {p} applies floor({p} x n_params {n_params}) = 0 coordinates; the smallest usable p is "
+                         f"1/{n_params} = {1.0 / n_params:.3g}")
+    return k
+
+
 def boost_statement(slot, w_g, gamma: float, n_vote: int):
     """The boosted update in numpy: ``fp32((double)w_g[c] + (double)gamma * (double)fp32(slot[c] - w_g[c]))`` for ``c < n_vote``,
     each fp64 operation rounded on its own.  Returns a float32 array ``[n_vote]``."""

@@ -14,78 +14,23 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "topk_select.cuh"
 
 namespace rlr {
 
 namespace {
 
-constexpr int kBins = 2048;          // 11-bit digits; the last pass uses 512 of them (9 bits)
-constexpr int kHistThreads = 512;
+__device__ __forceinline__ uint32_t key_of(float g, float p) { return magnitude_key(g - p); }
 
-// pass p: digit bits and the shift of the prefix fixed by the earlier passes
-__device__ __forceinline__ int digit_shift(int pass) { return pass == 0 ? 20 : (pass == 1 ? 9 : 0); }
-__device__ __forceinline__ uint32_t digit_mask(int pass) { return pass == 2 ? 0x1FFu : 0x7FFu; }
-__device__ __forceinline__ int prefix_shift(int pass) { return pass == 1 ? 20 : 9; }
-
-__device__ __forceinline__ uint32_t key_of(float g, float p) { return __float_as_uint(g - p) & 0x7FFFFFFFu; }
-
-struct SelectState {
-    uint32_t prefix;                 // key bits fixed so far (right-aligned)
-    uint32_t krem;                   // rank still to find inside the selected prefix, 1-based from the top
-};
-
-__global__ void __launch_bounds__(kHistThreads) topk_hist_kernel(const float* __restrict__ wg, const float* __restrict__ wp,
-                                                                  long long n4, int pass, const SelectState* __restrict__ st,
-                                                                  uint32_t* __restrict__ hist /*[kBins]*/) {
-    __shared__ uint32_t h[kBins];
-    for (int i = threadIdx.x; i < kBins; i += blockDim.x) h[i] = 0;
-    __syncthreads();
-    const int sh = digit_shift(pass);
-    const uint32_t dm = digit_mask(pass);
-    const int psh = prefix_shift(pass);
-    const uint32_t want = pass == 0 ? 0u : st->prefix;
-    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n4; q += (long long)gridDim.x * blockDim.x) {
+// Neurotoxin's keys: a[c] = bits(|fp32(w_g[c] - w_prev[c])|)
+struct DiffKeys {
+    const float* __restrict__ wg;
+    const float* __restrict__ wp;
+    __device__ __forceinline__ uint4 keys(long long q) const {
         const float4 g = ld_f4(wg + 4 * q), p = ld_f4(wp + 4 * q);
-        const uint32_t a[4] = {key_of(g.x, p.x), key_of(g.y, p.y), key_of(g.z, p.z), key_of(g.w, p.w)};
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-            if (pass == 0 || (a[j] >> psh) == want) atomicAdd(&h[(a[j] >> sh) & dm], 1u);
+        return make_uint4(key_of(g.x, p.x), key_of(g.y, p.y), key_of(g.z, p.z), key_of(g.w, p.w));
     }
-    __syncthreads();
-    for (int i = threadIdx.x; i < kBins; i += blockDim.x)
-        if (h[i]) atomicAdd(&hist[i], h[i]);
-}
-
-// One CTA of kBins/2 threads: the bin where the count from the top reaches krem.  Thread t holds the bins 2047-2t and 2046-2t; an
-// inclusive scan of the pair sums gives every thread the count above its pair, so exactly one thread sees the crossing.
-__global__ void __launch_bounds__(kBins / 2) topk_find_kernel(const uint32_t* __restrict__ hist, int pass, SelectState* st,
-                                                              long long k) {
-    __shared__ uint32_t warp_tot[kBins / 2 / 32];
-    const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
-    const uint32_t krem = pass == 0 ? (uint32_t)k : st->krem;
-    const uint32_t prefix = pass == 0 ? 0u : st->prefix;
-    const uint32_t hi = hist[kBins - 1 - 2 * t], lo = hist[kBins - 2 - 2 * t];
-    uint32_t s = hi + lo;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, s, o);
-        if (lane >= o) s += v;
-    }
-    if (lane == 31) warp_tot[wid] = s;
-    __syncthreads();
-    uint32_t base = 0;
-    for (int w = 0; w < wid; ++w) base += warp_tot[w];
-    const uint32_t incl = base + s, above = incl - (hi + lo);
-    __syncthreads();                 // every thread has read krem / prefix before the winner rewrites them
-    const int bits = pass == 2 ? 9 : 11;
-    if (above < krem && above + hi >= krem) {
-        st->prefix = (prefix << bits) | (uint32_t)(kBins - 1 - 2 * t);
-        st->krem = krem - above;
-    } else if (above + hi < krem && incl >= krem) {
-        st->prefix = (prefix << bits) | (uint32_t)(kBins - 2 - 2 * t);
-        st->krem = krem - above - hi;
-    }
-}
+};
 
 // M = {c < n_vote : a[c] >= max(tau, 1)} as bit words (bit c % 32 of word c / 32), |M| into *count, and w_prev <- w_g.  Each thread
 // takes one float4 (4 mask bits); the 8 lanes that share a word OR their nibbles together.
@@ -161,11 +106,6 @@ __global__ void __launch_bounds__(256) swap_samples_kernel(unsigned char* __rest
     }
 }
 
-inline int sweep_grid(long long n4, int threads, int num_sms, int per_sm) {
-    const long long want = (n4 + threads - 1) / threads, cap = (long long)num_sms * per_sm;
-    return (int)(want < 1 ? 1 : (want > cap ? cap : want));
-}
-
 }  // namespace
 
 cudaError_t launch_swap_samples(void* data, long long* targets, const long long* idx, void* side, long long* side_targets, long long n,
@@ -197,19 +137,11 @@ cudaError_t launch_neurotoxin_mask(const float* w_g, float* w_prev, long long n_
         RLR_CUDA_CHECK(cudaMemsetAsync(mask, 0, (size_t)words * sizeof(uint32_t), st));
         return cudaMemcpyAsync(w_prev, w_g, (size_t)n_vote * sizeof(float), cudaMemcpyDeviceToDevice, st);
     }
-    // three histograms and the select state, zeroed together
-    const size_t bytes = 3 * kBins * sizeof(uint32_t) + sizeof(SelectState);
-    Scratch scr(bytes, st);
+    Scratch scr(kSelectScratchBytes, st);
     uint32_t* hist = scr.as<uint32_t>();
     SelectState* sel = reinterpret_cast<SelectState*>(hist + 3 * kBins);
-    RLR_CUDA_CHECK(cudaMemsetAsync(hist, 0, bytes, st));
-    const int grid = sweep_grid(n4, kHistThreads, num_sms, 4);
-    for (int pass = 0; pass < 3; ++pass) {
-        topk_hist_kernel<<<grid, kHistThreads, 0, st>>>(w_g, w_prev, n4, pass, sel, hist + pass * kBins);
-        RLR_CUDA_CHECK(cudaGetLastError());
-        topk_find_kernel<<<1, kBins / 2, 0, st>>>(hist + pass * kBins, pass, sel, k);
-        RLR_CUDA_CHECK(cudaGetLastError());
-    }
+    RLR_CUDA_CHECK(cudaMemsetAsync(hist, 0, kSelectScratchBytes, st));
+    RLR_CUDA_CHECK(topk_select(DiffKeys{w_g, w_prev}, n4, k, hist, sel, sweep_grid(n4, kHistThreads, num_sms, 4), 0, st));
     neurotoxin_mask_kernel<<<sweep_grid(n4, 256, num_sms, 8), 256, 0, st>>>(w_g, w_prev, n4, sel, mask,
                                                                               reinterpret_cast<unsigned long long*>(count));
     return cudaGetLastError();

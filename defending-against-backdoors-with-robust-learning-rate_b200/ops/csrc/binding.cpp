@@ -515,6 +515,20 @@ void neurotoxin_mask(at::Tensor w_g, at::Tensor w_prev, int64_t n_vote, int64_t 
           "neurotoxin_mask");
 }
 
+void sparsefed(at::Tensor w_new, at::Tensor w, c10::optional<at::Tensor> w_bf16, at::Tensor e, int64_t n_vote, int64_t k, at::Tensor stats) {
+    CHECK_CUDA(w_new); CHECK_CUDA(w); CHECK_CUDA(e); CHECK_CUDA(stats);
+    TORCH_CHECK(w_new.scalar_type() == at::kFloat && w.scalar_type() == at::kFloat && e.scalar_type() == at::kFloat &&
+                stats.scalar_type() == at::kDouble && stats.numel() >= 3, "sparsefed: fp32 w_new / w / e and an fp64 stats[3]");
+    TORCH_CHECK(w_new.numel() == w.numel() && e.numel() >= n_vote && n_vote <= w.numel(), "sparsefed: w_new / w / e sizes");
+    if (w_bf16) {
+        CHECK_CUDA(*w_bf16);
+        TORCH_CHECK(w_bf16->scalar_type() == at::kBFloat16 && w_bf16->numel() == w.numel(), "sparsefed: bf16 shadow of w's size");
+    }
+    c10::cuda::CUDAGuard guard(w.device());
+    check(rlr::launch_sparsefed(w_new.data_ptr<float>(), w.data_ptr<float>(), w_bf16 ? w_bf16->data_ptr() : nullptr, e.data_ptr<float>(),
+                                n_vote, w.numel(), k, stats.data_ptr<double>(), num_sms(), cur_stream()), "sparsefed");
+}
+
 void boost_update(at::Tensor slot, at::Tensor w_g, double gamma, int64_t n_vote) {
     CHECK_CUDA(slot); CHECK_CUDA(w_g);
     TORCH_CHECK(slot.scalar_type() == at::kFloat && w_g.scalar_type() == at::kFloat);
@@ -638,6 +652,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("mask") = py::none(), py::arg("objective") = py::none());
     m.def("neurotoxin_mask", &neurotoxin_mask);
     m.def("boost_update", &boost_update);
+    m.def("sparsefed", &sparsefed);
     m.def("swap_samples", &swap_samples);
     m.def("pgd_project", &pgd_project, py::arg("w"), py::arg("w0"), py::arg("w_bf16"), py::arg("clip"), py::arg("d_sqnorm"),
           py::arg("n_pgd") = 0, py::arg("mask") = py::none());

@@ -216,6 +216,15 @@ cudaError_t launch_boost_update(float* slot, const float* w_g, long long n_vote,
 cudaError_t launch_swap_samples(void* data, long long* targets, const long long* idx, void* side, long long* side_targets, long long n,
                                 long long row_bytes, int num_sms, cudaStream_t st);
 
+// ---- SparseFed server step (sparsefed.cu) -----------------------------------------------------------------------------------------
+// After the plain server step wrote its fp32 result to w_new: over [0, n_vote) e <- fp32(e + fp32(w_new - w)), tau = the k-th largest
+// bits(|e|) (with multiplicity) by the on-device radix select, and on M = {c : bits(|e[c]|) >= max(tau, 1)} w <- fp32(w + e), e <- 0;
+// w[n_vote:] <- w_new[n_vote:]; the bf16 shadow (optional) <- bf16(w) everywhere.  stats (device fp64 [3]) = {|M|, float(tau),
+// ||e||_2}, the norm from per-CTA partials added in CTA order.  No host sync, no float atomics: bitwise reproducible.
+// n_vote % 4 == 0, n % 4 == 0, n_vote <= n, 1 <= k <= n_vote < 2^32.
+cudaError_t launch_sparsefed(const float* w_new, float* w, void* w_bf16, float* e, long long n_vote, long long n, long long k,
+                             double* stats, int num_sms, cudaStream_t st);
+
 // ---- loss / evaluation -----------------------------------------------------------------------------------
 // logits [B,C] (kind 0 fp32 / 1 bf16); writes dlogits (same kind, scaled by 1/B) and accumulates loss_sum / correct.
 cudaError_t launch_softmax_xent(const void* logits, int kind, const int64_t* labels, void* dlogits, float* loss_sum,

@@ -118,6 +118,10 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--server_beta1", type=float, default=0.9, help="server optimizer first-moment decay, in [0, 1)")
     p.add_argument("--server_beta2", type=float, default=0.99, help="adam / yogi second-moment decay, in [0, 1)")
     p.add_argument("--server_tau", type=float, default=1e-3, help="adagrad / adam / yogi adaptivity tau > 0 (v starts at tau^2)")
+    p.add_argument("--server_topk", type=float, default=0.0,
+                   help="SparseFed (Panda et al. 2022): every round the server applies only the k = floor(p * n_params) largest "
+                        "coordinates of its accumulated step (after the vote, the rule, noise and --server_opt) and carries the rest over "
+                        "as error feedback.  0 <= p <= 1 (0 = off).  The paper's setting adds --server_clip --clip L")
     p.add_argument("--select", type=str, default="none", choices=SELECTIONS,
                    help="participant selection before the --aggr rule: krum (Blanchard et al. 2017) admits the participant whose update "
                         "is closest to its K-F-2 nearest neighbours; multikrum the M best such scores; dnc (Shejwalkar and Houmansadr "
@@ -222,6 +226,10 @@ def finalize_args(args: argparse.Namespace) -> argparse.Namespace:
             raise ValueError(f"--{name} {getattr(args, name)} must lie in [0, 1)")
     if not getattr(args, "server_tau", 1.0) > 0:
         raise ValueError(f"--server_tau {args.server_tau} must be > 0")
+    topk = float(getattr(args, "server_topk", 0.0))
+    if not (math.isfinite(topk) and 0.0 <= topk <= 1.0):
+        raise ValueError(f"--server_topk {topk} must be a finite number in [0, 1]")
+    args.server_topk = topk
     if args.model == "auto":
         args.model = "cnn_cifar" if args.data == "cifar10" else "cnn_mnist"
     if args.aggr not in AGGREGATORS:
@@ -509,8 +517,9 @@ def make_args(**overrides) -> argparse.Namespace:
     return finalize_args(args)
 
 
-def print_exp_details(args) -> None:
-    """Experiment banner; same 14 fields as reference src/utils.py:287-303 plus engine fields."""
+def print_exp_details(args, n_params: int | None = None) -> None:
+    """Experiment banner; same 14 fields as reference src/utils.py:287-303 plus engine fields.  ``n_params``: the model's parameter count,
+    which sizes SparseFed's k (shown as ``-`` when not given)."""
     print("======================================")
     print(f"    Dataset: {args.data}")
     print(f"    Global Rounds: {args.rounds}")
@@ -530,6 +539,9 @@ def print_exp_details(args) -> None:
     print(f"    Crop pad / hflip: {args.crop_pad} / {args.hflip}")
     if getattr(args, "server_opt", "sgd") != "sgd":
         print(f"    Server optimizer (beta1 / beta2 / tau): {args.server_opt} ({args.server_beta1} / {args.server_beta2} / {args.server_tau})")
+    if getattr(args, "server_topk", 0.0) > 0:
+        k = math.floor(args.server_topk * n_params) if n_params is not None else "-"
+        print(f"    Server top-k (SparseFed): {args.server_topk} / {k}")
     if getattr(args, "select", "none") in ("krum", "multikrum"):
         print(f"    Selection (F / M): {args.select} ({args.select_f} / {args.select_m})")
     if getattr(args, "select", "none") == "dnc":

@@ -2,7 +2,7 @@
 
 Per-rank symmetric slab layout (byte offsets identical on every rank):
 
-    [ flags: uint32[3*world] (+pad to 4 KiB) | w_global fp32[n] | w_global bf16[n] | slot_0 fp32[n] | slot_1 ... ]
+    [ flags: uint32[3*world] (+pad to 4 KiB) | w_global fp32[n] | w_global bf16[n] | slot_0 fp32[n] | slot_1 ... ( | scratch fp32[n] ) ]
 
 Flag words of a rank: [0, world) barrier-in arrivals, [world, 2 world) barrier-out arrivals, [2 world, 3 world) broadcast-ready
 words ("slice r of the new global parameters has landed here", written by rank r).
@@ -35,6 +35,13 @@ coordinates -- and with every other transport each rank keeps the full vector (i
 histories (``--aggr foolsgold``) are laid out the same way: ``[num_agents][slice ∩ [0, n_vote)]`` on the fused multi-GPU path, the full
 ``[num_agents][n_vote]`` table on every rank otherwise.  FLDetector's state (``--detect fldetector``: the per-agent last-update table,
 the ring of the last N + 1 global updates and the previous global parameters) uses the same column layout.
+
+SparseFed (``--server_topk``; ``ops.sparsefed_statement``) runs replicated, not sharded: the unchanged aggregation kernel writes its fp32
+result ``w'`` into the ``scratch`` region (allocated only then; multicast to every rank on the fused multi-GPU path, which then runs the
+kernel with its barrier-out), and every rank runs the SparseFed passes locally over the whole vector on its own full copy of the error
+vector ``e``.  ``w'`` is identical on every rank, so ``e`` is too, at every world size: no histogram all-reduce, and rank 0 alone
+checkpoints it.  With the fused hand-off the rank's ``w_global`` is complete when the apply pass ends, so it then marks its own ready
+word of every slice with the round's epoch (no peer publishes during a barrier-out launch).
 """
 from __future__ import annotations
 
@@ -53,11 +60,12 @@ FLAG_BYTES = 4096
 class FusedAggregator:
     def __init__(self, ctx, n_total: int, n_vote: int, max_slots: int, backend: str = "auto", with_bf16: bool = True,
                  transport: str = "auto", server_opt=None, n_part: int | None = None, history_agents: int = 0, fld_agents: int = 0,
-                 fld_window: int = 0):
+                 fld_window: int = 0, topk_k: int = 0):
         """``server_opt``: optional ``dict(kind=..., beta1=..., beta2=..., tau=...)``; ``n_part``: participants per round (default
         every slot), which fixes whether the fused multi-GPU kernel or the gather fallback runs, and so the state layout;
         ``history_agents``: agents whose FoolsGold update history this aggregator keeps (``--aggr foolsgold``: ``--num_agents``; 0 = none);
-        ``fld_agents`` / ``fld_window``: agents and window N of the FLDetector state (``--detect fldetector``; 0 = none)."""
+        ``fld_agents`` / ``fld_window``: agents and window N of the FLDetector state (``--detect fldetector``; 0 = none);
+        ``topk_k``: SparseFed's k (``--server_topk``; 0 = off, nothing allocated)."""
         self.ctx = ctx
         # nccl / gloo back-ends: "gather" all-gathers every participant's parameters and runs the kernel on the copies (any
         # aggregator); "reduce" all-reduces per-coordinate partial sums (vote, weighted update sum) -- O(N) instead of O(K N)
@@ -83,11 +91,23 @@ class FusedAggregator:
         self.off_wb = self.off_wg + 4 * n
         self.off_slots = self.off_wb + 2 * n
         nbytes = self.off_slots + 4 * n * self.max_slots
+        self.topk_k = int(topk_k)
+        self.off_scratch = nbytes
+        if self.topk_k:
+            nbytes += 4 * n
         use_symm = backend == "fused" and ctx.is_dist
         self.buf = SymmetricBuffer(ctx, nbytes) if use_symm else SymmetricBuffer(_Solo(ctx), nbytes)
         self.w_global = self.buf.tensor(self.off_wg, n, torch.float32)
         self.w_bf16 = self.buf.tensor(self.off_wb, n, torch.bfloat16) if self.with_bf16 else None
         self.slots = [self.buf.tensor(self.off_slots + 4 * n * j, n, torch.float32) for j in range(self.max_slots)]
+        # SparseFed: the plain step's result w', the error vector e over [0, n_vote) and the round's (|M|, float(tau), ||e||) on the device
+        self.scratch = self.sparse_e = self.sparse_stats = None
+        if self.topk_k:
+            if not 1 <= self.topk_k <= self.n_vote:
+                raise ValueError(f"SparseFed k = {self.topk_k} must lie in [1, n_vote = {self.n_vote}]")
+            self.scratch = self.buf.tensor(self.off_scratch, n, torch.float32)
+            self.sparse_e = torch.zeros(self.n_vote, dtype=torch.float32, device=dev)
+            self.sparse_stats = torch.zeros(3, dtype=torch.float64, device=dev)
         self.flipped = torch.zeros(1, dtype=torch.int64, device=dev)
         self.flipped_is_partial = False   # True after a launch in which every rank counted only its own coordinate slice
         self.epoch = 0
@@ -111,6 +131,9 @@ class FusedAggregator:
                 self.out_ptrs = ops.PtrTable([self.buf.peer_ptr(r, self.off_wg) for r in range(world)], dev)
                 self.out_bf16_ptrs = (ops.PtrTable([self.buf.peer_ptr(r, self.off_wb) for r in range(world)], dev)
                                       if self.with_bf16 else None)
+            if self.topk_k:
+                self.scratch_ptrs = ops.PtrTable([self.buf.mc_ptr(self.off_scratch)] if self.use_multimem else
+                                                 [self.buf.peer_ptr(r, self.off_scratch) for r in range(world)], dev)
             # coordinate slices: multiples of 4, cover [0, n)
             per = (n // 4 + world - 1) // world * 4
             self.per = per
@@ -575,25 +598,57 @@ class FusedAggregator:
             wt = torch.as_tensor(weights, dtype=torch.float64).to(dev)
             sc = torch.as_tensor(scales, dtype=torch.float32).to(dev) if scales is not None else None
             table = self._agent_table(n_part) if members is None else self._member_table(idx)
+            sparse = self.topk_k > 0
+            # SparseFed: w' is multicast into every rank's scratch, behind the kernel's barrier-out (never the hand-off publication)
+            outs = self.scratch_ptrs.tensor if sparse else self.out_ptrs.tensor
+            outs_b = self.out_bf16_ptrs.tensor if (self.out_bf16_ptrs and not sparse) else None
             ops.ext().fused_aggregate(
                 table.tensor, wt, sc, total, self.w_global.data_ptr(),
-                self.out_ptrs.tensor, self.out_bf16_ptrs.tensor if self.out_bf16_ptrs else None, self.use_multimem,
+                outs, outs_b, self.use_multimem,
                 self.begin, self.end, self.n_vote, ops.MODE_IDS[mode], int(theta), float(server_lr), float(noise_std),
                 int(seed), int(rnd), self.flipped, self.flag_ptrs.tensor, self.local_sync, ctx.rank, ctx.world, self.epoch,
-                bool(self.handoff), *ops.opt_launch_args(self.opt))
+                bool(self.handoff) and not sparse, *ops.opt_launch_args(self.opt))
+            if sparse:
+                self._sparsefed()
+                if self.handoff:
+                    # this rank's w_global is complete: mark its own ready word of every slice (stream-ordered after the apply pass)
+                    world = ctx.world
+                    self.buf.tensor(self.off_flags, 3 * world, torch.int32)[2 * world:].fill_(self.epoch)
             if self.handoff:
                 self.epoch_dev.fill_(self.epoch)      # what the next round's consumers wait for (stream-ordered before their graphs)
             return
         # ---- baseline transports / single process ------------------------------------------------------------------
         if ctx.is_dist and self.transport == "reduce" and mode in ("avg", "sign") and members is None:
             self._aggregate_reduce(weights, mode, theta, server_lr, noise_std, seed, rnd, scales, total)
+            if self.topk_k:
+                self._sparsefed()
             return
         # gather participant params, run the kernel locally
         agents = self._participants(n_part, participants)
         if members is not None:
             agents = [agents[j] for j in idx]
+        sparse = self.topk_k > 0
         ops.fused_aggregate(self.w_global, agents, weights, mode, theta, server_lr, noise_std, seed, rnd, self.n_vote,
-                            scales, out=self.w_global, out_bf16=self.w_bf16, flipped=self.flipped, opt=self.opt, total_weight=total)
+                            scales, out=self.scratch if sparse else self.w_global, out_bf16=None if sparse else self.w_bf16,
+                            flipped=self.flipped, opt=self.opt, total_weight=total)
+        if sparse:
+            self._sparsefed()
+
+    def _sparsefed(self):
+        """SparseFed after the plain step wrote ``w'`` into ``scratch``: ``ops.sparsefed_step`` over the whole vector on this rank, which
+        updates ``w_global``, its bf16 shadow, the error vector and ``sparse_stats``."""
+        ops.sparsefed_step(self.w_global, self.scratch, self.sparse_e, self.n_vote, self.topk_k, self.sparse_stats, self.w_bf16)
+
+    def sparsefed_error(self):
+        """SparseFed's fp32 error vector ``[n_vote]`` on the host (identical on every rank: no collective)."""
+        return self.sparse_e.cpu()
+
+    def load_sparsefed_error(self, e):
+        if self.sparse_e is None:
+            raise ValueError("this aggregator keeps no SparseFed state (topk_k = 0)")
+        if tuple(e.shape) != (self.n_vote,):
+            raise ValueError(f"SparseFed error vector of shape {tuple(e.shape)}; this run keeps {self.n_vote} voted coordinates")
+        self.sparse_e.copy_(e.to(self.sparse_e.device))
 
     def _aggregate_reduce(self, weights, mode, theta, server_lr, noise_std, seed, rnd, scales, total_weight):
         """All-reduce transport: every rank folds its local participants into (vote, weighted sum), two all_reduce calls make them
@@ -613,9 +668,12 @@ class FusedAggregator:
             noise[self.n_vote:] = 0
         new, nflip = ops.aggregate_from_partials(self.w_global, vote, wsum, total_weight, mode, theta, server_lr,
                                                  noise, self.n_vote, self.opt)
-        self.w_global.copy_(new)
-        if self.w_bf16 is not None:
-            self.w_bf16.copy_(new.to(torch.bfloat16))
+        if self.topk_k:
+            self.scratch.copy_(new)                  # SparseFed's pass follows (aggregate)
+        else:
+            self.w_global.copy_(new)
+            if self.w_bf16 is not None:
+                self.w_bf16.copy_(new.to(torch.bfloat16))
         self.flipped += nflip
 
     def server_opt_state(self):

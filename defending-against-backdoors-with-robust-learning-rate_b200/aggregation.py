@@ -13,6 +13,9 @@ that launch too: the Gram matrix of the updates (``ops.pairwise_gram``) gives FL
 noise (``ops.flame_admit``), and the admitted participants' clipped updates are averaged with equal weights.  ``--aggr foolsgold`` keeps
 every agent's summed updates across rounds (``ops.history_accumulate``) and weights the mean by FoolsGold's ``ops.foolsgold_weights`` on
 the Gram matrix of those histories (``ops.history_gram``), so agents that keep pushing the model the same way lose their weight.
+``--aggr flare`` weights that launch by FLARE's trust: the MMD between the participants' penultimate-layer representations of a clean
+root set (``ops.flare_sums`` on the features the engine computes) and a softmax over how often each is among the others' nearest
+neighbours (``ops.flare_weights``).
 ``--detect fldetector`` is a stage ahead of the rule: every round it predicts each agent's update from its last one and an L-BFGS
 Hessian-vector product of the recent global updates (``ops.fld_hvp_coefficients`` on the Gram matrix of the update ring,
 ``ops.fld_hvp``), scores the distance to the prediction (``ops.fld_predict``) and, once the gap statistic finds a minority cluster of high
@@ -63,6 +66,7 @@ class Aggregation:
         self.last_rfa = None          # the RFA/* scalars of the last round (--aggr rfa)
         self.last_flame = None        # the FLAME/* scalars of the last round (--aggr flame)
         self.last_foolsgold = None    # the FoolsGold/* scalars of the last round (--aggr foolsgold)
+        self.last_flare = None        # the FLARE/* scalars of the last round (--aggr flare)
         self.history = None           # [num_agents][n_vote] FoolsGold histories of the in-process form (allocated on first use)
         self.opt = None               # full-length server optimizer state of the in-process form (allocated on first use)
         # FLDetector (--detect fldetector): host state identical on every rank, and the in-process form's tables (allocated on first use)
@@ -78,14 +82,17 @@ class Aggregation:
         self.last_sparse = None
 
     # ---- the server step ------------------------------------------------------------------------------------
-    def aggregate_updates(self, w_global, agent_params, cur_round, n_vote=None, root_params=None):
+    def aggregate_updates(self, w_global, agent_params, cur_round, n_vote=None, root_params=None, features=None):
         """In-process form: ``agent_params`` = {agent_id: flat local parameters}.  Updates ``w_global`` in place.  ``root_params``:
-        the server's root-trained parameters, needed by ``--aggr fltrust``."""
+        the server's root-trained parameters, needed by ``--aggr fltrust``; ``features``: fp32 ``[K][n][d]`` root-set features of the
+        participants in ``agent_params``' order, needed by ``--aggr flare``."""
         ids = list(agent_params.keys())
         ws = [agent_params[i] for i in ids]
         nv = n_vote if n_vote is not None else (self.layout.n_vote if self.layout else None)
         if self._fltrust and root_params is None:
             raise ValueError("--aggr fltrust needs the server's root parameters (root_params)")
+        if self._flare and features is None:
+            raise ValueError("--aggr flare needs the participants' root-set features (features)")
         clip = self._clip_scales(ops.update_norms(w_global, ws, nv)) if self._server_clip else None
         all_ids, all_ws = ids, ws
         n_voted = nv if nv is not None else w_global.numel()
@@ -99,7 +106,7 @@ class Aggregation:
         keep, weights, scales, total, noise_std = self._admission(ids, clip, detection, distances, dnc,
                                                                   lambda: ops.trust_stats(ws, root_params, w_global, nv), rfa_pass, gram,
                                                                   lambda members: self._history_pass(w_global, ws, ids, members, nv),
-                                                                  cur_round)
+                                                                  cur_round, lambda: features)
         if keep is not None and len(keep) < len(ids):
             ids, ws, weights = [ids[j] for j in keep], [ws[j] for j in keep], [weights[j] for j in keep]
             scales = scales[torch.as_tensor(keep, device=scales.device)] if scales is not None else None
@@ -127,9 +134,10 @@ class Aggregation:
             self.plot_sign_agreement(prev, w_global, ws, ids, cur_round)     # the vote that happened: admitted participants only
         return
 
-    def aggregate_slots(self, participants, cur_round):
+    def aggregate_slots(self, participants, cur_round, flare_local=None):
         """Engine form: participant j's parameters live in ``fused.slot_owner(j)``; updates every rank's global.  Under
-        ``--aggr fltrust`` the server's root job is position ``len(participants)``."""
+        ``--aggr fltrust`` the server's root job is position ``len(participants)``.  ``flare_local``: under ``--aggr flare``, this rank's
+        ``[max_slots][n][d]`` root-set features of the participants in its slots (``FusedAggregator.flare_features``)."""
         K = len(participants)
         diag = bool(self.args.diagnostics)
         norms = self.fused.update_norms(K) if self._server_clip or diag else None
@@ -149,7 +157,8 @@ class Aggregation:
             lambda: self.fused.trust_stats(K, K, gathered),
             lambda b, members: self.fused.rfa_sqdist(K, b, clip, members, copies),
             lambda members: self.fused.pairwise_gram(K, members, copies),
-            lambda members: self.fused.foolsgold_gram(K, participants, members, copies), cur_round)
+            lambda members: self.fused.foolsgold_gram(K, participants, members, copies), cur_round,
+            lambda: self.fused.flare_features(K, flare_local))
         if diag:   # the sign-agreement analysis needs the pre-step global parameters and every admitted participant's parameters
             prev = self.fused.w_global.clone()
             ws = [w.clone() for w in self.fused.gather_participants(K)]
@@ -171,13 +180,14 @@ class Aggregation:
     def _select(self):
         return getattr(self.args, "select", "none") != "none"
 
-    def _admission(self, ids, clip, detection, distances, dnc_grams, trust_stats, rfa_pass, gram, history, cur_round):
+    def _admission(self, ids, clip, detection, distances, dnc_grams, trust_stats, rfa_pass, gram, history, cur_round, features=None):
         """Admission of the participants ``ids`` shared by both forms of the step: FLDetector's ``detection()`` (``--detect``), which returns
         the positions of the agents it has not flagged (None while it has flagged nobody), or Krum / Multi-Krum on ``distances()`` or DnC
         on its Gram matrices ``dnc_grams()`` (``--select``),
         then FLTrust on ``trust_stats()`` (``--aggr fltrust``), RFA's weights from ``rfa_pass(b, members)`` (``--aggr rfa``), FLAME on
         the Gram matrix ``gram(members)`` (``--aggr flame``) or FoolsGold on ``history(members)``, the Gram matrix of the members' update
-        histories after this round's updates are folded in (``--aggr foolsgold``).  ``clip``: the server-clipping scales or None.  Returns
+        histories after this round's updates are folded in (``--aggr foolsgold``), or FLARE on the participants' root-set features
+        ``features()`` (``--aggr flare``).  ``clip``: the server-clipping scales or None.  Returns
         ``(members, weights, scales, total_weight, noise_std)`` for the step: members None admits everyone; weights are per position in
         ``ids``."""
         keep = self._admit(ids, cur_round, distances, dnc_grams) if self._select else (detection() if self._detect else None)
@@ -186,6 +196,9 @@ class Aggregation:
             return (*self._trust(trust_stats(), ids, keep, cur_round), noise_std)
         if self._flame:
             return self._flame_step(ids, keep, gram, cur_round)
+        if self._flare:
+            members, weights, total = self._flare_step(ids, keep, features, cur_round)
+            return members, weights, clip, total, noise_std
         weights = [float(self.agent_data_sizes[i]) for i in ids]
         if self._foolsgold:
             members, weights, total = self._foolsgold_step(ids, keep, weights, history, cur_round)
@@ -338,10 +351,15 @@ class Aggregation:
         return self.args.aggr == "foolsgold"
 
     @property
+    def _flare(self):
+        return self.args.aggr == "flare"
+
+    @property
     def _mode(self):
         """The aggregate kernel's rule: FLTrust is its weighted mean with trust weights and per-participant scales, RFA with its
-        Weiszfeld weights, FLAME with equal weights and its clip scales, FoolsGold with its weights times the data sizes."""
-        return "avg" if self._fltrust or self._rfa or self._flame or self._foolsgold else self.args.aggr
+        Weiszfeld weights, FLAME with equal weights and its clip scales, FoolsGold with its weights times the data sizes, FLARE with its
+        trust scores."""
+        return "avg" if self._fltrust or self._rfa or self._flame or self._foolsgold or self._flare else self.args.aggr
 
     def _history_pass(self, w_global, ws, ids, members, nv):
         """In-process form of the FoolsGold history pass: fold the updates of the participants at positions ``members`` into the rows of
@@ -379,6 +397,39 @@ class Aggregation:
                                "FoolsGold/Admitted": len(self.last_admitted)}
         if self.writer is not None:
             for k, v in self.last_foolsgold.items():
+                if v is not None:
+                    self.writer.add_scalar(k, v, cur_round)
+        return members, w, total
+
+    def _flare_step(self, ids, keep, features, cur_round):
+        """FLARE over the positions ``keep`` that selection or detection admitted (all when None): ``ops.flare`` on the candidates' rows of
+        ``features()`` (fp32 ``[K][n][d]``, identical on every rank).  Returns ``(members, weights, total_weight)`` for the step: F, the
+        candidates whose features are all finite, with weights ``fp32(TS_j)`` and total weight the sum of those fp32 weights (data sizes
+        are not used) -- or, when F is empty, every candidate with weight 0 and total weight 1, so the aggregate is 0 plus noise.  Records
+        ``last_admitted`` (F) and logs the mean trust of honest (ids >= num_corrupt) and corrupt candidates, the corrupt share of the
+        trust and the bandwidth sigma^2."""
+        K = len(ids)
+        cand = list(range(K)) if keep is None else [int(j) for j in keep]
+        Z = features()
+        if cand != list(range(K)):
+            Z = Z[torch.as_tensor(cand, dtype=torch.int64, device=Z.device)]
+        res = ops.flare(Z, self.args.flare_k, self.args.flare_tau)
+        members = [cand[j] for j in res.members]
+        w = [0.0] * K
+        for j, t in zip(cand, res.weights):
+            w[j] = float(np.float32(t))
+        total = sum(w[j] for j in members)
+        self.last_admitted = [ids[j] for j in members]
+        if not members:
+            members, w, total = cand, [0.0] * K, 1.0
+        nc = self.args.num_corrupt
+        honest = [float(t) for j, t in zip(cand, res.weights) if ids[j] >= nc]
+        corrupt = [float(t) for j, t in zip(cand, res.weights) if ids[j] < nc]
+        self.last_flare = {"FLARE/Avg_Honest_Trust": sum(honest) / len(honest) if honest else None,
+                           "FLARE/Avg_Corrupt_Trust": sum(corrupt) / len(corrupt) if corrupt else None,
+                           "FLARE/Corrupt_Weight": sum(corrupt), "FLARE/Bandwidth": res.sigma2}
+        if self.writer is not None:
+            for k, v in self.last_flare.items():
                 if v is not None:
                     self.writer.add_scalar(k, v, cur_round)
         return members, w, total

@@ -29,6 +29,7 @@ from .aggregation import Aggregation, server_opt_spec
 from .data import distribute_data, get_datasets, make_poisoned_val
 from .data.datasets import DeviceDataset, h5_to_device_dataset, load_fedemnist_client
 from .models import get_layout
+from .models.graph import feature_dim
 from .options import attack_schedule_set, is_attack_round, last_attack_round, print_exp_details
 from .parallel import FusedAggregator, init_distributed
 from .trainers import make_trainer
@@ -146,6 +147,14 @@ class FLEngine:
         if self.fused.w_bf16 is not None:
             self.fused.w_bf16.copy_(self.fused.w_global.to(torch.bfloat16))
         self.w_global = self.fused.w_global
+        # ---- FLARE: the clean root set every submitted model runs on, assembled once (eval normalisation, no augmentation), and this
+        # rank's [max_slots][|R|][d] block of its participants' penultimate-layer features.  Nothing is trained on R.
+        self.flare_x = self.flare_local = None
+        if args.aggr == "flare":
+            poisoned = [i for a in self.agents for i in a.poisoned_idxs]
+            root = draw_root_set(len(self.train_dataset), poisoned, args.root_size, args.seed)
+            self.flare_x, _ = self.train_dataset.batch(torch.as_tensor(root, device=dev))
+            self.flare_local = torch.zeros((max_slots, len(root), feature_dim(self.layout)), dtype=torch.float32, device=dev)
 
         self.trainer = make_trainer(args.trainer, self.layout, args, dev, max_shard)
         # Several agents per GPU and round can be trained concurrently: trainer i (own parameters, activations, CUDA graphs) runs
@@ -389,9 +398,22 @@ class FLEngine:
         self.timer.stop("local_train")
         self.timer.start("aggregate")
         self.last_collude = self._collude(chosen, rnd) if (attack and self.collude != "none") else None
-        self.aggregator.aggregate_slots(chosen, rnd)
+        if self.flare_x is not None:
+            self.aggregator.aggregate_slots(chosen, rnd, flare_local=self._flare_features(chosen))
+        else:
+            self.aggregator.aggregate_slots(chosen, rnd)
         self.timer.stop("aggregate")
         return {"chosen": chosen, "steps": steps, "h2d_bytes": h2d}
+
+    def _flare_features(self, chosen):
+        """FLARE: the root-set features of the participants this rank owns (``slot_owner``), from their final slots (after boosting and
+        collusion), into ``flare_local``; on the main stream, after the trainer streams have joined."""
+        fused = self.fused
+        for j in range(len(chosen)):
+            r, s = fused.slot_owner(j)
+            if r == self.ctx.rank:
+                self.flare_local[s].copy_(self.trainer.root_features(fused.slots[s], self.flare_x))
+        return self.flare_local
 
     def _neurotoxin_mask(self, attack: bool = True):
         """Start of a round with Neurotoxin on: the mask of the last global update ``w_global - w_prev`` (the top-k coordinates by
@@ -548,6 +570,10 @@ class FLEngine:
                 rec["flame_corrupt_admitted"] = self.aggregator.last_flame["FLAME/Corrupt_Admitted"]
                 rec["flame_clip_bound"] = self.aggregator.last_flame["FLAME/Clip_Bound"]
                 rec["flame_noise_std"] = self.aggregator.last_flame["FLAME/Noise_Std"]
+            if self.aggregator.last_flare is not None:
+                for key, tag in (("flare_avg_honest", "Avg_Honest_Trust"), ("flare_avg_corrupt", "Avg_Corrupt_Trust"),
+                                 ("flare_corrupt_weight", "Corrupt_Weight"), ("flare_bandwidth", "Bandwidth")):
+                    rec[key] = self.aggregator.last_flare[f"FLARE/{tag}"]
             if self.aggregator.last_foolsgold is not None:
                 rec["foolsgold_avg_honest"] = self.aggregator.last_foolsgold["FoolsGold/Avg_Honest_Weight"]
                 rec["foolsgold_avg_corrupt"] = self.aggregator.last_foolsgold["FoolsGold/Avg_Corrupt_Weight"]

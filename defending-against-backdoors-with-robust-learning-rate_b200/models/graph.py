@@ -187,6 +187,16 @@ class FlatLayout:
         return flat
 
 
+def head_index(layout) -> int:
+    """Index of the model's last ``linear`` node (the head); its input is the penultimate-layer representation."""
+    return max(i for i, nd in enumerate(layout.nodes) if nd.op == "linear")
+
+
+def feature_dim(layout) -> int:
+    """Width d of the penultimate-layer representation: the input features of the last ``linear`` node."""
+    return int(layout.nodes[head_index(layout)].attrs["cin"])
+
+
 class GraphNet(nn.Module):
     """PyTorch interpreter of the IR; parameters/buffers are views into the flat buffers ``w`` (and ``g``)."""
 
@@ -220,14 +230,19 @@ class GraphNet(nn.Module):
     def P(self, name):
         return self._parameters[name.replace(".", "__")]
 
-    def forward(self, x):
+    def forward(self, x, tap: bool = False):
+        """Logits of ``x`` (fp32); with ``tap`` the input of the last ``linear`` node instead (the penultimate-layer representation
+        FLARE compares, fp32 ``[B, d]``), the head itself not run."""
         cd = self.compute_dtype
         slots = {"x": x.to(cd)}
         if x.dim() == 4 and x.is_cuda:
             slots["x"] = slots["x"].contiguous(memory_format=torch.channels_last)
-        for nd in self.layout.nodes:
+        head = head_index(self.layout) if tap else -1
+        for i, nd in enumerate(self.layout.nodes):
             a = nd.attrs
             t = slots[nd.inp]
+            if i == head:
+                return t.float()
             if nd.op == "conv":
                 b = self.P(nd.name + ".bias").to(cd) if a.get("bias", True) else None
                 t = F.conv2d(t, self.P(nd.name + ".weight").to(cd), b, stride=a.get("stride", 1), padding=a.get("pad", 0))

@@ -341,10 +341,13 @@ class NativeNet:
         self.logits[:B].copy_(out)
         return self.logits[:B]
 
-    def forward_raw(self, x_nhwc, train: bool):
+    def forward_raw(self, x_nhwc, train: bool, tap: bool = False):
         """Forward pass; returns the head's output [B,classes] in the activation dtype, in place in its activation buffer (the
         training step hands it straight to the loss kernel -- no fp32 staging copy).  ``x_nhwc``: [B,H,W,C], or the first layer's
-        im2col matrix [B*Ho*Wo, 64] when ``stem_geometry()`` is not None (batch = rows / (Ho*Wo))."""
+        im2col matrix [B*Ho*Wo, 64] when ``stem_geometry()`` is not None (batch = rows / (Ho*Wo)).  ``tap``: stop before the head
+        (the last plan op, a linear layer) and return its input [B, d], the activation buffer of ``plan[-1].x``."""
+        if tap and self.plan[-1].kind != "linear":
+            raise ValueError("the feature tap needs a plan that ends in a linear head")
         B = x_nhwc.shape[0] if x_nhwc.dim() == 4 else x_nhwc.shape[0] // (self.plan[0].out_shape[0] * self.plan[0].out_shape[1])
         self._x, self._B, self._train = x_nhwc, B, train
         self._epoch = getattr(self, "_epoch", 0) + 1     # forward-pass id: lets stride-2 convs share their parity-split input copy
@@ -354,6 +357,8 @@ class NativeNet:
         if branch and getattr(self, "_branch_stream", None) is None:
             self._branch_stream = torch.cuda.Stream(self.device)
         for i, op in enumerate(self.plan):
+            if tap and i == len(self.plan) - 1:
+                return self.T(op.x, B).reshape(B, -1)
             if branch and op.saved.get("fork_before"):
                 self._branch_stream.wait_stream(torch.cuda.current_stream(self.device))      # the block input is final
             if branch and op.saved.get("join_before"):
@@ -757,3 +762,25 @@ class NativeTrainer:
             x = x_nchw.permute(0, 2, 3, 1).to(ACT).contiguous()
             return net.forward(x, False).clone()
         return fwd
+
+    @torch.no_grad()
+    def root_features(self, w, x):
+        """FLARE's features of parameters ``w`` on the normalised NCHW batch ``x``: the fp32 ``[B, d]`` input of the head in eval mode
+        (``w``'s own BatchNorm running statistics, no dropout), bf16 activations widened to fp32.  One feature executor per trainer:
+        ``w`` is copied into its fixed fp32 parameter buffer and bf16 shadow, so switching between slots rebuilds nothing and leaves the
+        executor ``eval_forward`` keeps alone.  ``--bs`` rows at a time."""
+        if getattr(self, "_feat", None) is None:
+            n = self.layout.n_total
+            net = NativeNet(self.layout, self.device, self.bs, self.net.impl, seed=self.args.seed)
+            fw = torch.zeros(n, dtype=torch.float32, device=self.device)
+            fwb = torch.zeros(n, dtype=ACT, device=self.device)
+            net.bind(fw, fwb, None)
+            self._feat = (net, fw, fwb)
+        net, fw, fwb = self._feat
+        fw.copy_(w)
+        fwb.copy_(w)
+        out = []
+        for s in range(0, x.shape[0], self.bs):
+            xb = x[s:s + self.bs].permute(0, 2, 3, 1).to(ACT).contiguous()
+            out.append(net.forward_raw(xb, False, tap=True).to(torch.float32, copy=True))
+        return torch.cat(out)

@@ -1361,6 +1361,132 @@ def sparsefed_k(p: float, n_params: int) -> int:
     return k
 
 
+# =====================================================================================================================
+# FLARE (Wang, Xiao, Chen, Hu, Lou, Hou, ASIA CCS 2022): trust from the MMD between the candidates' root-set representations
+# =====================================================================================================================
+class FlareResult(NamedTuple):
+    weights: np.ndarray        # float64 [K]: TS_j for the members of F, 0 for every other candidate
+    members: list              # F: the positions of the candidates whose features are all finite (ascending)
+    sigma2: float | None       # the pooled bandwidth sigma^2 (None when F pools fewer than two feature rows)
+    M: np.ndarray | None       # float64 [|F|][|F|] MMD matrix over F (None when no MMD pass ran)
+    counts: np.ndarray | None  # int64 [|F|] neighbour counts c_j (None when no MMD pass ran)
+
+
+def flare_sigma2(Z, members):
+    """FLARE's bandwidth (DESIGN.md section 3, step 4) in fp64 over the pooled feature rows of the candidates ``members``:
+    ``sigma^2 = (2N sum ||z||^2 - 2 ||sum z||^2) / (N (N - 1))``, the mean squared distance over distinct pooled pairs, N = |members| n.
+    None when N < 2."""
+    K, n, d = Z.shape
+    N = len(members) * n
+    if N < 2:
+        return None
+    X = Z[torch.as_tensor(members, dtype=torch.int64, device=Z.device)].reshape(N, d).double()
+    s1 = float((X * X).sum())
+    v = X.sum(0)
+    s2 = float((v * v).sum())
+    return (2.0 * N * s1 - 2.0 * s2) / (N * (N - 1.0))
+
+
+def flare_sums_statement(Z, finite, sigma2):
+    """fp64 statement of the MMD pass: ``S[i][j] = sum_{a in Z_i, b in Z_j} exp(-||a - b||^2 / sigma^2)`` (float64 numpy ``[K][K]``,
+    symmetric) between the finite candidates (``finite[k]``), 0 wherever a non-finite candidate takes part.  Distances are taken from
+    direct differences in fp64."""
+    K, n, d = Z.shape
+    fin = [k for k in range(K) if bool(finite[k])]
+    S = np.zeros((K, K), dtype=np.float64)
+    if not fin:
+        return S
+    X = Z.double()
+    for a, i in enumerate(fin):
+        for j in fin[a:]:
+            D = torch.cdist(X[i], X[j], compute_mode="donot_use_mm_for_euclid_dist") ** 2
+            S[i, j] = S[j, i] = float(torch.exp(-D / float(sigma2)).sum())
+    return S
+
+
+def flare_sums(Z, finite, sigma2):
+    """The MMD pass: ``flare_sums_statement``'s matrix.  On CUDA one launch of ``flare_mmd_kernel`` (ops/csrc/flare.cu) covers every pair
+    (i <= j): fp32 distances from direct differences, expf, fp64 sums added in a fixed order (bitwise reproducible); on CPU it evaluates
+    the statement."""
+    K = Z.shape[0]
+    if not Z.is_cuda:
+        return flare_sums_statement(Z, finite.cpu().tolist(), sigma2)
+    out = torch.empty(K * (K + 1) // 2, dtype=torch.float64, device=Z.device)
+    ext().flare_mmd(Z.contiguous(), finite.to(torch.bool).contiguous(), 1.0 / float(sigma2), out)
+    p = out.cpu().numpy()
+    S = np.zeros((K, K), dtype=np.float64)
+    iu = np.triu_indices(K)                                 # row by row: (0, 0), (0, 1), ..., (1, 1), ... as the kernel numbers its pairs
+    S[iu] = p
+    S.T[iu] = p
+    return S
+
+
+def flare_mmd_matrix(S, members, n: int):
+    """FLARE's biased MMD estimates over the candidates ``members`` from the kernel sums ``S`` (``[K][K]``):
+    ``M_ij = max(0, S_ii/n^2 + S_jj/n^2 - 2 S_ij/n^2)``, float64 numpy ``[|members|][|members|]``, symmetric with a zero diagonal."""
+    idx = np.asarray(members, dtype=np.int64)
+    s = np.asarray(S, dtype=np.float64)[np.ix_(idx, idx)]
+    nn = float(n) * float(n)
+    diag = np.diag(s) / nn
+    return np.maximum(0.0, (diag[:, None] + diag[None, :]) - 2.0 * s / nn)
+
+
+def flare_weights(M, ids, k=None, tau: float = 1.0):
+    """FLARE's host half (DESIGN.md section 3, steps 6 and 7) in fp64, over the members of F listed by their positions ``ids``
+    (ascending) with their MMD matrix ``M``.  ``k`` (default ``floor(|F|/2)``) is capped at ``|F| - 1``; ``NN(i)`` = the ``k`` other
+    members with the smallest ``M_ij``, ties to the lower position; ``c_j`` counts the members whose neighbour lists hold j; ``TS_j =
+    exp((c_j - max c)/tau) / sum_l exp((c_l - max c)/tau)``, the denominator added in position order.  Returns ``(TS float64 [|F|],
+    c int64 [|F|])``."""
+    M = np.asarray(M, dtype=np.float64)
+    ids = np.asarray(ids, dtype=np.int64)
+    F = len(ids)
+    if F == 0:
+        return np.zeros(0, dtype=np.float64), np.zeros(0, dtype=np.int64)
+    k = F // 2 if k is None else int(k)
+    k = max(0, min(k, F - 1))
+    counts = np.zeros(F, dtype=np.int64)
+    for i in range(F):
+        others = np.asarray([j for j in range(F) if j != i], dtype=np.int64)
+        if k and others.size:
+            order = others[np.lexsort((ids[others], M[i, others]))]     # by M_ij, then by position
+            counts[order[:k]] += 1
+    e = np.exp((counts - counts.max()).astype(np.float64) / float(tau))
+    tot = 0.0
+    for v in e:
+        tot += float(v)
+    return e / tot, counts
+
+
+def flare(Z, k=None, tau: float = 1.0, sums=None):
+    """FLARE's weights (DESIGN.md section 3, steps 3 to 7 and the special cases) from the candidates' features ``Z`` (fp32 ``[K][n][d]``):
+    F = the candidates whose features are all finite; ``|F| = 1``: weight 1, no MMD pass; sigma^2 (``flare_sigma2``) not finite or <= 0:
+    weight 1/|F| each, no MMD pass; else the MMD pass ``sums(Z, finite, sigma^2)`` (default ``flare_sums``: the device kernel on CUDA),
+    ``flare_mmd_matrix`` and ``flare_weights``.  ``|F| = 0`` returns zero weights (the caller runs the nobody-trusted step)."""
+    K, n, d = Z.shape
+    finite = torch.isfinite(Z.reshape(K, -1)).all(1)
+    F = [j for j, f in enumerate(finite.cpu().tolist()) if f]
+    w = np.zeros(K, dtype=np.float64)
+    if not F:
+        return FlareResult(w, F, None, None, None)
+    s2 = flare_sigma2(Z, F)
+    if len(F) == 1:
+        w[F[0]] = 1.0
+        return FlareResult(w, F, s2, None, None)
+    if not (s2 is not None and math.isfinite(s2) and s2 > 0):
+        w[F] = 1.0 / len(F)
+        return FlareResult(w, F, s2, None, None)
+    S = (sums or flare_sums)(Z, finite, s2)
+    M = flare_mmd_matrix(S, F, n)
+    ts, counts = flare_weights(M, F, k, tau)
+    w[F] = ts
+    return FlareResult(w, F, s2, M, counts)
+
+
+def flare_statement(Z, k=None, tau: float = 1.0):
+    """The fp64 statement of FLARE's weights: ``flare`` with the MMD pass evaluated by ``flare_sums_statement`` on any device."""
+    return flare(Z, k, tau, sums=lambda z, fin, s2: flare_sums_statement(z, fin.cpu().tolist(), s2))
+
+
 def boost_statement(slot, w_g, gamma: float, n_vote: int):
     """The boosted update in numpy: ``fp32((double)w_g[c] + (double)gamma * (double)fp32(slot[c] - w_g[c]))`` for ``c < n_vote``,
     each fp64 operation rounded on its own.  Returns a float32 array ``[n_vote]``."""

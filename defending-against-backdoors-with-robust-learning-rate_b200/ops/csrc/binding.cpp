@@ -529,6 +529,19 @@ void sparsefed(at::Tensor w_new, at::Tensor w, c10::optional<at::Tensor> w_bf16,
                                 n_vote, w.numel(), k, stats.data_ptr<double>(), num_sms(), cur_stream()), "sparsefed");
 }
 
+void flare_mmd(at::Tensor z, at::Tensor finite, double inv_s2, at::Tensor out) {
+    CHECK_CUDA(z); CHECK_CUDA(finite); CHECK_CUDA(out);
+    TORCH_CHECK(z.scalar_type() == at::kFloat && z.dim() == 3 && z.is_contiguous(), "flare_mmd: contiguous fp32 features [K][n][d]");
+    const int64_t K = z.size(0);
+    TORCH_CHECK(finite.scalar_type() == at::kBool && finite.numel() == K && finite.is_contiguous(), "flare_mmd: bool finite[K]");
+    TORCH_CHECK(out.scalar_type() == at::kDouble && out.numel() == K * (K + 1) / 2 && out.is_contiguous(), "flare_mmd: fp64 out[K (K + 1) / 2]");
+    TORCH_CHECK(K >= 1 && z.size(1) >= 1 && z.size(2) >= 1 && K < (1LL << 31) && z.size(1) < (1LL << 31) && z.size(2) < (1LL << 31),
+                "flare_mmd: empty or oversized features");
+    c10::cuda::CUDAGuard guard(z.device());
+    check(rlr::launch_flare_mmd(z.data_ptr<float>(), reinterpret_cast<const unsigned char*>(finite.data_ptr()), (int)K, (int)z.size(1),
+                                (int)z.size(2), (float)inv_s2, out.data_ptr<double>(), cur_stream()), "flare_mmd");
+}
+
 void boost_update(at::Tensor slot, at::Tensor w_g, double gamma, int64_t n_vote) {
     CHECK_CUDA(slot); CHECK_CUDA(w_g);
     TORCH_CHECK(slot.scalar_type() == at::kFloat && w_g.scalar_type() == at::kFloat);
@@ -653,6 +666,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("neurotoxin_mask", &neurotoxin_mask);
     m.def("boost_update", &boost_update);
     m.def("sparsefed", &sparsefed);
+    m.def("flare_mmd", &flare_mmd);
     m.def("swap_samples", &swap_samples);
     m.def("pgd_project", &pgd_project, py::arg("w"), py::arg("w0"), py::arg("w_bf16"), py::arg("clip"), py::arg("d_sqnorm"),
           py::arg("n_pgd") = 0, py::arg("mask") = py::none());

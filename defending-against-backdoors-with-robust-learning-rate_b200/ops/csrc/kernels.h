@@ -225,6 +225,13 @@ cudaError_t launch_swap_samples(void* data, long long* targets, const long long*
 cudaError_t launch_sparsefed(const float* w_new, float* w, void* w_bf16, float* e, long long n_vote, long long n, long long k,
                              double* stats, int num_sms, cudaStream_t st);
 
+// ---- FLARE MMD pass (flare.cu) -----------------------------------------------------------------------------------------------------
+// z: [K][n][d] fp32 penultimate-layer features of K candidates on the n root samples; finite[k] = 1 when every feature of candidate k is
+// finite.  out (device fp64 [K (K + 1) / 2], pairs (i <= j) numbered row by row): S_ij = sum_{a, b} expf(-||z_i[a] - z_j[b]||^2 * inv_s2),
+// each distance an fp32 sum of direct differences (a - b)^2 in ascending coordinate order; 0 for a pair with a non-finite candidate.
+// Per-CTA fp64 partials added in tile order: no float atomics, bitwise reproducible.
+cudaError_t launch_flare_mmd(const float* z, const unsigned char* finite, int K, int n, int d, float inv_s2, double* out, cudaStream_t st);
+
 // ---- loss / evaluation -----------------------------------------------------------------------------------
 // logits [B,C] (kind 0 fp32 / 1 bf16); writes dlogits (same kind, scaled by 1/B) and accumulates loss_sum / correct.
 cudaError_t launch_softmax_xent(const void* logits, int kind, const int64_t* labels, void* dlogits, float* loss_sum,

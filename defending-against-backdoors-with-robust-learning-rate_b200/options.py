@@ -14,8 +14,9 @@ import math
 import torch
 
 DATASETS = ("fmnist", "fedemnist", "cifar10")
-AGGREGATORS = ("avg", "comed", "sign", "fltrust", "rfa", "flame", "foolsgold")
-ROOT_SIZE = 100                  # FLTrust root set: the paper's 100 clean samples
+AGGREGATORS = ("avg", "comed", "sign", "fltrust", "rfa", "flame", "foolsgold", "flare")
+ROOT_SIZE = 100                  # FLTrust / FLARE root set: the paper's 100 clean samples
+FLARE_TAU = 1.0                  # FLARE: temperature of the softmax over the neighbour counts
 RFA_ITERS = 3                    # RFA: a few smoothed Weiszfeld passes per round
 RFA_NU = 1e-6                    # RFA smoothing: distances below nu count as nu
 FLAME_LAMBDA = 1e-3              # FLAME noise factor: the paper's value for image classification
@@ -51,7 +52,9 @@ def build_parser() -> argparse.ArgumentParser:
                    help="aggregation rule: avg | comed | sign | fltrust (trust-weighted mean against a server-trained root update) | "
                         "rfa (smoothed geometric median by Weiszfeld passes, Pillutla et al. 2022) | flame (cosine clustering, "
                         "median-norm clipping and adaptive noise, Nguyen et al. 2022) | foolsgold (a weighted mean that "
-                        "down-weights agents whose summed update histories are too similar to another's, Fung et al. 2020)")
+                        "down-weights agents whose summed update histories are too similar to another's, Fung et al. 2020) | flare (a "
+                        "weighted mean that trusts the models whose penultimate-layer representations of a clean root set lie among the "
+                        "others' nearest by MMD, Wang et al. 2022)")
     p.add_argument("--local_ep", type=int, default=2, help="number of local epochs: E")
     p.add_argument("--bs", type=int, default=256, help="local batch size: B")
     p.add_argument("--client_lr", type=float, default=0.1, help="clients' learning rate")
@@ -140,8 +143,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--dnc_frac", type=float, default=None,
                    help=f"--select dnc: filtering fraction c >= 0; each subsample removes floor(c F) participants (default {DNC_FRAC})")
     p.add_argument("--root_size", type=int, default=None,
-                   help=f"--aggr fltrust: clean training samples the server trains its root update on each round (default {ROOT_SIZE}); "
-                        "drawn once from --seed, never a poisoned sample")
+                   help=f"--aggr fltrust / flare: clean training samples the server trains its root update on each round (fltrust) or "
+                        f"runs every submitted model on (flare) (default {ROOT_SIZE}); drawn once from --seed, never a poisoned sample")
     p.add_argument("--rfa_iters", type=int, default=None,
                    help=f"--aggr rfa: smoothed Weiszfeld passes per round (default {RFA_ITERS}; 0 = the avg step).  Each pass reweights "
                         "every participant by its data size over its distance to the current weighted mean; a fixed count keeps the "
@@ -151,6 +154,11 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--flame_lambda", type=float, default=None,
                    help=f"--aggr flame: noise factor lambda >= 0; the round's Gaussian noise has std lambda * S, S the median update norm "
                         f"the admitted updates are clipped to (default {FLAME_LAMBDA})")
+    p.add_argument("--flare_k", type=int, default=None,
+                   help="--aggr flare: neighbours k >= 1 each candidate votes for (default per round floor(|F|/2), F the candidates "
+                        "with finite features; capped at |F| - 1)")
+    p.add_argument("--flare_tau", type=float, default=None,
+                   help=f"--aggr flare: temperature tau > 0 of the softmax that turns neighbour counts into trust (default {FLARE_TAU})")
     p.add_argument("--detect", type=str, default="none", choices=DETECTORS,
                    help="detection ahead of the --aggr rule: fldetector (Zhang et al. 2022) predicts every agent's update from its last "
                         "one and an L-BFGS Hessian estimate, scores how far each update lies from its prediction, and once the gap "
@@ -244,6 +252,7 @@ def finalize_args(args: argparse.Namespace) -> argparse.Namespace:
         raise ValueError(f"--crop_pad {args.crop_pad} must lie in [0, {side}) for --data {args.data} ({meta.height}x{meta.width} images)")
     _finalize_select(args)
     _finalize_fltrust(args)
+    _finalize_flare(args)
     _finalize_rfa(args)
     _finalize_flame(args)
     _finalize_attack(args)
@@ -417,19 +426,36 @@ def _finalize_rfa(args) -> None:
 
 
 def _finalize_fltrust(args) -> None:
-    """Validate the FLTrust flags and resolve ``root_size`` in place (``ROOT_SIZE`` by default under ``--aggr fltrust``)."""
+    """Validate the FLTrust flags and resolve ``root_size`` in place (``ROOT_SIZE`` by default under ``--aggr fltrust`` or ``flare``)."""
     root_size = getattr(args, "root_size", None)
-    if args.aggr != "fltrust":
+    if args.aggr not in ("fltrust", "flare"):
         if root_size is not None:
-            raise ValueError("--root_size needs --aggr fltrust")
+            raise ValueError("--root_size needs --aggr fltrust or flare")
         return
-    if getattr(args, "server_clip", False):
+    if args.aggr == "fltrust" and getattr(args, "server_clip", False):
         raise ValueError("--server_clip does not combine with --aggr fltrust, which rescales every update to the root update's norm")
     if root_size is None:
         root_size = ROOT_SIZE
     if root_size < 1:
         raise ValueError(f"--root_size {root_size} must be >= 1")
     args.root_size = int(root_size)
+
+
+def _finalize_flare(args) -> None:
+    """Validate the FLARE flags and resolve ``flare_tau`` in place (``FLARE_TAU`` by default under ``--aggr flare``); ``flare_k`` stays None
+    for the per-round default."""
+    k, tau = getattr(args, "flare_k", None), getattr(args, "flare_tau", None)
+    if args.aggr != "flare":
+        if k is not None or tau is not None:
+            raise ValueError("--flare_k / --flare_tau need --aggr flare")
+        return
+    if k is not None and (int(k) != k or k < 1):
+        raise ValueError(f"--flare_k {k} must be an integer >= 1")
+    tau = FLARE_TAU if tau is None else tau
+    if not (math.isfinite(tau) and tau > 0):
+        raise ValueError(f"--flare_tau {tau} must be a finite number > 0")
+    args.flare_k = None if k is None else int(k)
+    args.flare_tau = float(tau)
 
 
 def dnc_fewest(args) -> int:
@@ -548,6 +574,8 @@ def print_exp_details(args, n_params: int | None = None) -> None:
         print(f"    Selection DnC (F / c / b / T): {args.select_f} / {args.dnc_frac} / {args.dnc_dim} / {args.dnc_iters}")
     if args.aggr == "fltrust":
         print(f"    Root set: {args.root_size}")
+    if args.aggr == "flare":
+        print(f"    FLARE (root / k / tau): {args.root_size} / {'floor(|F|/2)' if args.flare_k is None else args.flare_k} / {args.flare_tau}")
     if args.aggr == "rfa":
         print(f"    RFA passes / nu: {args.rfa_iters} / {args.rfa_nu}")
     if args.aggr == "flame":

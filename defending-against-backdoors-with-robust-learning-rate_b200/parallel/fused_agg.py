@@ -386,6 +386,17 @@ class FusedAggregator:
             dev2 = ops.collude_write(hon, cor, outs, self.w_global, self.n_vote, mode, direction, z, gamma)
         return {"gamma": gamma, "deviation": math.sqrt(max(0.0, float(dev2.reshape(-1)[0])))}
 
+    def flare_features(self, n_part: int, local):
+        """FLARE's features of the round's ``n_part`` participants, fp32 ``[n_part][n][d]`` ordered by participant position and identical
+        on every rank.  ``local``: this rank's ``[max_slots][n][d]`` block, row s holding the features of the participant in its slot s
+        (``slot_owner``).  With several ranks, on every transport (fused, gather and reduce alike), the blocks are all-gathered
+        (``ctx.all_gather``) and reordered, so every rank runs the MMD pass on the same bytes; with one process the block is the result."""
+        ctx = self.ctx
+        if not ctx.is_dist:
+            return local[:n_part]
+        allp = ctx.all_gather(local)                                     # [world, max_slots, n, d]
+        return torch.stack([allp[r, s] for r, s in map(self.slot_owner, range(n_part))])
+
     def pairwise_gram(self, n_part: int, members=None, participants=None):
         """FLAME Gram pass (``ops.gram_statement``): the float64 Gram matrix of the updates ``w_j - w_global`` of the participants at
         positions ``members`` (ascending; every one of the round's ``n_part`` when None) over ``[0, n_vote)``, identical on every rank.

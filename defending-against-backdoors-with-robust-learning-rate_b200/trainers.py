@@ -151,6 +151,18 @@ class TorchTrainer:
         net.eval()
         return lambda x: net(x)
 
+    @torch.no_grad()
+    def root_features(self, w, x):
+        """FLARE's features of parameters ``w`` on the normalised NCHW batch ``x``: the fp32 ``[B, d]`` input of the head in eval mode
+        (``w``'s own BatchNorm running statistics, no dropout), through one feature ``GraphNet`` per trainer rebound to ``w``, ``--bs``
+        rows at a time."""
+        if getattr(self, "_feat_net", None) is None:
+            self._feat_net = GraphNet(self.layout, w, None, self.compute_dtype)
+            self._feat_net.eval()
+        else:
+            self._feat_net.bind(w, None)
+        return torch.cat([self._feat_net(x[s:s + self.bs], tap=True) for s in range(0, x.shape[0], self.bs)])
+
 
 def make_trainer(kind, layout, args, device, max_shard):
     dev = torch.device(device)

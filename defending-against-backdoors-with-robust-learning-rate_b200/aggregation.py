@@ -16,6 +16,9 @@ the Gram matrix of those histories (``ops.history_gram``), so agents that keep p
 ``--aggr flare`` weights that launch by FLARE's trust: the MMD between the participants' penultimate-layer representations of a clean
 root set (``ops.flare_sums`` on the features the engine computes) and a softmax over how often each is among the others' nearest
 neighbours (``ops.flare_weights``).
+``--aggr deepsight`` runs that launch with equal weights over DeepSight's accepted clusters, clipped to the median norm: the statistics
+of the participants' output layers and of their behaviour on random inputs (``ops.deepsight_stats`` on the logits the engine computes)
+label and cluster them (``ops.deepsight_decide``).
 ``--detect fldetector`` is a stage ahead of the rule: every round it predicts each agent's update from its last one and an L-BFGS
 Hessian-vector product of the recent global updates (``ops.fld_hvp_coefficients`` on the Gram matrix of the update ring,
 ``ops.fld_hvp``), scores the distance to the prediction (``ops.fld_predict``) and, once the gap statistic finds a minority cluster of high
@@ -33,7 +36,7 @@ import torch
 import torch.nn.functional as F
 
 from . import ops
-from .models.graph import GraphNet
+from .models.graph import GraphNet, head_slices
 
 
 def server_opt_spec(args):
@@ -67,6 +70,7 @@ class Aggregation:
         self.last_flame = None        # the FLAME/* scalars of the last round (--aggr flame)
         self.last_foolsgold = None    # the FoolsGold/* scalars of the last round (--aggr foolsgold)
         self.last_flare = None        # the FLARE/* scalars of the last round (--aggr flare)
+        self.last_deepsight = None    # the DeepSight/* scalars of the last round (--aggr deepsight)
         self.history = None           # [num_agents][n_vote] FoolsGold histories of the in-process form (allocated on first use)
         self.opt = None               # full-length server optimizer state of the in-process form (allocated on first use)
         # FLDetector (--detect fldetector): host state identical on every rank, and the in-process form's tables (allocated on first use)
@@ -82,10 +86,12 @@ class Aggregation:
         self.last_sparse = None
 
     # ---- the server step ------------------------------------------------------------------------------------
-    def aggregate_updates(self, w_global, agent_params, cur_round, n_vote=None, root_params=None, features=None):
+    def aggregate_updates(self, w_global, agent_params, cur_round, n_vote=None, root_params=None, features=None, logits=None,
+                          global_logits=None):
         """In-process form: ``agent_params`` = {agent_id: flat local parameters}.  Updates ``w_global`` in place.  ``root_params``:
         the server's root-trained parameters, needed by ``--aggr fltrust``; ``features``: fp32 ``[K][n][d]`` root-set features of the
-        participants in ``agent_params``' order, needed by ``--aggr flare``."""
+        participants in ``agent_params``' order, needed by ``--aggr flare``; ``logits`` / ``global_logits``: fp32 ``[K][S N][P]`` logits
+        of those participants and ``[S N][P]`` of ``w_global`` on DeepSight's random inputs, needed by ``--aggr deepsight``."""
         ids = list(agent_params.keys())
         ws = [agent_params[i] for i in ids]
         nv = n_vote if n_vote is not None else (self.layout.n_vote if self.layout else None)
@@ -93,6 +99,8 @@ class Aggregation:
             raise ValueError("--aggr fltrust needs the server's root parameters (root_params)")
         if self._flare and features is None:
             raise ValueError("--aggr flare needs the participants' root-set features (features)")
+        if self._deepsight and (logits is None or global_logits is None):
+            raise ValueError("--aggr deepsight needs the participants' and the global model's logits (logits, global_logits)")
         clip = self._clip_scales(ops.update_norms(w_global, ws, nv)) if self._server_clip else None
         all_ids, all_ws = ids, ws
         n_voted = nv if nv is not None else w_global.numel()
@@ -106,7 +114,10 @@ class Aggregation:
         keep, weights, scales, total, noise_std = self._admission(ids, clip, detection, distances, dnc,
                                                                   lambda: ops.trust_stats(ws, root_params, w_global, nv), rfa_pass, gram,
                                                                   lambda members: self._history_pass(w_global, ws, ids, members, nv),
-                                                                  cur_round, lambda: features)
+                                                                  cur_round, lambda: features,
+                                                                  lambda: (ops.deepsight_stats(logits, global_logits, ws, w_global,
+                                                                                               head_slices(self.layout)),
+                                                                           ops.update_norms(w_global, ws, nv)))
         if keep is not None and len(keep) < len(ids):
             ids, ws, weights = [ids[j] for j in keep], [ws[j] for j in keep], [weights[j] for j in keep]
             scales = scales[torch.as_tensor(keep, device=scales.device)] if scales is not None else None
@@ -134,10 +145,12 @@ class Aggregation:
             self.plot_sign_agreement(prev, w_global, ws, ids, cur_round)     # the vote that happened: admitted participants only
         return
 
-    def aggregate_slots(self, participants, cur_round, flare_local=None):
+    def aggregate_slots(self, participants, cur_round, flare_local=None, deepsight_local=None):
         """Engine form: participant j's parameters live in ``fused.slot_owner(j)``; updates every rank's global.  Under
         ``--aggr fltrust`` the server's root job is position ``len(participants)``.  ``flare_local``: under ``--aggr flare``, this rank's
-        ``[max_slots][n][d]`` root-set features of the participants in its slots (``FusedAggregator.flare_features``)."""
+        ``[max_slots][n][d]`` root-set features of the participants in its slots (``FusedAggregator.flare_features``).
+        ``deepsight_local``: under ``--aggr deepsight``, this rank's ``[max_slots][(S + 2) P]`` DeepSight statistics of the participants
+        in its slots (``ops.deepsight_stats``), all-gathered the same way."""
         K = len(participants)
         diag = bool(self.args.diagnostics)
         norms = self.fused.update_norms(K) if self._server_clip or diag else None
@@ -158,7 +171,8 @@ class Aggregation:
             lambda b, members: self.fused.rfa_sqdist(K, b, clip, members, copies),
             lambda members: self.fused.pairwise_gram(K, members, copies),
             lambda members: self.fused.foolsgold_gram(K, participants, members, copies), cur_round,
-            lambda: self.fused.flare_features(K, flare_local))
+            lambda: self.fused.flare_features(K, flare_local),
+            lambda: (self.fused.gather_slot_rows(K, deepsight_local), norms if norms is not None else self.fused.update_norms(K)))
         if diag:   # the sign-agreement analysis needs the pre-step global parameters and every admitted participant's parameters
             prev = self.fused.w_global.clone()
             ws = [w.clone() for w in self.fused.gather_participants(K)]
@@ -180,14 +194,16 @@ class Aggregation:
     def _select(self):
         return getattr(self.args, "select", "none") != "none"
 
-    def _admission(self, ids, clip, detection, distances, dnc_grams, trust_stats, rfa_pass, gram, history, cur_round, features=None):
+    def _admission(self, ids, clip, detection, distances, dnc_grams, trust_stats, rfa_pass, gram, history, cur_round, features=None,
+                   deepsight=None):
         """Admission of the participants ``ids`` shared by both forms of the step: FLDetector's ``detection()`` (``--detect``), which returns
         the positions of the agents it has not flagged (None while it has flagged nobody), or Krum / Multi-Krum on ``distances()`` or DnC
         on its Gram matrices ``dnc_grams()`` (``--select``),
         then FLTrust on ``trust_stats()`` (``--aggr fltrust``), RFA's weights from ``rfa_pass(b, members)`` (``--aggr rfa``), FLAME on
         the Gram matrix ``gram(members)`` (``--aggr flame``) or FoolsGold on ``history(members)``, the Gram matrix of the members' update
         histories after this round's updates are folded in (``--aggr foolsgold``), or FLARE on the participants' root-set features
-        ``features()`` (``--aggr flare``).  ``clip``: the server-clipping scales or None.  Returns
+        ``features()`` (``--aggr flare``), or DeepSight on ``deepsight()``, the participants' statistics and update norms (``--aggr
+        deepsight``).  ``clip``: the server-clipping scales or None.  Returns
         ``(members, weights, scales, total_weight, noise_std)`` for the step: members None admits everyone; weights are per position in
         ``ids``."""
         keep = self._admit(ids, cur_round, distances, dnc_grams) if self._select else (detection() if self._detect else None)
@@ -199,6 +215,8 @@ class Aggregation:
         if self._flare:
             members, weights, total = self._flare_step(ids, keep, features, cur_round)
             return members, weights, clip, total, noise_std
+        if self._deepsight:
+            return (*self._deepsight_step(ids, keep, deepsight, cur_round), noise_std)
         weights = [float(self.agent_data_sizes[i]) for i in ids]
         if self._foolsgold:
             members, weights, total = self._foolsgold_step(ids, keep, weights, history, cur_round)
@@ -355,11 +373,15 @@ class Aggregation:
         return self.args.aggr == "flare"
 
     @property
+    def _deepsight(self):
+        return self.args.aggr == "deepsight"
+
+    @property
     def _mode(self):
         """The aggregate kernel's rule: FLTrust is its weighted mean with trust weights and per-participant scales, RFA with its
         Weiszfeld weights, FLAME with equal weights and its clip scales, FoolsGold with its weights times the data sizes, FLARE with its
-        trust scores."""
-        return "avg" if self._fltrust or self._rfa or self._flame or self._foolsgold or self._flare else self.args.aggr
+        trust scores, DeepSight with equal weights and its clip scales."""
+        return "avg" if self._fltrust or self._rfa or self._flame or self._foolsgold or self._flare or self._deepsight else self.args.aggr
 
     def _history_pass(self, w_global, ws, ids, members, nv):
         """In-process form of the FoolsGold history pass: fold the updates of the participants at positions ``members`` into the rows of
@@ -433,6 +455,39 @@ class Aggregation:
                 if v is not None:
                     self.writer.add_scalar(k, v, cur_round)
         return members, w, total
+
+    def _deepsight_step(self, ids, keep, deepsight, cur_round):
+        """DeepSight over the positions ``keep`` that selection or detection admitted (all when None): ``ops.deepsight_decide`` on the
+        candidates' rows of ``deepsight()`` = (statistics ``[K][(S + 2) P]``, update norms ``[K]``), identical on every rank.  Returns
+        ``(members, weights, scales, total_weight)`` for the step: the accepted positions with weight 1 each, total weight their count
+        and the clip scales -- or, when nobody is accepted, every candidate with weight 0 and total weight 1, so the aggregate is 0 plus
+        noise.  Records ``last_admitted`` and logs the accepted and suspicious counts, the corrupt ones among them (ids < num_corrupt),
+        the number of final clusters over the finite candidates and the clip bound."""
+        K = len(ids)
+        cand = list(range(K)) if keep is None else [int(j) for j in keep]
+        stats, norms = deepsight()
+        idx = torch.as_tensor(cand, dtype=torch.int64)
+        res = ops.deepsight_decide(stats.detach().cpu()[idx], norms.detach().double().cpu()[idx], [ids[j] for j in cand],
+                                   self.args.deepsight_tau)
+        members = [cand[j] for j in res.members]
+        scales = torch.ones(K, dtype=torch.float32)
+        scales[idx] = res.scales
+        weights, total = [1.0] * K, float(len(members))
+        self.last_admitted = [ids[j] for j in members]
+        if not members:
+            members, weights, total = cand, [0.0] * K, 1.0
+        nc = self.args.num_corrupt
+        sus = [ids[cand[j]] for j in range(len(cand)) if res.suspicious[j]]
+        self.last_deepsight = {"DeepSight/Accepted": len(self.last_admitted),
+                               "DeepSight/Corrupt_Accepted": sum(1 for i in self.last_admitted if i < nc),
+                               "DeepSight/Suspicious": len(sus), "DeepSight/Corrupt_Suspicious": sum(1 for i in sus if i < nc),
+                               "DeepSight/Clusters": len({int(v) for v in res.labels if v >= 0}),
+                               "DeepSight/Clip_Bound": res.clip_bound}
+        if self.writer is not None:
+            for k, v in self.last_deepsight.items():
+                if v is not None:
+                    self.writer.add_scalar(k, v, cur_round)
+        return members, weights, scales, total
 
     def _flame_step(self, ids, keep, gram, cur_round):
         """FLAME over the positions ``keep`` that selection admitted (all when None): ``ops.flame_admit`` on ``gram(candidates)``.

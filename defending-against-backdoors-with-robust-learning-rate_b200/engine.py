@@ -29,7 +29,7 @@ from .aggregation import Aggregation, server_opt_spec
 from .data import distribute_data, get_datasets, make_poisoned_val
 from .data.datasets import DeviceDataset, h5_to_device_dataset, load_fedemnist_client
 from .models import get_layout
-from .models.graph import feature_dim
+from .models.graph import feature_dim, head_slices
 from .options import attack_schedule_set, is_attack_round, last_attack_round, print_exp_details
 from .parallel import FusedAggregator, init_distributed
 from .trainers import make_trainer
@@ -155,6 +155,13 @@ class FLEngine:
             root = draw_root_set(len(self.train_dataset), poisoned, args.root_size, args.seed)
             self.flare_x, _ = self.train_dataset.batch(torch.as_tensor(root, device=dev))
             self.flare_local = torch.zeros((max_slots, len(root), feature_dim(self.layout)), dtype=torch.float32, device=dev)
+        # ---- DeepSight: its random inputs (S seeds of --deepsight_samples images, drawn once from --seed) and this rank's
+        # [max_slots][(S + 2) P] block of its participants' statistics.  A head without a bias is refused here.
+        self.ds_x = self.ds_local = None
+        if args.aggr == "deepsight":
+            self.ds_head = head_slices(self.layout)
+            self.ds_x = ops.deepsight_inputs(self.train_dataset.meta, args.seed, args.deepsight_samples, dev)
+            self.ds_local = torch.zeros((max_slots, (ops.DEEPSIGHT_SEEDS + 2) * self.ds_head[2]), dtype=torch.float64, device=dev)
 
         self.trainer = make_trainer(args.trainer, self.layout, args, dev, max_shard)
         # Several agents per GPU and round can be trained concurrently: trainer i (own parameters, activations, CUDA graphs) runs
@@ -400,6 +407,8 @@ class FLEngine:
         self.last_collude = self._collude(chosen, rnd) if (attack and self.collude != "none") else None
         if self.flare_x is not None:
             self.aggregator.aggregate_slots(chosen, rnd, flare_local=self._flare_features(chosen))
+        elif self.ds_x is not None:
+            self.aggregator.aggregate_slots(chosen, rnd, deepsight_local=self._deepsight_stats(chosen))
         else:
             self.aggregator.aggregate_slots(chosen, rnd)
         self.timer.stop("aggregate")
@@ -414,6 +423,19 @@ class FLEngine:
             if r == self.ctx.rank:
                 self.flare_local[s].copy_(self.trainer.root_features(fused.slots[s], self.flare_x))
         return self.flare_local
+
+    def _deepsight_stats(self, chosen):
+        """DeepSight: the statistics of the participants this rank owns (``slot_owner``), from their final slots (after boosting and
+        collusion) and the global model's logits on the random inputs, into ``ds_local``; on the main stream, after the trainer streams
+        have joined.  One statistics pass covers every owned slot."""
+        fused = self.fused
+        owned = [s for r, s in map(fused.slot_owner, range(len(chosen))) if r == self.ctx.rank]
+        if owned:
+            zg = self.trainer.root_features(self.w_global, self.ds_x, tap=False)
+            z = torch.stack([self.trainer.root_features(fused.slots[s], self.ds_x, tap=False) for s in owned])
+            st = ops.deepsight_stats(z, zg, [fused.slots[s] for s in owned], self.w_global, self.ds_head)
+            self.ds_local[torch.as_tensor(owned, dtype=torch.int64, device=self.ds_local.device)] = st.to(self.ds_local.device)
+        return self.ds_local
 
     def _neurotoxin_mask(self, attack: bool = True):
         """Start of a round with Neurotoxin on: the mask of the last global update ``w_global - w_prev`` (the top-k coordinates by
@@ -574,6 +596,10 @@ class FLEngine:
                 for key, tag in (("flare_avg_honest", "Avg_Honest_Trust"), ("flare_avg_corrupt", "Avg_Corrupt_Trust"),
                                  ("flare_corrupt_weight", "Corrupt_Weight"), ("flare_bandwidth", "Bandwidth")):
                     rec[key] = self.aggregator.last_flare[f"FLARE/{tag}"]
+            if self.aggregator.last_deepsight is not None:
+                for key in ("accepted", "corrupt_accepted", "suspicious", "corrupt_suspicious", "clusters", "clip_bound"):
+                    tag = "_".join(w.capitalize() for w in key.split("_"))
+                    rec[f"deepsight_{key}"] = self.aggregator.last_deepsight[f"DeepSight/{tag}"]
             if self.aggregator.last_foolsgold is not None:
                 rec["foolsgold_avg_honest"] = self.aggregator.last_foolsgold["FoolsGold/Avg_Honest_Weight"]
                 rec["foolsgold_avg_corrupt"] = self.aggregator.last_foolsgold["FoolsGold/Avg_Corrupt_Weight"]

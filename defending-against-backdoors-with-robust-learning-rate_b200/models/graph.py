@@ -197,6 +197,16 @@ def feature_dim(layout) -> int:
     return int(layout.nodes[head_index(layout)].attrs["cin"])
 
 
+def head_slices(layout):
+    """``(w_off, b_off, P, d)`` of the model's head (the last ``linear`` node): its weight ``[P][d]`` and bias ``[P]`` in the flat vector.
+    DeepSight reads both, so a head without a bias is refused."""
+    nd = layout.nodes[head_index(layout)]
+    if nd.name + ".bias" not in layout.by_name:
+        raise ValueError(f"--aggr deepsight needs a head with a bias; {nd.name} has none")
+    a = nd.attrs
+    return layout.by_name[nd.name + ".weight"].offset, layout.by_name[nd.name + ".bias"].offset, int(a["cout"]), int(a["cin"])
+
+
 class GraphNet(nn.Module):
     """PyTorch interpreter of the IR; parameters/buffers are views into the flat buffers ``w`` (and ``g``)."""
 

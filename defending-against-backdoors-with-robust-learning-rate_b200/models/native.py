@@ -764,9 +764,10 @@ class NativeTrainer:
         return fwd
 
     @torch.no_grad()
-    def root_features(self, w, x):
+    def root_features(self, w, x, tap: bool = True):
         """FLARE's features of parameters ``w`` on the normalised NCHW batch ``x``: the fp32 ``[B, d]`` input of the head in eval mode
-        (``w``'s own BatchNorm running statistics, no dropout), bf16 activations widened to fp32.  One feature executor per trainer:
+        (``w``'s own BatchNorm running statistics, no dropout), bf16 activations widened to fp32; ``tap=False``: the head's output, the
+        fp32 ``[B, classes]`` logits (DeepSight's random-input behaviour).  One feature executor per trainer:
         ``w`` is copied into its fixed fp32 parameter buffer and bf16 shadow, so switching between slots rebuilds nothing and leaves the
         executor ``eval_forward`` keeps alone.  ``--bs`` rows at a time."""
         if getattr(self, "_feat", None) is None:
@@ -782,5 +783,5 @@ class NativeTrainer:
         out = []
         for s in range(0, x.shape[0], self.bs):
             xb = x[s:s + self.bs].permute(0, 2, 3, 1).to(ACT).contiguous()
-            out.append(net.forward_raw(xb, False, tap=True).to(torch.float32, copy=True))
+            out.append(net.forward_raw(xb, False, tap=tap).to(torch.float32, copy=True))
         return torch.cat(out)

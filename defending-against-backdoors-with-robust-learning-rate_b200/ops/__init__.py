@@ -1487,6 +1487,296 @@ def flare_statement(Z, k=None, tau: float = 1.0):
     return flare(Z, k, tau, sums=lambda z, fin, s2: flare_sums_statement(z, fin.cpu().tolist(), s2))
 
 
+# =====================================================================================================================
+# DeepSight (Rieger, Nguyen, Miettinen, Sadeghi, NDSS 2022): output-layer energy, random-input behaviour and per-cluster acceptance
+# =====================================================================================================================
+DEEPSIGHT_SEEDS = 3              # S: seeds of random inputs, one DDif clustering each
+
+
+def deepsight_inputs(meta, seed: int, n: int, device, seeds: int = DEEPSIGHT_SEEDS):
+    """DeepSight's random inputs: ``seeds`` blocks of ``n`` images of the dataset's shape, normalised NCHW fp32 ``[seeds n][C][H][W]``.
+    Block s holds uniform uint8 pixels (uniform floats in [0, 1) when the dataset stores floats), drawn on the host from a generator
+    seeded by ``(seed, s)`` alone -- identical on every rank, in every round and after a resume -- and normalised by the dataset's mean and
+    std through ``gather_normalize``, like real images (no augmentation)."""
+    raw = []
+    for s in range(seeds):
+        gen = torch.Generator().manual_seed((int(seed) * 1000003 + 7919 * (s + 1)) & 0x7FFFFFFFFFFFFFFF)
+        shape = (int(n), meta.height, meta.width, meta.channels)
+        raw.append(torch.rand(shape, generator=gen) if meta.is_float else torch.randint(0, 256, shape, generator=gen, dtype=torch.uint8))
+    data = torch.cat(raw).to(device)
+    return gather_normalize(data, torch.arange(data.shape[0], dtype=torch.int64, device=data.device), meta.mean, meta.std)
+
+
+def _deepsight_lse(z):
+    """fp64 log-sum-exp of the fp32 logits' last axis: ``max + log(sum_c exp(z_c - max))``, the sum over c ascending; NaN for a row with
+    a non-finite logit."""
+    z = np.asarray(z, dtype=np.float64)
+    with np.errstate(all="ignore"):
+        mx = z.max(axis=-1, keepdims=True)
+        lse = mx[..., 0] + np.log(np.cumsum(np.exp(z - mx), axis=-1)[..., -1])
+    return np.where(np.isfinite(z).all(axis=-1), lse, np.nan)
+
+
+def deepsight_stats_statement(logits, g_logits, w_agents, w_global, head, seeds: int = DEEPSIGHT_SEEDS):
+    """fp64 statement of the DeepSight statistics pass (DESIGN.md section 3).  ``logits``: fp32 ``[K][seeds N][P]`` eval-mode logits of the
+    candidates on the random inputs, ``g_logits``: the global model's ``[seeds N][P]``; ``w_agents``: the candidates' flat parameters;
+    ``head``: ``(w_off, b_off, P, d)`` of the last linear layer (``models.graph.head_slices``).  Returns float64 ``[K][(seeds + 2) P]``,
+    per candidate ``DDif [seeds][P]`` (``(1/N) sum_m exp((z_k - lse z_k) - (z_g - lse z_g))``, m ascending), ``eps [P]`` (``|fp32(db_c)|``
+    then ``|fp32(dW_cj)|`` for ascending j, added left to right) and ``db [P]``."""
+    w_off, b_off, P, d = (int(v) for v in head)
+    z = logits.detach().float().cpu().numpy()
+    zg = g_logits.detach().float().cpu().numpy()
+    K, SN, _ = z.shape
+    N = SN // seeds
+    with np.errstate(all="ignore"):
+        a = z.astype(np.float64) - _deepsight_lse(z)[..., None]
+        b = zg.astype(np.float64) - _deepsight_lse(zg)[..., None]
+        terms = np.exp(a - b[None]).reshape(K, seeds, N, P)
+        ddif = np.cumsum(terms, axis=2)[:, :, -1, :] / float(N)
+    wg = w_global.detach().float().cpu().numpy()
+    out = np.empty((K, (seeds + 2) * P), dtype=np.float64)
+    for k, w in enumerate(w_agents):
+        wk = w.detach().float().cpu().numpy()
+        dW = (wk[w_off:w_off + P * d] - wg[w_off:w_off + P * d]).reshape(P, d)          # fp32 differences
+        db = wk[b_off:b_off + P] - wg[b_off:b_off + P]
+        terms = np.abs(np.concatenate([db[:, None], dW], axis=1).astype(np.float64))
+        out[k, :seeds * P] = ddif[k].reshape(-1)
+        out[k, seeds * P:(seeds + 1) * P] = np.cumsum(terms, axis=1)[:, -1]
+        out[k, (seeds + 1) * P:] = db.astype(np.float64)
+    return torch.from_numpy(out)
+
+
+def deepsight_stats(logits, g_logits, w_agents, w_global, head, seeds: int = DEEPSIGHT_SEEDS):
+    """The DeepSight statistics pass: ``deepsight_stats_statement``'s float64 ``[K][(seeds + 2) P]``.  On CUDA one ``deepsight_stats``
+    launch pair (ops/csrc/deepsight.cu): one thread per output adding its terms in the stated order, bitwise reproducible; on CPU the
+    statement."""
+    if not logits.is_cuda:
+        return deepsight_stats_statement(logits, g_logits, w_agents, w_global, head, seeds)
+    w_off, b_off, P, d = (int(v) for v in head)
+    K = logits.shape[0]
+    tab = PtrTable([w.data_ptr() for w in w_agents], logits.device, w_agents)
+    for w in (*w_agents, w_global):
+        assert w.is_cuda and w.dtype == torch.float32 and w.is_contiguous() and w.numel() >= max(w_off + P * d, b_off + P)
+    out = torch.empty((K, (seeds + 2) * P), dtype=torch.float64, device=logits.device)
+    ext().deepsight_stats(logits.float().contiguous(), g_logits.float().contiguous(), tab.tensor, w_global.data_ptr(), w_off, b_off,
+                          int(seeds), d, out)
+    return out
+
+
+def _prim_edges(d):
+    """The ``n - 1`` edges ``(weight, u, v)`` of a minimum spanning tree of the symmetric distances ``d`` by Prim's algorithm (as in
+    ``_first_cluster``).  Every minimum spanning tree has the same components under ``weight <= h`` for each h: those of ``{d <= h}``."""
+    n = d.shape[0]
+    in_tree = np.zeros(n, dtype=bool)
+    in_tree[0] = True
+    best, parent = d[0].copy(), np.zeros(n, dtype=np.int64)
+    edges = []
+    for _ in range(n - 1):
+        out = np.flatnonzero(~in_tree)
+        k = int(out[np.argmin(best[out])])
+        edges.append((float(best[k]), int(parent[k]), k))
+        in_tree[k] = True
+        closer = d[k] < best
+        parent[closer] = k
+        best[closer] = d[k][closer]
+    return edges
+
+
+def _components(points, edges):
+    """Connected components of ``points`` under ``edges`` (``(w, u, v)``), each a sorted list, ordered by their smallest point."""
+    root = {p: p for p in points}
+
+    def find(x):
+        while root[x] != x:
+            root[x] = root[root[x]]
+            x = root[x]
+        return x
+    for _, u, v in edges:
+        a, b = find(u), find(v)
+        if a != b:
+            root[max(a, b)] = min(a, b)
+    comp = {}
+    for p in sorted(points):
+        comp.setdefault(find(p), []).append(p)
+    return sorted(comp.values(), key=lambda c: c[0])
+
+
+def hdbscan_labels(D, min_cluster_size: int):
+    """HDBSCAN labels of the symmetric distances ``D`` (float64 ``[n][n]``, finite): scikit-learn's ``HDBSCAN(metric="precomputed",
+    min_samples=1, min_cluster_size=m, allow_single_cluster=True)`` with equal distances entering together, so the labels do not depend
+    on the order of the points.  Level by level from the top: at the largest distance h left inside a cluster, the clusters' points
+    split into the connected components of ``{d < h}`` at lambda = 1/h (+inf for h = 0).  Two or more components of at least m points
+    are new clusters born at lambda and the cluster ends; with one, the cluster goes on as it; the points of the smaller components leave
+    at lambda.  The stability of a cluster is ``sum (lambda_leave - lambda_birth)`` over its points (the root is born at 0); excess of
+    mass selects among every cluster, the root included; the points of a selected cluster take its label, and when the root is the one
+    selected, only the points that leave it at its last lambda or later.  Every other point is noise (-1), as is a lone point.  Labels
+    are numbered by their clusters' smallest point.  Returns int64 ``[n]``."""
+    d = np.asarray(D, dtype=np.float64)
+    n = d.shape[0]
+    m = int(min_cluster_size)
+    if m < 2:
+        raise ValueError(f"hdbscan_labels: min_cluster_size {m} must be >= 2")
+    labels = np.full(n, -1, dtype=np.int64)
+    if n < 2:
+        return labels
+    birth, parent, stab, children, death = [0.0], [-1], [0.0], [[]], [0.0]
+    leave = {}                                   # point -> (cluster it leaves, lambda)
+    work = [(0, list(range(n)), _prim_edges(d))]
+    while work:
+        c, pts, edges = work.pop()
+        while True:
+            h = max(e[0] for e in edges)
+            lam = 1.0 / h if h > 0 else math.inf
+            kept = [e for e in edges if e[0] < h]
+            comps = _components(pts, kept)
+            big = [q for q in comps if len(q) >= m]
+            for q in comps:
+                if len(q) < m:
+                    for p in q:
+                        leave[p] = (c, lam)
+                        stab[c] += lam - birth[c]
+            death[c] = lam
+            if len(big) >= 2:
+                for q in big:
+                    stab[c] += (lam - birth[c]) * len(q)
+                    qs = set(q)
+                    cid = len(birth)
+                    birth.append(lam); parent.append(c); stab.append(0.0); children.append([]); death.append(lam)
+                    children[c].append(cid)
+                    work.append((cid, q, [e for e in kept if e[1] in qs]))
+                break
+            if not big:
+                break
+            pts = big[0]
+            qs = set(pts)
+            edges = [e for e in kept if e[1] in qs]
+    n_cl = len(birth)
+    selected = [False] * n_cl
+    value = list(stab)
+    for c in range(n_cl - 1, -1, -1):            # children are numbered after their parents
+        sub = sum(value[ch] for ch in children[c])
+        if sub > value[c]:
+            value[c] = sub
+        else:
+            selected[c] = True
+            todo = list(children[c])
+            while todo:
+                x = todo.pop()
+                selected[x] = False
+                todo.extend(children[x])
+    for p in range(n):
+        c, lam = leave[p]
+        while c != -1 and not selected[c]:
+            c = parent[c]
+        if c > 0 or (c == 0 and lam >= death[0]):
+            labels[p] = c
+    out = np.full(n, -1, dtype=np.int64)
+    names = {}
+    for p in range(n):
+        if labels[p] >= 0:
+            out[p] = names.setdefault(int(labels[p]), len(names))
+    return out
+
+
+def _partition_indicator(labels):
+    """``A[i][j] = 0`` when points i and j share a part of the partition of ``labels`` (every noise point, -1, its own part), 1 else."""
+    lab = np.asarray(labels, dtype=np.int64)
+    same = (lab[:, None] == lab[None, :]) & (lab[:, None] >= 0)
+    A = np.where(same, 0, 1).astype(np.int64)
+    np.fill_diagonal(A, 0)
+    return A
+
+
+def _pair_sum(f, X):
+    """Symmetric float64 ``[n][n]`` of ``sum_c f(x_i, x_j)_c`` for the rows of ``X``, each sum left to right (content-only, so equal rows
+    give equal entries wherever they stand)."""
+    n = X.shape[0]
+    out = np.zeros((n, n), dtype=np.float64)
+    for i in range(n):
+        if i + 1 < n:
+            v = np.cumsum(f(X[i][None, :], X[i + 1:]), axis=1)[:, -1]
+            out[i, i + 1:] = v
+            out[i + 1:, i] = v
+        out[i, i] = np.cumsum(f(X[i], X[i]))[-1] if X.shape[1] else 0.0
+    return out
+
+
+class DeepSightResult(NamedTuple):
+    members: list              # A: the accepted positions (ascending)
+    scales: torch.Tensor       # float32 [K]: s_k = fp32(min(1, S_clip / e_k)) (1 when e_k = 0 or k is not finite)
+    clip_bound: float | None   # S_clip = median over F of e_k (None when F is empty)
+    labels: np.ndarray         # int64 [K]: the final part of each candidate (numbered in agent-id order), -1 outside F
+    suspicious: np.ndarray     # bool [K]: TE_k <= median_F(TE) / 2 (False outside F)
+    te: np.ndarray             # int64 [K]: threshold exceedings (-1 outside F)
+    finite: list               # F: the positions of the finite candidates (ascending)
+
+
+def deepsight_decide(stats, norms, ids, tau: float, seeds: int = DEEPSIGHT_SEEDS):
+    """DeepSight's decision on the host, in fp64 (DESIGN.md section 3), from the candidates' statistics ``stats`` (float64
+    ``[K][(seeds + 2) P]``, ``deepsight_stats_statement``'s layout), their update norms ``norms`` (``[K]``) and agent ids ``ids``.
+    The candidates are taken in agent-id order, so the result does not depend on their positions.  Returns a ``DeepSightResult``."""
+    st = np.asarray(torch.as_tensor(stats).detach().double().cpu().numpy(), dtype=np.float64)
+    e_all = np.asarray(torch.as_tensor(norms).detach().double().cpu().numpy(), dtype=np.float64).reshape(-1)
+    K = st.shape[0]
+    if len(ids) != K or e_all.shape[0] != K:
+        raise ValueError(f"deepsight_decide: statistics of {K} candidates, {e_all.shape[0]} norms and {len(ids)} ids")
+    P = st.shape[1] // (seeds + 2) if K else 0
+    ddif = st[:, :seeds * P].reshape(K, seeds, P)
+    eps = st[:, seeds * P:(seeds + 1) * P]
+    db = st[:, (seeds + 1) * P:]
+    with np.errstate(all="ignore"):
+        e2 = eps * eps
+        tot = np.cumsum(e2, axis=1)[:, -1] if P else np.zeros(K)
+        neup = np.where(tot[:, None] > 0, e2 / np.where(tot > 0, tot, 1.0)[:, None], 0.0)
+        top = neup.max(axis=1) if P else np.zeros(K)
+        te = (neup > max(0.01, 1.0 / max(P, 1)) * top[:, None]).sum(axis=1).astype(np.int64)
+    ok = np.isfinite(st).all(axis=1) & np.isfinite(neup).all(axis=1) & np.isfinite(e_all)
+    F = sorted((k for k in range(K) if ok[k]), key=lambda k: ids[k])      # agent-id order
+    labels = np.full(K, -1, dtype=np.int64)
+    sus = np.zeros(K, dtype=bool)
+    te_out = np.where(ok, te, -1)
+    scales = np.ones(K, dtype=np.float32)
+    if not F:
+        return DeepSightResult([], torch.from_numpy(scales), None, labels, sus, te_out, [])
+    Fi = np.asarray(F, dtype=np.int64)
+    B = float(np.median(te[Fi])) / 2.0
+    sus[Fi] = te[Fi] <= B
+    with np.errstate(all="ignore"):
+        x = db[Fi]
+        G = _pair_sum(lambda a, b: a * b, x)
+        q = np.diag(G).copy()
+        nrm = np.sqrt(np.outer(q, q))
+        d_cos = 1.0 - np.clip(np.where(nrm > 0, G / np.where(nrm > 0, nrm, 1.0), 0.0), -1.0, 1.0)
+    np.fill_diagonal(d_cos, 0.0)
+    euclid = lambda X: np.sqrt(_pair_sum(lambda a, b: (a - b) * (a - b), X))
+    merged = seeds * _partition_indicator(hdbscan_labels(d_cos, 2)) + seeds * _partition_indicator(hdbscan_labels(euclid(neup[Fi]), 2))
+    for s in range(seeds):
+        merged = merged + _partition_indicator(hdbscan_labels(euclid(ddif[Fi, s]), 2))
+    final = hdbscan_labels(merged.astype(np.float64), 2)
+    parts = {}
+    for j, lab in enumerate(final.tolist()):
+        parts.setdefault(lab if lab >= 0 else -1 - j, []).append(j)     # a noise point is a part of its own
+    accepted = []
+    for pid, (key, q) in enumerate(sorted(parts.items(), key=lambda kv: kv[1][0])):
+        for j in q:
+            labels[F[j]] = pid
+        if sum(int(sus[F[j]]) for j in q) / len(q) < float(tau):
+            accepted.extend(F[j] for j in q)
+    S_clip = float(np.median(e_all[Fi]))
+    for k in F:
+        if e_all[k] > 0:
+            scales[k] = np.float32(min(1.0, S_clip / float(e_all[k])))
+    return DeepSightResult(sorted(accepted), torch.from_numpy(scales), S_clip, labels, sus, te_out, sorted(F))
+
+
+def deepsight_statement(logits, g_logits, w_agents, w_global, head, ids, tau: float, n_vote=None, seeds: int = DEEPSIGHT_SEEDS):
+    """The fp64 statement of DeepSight's admission: ``deepsight_decide`` on ``deepsight_stats_statement`` and the fp64 update norms
+    over the voted coordinates ``[0, n_vote)``."""
+    nv = w_global.numel() if n_vote is None else int(n_vote)
+    norms = torch.stack([(w[:nv].double() - w_global[:nv].double()).norm() for w in w_agents]).cpu()
+    return deepsight_decide(deepsight_stats_statement(logits, g_logits, w_agents, w_global, head, seeds), norms, ids, tau, seeds)
+
+
 def boost_statement(slot, w_g, gamma: float, n_vote: int):
     """The boosted update in numpy: ``fp32((double)w_g[c] + (double)gamma * (double)fp32(slot[c] - w_g[c]))`` for ``c < n_vote``,
     each fp64 operation rounded on its own.  Returns a float32 array ``[n_vote]``."""

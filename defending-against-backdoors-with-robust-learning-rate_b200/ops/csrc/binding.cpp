@@ -542,6 +542,27 @@ void flare_mmd(at::Tensor z, at::Tensor finite, double inv_s2, at::Tensor out) {
                                 (int)z.size(2), (float)inv_s2, out.data_ptr<double>(), cur_stream()), "flare_mmd");
 }
 
+void deepsight_stats(at::Tensor z, at::Tensor zg, at::Tensor slot_ptrs, int64_t wg_ptr, int64_t w_off, int64_t b_off, int64_t S,
+                     int64_t d, at::Tensor out) {
+    CHECK_CUDA(z); CHECK_CUDA(zg); CHECK_CUDA(slot_ptrs); CHECK_CUDA(out);
+    TORCH_CHECK(z.scalar_type() == at::kFloat && z.dim() == 3 && z.is_contiguous(), "deepsight_stats: contiguous fp32 logits [K][S N][P]");
+    const int64_t K = z.size(0), SN = z.size(1), P = z.size(2);
+    TORCH_CHECK(K >= 1 && S >= 1 && SN >= 1 && SN % S == 0 && K < (1LL << 31) && SN < (1LL << 31) && d >= 1 && d < (1LL << 31),
+                "deepsight_stats: empty or oversized logits, or S does not divide their rows");
+    TORCH_CHECK(P >= 1 && P <= rlr::kDeepSightMaxClasses, "deepsight_stats: ", P, " classes; the pass takes 1 to ",
+                rlr::kDeepSightMaxClasses);
+    TORCH_CHECK(zg.scalar_type() == at::kFloat && zg.is_contiguous() && zg.dim() == 2 && zg.size(0) == SN && zg.size(1) == P,
+                "deepsight_stats: contiguous fp32 global logits [S N][P]");
+    TORCH_CHECK(slot_ptrs.scalar_type() == at::kLong && slot_ptrs.numel() == K, "deepsight_stats: int64 pointer table [K]");
+    TORCH_CHECK(wg_ptr && w_off >= 0 && b_off >= 0, "deepsight_stats: global parameters and head offsets");
+    TORCH_CHECK(out.scalar_type() == at::kDouble && out.is_contiguous() && out.numel() == K * (S + 2) * P,
+                "deepsight_stats: fp64 out[K][(S + 2) P]");
+    c10::cuda::CUDAGuard guard(z.device());
+    check(rlr::launch_deepsight_stats(z.data_ptr<float>(), zg.data_ptr<float>(), reinterpret_cast<const float* const*>(slot_ptrs.data_ptr()),
+                                      reinterpret_cast<const float*>(wg_ptr), w_off, b_off, (int)K, (int)S, (int)(SN / S), (int)P, (int)d,
+                                      out.data_ptr<double>(), cur_stream()), "deepsight_stats");
+}
+
 void boost_update(at::Tensor slot, at::Tensor w_g, double gamma, int64_t n_vote) {
     CHECK_CUDA(slot); CHECK_CUDA(w_g);
     TORCH_CHECK(slot.scalar_type() == at::kFloat && w_g.scalar_type() == at::kFloat);
@@ -667,6 +688,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("boost_update", &boost_update);
     m.def("sparsefed", &sparsefed);
     m.def("flare_mmd", &flare_mmd);
+    m.def("deepsight_stats", &deepsight_stats);
     m.def("swap_samples", &swap_samples);
     m.def("pgd_project", &pgd_project, py::arg("w"), py::arg("w0"), py::arg("w_bf16"), py::arg("clip"), py::arg("d_sqnorm"),
           py::arg("n_pgd") = 0, py::arg("mask") = py::none());

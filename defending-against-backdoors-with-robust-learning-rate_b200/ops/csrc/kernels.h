@@ -232,6 +232,16 @@ cudaError_t launch_sparsefed(const float* w_new, float* w, void* w_bf16, float* 
 // Per-CTA fp64 partials added in tile order: no float atomics, bitwise reproducible.
 cudaError_t launch_flare_mmd(const float* z, const unsigned char* finite, int K, int n, int d, float inv_s2, double* out, cudaStream_t st);
 
+// ---- DeepSight statistics pass (deepsight.cu) -------------------------------------------------------------------------------------
+// z: [K][S N][P] fp32 eval-mode logits of K candidates on S seeds of N random inputs, zg: [S N][P] the global model's; slots: [K] flat
+// fp32 parameters of the candidates, wg the global ones, the head weight [P][d] at w_off and its bias [P] at b_off.  out (device fp64
+// [K][(S + 2) P]) per candidate: DDif [S][P] (each an fp64 mean over its seed's rows in ascending order), eps [P] (|db_c| then
+// |dW_cj| for ascending j, added left to right) and db [P] = fp32(b_k - b_g).  One thread per output: bitwise reproducible.
+// 1 <= P <= kDeepSightMaxClasses; anything else returns cudaErrorInvalidValue.
+constexpr int kDeepSightMaxClasses = 1024;
+cudaError_t launch_deepsight_stats(const float* z, const float* zg, const float* const* slots, const float* wg, long long w_off,
+                                   long long b_off, int K, int S, int N, int P, int d, double* out, cudaStream_t st);
+
 // ---- loss / evaluation -----------------------------------------------------------------------------------
 // logits [B,C] (kind 0 fp32 / 1 bf16); writes dlogits (same kind, scaled by 1/B) and accumulates loss_sum / correct.
 cudaError_t launch_softmax_xent(const void* logits, int kind, const int64_t* labels, void* dlogits, float* loss_sum,

@@ -14,11 +14,13 @@ import math
 import torch
 
 DATASETS = ("fmnist", "fedemnist", "cifar10")
-AGGREGATORS = ("avg", "comed", "sign", "fltrust", "rfa", "flame", "foolsgold", "flare")
+AGGREGATORS = ("avg", "comed", "sign", "fltrust", "rfa", "flame", "foolsgold", "flare", "deepsight")
 ROOT_SIZE = 100                  # FLTrust / FLARE root set: the paper's 100 clean samples
 FLARE_TAU = 1.0                  # FLARE: temperature of the softmax over the neighbour counts
 RFA_ITERS = 3                    # RFA: a few smoothed Weiszfeld passes per round
 RFA_NU = 1e-6                    # RFA smoothing: distances below nu count as nu
+DEEPSIGHT_SAMPLES = 256          # DeepSight: random inputs per seed (this project's choice; the paper does not fix one)
+DEEPSIGHT_TAU = 1.0 / 3.0        # DeepSight: a cluster is accepted when fewer than tau of its members are suspicious
 FLAME_LAMBDA = 1e-3              # FLAME noise factor: the paper's value for image classification
 LIFESPAN_THRESHOLD = 0.5         # poison accuracy below which the backdoor counts as gone
 SERVER_OPTS = ("sgd", "momentum", "adagrad", "adam", "yogi")
@@ -54,7 +56,9 @@ def build_parser() -> argparse.ArgumentParser:
                         "median-norm clipping and adaptive noise, Nguyen et al. 2022) | foolsgold (a weighted mean that "
                         "down-weights agents whose summed update histories are too similar to another's, Fung et al. 2020) | flare (a "
                         "weighted mean that trusts the models whose penultimate-layer representations of a clean root set lie among the "
-                        "others' nearest by MMD, Wang et al. 2022)")
+                        "others' nearest by MMD, Wang et al. 2022) | deepsight (clusters the models by their output-layer energy, "
+                        "update direction and behaviour on random inputs, and drops clusters of models whose output layer was trained "
+                        "on few labels, then averages the rest clipped to the median norm, Rieger et al. 2022)")
     p.add_argument("--local_ep", type=int, default=2, help="number of local epochs: E")
     p.add_argument("--bs", type=int, default=256, help="local batch size: B")
     p.add_argument("--client_lr", type=float, default=0.1, help="clients' learning rate")
@@ -159,6 +163,13 @@ def build_parser() -> argparse.ArgumentParser:
                         "with finite features; capped at |F| - 1)")
     p.add_argument("--flare_tau", type=float, default=None,
                    help=f"--aggr flare: temperature tau > 0 of the softmax that turns neighbour counts into trust (default {FLARE_TAU})")
+    p.add_argument("--deepsight_samples", type=int, default=None,
+                   help=f"--aggr deepsight: random inputs per seed, an integer >= 1 (default {DEEPSIGHT_SAMPLES}); every submitted model "
+                        "and the global model run on 3 seeds of them, drawn once from --seed")
+    p.add_argument("--deepsight_tau", type=float, default=None,
+                   help="--aggr deepsight: a cluster of models is accepted when the share of suspicious models in it is below tau, "
+                        "0 < tau <= 1 (default 1/3).  DeepSight guarantees no number of accepted models: a --robustLR_threshold above "
+                        "the accepted count flips every coordinate")
     p.add_argument("--detect", type=str, default="none", choices=DETECTORS,
                    help="detection ahead of the --aggr rule: fldetector (Zhang et al. 2022) predicts every agent's update from its last "
                         "one and an L-BFGS Hessian estimate, scores how far each update lies from its prediction, and once the gap "
@@ -255,6 +266,7 @@ def finalize_args(args: argparse.Namespace) -> argparse.Namespace:
     _finalize_flare(args)
     _finalize_rfa(args)
     _finalize_flame(args)
+    _finalize_deepsight(args)
     _finalize_attack(args)
     _finalize_collude(args)
     _finalize_detect(args)
@@ -458,6 +470,26 @@ def _finalize_flare(args) -> None:
     args.flare_tau = float(tau)
 
 
+def _finalize_deepsight(args) -> None:
+    """Validate the DeepSight flags and resolve ``deepsight_samples`` / ``deepsight_tau`` in place (``DEEPSIGHT_SAMPLES`` /
+    ``DEEPSIGHT_TAU`` by default under ``--aggr deepsight``).  No ``--server_clip``: DeepSight clips to the median norm itself.  It
+    guarantees no number of accepted voters, so, as under FLTrust, the RLR threshold is not checked against one."""
+    n, tau = getattr(args, "deepsight_samples", None), getattr(args, "deepsight_tau", None)
+    if args.aggr != "deepsight":
+        if n is not None or tau is not None:
+            raise ValueError("--deepsight_samples / --deepsight_tau need --aggr deepsight")
+        return
+    n = DEEPSIGHT_SAMPLES if n is None else n
+    if int(n) != n or n < 1:
+        raise ValueError(f"--deepsight_samples {n} must be an integer >= 1")
+    tau = DEEPSIGHT_TAU if tau is None else tau
+    if not (math.isfinite(tau) and 0 < tau <= 1):
+        raise ValueError(f"--deepsight_tau {tau} must be a finite number in (0, 1]")
+    if getattr(args, "server_clip", False):
+        raise ValueError("--server_clip does not combine with --aggr deepsight, which clips every update to the round's median norm")
+    args.deepsight_samples, args.deepsight_tau = int(n), float(tau)
+
+
 def dnc_fewest(args) -> int:
     """The fewest participants ``--select dnc`` can admit: ``K - T floor(c F)``, every iteration removing others."""
     K = max(1, math.floor(args.num_agents * args.agent_frac))
@@ -576,6 +608,8 @@ def print_exp_details(args, n_params: int | None = None) -> None:
         print(f"    Root set: {args.root_size}")
     if args.aggr == "flare":
         print(f"    FLARE (root / k / tau): {args.root_size} / {'floor(|F|/2)' if args.flare_k is None else args.flare_k} / {args.flare_tau}")
+    if args.aggr == "deepsight":
+        print(f"    DeepSight (seeds x samples / tau): 3 x {args.deepsight_samples} / {args.deepsight_tau:.4g}")
     if args.aggr == "rfa":
         print(f"    RFA passes / nu: {args.rfa_iters} / {args.rfa_nu}")
     if args.aggr == "flame":

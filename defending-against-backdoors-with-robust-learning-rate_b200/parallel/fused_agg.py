@@ -391,10 +391,17 @@ class FusedAggregator:
         on every rank.  ``local``: this rank's ``[max_slots][n][d]`` block, row s holding the features of the participant in its slot s
         (``slot_owner``).  With several ranks, on every transport (fused, gather and reduce alike), the blocks are all-gathered
         (``ctx.all_gather``) and reordered, so every rank runs the MMD pass on the same bytes; with one process the block is the result."""
+        return self.gather_slot_rows(n_part, local)
+
+    def gather_slot_rows(self, n_part: int, local):
+        """The per-participant rows of the round's ``n_part`` participants, ``[n_part][...]`` ordered by participant position and
+        identical on every rank.  ``local``: this rank's ``[max_slots][...]`` block, row s holding the row of the participant in its slot
+        s (``slot_owner``).  With several ranks, on every transport (fused, gather and reduce alike), the blocks are all-gathered
+        (``ctx.all_gather``) and reordered; with one process the block is the result."""
         ctx = self.ctx
         if not ctx.is_dist:
             return local[:n_part]
-        allp = ctx.all_gather(local)                                     # [world, max_slots, n, d]
+        allp = ctx.all_gather(local)                                     # [world, max_slots, ...]
         return torch.stack([allp[r, s] for r, s in map(self.slot_owner, range(n_part))])
 
     def pairwise_gram(self, n_part: int, members=None, participants=None):

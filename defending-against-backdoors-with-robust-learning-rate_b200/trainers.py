@@ -152,16 +152,16 @@ class TorchTrainer:
         return lambda x: net(x)
 
     @torch.no_grad()
-    def root_features(self, w, x):
+    def root_features(self, w, x, tap: bool = True):
         """FLARE's features of parameters ``w`` on the normalised NCHW batch ``x``: the fp32 ``[B, d]`` input of the head in eval mode
         (``w``'s own BatchNorm running statistics, no dropout), through one feature ``GraphNet`` per trainer rebound to ``w``, ``--bs``
-        rows at a time."""
+        rows at a time.  ``tap=False``: the fp32 ``[B, classes]`` logits instead (DeepSight's random-input behaviour)."""
         if getattr(self, "_feat_net", None) is None:
             self._feat_net = GraphNet(self.layout, w, None, self.compute_dtype)
             self._feat_net.eval()
         else:
             self._feat_net.bind(w, None)
-        return torch.cat([self._feat_net(x[s:s + self.bs], tap=True) for s in range(0, x.shape[0], self.bs)])
+        return torch.cat([self._feat_net(x[s:s + self.bs], tap=tap) for s in range(0, x.shape[0], self.bs)])
 
 
 def make_trainer(kind, layout, args, device, max_shard):

@@ -84,6 +84,9 @@ class Aggregation:
         # SparseFed (--server_topk) of the in-process form: the error vector [n_vote] (allocated on first use) and the last round's fields
         self.sparse_e = None
         self.last_sparse = None
+        # CRFL (--param_clip / --param_noise) of the in-process form: the real-coordinate mask (built on first use) and the last round's fields
+        self.crfl_mask = None
+        self.last_crfl = None
 
     # ---- the server step ------------------------------------------------------------------------------------
     def aggregate_updates(self, w_global, agent_params, cur_round, n_vote=None, root_params=None, features=None, logits=None,
@@ -126,7 +129,10 @@ class Aggregation:
         if self.opt is None:
             self.opt = ops.ServerOptState(n=w_global.numel(), device=w_global.device, **server_opt_spec(self.args))
         p = float(getattr(self.args, "server_topk", 0.0))
-        out = torch.empty_like(w_global) if p > 0 else w_global      # SparseFed: the plain step's result w' goes to a scratch vector
+        rho, sigma = float(getattr(self.args, "param_clip", 0.0)), float(getattr(self.args, "param_noise", 0.0))
+        crfl = rho > 0 or sigma > 0
+        # SparseFed / CRFL: the plain step's result w' goes to a scratch vector
+        out = torch.empty_like(w_global) if (p > 0 or crfl) else w_global
         ops.fused_aggregate(w_global, ws, weights, self._mode, self.args.robustLR_threshold, self.server_lr, noise_std, self.args.seed,
                             cur_round,
                             n_vote if n_vote is not None else (self.layout.n_vote if self.layout else None),
@@ -139,6 +145,16 @@ class Aggregation:
             ops.sparsefed_step(w_global, out, self.sparse_e, n_voted, k, stats)
             s = stats.tolist()
             self.last_sparse = {"sparse_applied": int(s[0]), "sparse_threshold": s[1], "sparse_error_norm": s[2]}
+            out = w_global                                            # CRFL's pass follows in place
+        if crfl:
+            if self.layout is None:
+                raise ValueError("--param_clip / --param_noise need the model's layout (its real-coordinate mask)")
+            if self.crfl_mask is None:
+                self.crfl_mask = ops.real_mask(self.layout).to(w_global.device)
+            stats = torch.zeros(2, dtype=torch.float64, device=w_global.device)
+            ops.crfl_step(w_global, out, self.crfl_mask, self.layout.n_vote, rho, sigma, self.args.seed, cur_round, stats)
+            s = stats.tolist()
+            self.last_crfl = {"param_norm": s[0], "param_scale": s[1]}
         self.last_flipped = flipped
         if self.args.diagnostics:
             self.plot_norms(dict(zip(all_ids, ops.update_norms(prev, all_ws, nv).tolist())), cur_round)

@@ -30,7 +30,8 @@ from .data import distribute_data, get_datasets, make_poisoned_val
 from .data.datasets import DeviceDataset, h5_to_device_dataset, load_fedemnist_client
 from .models import get_layout
 from .models.graph import feature_dim, head_slices
-from .options import attack_schedule_set, is_attack_round, last_attack_round, print_exp_details
+from .options import (CERTIFY_ALPHA, CERTIFY_N, CERTIFY_N0, attack_schedule_set, is_attack_round, last_attack_round,
+                      print_exp_details)
 from .parallel import FusedAggregator, init_distributed
 from .trainers import make_trainer
 from .utils import (MetricLogger, PhaseTimer, backdoor_lifespan, get_loss_n_accuracy, load_checkpoint, restore_server_opt,
@@ -136,11 +137,16 @@ class FLEngine:
         p = float(getattr(args, "server_topk", 0.0))
         self.topk_k = ops.sparsefed_k(p, self.layout.n_params) if p > 0 else 0
         self.last_sparse = None
+        # CRFL (--param_clip / --param_noise; DESIGN.md section 3): the clip-and-perturb pass after the server step, keyed by (seed, round)
+        self.crfl = getattr(args, "param_clip", 0.0) > 0 or getattr(args, "param_noise", 0.0) > 0
+        self.last_crfl = None
+        self.last_certify = None
         self.fused = FusedAggregator(ctx, self.layout.n_total, self.layout.n_vote, max_slots, backend,
                                      transport=getattr(args, "agg_transport", "auto"), server_opt=server_opt_spec(args),
                                      n_part=self.n_part, history_agents=args.num_agents if args.aggr == "foolsgold" else 0,
                                      fld_agents=args.num_agents if self.detect else 0, fld_window=args.fld_window if self.detect else 0,
-                                     topk_k=self.topk_k)
+                                     topk_k=self.topk_k,
+                                     crfl=(args.param_clip, args.param_noise, ops.real_mask(self.layout)) if self.crfl else None)
         init = torch.zeros(self.layout.n_total, dtype=torch.float32)
         self.layout.init_(init, args.seed)
         self.fused.w_global.copy_(init.to(dev))
@@ -490,9 +496,15 @@ class FLEngine:
             parts.append(self.masked_coords.double())                   # |M| of the round, read with the same copy
         if self.topk_k:
             parts.append(self.fused.sparse_stats)                       # SparseFed's |M|, tau and ||e||, likewise
+        if self.crfl:
+            parts.append(self.fused.crfl_stats)                         # CRFL's pre-clip norm and scale, likewise
         vals = torch.cat(parts).cpu()
         if self.neurotoxin_k is not None:
             self.last_masked_coords = int(vals[2])
+        if self.crfl:
+            s = vals[-2:].tolist()
+            self.last_crfl = {"param_norm": s[0], "param_scale": s[1]}
+            vals = vals[:-2]
         if self.topk_k:
             s = vals[-3:].tolist()
             self.last_sparse = {"sparse_applied": int(s[0]), "sparse_threshold": s[1], "sparse_error_norm": s[2]}
@@ -539,6 +551,75 @@ class FLEngine:
                     print(f"| Backdoor lifespan: {span} rounds |")
         return out
 
+    # ---- CRFL certification (DESIGN.md section 3) ----------------------------------------------------------
+    @torch.no_grad()
+    def certify(self):
+        """Certify the current global model w on the validation and the poisoned validation set by parameter smoothing (Cohen et al.'s
+        CERTIFY in parameter space, sigma = ``--param_noise``).  Draw m < n0 + n writes w + sigma z_m into the trainer's certification
+        executor (``ops.crfl_smooth``, stream ``ops.crfl_stream(m, certify=True)``) and sweeps both datasets, whose batches are assembled
+        and normalised once; every row's vote lands in int32 counts (``ops.vote_count``): selection counts for m < n0, estimation counts
+        after.  With several ranks draw m runs on rank m % world and the counts are all-reduced, so the result does not depend on the
+        world size.  Returns ``{"val": ..., "poison": ...}``, each a dict of the per-input ``pred`` (-1 = abstain), ``radius`` (L2 in
+        parameter space), ``p_a``, ``labels`` and the ``selection`` / ``estimation`` counts, plus ``acc``, ``abstain`` and ``certified``
+        (the certified accuracy at R / sigma in ``ops.CERTIFY_RATIOS``)."""
+        args, ctx = self.args, self.ctx
+        sigma = float(getattr(args, "param_noise", 0.0))
+        if not sigma > 0:
+            raise ValueError("certification smooths with the training noise and needs --param_noise > 0")
+        n0 = int(getattr(args, "certify_n0", None) or CERTIFY_N0)
+        n = int(getattr(args, "certify_n", None) or CERTIFY_N)
+        alpha = float(getattr(args, "certify_alpha", None) or CERTIFY_ALPHA)
+        w = self.global_params()
+        cw, cwb, prepare, forward = self.trainer.certify_executor()
+        mask = self.fused.crfl_mask if self.fused.crfl_mask is not None else ops.real_mask(self.layout).to(w.device)
+        sets = []
+        for name, ds in (("val", self.val_dataset), ("poison", self.poisoned_val)):
+            N = len(ds)
+            idx = torch.arange(N, device=ds.device)
+            batches, labels = [], []
+            for s in range(0, N, args.bs):
+                x, y = ds.batch(idx[s:s + args.bs])
+                batches.append((s, prepare(x)))
+                labels.append(y)
+            y = torch.cat(labels) if labels else torch.zeros(0, dtype=torch.int64)
+            sets.append((name, batches, y, torch.zeros((2, N, self.n_classes), dtype=torch.int32, device=w.device)))
+        for m in range(ctx.rank, n0 + n, ctx.world):
+            ops.crfl_smooth(w, mask, self.layout.n_vote, sigma, args.seed, m, cw, cwb)
+            for _, batches, _, counts in sets:
+                c = counts[0 if m < n0 else 1]
+                for s, xb in batches:
+                    ops.vote_count(forward(xb), c, s)
+        out = {}
+        for name, _, y, counts in sets:
+            if ctx.is_dist:
+                ctx.all_reduce_sum(counts)
+            cnt = counts.cpu().numpy()
+            labels = y.cpu().numpy()
+            pred, radius, pa = ops.certify_decision(cnt[0], cnt[1], n, alpha, sigma)
+            total = max(1, labels.size)
+            out[name] = {"pred": pred, "radius": radius, "p_a": pa, "labels": labels, "selection": cnt[0], "estimation": cnt[1],
+                         "acc": float(np.sum(pred == labels)) / total, "abstain": float(np.sum(pred < 0)) / total,
+                         "certified": ops.certified_accuracy(pred, radius, labels, sigma)}
+        self.last_certify = out
+        return out
+
+    def _certify_record(self, rnd: int):
+        """Run ``certify()`` and report it: the stdout line, the Certify/* TensorBoard tags and the ``certify_*`` record fields."""
+        args = self.args
+        res = self.certify()
+        rec = {}
+        for name, tag in (("val", "Val"), ("poison", "Poison")):
+            r = res[name]
+            rec[f"certify_{name}_acc"], rec[f"certify_{name}_abstain"] = r["acc"], r["abstain"]
+            rec[f"certify_{name}_certified"] = r["certified"]
+            self.logger.add_scalar(f"Certify/{tag}_Accuracy", r["acc"], rnd)
+            self.logger.add_scalar(f"Certify/{tag}_Abstain", r["abstain"], rnd)
+        if self.verbose:
+            print(f"| Certified (sigma {args.param_noise}, n0/n {args.certify_n0}/{args.certify_n}, alpha {args.certify_alpha}): "
+                  f"val acc {res['val']['acc']:.3f} / abstain {res['val']['abstain']:.3f} | "
+                  f"poison acc {res['poison']['acc']:.3f} / abstain {res['poison']['abstain']:.3f} |")
+        return rec
+
     # ---- the training loop --------------------------------------------------------------------------------
     def fit(self, rounds: int | None = None):
         args = self.args
@@ -567,6 +648,10 @@ class FLEngine:
                 rec.update(self.last_sparse)
                 for key, tag in (("sparse_applied", "Applied"), ("sparse_threshold", "Threshold"), ("sparse_error_norm", "Error_Norm")):
                     self.logger.add_scalar(f"SparseFed/{tag}", self.last_sparse[key], rnd)
+            if self.last_crfl is not None:
+                rec.update(self.last_crfl)
+                self.logger.add_scalar("ParamClip/Norm", self.last_crfl["param_norm"], rnd)
+                self.logger.add_scalar("ParamClip/Scale", self.last_crfl["param_scale"], rnd)
             if self.last_collude is not None:
                 rec.update(self.last_collude)
                 for key, tag in (("collude_honest", "Honest"), ("collude_deviation", "Deviation"), ("collude_z", "Z")):
@@ -608,6 +693,8 @@ class FLEngine:
                 rec.update(self.aggregator.last_fld)
                 if "fld_flagged" in rec and self.verbose:
                     print(f"| FLDetector: flagged {rec['fld_flagged']} in round {rnd} ({rec['fld_corrupt_flagged']} corrupt) |")
+            if rnd == rounds and getattr(args, "certify", False):
+                rec.update(self._certify_record(rnd))
             rec.update({f"ms_{k}": v for k, v in self.timer.elapsed().items()})
             if args.profile_phases and self.verbose:
                 print({k: round(v, 3) for k, v in rec.items() if k.startswith("ms_")})

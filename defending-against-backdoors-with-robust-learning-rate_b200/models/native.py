@@ -785,3 +785,18 @@ class NativeTrainer:
             xb = x[s:s + self.bs].permute(0, 2, 3, 1).to(ACT).contiguous()
             out.append(net.forward_raw(xb, False, tap=tap).to(torch.float32, copy=True))
         return torch.cat(out)
+
+    @torch.no_grad()
+    def certify_executor(self):
+        """CRFL certification's executor, built once: ``(w, w_bf16, prepare, forward)``.  A native eval executor of its own bound to a
+        dedicated fp32 parameter buffer ``w`` and bf16 shadow ``w_bf16``, both rewritten by ``ops.crfl_smooth`` in one pass per draw;
+        ``prepare(x)`` turns a normalised NCHW batch (at most ``--bs`` rows) into the NHWC activation input once, and ``forward(xb)``
+        returns the fp32 logits in eval mode (a view of the executor's logits buffer, valid until its next forward)."""
+        if getattr(self, "_cert", None) is None:
+            n = self.layout.n_total
+            net = NativeNet(self.layout, self.device, self.bs, self.net.impl, seed=self.args.seed)
+            w = torch.zeros(n, dtype=torch.float32, device=self.device)
+            wb = torch.zeros(n, dtype=ACT, device=self.device)
+            net.bind(w, wb, None)
+            self._cert = (w, wb, lambda x: x.permute(0, 2, 3, 1).to(ACT).contiguous(), lambda xb: net.forward(xb, False))
+        return self._cert

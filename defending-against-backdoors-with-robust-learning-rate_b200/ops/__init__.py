@@ -1362,6 +1362,199 @@ def sparsefed_k(p: float, n_params: int) -> int:
 
 
 # =====================================================================================================================
+# CRFL (Xie, Chen, Chen, Li, ICML 2021): clip and perturb the global model every round, certify it by parameter smoothing
+# =====================================================================================================================
+_CRFL_TRAIN_TAG = 0x3C6EF372FE94F82B     # domain tags of the training noise and the certification draws (SHA-512 IV words, like
+_CRFL_CERT_TAG = 0xA54FF53A5F1D36F1      # _AUGMENT_TAG): keep both apart from every other Philox stream
+CERTIFY_RATIOS = (0.0, 0.5, 1.0, 1.5, 2.0)   # R / sigma at which the certified accuracy is reported
+
+
+def crfl_stream(index: int, certify: bool = False) -> int:
+    """Philox stream word of CRFL's training noise in round ``index`` (``certify=False``) or of certification draw ``index``: a splitmix64
+    hash of the domain tag and the index, in the style of ``augment_stream``.  Bit 63 is set, so the word is never an augmentation word
+    (kept below 2^63) nor the aggregate noise's bare round number; bit 62 tells training from certification, so those two never meet.
+    The key is ``--seed``; the counter is the coordinate / 4."""
+    z = ((_CRFL_CERT_TAG if certify else _CRFL_TRAIN_TAG) + (int(index) + 1) * 0x9E3779B97F4A7C15) & _M64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _M64
+    z ^= z >> 31
+    return (z & (2 ** 62 - 1)) | (1 << 63) | (int(bool(certify)) << 62)
+
+
+def _i64(word: int) -> int:
+    """An unsigned 64-bit word as the int64 the bindings take."""
+    word = int(word) & _M64
+    return word - 2 ** 64 if word >= 2 ** 63 else word
+
+
+def real_mask(layout):
+    """CRFL's real-coordinate mask of a ``FlatLayout``: int32 bit words over ``[0, n_vote)`` in Neurotoxin's format (bit ``c % 32`` of word
+    ``c // 32``), set for the ``layout.n_params`` coordinates inside parameter tensors and clear on the alignment padding."""
+    nv = int(layout.n_vote)
+    m = np.zeros(mask_words(nv) * 32, dtype=bool)
+    for p in layout.params:
+        m[p.offset:p.offset + p.numel] = True
+    return torch.from_numpy(np.packbits(m, bitorder="little").view("<u4").astype(np.uint32).view(np.int32).copy())
+
+
+def philox_normals(seed: int, stream: int, n: int):
+    """fp64 Box-Muller of the Philox words behind ``philox_normal4`` (common.cuh) for coordinates ``[0, n)`` (``n % 4 == 0``): counter
+    c / 4, lane c % 4 = (r0 cos 2 pi u1, r0 sin 2 pi u1, r1 cos 2 pi u3, r1 sin 2 pi u3), r = sqrt(-2 ln u), u = ((x >> 8) + 1) / 2^24."""
+    n4 = int(n) // 4
+    u = philox4x32(np.arange(n4, dtype=np.uint64), stream, seed)
+    unit = [((x >> np.uint32(8)).astype(np.float64) + 1.0) / 16777216.0 for x in u]
+    r0, r1 = np.sqrt(-2.0 * np.log(unit[0])), np.sqrt(-2.0 * np.log(unit[2]))
+    z = np.empty((n4, 4), dtype=np.float64)
+    c1, s1 = _cos_sin_pi(2.0 * unit[1])
+    c3, s3 = _cos_sin_pi(2.0 * unit[3])
+    z[:, 0], z[:, 1], z[:, 2], z[:, 3] = r0 * c1, r0 * s1, r1 * c3, r1 * s3
+    return z.reshape(-1)
+
+
+def _cos_sin_pi(t):
+    """``(cos(pi t), sin(pi t))`` in fp64 with exact argument reduction, as ``sincospif`` reduces: t = q/2 + f with q = rint(2 t) and
+    |f| <= 1/4 exact, so the zeros at quarter turns are exact zeros."""
+    q = np.rint(2.0 * t)
+    f = t - 0.5 * q
+    c, s = np.cos(np.pi * f), np.sin(np.pi * f)
+    k = q.astype(np.int64) & 3
+    cos = np.select([k == 0, k == 1, k == 2], [c, -s, -c], s)
+    sin = np.select([k == 0, k == 1, k == 2], [s, c, -s], -c)
+    return cos, sin
+
+
+def crfl_statement(w_new, mask, n_vote: int, rho: float, sigma: float, seed: int, stream: int, z=None):
+    """CRFL's clip-and-perturb pass in numpy, after the complete server step wrote ``w_new`` (fp32 ``[n]``); ``mask``: ``real_mask`` words.
+
+    * ``q = sum w_new[c]^2`` in fp64 over the real coordinates (each square exact, the sum in numpy's fixed order);
+    * ``s = 1`` if ``rho`` is 0 (no clip), ``q <= rho^2`` or ``q`` is not finite, else ``fp32(rho / sqrt(q))``;
+    * on real coordinates ``w = fp32(fp32(w_new s) + fp32(fp32(sigma) z))`` with ``z = fp32(philox_normals)`` (or the given fp32 ``z``
+      ``[n_vote]``), no noise term at ``sigma = 0``; every other coordinate keeps ``w_new``.
+
+    Returns ``(w fp32 [n], sqrt(q), s)``."""
+    n_vote = int(n_vote)
+    wn = (w_new.detach().cpu().numpy() if torch.is_tensor(w_new) else np.asarray(w_new)).astype(np.float32, copy=True)
+    words = mask.detach().cpu() if torch.is_tensor(mask) else torch.from_numpy(np.asarray(mask).view(np.int32))
+    real = mask_bits(words, n_vote).numpy()
+    v = wn[:n_vote]
+    x = v[real].astype(np.float64)
+    q = float(np.sum(x * x))
+    s = np.float32(1.0)
+    rho = float(rho)
+    if rho > 0 and math.isfinite(q) and q > rho * rho:
+        s = np.float32(rho / math.sqrt(q))
+    with np.errstate(invalid="ignore", over="ignore"):
+        o = np.where(real, v * s, v).astype(np.float32)
+        if sigma > 0:
+            zz = philox_normals(seed, stream, n_vote).astype(np.float32) if z is None else np.asarray(z, dtype=np.float32)[:n_vote]
+            o = np.where(real, o + np.float32(sigma) * zz, o).astype(np.float32)
+    wn[:n_vote] = o
+    return wn, math.sqrt(q), float(s)
+
+
+def crfl_step(w, w_new, mask, n_vote: int, rho: float, sigma: float, seed: int, rnd: int, stats, w_bf16=None):
+    """CRFL's clip-and-perturb pass of round ``rnd`` (``crfl_statement`` with the stream ``crfl_stream(rnd)``): ``w`` (and its bf16 shadow,
+    when given) becomes the clipped, perturbed ``w_new``; ``w`` may be ``w_new``.  ``rho = 0``: no clip.  The float64 ``stats[:2]`` =
+    ``(sqrt(q), s)``.  On the GPU the norm, the ordered sum and the apply pass queue without a host sync."""
+    stream = crfl_stream(rnd)
+    if w.is_cuda:
+        ext().crfl_clip_noise(w_new, w, w_bf16, mask, int(n_vote), float(rho) if rho > 0 else math.inf, float(sigma), _i64(seed),
+                              _i64(stream), stats)
+        return
+    out, norm, s = crfl_statement(w_new, mask, n_vote, rho, sigma, seed, stream)
+    w.copy_(torch.from_numpy(out))
+    if w_bf16 is not None:
+        w_bf16.copy_(w.to(torch.bfloat16))
+    stats[:2].copy_(torch.tensor([norm, s], dtype=torch.float64))
+
+
+def crfl_smooth(w, mask, n_vote: int, sigma: float, seed: int, m: int, out, out_bf16=None):
+    """Parameters of certification draw ``m``: ``out = fp32(w + fp32(sigma z_m))`` on the real coordinates, ``w`` elsewhere, with
+    ``z_m`` on the stream ``crfl_stream(m, certify=True)``; the bf16 shadow ``out_bf16`` (when given) is written in the same pass."""
+    stream = crfl_stream(m, certify=True)
+    if w.is_cuda:
+        ext().crfl_smooth(w, out, out_bf16, mask, int(n_vote), float(sigma), _i64(seed), _i64(stream))
+        return
+    o, _, _ = crfl_statement(w, mask, n_vote, 0.0, sigma, seed, stream)
+    out.copy_(torch.from_numpy(o))
+    if out_bf16 is not None:
+        out_bf16.copy_(out.to(torch.bfloat16))
+
+
+def vote_count(logits, counts, row0: int = 0):
+    """``counts[row0 + r][argmax(logits[r])] += 1`` for every row ``r`` of the fp32 ``[rows][classes]`` logits: the lowest class on ties,
+    no vote for a row with a non-finite logit.  ``counts``: int32 ``[inputs][classes]``."""
+    if logits.is_cuda:
+        ext().vote_count(logits if logits.dtype == torch.float32 and logits.is_contiguous() else logits.float().contiguous(), counts,
+                         int(row0))
+        return
+    x = logits.float()
+    ok = torch.isfinite(x).all(1)
+    rows = torch.arange(x.shape[0])[ok] + int(row0)
+    counts.index_put_((rows, x.argmax(1)[ok]), torch.ones(rows.numel(), dtype=counts.dtype), accumulate=True)
+
+
+def clopper_pearson_lower(k, n: int, alpha: float):
+    """One-sided Clopper-Pearson lower bounds of ``k`` successes in ``n`` trials at level ``alpha``: the alpha-quantile of
+    Beta(k, n - k + 1), i.e. the p with P(Bin(n, p) >= k) = alpha, and 0 for k = 0.  Bisection in fp64 on the exact binomial tail (log
+    terms from ``lgamma``, summed with the largest factored out); the bisection keeps the side whose tail is <= alpha, so the bound is
+    never above the exact quantile by more than the last interval.  ``k``: an integer or an array; returns a float64 array."""
+    k = np.atleast_1d(np.asarray(k, dtype=np.int64))
+    n = int(n)
+    if np.any(k < 0) or np.any(k > n):
+        raise ValueError(f"success counts must lie in [0, n = {n}]")
+    out = np.zeros(k.shape, dtype=np.float64)
+    pos = np.flatnonzero(k > 0)
+    if pos.size == 0:
+        return out
+    lf = np.array([math.lgamma(j + 1.0) for j in range(n + 1)])
+    j = np.arange(n + 1, dtype=np.float64)
+    logc = lf[n] - lf - lf[::-1]
+    la = math.log(alpha)
+    step = max(1, (1 << 22) // (n + 1))
+    for c0 in range(0, pos.size, step):
+        kk = k[pos[c0:c0 + step]].astype(np.float64)[:, None]
+        lo, hi = np.zeros(kk.shape[0]), np.ones(kk.shape[0])
+        for _ in range(64):
+            mid = 0.5 * (lo + hi)
+            t = logc[None, :] + j[None, :] * np.log(mid)[:, None] + (n - j)[None, :] * np.log1p(-mid)[:, None]
+            t = np.where(j[None, :] >= kk, t, -np.inf)
+            mx = t.max(1)
+            lt = mx + np.log(np.exp(t - mx[:, None]).sum(1))
+            up = lt > la
+            hi, lo = np.where(up, mid, hi), np.where(up, lo, mid)
+        out[pos[c0:c0 + step]] = lo
+    return out
+
+
+def certify_decision(selection, estimation, n: int, alpha: float, sigma: float):
+    """Cohen et al.'s CERTIFY on the vote counts of every input (int ``[inputs][classes]``: the selection draws and the ``n`` estimation
+    draws): ``c = argmax(selection)`` (lowest class on ties), ``n_A = estimation[c]``, ``p_A = clopper_pearson_lower(n_A, n, alpha)``;
+    predict c with radius ``R = sigma Phi^-1(p_A)`` when ``p_A > 1/2``, else abstain.  fp64 on the host, one bound per distinct ``n_A``.
+    Returns ``(prediction int64 [inputs] (-1 = abstain), radius float64 [inputs], p_A float64 [inputs])``."""
+    from statistics import NormalDist
+    sel, est = np.asarray(selection), np.asarray(estimation)
+    c = sel.argmax(1) if sel.shape[0] else np.zeros(0, dtype=np.int64)
+    n_a = est[np.arange(est.shape[0]), c]
+    uniq, inv = np.unique(n_a, return_inverse=True)
+    pa_u = clopper_pearson_lower(uniq, n, alpha)
+    inv_cdf = NormalDist().inv_cdf
+    r_u = np.array([float(sigma) * inv_cdf(p) if p > 0.5 else 0.0 for p in pa_u], dtype=np.float64)
+    pa, radius = pa_u[inv].reshape(-1), r_u[inv].reshape(-1)
+    pred = np.where(pa > 0.5, c, -1).astype(np.int64)
+    return pred, radius, pa
+
+
+def certified_accuracy(pred, radius, labels, sigma: float, ratios=CERTIFY_RATIOS):
+    """Share of inputs predicted correctly with a radius ``R >= r sigma``, for each ``r`` of ``ratios``."""
+    pred, radius, labels = np.asarray(pred), np.asarray(radius), np.asarray(labels)
+    if pred.size == 0:
+        return [0.0 for _ in ratios]
+    ok = pred == labels
+    return [float(np.mean(ok & (radius >= r * float(sigma)))) for r in ratios]
+
+
+# =====================================================================================================================
 # FLARE (Wang, Xiao, Chen, Hu, Lou, Hou, ASIA CCS 2022): trust from the MMD between the candidates' root-set representations
 # =====================================================================================================================
 class FlareResult(NamedTuple):

@@ -529,6 +529,51 @@ void sparsefed(at::Tensor w_new, at::Tensor w, c10::optional<at::Tensor> w_bf16,
                                 n_vote, w.numel(), k, stats.data_ptr<double>(), num_sms(), cur_stream()), "sparsefed");
 }
 
+static void crfl_check(const char* what, const at::Tensor& src, const at::Tensor& dst, const c10::optional<at::Tensor>& dst_bf16,
+                       const at::Tensor& mask, int64_t n_vote) {
+    CHECK_CUDA(src); CHECK_CUDA(dst); CHECK_CUDA(mask);
+    TORCH_CHECK(src.scalar_type() == at::kFloat && dst.scalar_type() == at::kFloat && src.is_contiguous() && dst.is_contiguous() &&
+                src.numel() == dst.numel(), what, ": contiguous fp32 source and destination of one size");
+    TORCH_CHECK(mask.scalar_type() == at::kInt && mask.is_contiguous() && mask.numel() * 32 >= n_vote && n_vote <= src.numel(),
+                what, ": int32 mask words covering [0, n_vote)");
+    if (dst_bf16) {
+        CHECK_CUDA(*dst_bf16);
+        TORCH_CHECK(dst_bf16->scalar_type() == at::kBFloat16 && dst_bf16->numel() == dst.numel(), what, ": bf16 shadow of the destination's size");
+    }
+}
+
+void crfl_clip_noise(at::Tensor w_new, at::Tensor w, c10::optional<at::Tensor> w_bf16, at::Tensor mask, int64_t n_vote, double rho,
+                     double sigma, int64_t seed, int64_t stream, at::Tensor stats) {
+    crfl_check("crfl_clip_noise", w_new, w, w_bf16, mask, n_vote);
+    CHECK_CUDA(stats);
+    TORCH_CHECK(stats.scalar_type() == at::kDouble && stats.numel() >= 2, "crfl_clip_noise: an fp64 stats[2]");
+    c10::cuda::CUDAGuard guard(w.device());
+    check(rlr::launch_crfl_clip_noise(w_new.data_ptr<float>(), w.data_ptr<float>(), w_bf16 ? w_bf16->data_ptr() : nullptr,
+                                      reinterpret_cast<const uint32_t*>(mask.data_ptr<int>()), n_vote, w.numel(), rho, (float)sigma,
+                                      (unsigned long long)seed, (unsigned long long)stream, stats.data_ptr<double>(), num_sms(), cur_stream()),
+          "crfl_clip_noise");
+}
+
+void crfl_smooth(at::Tensor w, at::Tensor out, c10::optional<at::Tensor> out_bf16, at::Tensor mask, int64_t n_vote, double sigma,
+                 int64_t seed, int64_t stream) {
+    crfl_check("crfl_smooth", w, out, out_bf16, mask, n_vote);
+    c10::cuda::CUDAGuard guard(w.device());
+    check(rlr::launch_crfl_smooth(w.data_ptr<float>(), out.data_ptr<float>(), out_bf16 ? out_bf16->data_ptr() : nullptr,
+                                  reinterpret_cast<const uint32_t*>(mask.data_ptr<int>()), n_vote, w.numel(), (float)sigma,
+                                  (unsigned long long)seed, (unsigned long long)stream, num_sms(), cur_stream()),
+          "crfl_smooth");
+}
+
+void vote_count(at::Tensor logits, at::Tensor counts, int64_t row0) {
+    CHECK_CUDA(logits); CHECK_CUDA(counts);
+    TORCH_CHECK(logits.scalar_type() == at::kFloat && logits.dim() == 2 && logits.is_contiguous(), "vote_count: contiguous fp32 logits [rows][classes]");
+    TORCH_CHECK(counts.scalar_type() == at::kInt && counts.dim() == 2 && counts.is_contiguous() && counts.size(1) == logits.size(1) &&
+                row0 >= 0 && row0 + logits.size(0) <= counts.size(0), "vote_count: int32 counts [inputs][classes] holding rows row0 ..");
+    c10::cuda::CUDAGuard guard(logits.device());
+    check(rlr::launch_vote_count(logits.data_ptr<float>(), logits.size(0), (int)logits.size(1), counts.data_ptr<int>(), row0, cur_stream()),
+          "vote_count");
+}
+
 void flare_mmd(at::Tensor z, at::Tensor finite, double inv_s2, at::Tensor out) {
     CHECK_CUDA(z); CHECK_CUDA(finite); CHECK_CUDA(out);
     TORCH_CHECK(z.scalar_type() == at::kFloat && z.dim() == 3 && z.is_contiguous(), "flare_mmd: contiguous fp32 features [K][n][d]");
@@ -687,6 +732,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("neurotoxin_mask", &neurotoxin_mask);
     m.def("boost_update", &boost_update);
     m.def("sparsefed", &sparsefed);
+    m.def("crfl_clip_noise", &crfl_clip_noise);
+    m.def("crfl_smooth", &crfl_smooth);
+    m.def("vote_count", &vote_count);
     m.def("flare_mmd", &flare_mmd);
     m.def("deepsight_stats", &deepsight_stats);
     m.def("swap_samples", &swap_samples);

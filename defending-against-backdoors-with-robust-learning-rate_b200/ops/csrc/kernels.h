@@ -225,6 +225,22 @@ cudaError_t launch_swap_samples(void* data, long long* targets, const long long*
 cudaError_t launch_sparsefed(const float* w_new, float* w, void* w_bf16, float* e, long long n_vote, long long n, long long k,
                              double* stats, int num_sms, cudaStream_t st);
 
+// ---- CRFL (crfl.cu) ---------------------------------------------------------------------------------------------------------------
+// Clip and perturb after the complete server step, which wrote w_new: q = sum of w_new[c]^2 (fp64, fixed order) over the real coordinates
+// (bit c of mask, words over [0, n_vote)), s = 1 if q <= rho^2 or q is not finite else fp32(rho / sqrt(q)); on real coordinates
+// w = fp32(fp32(w_new s) + fp32(sigma z)) (no noise term at sigma = 0), elsewhere w = w_new; the bf16 shadow (optional) <- bf16(w).
+// z = philox_normal4(Philox(seed), c / 4, stream), lane c % 4.  stats (device fp64 [2]) = {sqrt(q), s}.  w may alias w_new; rho = +inf:
+// no clip.  No host sync, no atomics.  n_vote % 4 == 0, n % 4 == 0, n_vote <= n.
+cudaError_t launch_crfl_clip_noise(const float* w_new, float* w, void* w_bf16, const uint32_t* mask, long long n_vote, long long n,
+                                   double rho, float sigma, unsigned long long seed, unsigned long long stream, double* stats,
+                                   int num_sms, cudaStream_t st);
+// Smoothing parameters of one certification draw: out = fp32(w + fp32(sigma z)) on real coordinates, w elsewhere, and its bf16 shadow.
+cudaError_t launch_crfl_smooth(const float* w, float* out, void* out_bf16, const uint32_t* mask, long long n_vote, long long n, float sigma,
+                               unsigned long long seed, unsigned long long stream, int num_sms, cudaStream_t st);
+// counts[row0 + r][argmax of logits row r] += 1 for r < rows (fp32 [rows][classes]; lowest class on ties; no vote for a row with a
+// non-finite logit).  One thread per row, no atomics.
+cudaError_t launch_vote_count(const float* logits, long long rows, int classes, int* counts, long long row0, cudaStream_t st);
+
 // ---- FLARE MMD pass (flare.cu) -----------------------------------------------------------------------------------------------------
 // z: [K][n][d] fp32 penultimate-layer features of K candidates on the n root samples; finite[k] = 1 when every feature of candidate k is
 // finite.  out (device fp64 [K (K + 1) / 2], pairs (i <= j) numbered row by row): S_ij = sum_{a, b} expf(-||z_i[a] - z_j[b]||^2 * inv_s2),

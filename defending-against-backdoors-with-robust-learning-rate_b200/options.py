@@ -23,6 +23,9 @@ DEEPSIGHT_SAMPLES = 256          # DeepSight: random inputs per seed (this proje
 DEEPSIGHT_TAU = 1.0 / 3.0        # DeepSight: a cluster is accepted when fewer than tau of its members are suspicious
 FLAME_LAMBDA = 1e-3              # FLAME noise factor: the paper's value for image classification
 LIFESPAN_THRESHOLD = 0.5         # poison accuracy below which the backdoor counts as gone
+CERTIFY_N0 = 100                 # CRFL certification: selection draws (this project's choice, in the style of Cohen et al.)
+CERTIFY_N = 1000                 # ... estimation draws (likewise)
+CERTIFY_ALPHA = 1e-3             # ... failure probability of each input's certificate (likewise)
 SERVER_OPTS = ("sgd", "momentum", "adagrad", "adam", "yogi")
 SELECTIONS = ("none", "krum", "multikrum", "dnc")
 DNC_DIM = 10000                  # DnC: coordinates per subsample b
@@ -129,6 +132,22 @@ def build_parser() -> argparse.ArgumentParser:
                    help="SparseFed (Panda et al. 2022): every round the server applies only the k = floor(p * n_params) largest "
                         "coordinates of its accumulated step (after the vote, the rule, noise and --server_opt) and carries the rest over "
                         "as error feedback.  0 <= p <= 1 (0 = off).  The paper's setting adds --server_clip --clip L")
+    p.add_argument("--param_clip", type=float, default=0.0,
+                   help="CRFL (Xie et al. 2021): after every round's complete server step (vote, rule, noise, --server_opt, --server_topk) "
+                        "the global model's real parameters are scaled by min(1, rho / ||w||).  rho > 0 (0 = off)")
+    p.add_argument("--param_noise", type=float, default=0.0,
+                   help="CRFL: after the clip, every real parameter gets sigma * z, z ~ N(0, 1) keyed by (--seed, round, coordinate), in every "
+                        "round including the last.  sigma >= 0 (0 = off)")
+    p.add_argument("--certify", action="store_true",
+                   help="CRFL: after the last round certify the final global model on the validation and the poisoned validation set by "
+                        "parameter smoothing with sigma = --param_noise (needs --param_noise > 0): a prediction per input, or an "
+                        "abstention, with an L2 radius in parameter space")
+    p.add_argument("--certify_n0", type=int, default=None,
+                   help=f"--certify: noisy models that select each input's class, an integer >= 1 (default {CERTIFY_N0})")
+    p.add_argument("--certify_n", type=int, default=None,
+                   help=f"--certify: noisy models that estimate the selected class's probability, an integer >= 1 (default {CERTIFY_N})")
+    p.add_argument("--certify_alpha", type=float, default=None,
+                   help=f"--certify: failure probability of each input's certificate, 0 < alpha < 1 (default {CERTIFY_ALPHA})")
     p.add_argument("--select", type=str, default="none", choices=SELECTIONS,
                    help="participant selection before the --aggr rule: krum (Blanchard et al. 2017) admits the participant whose update "
                         "is closest to its K-F-2 nearest neighbours; multikrum the M best such scores; dnc (Shejwalkar and Houmansadr "
@@ -267,6 +286,7 @@ def finalize_args(args: argparse.Namespace) -> argparse.Namespace:
     _finalize_rfa(args)
     _finalize_flame(args)
     _finalize_deepsight(args)
+    _finalize_crfl(args)
     _finalize_attack(args)
     _finalize_collude(args)
     _finalize_detect(args)
@@ -575,6 +595,34 @@ def make_args(**overrides) -> argparse.Namespace:
     return finalize_args(args)
 
 
+def _finalize_crfl(args) -> None:
+    """Validate the CRFL flags and resolve ``certify_n0`` / ``certify_n`` / ``certify_alpha`` in place (defaults under ``--certify``)."""
+    rho, sigma = float(getattr(args, "param_clip", 0.0)), float(getattr(args, "param_noise", 0.0))
+    if not (math.isfinite(rho) and rho >= 0.0):
+        raise ValueError(f"--param_clip {rho} must be a finite number > 0 (0 = off)")
+    if not (math.isfinite(sigma) and sigma >= 0.0):
+        raise ValueError(f"--param_noise {sigma} must be a finite number >= 0 (0 = off)")
+    args.param_clip, args.param_noise = rho, sigma
+    certify = bool(getattr(args, "certify", False))
+    n0, n, alpha = (getattr(args, k, None) for k in ("certify_n0", "certify_n", "certify_alpha"))
+    if not certify:
+        if n0 is not None or n is not None or alpha is not None:
+            raise ValueError("--certify_n0 / --certify_n / --certify_alpha need --certify")
+        return
+    if sigma <= 0.0:
+        raise ValueError("--certify smooths with the training noise sigma and needs --param_noise > 0")
+    n0 = CERTIFY_N0 if n0 is None else n0
+    n = CERTIFY_N if n is None else n
+    alpha = CERTIFY_ALPHA if alpha is None else float(alpha)
+    if int(n0) != n0 or n0 < 1:
+        raise ValueError(f"--certify_n0 {n0} must be an integer >= 1")
+    if int(n) != n or n < 1:
+        raise ValueError(f"--certify_n {n} must be an integer >= 1")
+    if not 0.0 < alpha < 1.0:
+        raise ValueError(f"--certify_alpha {alpha} must lie strictly between 0 and 1")
+    args.certify, args.certify_n0, args.certify_n, args.certify_alpha = True, int(n0), int(n), alpha
+
+
 def print_exp_details(args, n_params: int | None = None) -> None:
     """Experiment banner; same 14 fields as reference src/utils.py:287-303 plus engine fields.  ``n_params``: the model's parameter count,
     which sizes SparseFed's k (shown as ``-`` when not given)."""
@@ -600,6 +648,10 @@ def print_exp_details(args, n_params: int | None = None) -> None:
     if getattr(args, "server_topk", 0.0) > 0:
         k = math.floor(args.server_topk * n_params) if n_params is not None else "-"
         print(f"    Server top-k (SparseFed): {args.server_topk} / {k}")
+    if getattr(args, "param_clip", 0.0) > 0 or getattr(args, "param_noise", 0.0) > 0:
+        print(f"    CRFL (param clip rho / noise sigma): {args.param_clip} / {args.param_noise}")
+    if getattr(args, "certify", False):
+        print(f"    Certify (n0 / n / alpha): {args.certify_n0} / {args.certify_n} / {args.certify_alpha}")
     if getattr(args, "select", "none") in ("krum", "multikrum"):
         print(f"    Selection (F / M): {args.select} ({args.select_f} / {args.select_m})")
     if getattr(args, "select", "none") == "dnc":

@@ -42,6 +42,11 @@ kernel with its barrier-out), and every rank runs the SparseFed passes locally o
 vector ``e``.  ``w'`` is identical on every rank, so ``e`` is too, at every world size: no histogram all-reduce, and rank 0 alone
 checkpoints it.  With the fused hand-off the rank's ``w_global`` is complete when the apply pass ends, so it then marks its own ready
 word of every slice with the round's epoch (no peer publishes during a barrier-out launch).
+
+CRFL's clip-and-perturb pass (``--param_clip`` / ``--param_noise``; ``ops.crfl_statement``) runs the same way, replicated after the
+complete server step: ``w'`` lands in ``scratch``, and every rank clips and perturbs the whole vector locally into ``w_global`` and its
+bf16 shadow (in place on ``w_global`` after SparseFed when both are on).  The noise is keyed by (seed, round, coordinate), so every rank
+draws the same vector and there is no state to keep.
 """
 from __future__ import annotations
 
@@ -60,12 +65,13 @@ FLAG_BYTES = 4096
 class FusedAggregator:
     def __init__(self, ctx, n_total: int, n_vote: int, max_slots: int, backend: str = "auto", with_bf16: bool = True,
                  transport: str = "auto", server_opt=None, n_part: int | None = None, history_agents: int = 0, fld_agents: int = 0,
-                 fld_window: int = 0, topk_k: int = 0):
+                 fld_window: int = 0, topk_k: int = 0, crfl=None):
         """``server_opt``: optional ``dict(kind=..., beta1=..., beta2=..., tau=...)``; ``n_part``: participants per round (default
         every slot), which fixes whether the fused multi-GPU kernel or the gather fallback runs, and so the state layout;
         ``history_agents``: agents whose FoolsGold update history this aggregator keeps (``--aggr foolsgold``: ``--num_agents``; 0 = none);
         ``fld_agents`` / ``fld_window``: agents and window N of the FLDetector state (``--detect fldetector``; 0 = none);
-        ``topk_k``: SparseFed's k (``--server_topk``; 0 = off, nothing allocated)."""
+        ``topk_k``: SparseFed's k (``--server_topk``; 0 = off, nothing allocated); ``crfl``: ``(rho, sigma, mask)`` of CRFL's
+        clip-and-perturb pass (``--param_clip`` / ``--param_noise``, ``ops.real_mask`` words; None = off, nothing allocated)."""
         self.ctx = ctx
         # nccl / gloo back-ends: "gather" all-gathers every participant's parameters and runs the kernel on the copies (any
         # aggregator); "reduce" all-reduces per-coordinate partial sums (vote, weighted update sum) -- O(N) instead of O(K N)
@@ -92,8 +98,10 @@ class FusedAggregator:
         self.off_slots = self.off_wb + 2 * n
         nbytes = self.off_slots + 4 * n * self.max_slots
         self.topk_k = int(topk_k)
+        self.crfl = None if crfl is None else (float(crfl[0]), float(crfl[1]))
+        post = bool(self.topk_k) or self.crfl is not None        # a pass after the plain step: w' goes to scratch
         self.off_scratch = nbytes
-        if self.topk_k:
+        if post:
             nbytes += 4 * n
         use_symm = backend == "fused" and ctx.is_dist
         self.buf = SymmetricBuffer(ctx, nbytes) if use_symm else SymmetricBuffer(_Solo(ctx), nbytes)
@@ -102,12 +110,18 @@ class FusedAggregator:
         self.slots = [self.buf.tensor(self.off_slots + 4 * n * j, n, torch.float32) for j in range(self.max_slots)]
         # SparseFed: the plain step's result w', the error vector e over [0, n_vote) and the round's (|M|, float(tau), ||e||) on the device
         self.scratch = self.sparse_e = self.sparse_stats = None
+        if post:
+            self.scratch = self.buf.tensor(self.off_scratch, n, torch.float32)
         if self.topk_k:
             if not 1 <= self.topk_k <= self.n_vote:
                 raise ValueError(f"SparseFed k = {self.topk_k} must lie in [1, n_vote = {self.n_vote}]")
-            self.scratch = self.buf.tensor(self.off_scratch, n, torch.float32)
             self.sparse_e = torch.zeros(self.n_vote, dtype=torch.float32, device=dev)
             self.sparse_stats = torch.zeros(3, dtype=torch.float64, device=dev)
+        # CRFL: the real-coordinate mask words and the round's (pre-clip norm, scale) on the device
+        self.crfl_mask = self.crfl_stats = None
+        if self.crfl is not None:
+            self.crfl_mask = crfl[2].to(dev)
+            self.crfl_stats = torch.zeros(2, dtype=torch.float64, device=dev)
         self.flipped = torch.zeros(1, dtype=torch.int64, device=dev)
         self.flipped_is_partial = False   # True after a launch in which every rank counted only its own coordinate slice
         self.epoch = 0
@@ -131,7 +145,7 @@ class FusedAggregator:
                 self.out_ptrs = ops.PtrTable([self.buf.peer_ptr(r, self.off_wg) for r in range(world)], dev)
                 self.out_bf16_ptrs = (ops.PtrTable([self.buf.peer_ptr(r, self.off_wb) for r in range(world)], dev)
                                       if self.with_bf16 else None)
-            if self.topk_k:
+            if post:
                 self.scratch_ptrs = ops.PtrTable([self.buf.mc_ptr(self.off_scratch)] if self.use_multimem else
                                                  [self.buf.peer_ptr(r, self.off_scratch) for r in range(world)], dev)
             # coordinate slices: multiples of 4, cover [0, n)
@@ -616,20 +630,20 @@ class FusedAggregator:
             wt = torch.as_tensor(weights, dtype=torch.float64).to(dev)
             sc = torch.as_tensor(scales, dtype=torch.float32).to(dev) if scales is not None else None
             table = self._agent_table(n_part) if members is None else self._member_table(idx)
-            sparse = self.topk_k > 0
-            # SparseFed: w' is multicast into every rank's scratch, behind the kernel's barrier-out (never the hand-off publication)
-            outs = self.scratch_ptrs.tensor if sparse else self.out_ptrs.tensor
-            outs_b = self.out_bf16_ptrs.tensor if (self.out_bf16_ptrs and not sparse) else None
+            post = self.scratch is not None
+            # SparseFed / CRFL: w' is multicast into every rank's scratch, behind the kernel's barrier-out (never the hand-off publication)
+            outs = self.scratch_ptrs.tensor if post else self.out_ptrs.tensor
+            outs_b = self.out_bf16_ptrs.tensor if (self.out_bf16_ptrs and not post) else None
             ops.ext().fused_aggregate(
                 table.tensor, wt, sc, total, self.w_global.data_ptr(),
                 outs, outs_b, self.use_multimem,
                 self.begin, self.end, self.n_vote, ops.MODE_IDS[mode], int(theta), float(server_lr), float(noise_std),
                 int(seed), int(rnd), self.flipped, self.flag_ptrs.tensor, self.local_sync, ctx.rank, ctx.world, self.epoch,
-                bool(self.handoff) and not sparse, *ops.opt_launch_args(self.opt))
-            if sparse:
-                self._sparsefed()
+                bool(self.handoff) and not post, *ops.opt_launch_args(self.opt))
+            if post:
+                self._post_passes(seed, rnd)
                 if self.handoff:
-                    # this rank's w_global is complete: mark its own ready word of every slice (stream-ordered after the apply pass)
+                    # this rank's w_global is complete: mark its own ready word of every slice (stream-ordered after the last pass)
                     world = ctx.world
                     self.buf.tensor(self.off_flags, 3 * world, torch.int32)[2 * world:].fill_(self.epoch)
             if self.handoff:
@@ -638,19 +652,30 @@ class FusedAggregator:
         # ---- baseline transports / single process ------------------------------------------------------------------
         if ctx.is_dist and self.transport == "reduce" and mode in ("avg", "sign") and members is None:
             self._aggregate_reduce(weights, mode, theta, server_lr, noise_std, seed, rnd, scales, total)
-            if self.topk_k:
-                self._sparsefed()
+            if self.scratch is not None:
+                self._post_passes(seed, rnd)
             return
         # gather participant params, run the kernel locally
         agents = self._participants(n_part, participants)
         if members is not None:
             agents = [agents[j] for j in idx]
-        sparse = self.topk_k > 0
+        post = self.scratch is not None
         ops.fused_aggregate(self.w_global, agents, weights, mode, theta, server_lr, noise_std, seed, rnd, self.n_vote,
-                            scales, out=self.scratch if sparse else self.w_global, out_bf16=None if sparse else self.w_bf16,
+                            scales, out=self.scratch if post else self.w_global, out_bf16=None if post else self.w_bf16,
                             flipped=self.flipped, opt=self.opt, total_weight=total)
-        if sparse:
+        if post:
+            self._post_passes(seed, rnd)
+
+    def _post_passes(self, seed, rnd):
+        """The passes after the plain step wrote ``w'`` into ``scratch``, on this rank over the whole vector: SparseFed, then CRFL's clip
+        and noise (in place on ``w_global`` when SparseFed ran, from ``scratch`` otherwise).  Each writes ``w_global`` and its shadow."""
+        src = self.scratch
+        if self.topk_k:
             self._sparsefed()
+            src = self.w_global
+        if self.crfl is not None:
+            ops.crfl_step(self.w_global, src, self.crfl_mask, self.n_vote, self.crfl[0], self.crfl[1], seed, rnd, self.crfl_stats,
+                          self.w_bf16)
 
     def _sparsefed(self):
         """SparseFed after the plain step wrote ``w'`` into ``scratch``: ``ops.sparsefed_step`` over the whole vector on this rank, which
@@ -686,8 +711,8 @@ class FusedAggregator:
             noise[self.n_vote:] = 0
         new, nflip = ops.aggregate_from_partials(self.w_global, vote, wsum, total_weight, mode, theta, server_lr,
                                                  noise, self.n_vote, self.opt)
-        if self.topk_k:
-            self.scratch.copy_(new)                  # SparseFed's pass follows (aggregate)
+        if self.scratch is not None:
+            self.scratch.copy_(new)                  # SparseFed's / CRFL's passes follow (aggregate)
         else:
             self.w_global.copy_(new)
             if self.w_bf16 is not None:

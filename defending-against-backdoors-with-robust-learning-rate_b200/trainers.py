@@ -164,6 +164,18 @@ class TorchTrainer:
         return torch.cat([self._feat_net(x[s:s + self.bs], tap=tap) for s in range(0, x.shape[0], self.bs)])
 
 
+    @torch.no_grad()
+    def certify_executor(self):
+        """CRFL certification's executor, built once: ``(w, w_bf16, prepare, forward)``.  ``w`` is a dedicated fp32 parameter buffer that
+        ``ops.crfl_smooth`` rewrites for every draw (this trainer reads no bf16 shadow: ``w_bf16`` is None); ``prepare(x)`` turns a
+        normalised NCHW batch into the executor's input once, and ``forward(xb)`` returns its fp32 logits in eval mode."""
+        if getattr(self, "_cert", None) is None:
+            w = torch.zeros(self.layout.n_total, dtype=torch.float32, device=self.device)
+            net = GraphNet(self.layout, w, None, self.compute_dtype)
+            net.eval()
+            self._cert = (w, None, lambda x: x.contiguous(), lambda xb: net(xb).float())
+        return self._cert
+
 def make_trainer(kind, layout, args, device, max_shard):
     dev = torch.device(device)
     if kind == "auto":
